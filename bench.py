@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- GCRA decisions/sec on B200 (BASELINE.json metric), one JSON line.
+"""bench.py -- GCRA decisions/sec on one H100 or more (BASELINE.json metric), one JSON line.
 
 A "step" is one tick: one pass of the hot path over one batch of 2^20 synthetic requests.
 
@@ -20,6 +20,10 @@ parity       the CPU oracle (C++ restatement of the reference; the reference is 
              here) replays the SAME trace: at N=1 the whole 10 M-key trace (warm pass + every tick), at
              N>1 a key subset (the hottest keys + sampled cold keys; keys are independent) of the first ticks
 cpu_baseline that oracle replay, timed (single thread = the reference's design point)
+
+`--dump-outputs DIR` writes the results of the last timed tick (rank 0's slice at N>1), one float64 array per
+result field, as DIR/<field>.npy: the inputs are generated from fixed seeds, so two builds run with the same
+arguments can be compared output for output.
 
 `--impl reference` times the CPU restatement on all host cores (hash-sharded stores, built ONCE at the
 full key count) on the same config instead.
@@ -49,18 +53,16 @@ UNIT = "decisions/s"
 REF_TICKS_PER_STEP = 2
 
 
-def measured_peak_gbs():
-    try:
-        return float(json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["hbm_gbs"]), "measured"
-    except Exception:
-        return 6650.0, "fallback"
+RESULT_FIELDS = ("remaining", "reset_after_ns", "retry_after_ns", "status", "allowed")
+# NVIDIA's data sheet for the H100 SXM (HBM3): a bound, not a reached figure
+PEAK_HBM_GBS = 3350.0
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons / power limit during the timed region (read-only queries)."""
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,"
          "clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
-         "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
+         "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap,power.limit")
 
     def __init__(self, gpu=0):
         self.gpu, self.rows, self.proc = gpu, [], None
@@ -81,24 +83,25 @@ class ClockSampler:
 
     def stop(self):
         if not self.proc:
-            return {"sm_mhz": None, "sm_max_mhz": None, "reasons": ["nvidia-smi unavailable"]}
+            return {"sm_mhz": None, "sm_max_mhz": None, "power_limit_w": None, "reasons": ["nvidia-smi unavailable"]}
         self.proc.terminate()
         try:
             self.proc.wait(timeout=2)
         except Exception:
             self.proc.kill()
-        sm, mx, reasons = [], [], set()
+        sm, mx, limit, reasons = [], [], None, set()
         names = ["hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown", "sw_power_cap"]
         for r in self.rows:
             try:
                 sm.append(float(r[1])); mx.append(float(r[2]))
+                limit = float(r[9])
                 for nm, v in zip(names, r[5:9]):
                     if v.lower().startswith("active"):
                         reasons.add(nm)
             except Exception:
                 pass
         return {"sm_mhz": float(np.median(sm)) if sm else None,
-                "sm_max_mhz": float(max(mx)) if mx else None,
+                "sm_max_mhz": float(max(mx)) if mx else None, "power_limit_w": limit,
                 "samples": len(sm), "reasons": sorted(reasons)}
 
 
@@ -154,8 +157,6 @@ def run_reference(args, rank, world):
         _, sec = oracle.replay_sharded(stores, tr)               # timed: the decision loops only
         if s >= W:
             vals.append(len(tr) / sec)
-        if time.time() - t0 > 270 and len(vals) >= 3:
-            break
     value = float(np.median(vals))
     line = {
         "impl": "reference", "metric": METRIC, "value": value, "unit": UNIT, "n_gpus": args.gpus,
@@ -228,6 +229,8 @@ def main():
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--no-sweep", action="store_true")
     ap.add_argument("--sustain-sec", type=float, default=0.5)
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed tick's results as DIR/<field>.npy (float64)")
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -252,7 +255,8 @@ def main():
     W, K = max(args.warmup, 3), args.steps
     n_local_keys = args.keys
     n_keys = n_local_keys * world
-    peak, peak_kind = measured_peak_gbs()
+    peak, peak_kind = PEAK_HBM_GBS, "datasheet"
+    props = torch.cuda.get_device_properties(dev)
 
     # ---------------------------------------------------------------- synthetic workload
     t0 = time.time()
@@ -348,6 +352,8 @@ def main():
     res_np = res_all[W:]
     n_allowed = int(res_np["allowed"].sum())
     n_ok = int((res_np["status"] == 0).sum())
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, res_all[W + K - 1])
 
     # ---------------------------------------------------------------- sustained: the resident ticks cycled
     sustained = None
@@ -587,16 +593,24 @@ def main():
                                 "(BASELINE configs[4] shape)" % (n_keys // 1_000_000, world)),
                    "sharded_pipeline": (None if world == 1 else sh.describe()),
                    "keys": n_keys, "tick": TICK, "request_bytes": 48, "result_bytes": 32,
-                   "l2": "no flush: table %.2f GB and a distinct 80 MB tick per step exceed the 126 MB L2"
-                         % (stats1["table_slots"] * 32 / 1e9),
+                   "l2": "no flush: table %.2f GB and a distinct 80 MB tick per step exceed the %d MB L2"
+                         % (stats1["table_slots"] * 32 / 1e9, props.L2_cache_size >> 20),
                    "allowed_fraction": n_allowed / max(n_ok, 1), "gen_seconds": round(gen_s, 1)},
         "host_enqueue_ms_per_step": {"min": min(step_ms), "median": float(np.median(step_ms)), "max": max(step_ms)},
         "roofline": roof, "sweep": sweep, "sustained": sustained, "parity": parity, "cpu_baseline": cpu, "e2e": e2e,
-        "gpu_launches": int(launches), "clocks": clocks,
+        "gpu_launches": int(launches), "device": props.name, "clocks": clocks,
     }
     print(json.dumps(line), flush=True)
     if dist:
         dist.destroy_process_group()
+
+
+def dump_outputs(out_dir, res):
+    """What a caller of the timed path receives for one tick: every result field as float64 (exact: the fields are
+    integers below 2^53 for the benchmark's policies), 2^20 rows x 8 B x 5 fields = 40 MiB."""
+    os.makedirs(out_dir, exist_ok=True)
+    for f in RESULT_FIELDS:
+        np.save(os.path.join(out_dir, f + ".npy"), res[f].astype(np.float64))
 
 
 def sharded_parity(tc, oracle, dist, rank, world, n_keys, n_local_keys, tr, res_all, W, K, n_ticks=4):

@@ -1,5 +1,5 @@
 /*
- * gcra_b200.h -- C ABI of the B200-native batched GCRA rate-limit engine.
+ * gcra_b200.h -- C ABI of the H100-native (sm_90a) batched GCRA rate-limit engine.
  *
  * This is the drop-in boundary for ONE path of lazureykis/throttlecrab: the GCRA
  * decide-and-update behind `RateLimiter::rate_limit` over a `Store`, plus the

@@ -1,4 +1,4 @@
-"""throttlecrab_b200 -- B200-native batched GCRA rate-limit engine (host-side mirror).
+"""throttlecrab_b200 -- H100-native batched GCRA rate-limit engine (host-side mirror).
 
 Mirrors the part of lazureykis/throttlecrab's library API that sits on the hot path:
 

@@ -15,7 +15,7 @@ _ROOT = os.path.dirname(_PKG)
 _SRC = os.path.join(_PKG, "csrc")
 SO_PATH = os.environ.get("GCRA_SO") or os.path.join(_PKG, "libgcra_b200.so")   # GCRA_SO: tuning variants
 
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+NVCC_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
               "--shared", "-Xcompiler", "-fPIC", "-Xcompiler", "-pthread", "-ldl"]
 
 REQ_DTYPE = np.dtype([("key_hash", "<u8"), ("max_burst", "<i8"), ("count_per_period", "<i8"),
@@ -51,7 +51,7 @@ def sources():
 
 
 def build(force=False, verbose=False):
-    """nvcc cross-compiles for sm_100a without a GPU; the .so is kept in-tree."""
+    """nvcc cross-compiles for sm_90a (H100) without a GPU; the .so is kept in-tree."""
     srcs = sources()
     if os.environ.get("GCRA_SO"):
         return SO_PATH                      # a prebuilt tuning variant

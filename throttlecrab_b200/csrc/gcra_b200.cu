@@ -172,6 +172,7 @@ struct Scratch {
 
 struct gcra_engine {
     int device = 0;
+    uint32_t sms = 0;                // streaming multiprocessors of the device: sizes the grids of the streaming kernels
     cudaStream_t stream = nullptr, in_stream = nullptr, out_stream = nullptr, aux_stream = nullptr, aux2_stream = nullptr;
     Table tab{};
     uint32_t total_lines = 0;
@@ -232,7 +233,7 @@ struct gcra_engine {
     uint32_t index_min = 0;          // batches of at least this many rows take the index-order pipeline (0: never)
     int prefetch_state = 0;
     uint32_t max_tiles = 0;
-    uint32_t grid_probe[2] = {592, 592}, grid_decide[2] = {444, 444};   // resident CTAs of the persistent kernels [compact]
+    uint32_t grid_probe[2] = {}, grid_decide[2] = {};   // resident CTAs of the persistent kernels [compact]
     uint32_t dbg = 0;                // timing experiments only (gcra_debug_set): skips parts of pass B
     uint32_t last_nres = 0, last_nres_rows = 0;   // newest residue size that has reached the host (and its batch's rows)
     bool adaptive = true;            // choose the pipeline from the residue feedback (off when a test / env forces one)
@@ -282,7 +283,7 @@ static int alloc_table(gcra_engine *h, uint64_t capacity, Table &t, uint32_t &to
     t.null_slot = total_lines * 4 - 1;
     t.slot_bits = ceil_log2((uint64_t)total_lines * 4);
     t.counters = counters;
-    uint32_t grid = (uint32_t)std::min<size_t>((slots + TILE_THREADS - 1) / TILE_THREADS, 148 * 16);
+    uint32_t grid = (uint32_t)std::min<size_t>((slots + TILE_THREADS - 1) / TILE_THREADS, 16 * h->sms);
     clear_slots_kernel<<<grid, TILE_THREADS, 0, h->stream>>>(t, 0, slots);
     h->launches++;
     CK(cudaGetLastError());
@@ -313,7 +314,7 @@ static int do_sweep(gcra_engine *h, int64_t now_ns, uint64_t *removed) {
     CK(cudaDeviceSynchronize());   // the sweep is exclusive: batches may be in flight on caller streams
     RC(refresh_counters(h, true));
     uint64_t before = h->h_counters[C_SWEPT];
-    uint32_t grid = (uint32_t)std::min<uint64_t>(((uint64_t)h->total_lines * 2 + TILE_THREADS * SWEEP_UNROLL - 1) / (TILE_THREADS * SWEEP_UNROLL), 148 * 16);
+    uint32_t grid = (uint32_t)std::min<uint64_t>(((uint64_t)h->total_lines * 2 + TILE_THREADS * SWEEP_UNROLL - 1) / (TILE_THREADS * SWEEP_UNROLL), 16 * h->sms);
     CK(cudaEventRecord(h->ev_sweep[0], h->stream));
     static const int sweep_mode = getenv("GCRA_SWEEP_MODE") ? atoi(getenv("GCRA_SWEEP_MODE")) : 0;
     sweep_kernel<<<grid, TILE_THREADS, 0, h->stream>>>(h->tab, (u64)h->total_lines * 4, now_ns, sweep_mode);
@@ -333,7 +334,7 @@ static int do_sweep(gcra_engine *h, int64_t now_ns, uint64_t *removed) {
 static int purge(gcra_engine *h) {
     CK(cudaDeviceSynchronize());
     const uint64_t slots = (uint64_t)h->total_lines * 4;
-    uint32_t grid = (uint32_t)std::min<uint64_t>((slots + TILE_THREADS - 1) / TILE_THREADS, 148 * 16);
+    uint32_t grid = (uint32_t)std::min<uint64_t>((slots + TILE_THREADS - 1) / TILE_THREADS, 16 * h->sms);
     purge_kernel<<<grid, TILE_THREADS, 0, h->stream>>>(h->tab, slots);
     h->launches++;
     CK(cudaGetLastError());
@@ -364,7 +365,7 @@ static int grow(gcra_engine *h, uint64_t need) {
     CK(cudaMemsetAsync(ncounters, 0, C_COUNT * sizeof(u64), h->stream));
     int rc = alloc_table(h, newcap, nt, nl, ncounters);
     if (rc) return rc;
-    uint32_t grid = std::min<uint32_t>((h->total_lines + TILE_THREADS - 1) / TILE_THREADS, 148 * 8);
+    uint32_t grid = std::min<uint32_t>((h->total_lines + TILE_THREADS - 1) / TILE_THREADS, 8 * h->sms);
     rehash_kernel<<<grid, TILE_THREADS, 0, h->stream>>>(h->tab, (u64)h->total_lines * 4, nt);
     h->launches++;
     CK(cudaGetLastError());
@@ -548,7 +549,7 @@ static int enqueue_sort(gcra_engine *h, Scratch &sc, uint32_t n_max, const u32 *
         // fixed grid, all CTAs resident (grid barriers), the kernels loop over the tiles: sized for about twice the
         // residue the host saw last (a barrier over few CTAs is cheaper), any size is correct
         const uint32_t guess = (uint32_t)std::min<uint64_t>(std::max<uint64_t>(2ULL * h->last_nres, n_max / 8) + 8 * SORT_TILE, n_max);
-        stiles = std::max<uint32_t>(std::min<uint32_t>((guess + SORT_TILE - 1) / SORT_TILE, 2 * 148), 8);
+        stiles = std::max<uint32_t>(std::min<uint32_t>((guess + SORT_TILE - 1) / SORT_TILE, 2 * h->sms), 8);
     }
     u64 *src = sc.keys_a, *dst = sc.keys_b;
     uint32_t shift = 32;
@@ -579,7 +580,7 @@ static int enqueue_decide_sorted_t(gcra_engine *h, Scratch &sc, uint32_t n_max, 
     if (BY_ROW) CK(cudaMemsetAsync(sc.long_count, 0, 2 * sizeof(u32), st));
     const uint32_t warps = (n_max + 31) / 32;
     uint32_t grid = (warps + DECIDE_THREADS / 32 - 1) / (DECIDE_THREADS / 32);
-    if (n_dev) grid = std::min<uint32_t>(grid, 4 * 148);
+    if (n_dev) grid = std::min<uint32_t>(grid, 4 * h->sms);
     decide_kernel<BY_ROW><<<grid, DECIDE_THREADS, 0, st>>>(h->tab, src, sc.drec, n_max, n_dev, om, sc.long_runs, sc.giant_runs,
                                                            sc.long_count, 0);
     h->launches++;
@@ -588,13 +589,13 @@ static int enqueue_decide_sorted_t(gcra_engine *h, Scratch &sc, uint32_t n_max, 
         // stream and overlaps the cluster kernel (fork/join with events)
         CK(cudaEventRecord(sc.ev_fork, st));
         CK(cudaStreamWaitEvent(h->aux_stream, sc.ev_fork, 0));
-        decide_runs_kernel<1, BY_ROW><<<148, LONG_THREADS, 0, h->aux_stream>>>(h->tab, src, sc.drec, om, sc.long_runs, sc.long_count);
+        decide_runs_kernel<1, BY_ROW><<<h->sms, LONG_THREADS, 0, h->aux_stream>>>(h->tab, src, sc.drec, om, sc.long_runs, sc.long_count);
         CK(cudaEventRecord(sc.ev_join, h->aux_stream));
         RC(launch_giant<BY_ROW>(h, sc, src, om, st));   // hottest keys: one cluster per run
         CK(cudaStreamWaitEvent(st, sc.ev_join, 0));
         h->launches += 2;
     } else if (n_max >= LONG_RUN_MIN) {
-        decide_runs_kernel<1, BY_ROW><<<148, LONG_THREADS, 0, st>>>(h->tab, src, sc.drec, om, sc.long_runs, sc.long_count);
+        decide_runs_kernel<1, BY_ROW><<<h->sms, LONG_THREADS, 0, st>>>(h->tab, src, sc.drec, om, sc.long_runs, sc.long_count);
         h->launches++;
     }
     return GCRA_OK;
@@ -702,7 +703,7 @@ static int enqueue_mid_index(gcra_engine *h, Scratch &sc, Scratch &next, const B
     }
     const uint32_t rows = view_max_rows(v);
     const uint32_t grid = std::min<uint32_t>((rows + TILE_THREADS - 1) / TILE_THREADS, h->grid_decide[compact ? 1 : 0]);   // persistent CTAs
-    const uint32_t rgrid = std::min<uint32_t>((rows + RES_TILE - 1) / RES_TILE + v.nseg, 6 * 148);
+    const uint32_t rgrid = std::min<uint32_t>((rows + RES_TILE - 1) / RES_TILE + v.nseg, 6 * h->sms);
     u32 *ctrl = reinterpret_cast<u32 *>(sc.ctrl_block);
     u64 *status = sc.ctrl_block + 2;
     if (compact) {
@@ -962,6 +963,10 @@ int32_t gcra_create(const gcra_config *cfg, gcra_engine **out) {
     if (cfg->device < 0 || cfg->device >= ndev) return fail("bad device ordinal", cudaErrorInvalidDevice);
     h->device = cfg->device;
     if ((e = cudaSetDevice(h->device)) != cudaSuccess) return fail("cudaSetDevice", e);
+    int sms = 0;
+    if ((e = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, h->device)) != cudaSuccess || sms <= 0)
+        return fail("cudaDevAttrMultiProcessorCount", e);
+    h->sms = (uint32_t)sms;
     if (const char *g = getenv("GCRA_L2_FETCH")) cudaDeviceSetLimit(cudaLimitMaxL2FetchGranularity, (size_t)atoi(g));
     if ((e = cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking)) != cudaSuccess) return fail("stream", e);
     cudaStreamCreateWithFlags(&h->in_stream, cudaStreamNonBlocking);
@@ -1016,8 +1021,9 @@ int32_t gcra_create(const gcra_config *cfg, gcra_engine **out) {
         if (const char *g = getenv("GCRA_ADAPTIVE")) h->adaptive = atoi(g) != 0;
         h->prefetch_state = 0;
         if (const char *g = getenv("GCRA_PREFETCH")) h->prefetch_state = atoi(g);
-        int sms = 148, nb = 0;
-        cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, h->device);
+        int nb = 0;
+        h->grid_probe[0] = h->grid_probe[1] = 4 * h->sms;      // used when the occupancy query fails
+        h->grid_decide[0] = h->grid_decide[1] = 3 * h->sms;
         if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, probe_kernel<false>, TILE_THREADS, 0) == cudaSuccess && nb > 0) h->grid_probe[0] = (uint32_t)(nb * sms);
         if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, probe_kernel<true>, TILE_THREADS, 0) == cudaSuccess && nb > 0) h->grid_probe[1] = (uint32_t)(nb * sms);
         if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, decide_index_kernel<false>, TILE_THREADS, 0) == cudaSuccess && nb > 0) h->grid_decide[0] = (uint32_t)(nb * sms);

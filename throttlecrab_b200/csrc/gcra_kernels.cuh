@@ -1,4 +1,4 @@
-// gcra_kernels.cuh -- the sm_100a kernels of the batched GCRA engine.
+// gcra_kernels.cuh -- the sm_90a (H100) kernels of the batched GCRA engine.
 //
 //   K1a ingest  : bulk-async (TMA, UBLKCP) staging of a request tile into shared memory, per-request
 //                 validation + parameter derivation (rate_limiter.rs:111-122), key -> slot probe/claim

@@ -16,8 +16,7 @@ route (partition, count exchange, request all-to-all), decide (the engine's kern
 (result all-to-all, un-permutation).  Each stage's collectives use their own communicator so that
 NCCL does not serialise the stages of neighbouring ticks; tick i+1 is routed while tick i is decided
 and tick i-1's results travel back.  `DEPTH` buffer sets are cycled; `finish()` drains.
-`step()` = submit + finish (blocking).  Measured stage times (2 x B200, 2^20-request ticks):
-partition 0.07 ms, counts 0.10, requests 0.12, decide 0.34, results 0.16, unpermute 0.03.
+`step()` = submit + finish (blocking).
 
 torch is plumbing only: device buffers, the NCCL process group and stream/event ordering.
 """

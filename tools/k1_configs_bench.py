@@ -23,8 +23,7 @@ ap.add_argument("--configs", default="zipf,hot100,uniform100m")
 ap.add_argument("--steps", type=int, default=12)
 args = ap.parse_args()
 TICK, W, K = 1 << 20, 3, args.steps
-peak = float(json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))["hbm_gbs"]) \
-    if os.path.exists(os.path.join(ROOT, "MEASURED_PEAKS.json")) else 6650.0
+peak = 3350.0        # GB/s, NVIDIA's data sheet for the H100 SXM (HBM3): a bound, not a reached figure
 dev = torch.device("cuda", 0)
 stream = torch.cuda.Stream(dev)
 torch.cuda.set_stream(stream)
@@ -75,7 +74,7 @@ for name in args.configs.split(","):
     ph = st.last_kernel_ms()
     print(json.dumps({"config": name, "keys": n_keys, "tick": TICK, "ms_per_tick": ms,
                       "decisions_per_s": TICK / ms * 1e3, "allowed_fraction": n_allowed / (K * TICK),
-                      "k1_algorithmic_GBps": alg / (ms * K) / 1e6, "frac_of_measured_peak": alg / (ms * K) / 1e6 / peak,
+                      "k1_algorithmic_GBps": alg / (ms * K) / 1e6, "frac_of_datasheet_peak": alg / (ms * K) / 1e6 / peak,
                       "last_tick_phase_ms": {"ingest": ph[1], "order": ph[2], "decide": ph[3]},
                       "table_slots": st.stats()["table_slots"], "stash_entries": st.stats()["stash_entries"]}),
           flush=True)
