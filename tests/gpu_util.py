@@ -37,6 +37,19 @@ def replay_both(req, capacity, batch, max_batch=None, store_cls=None, oracle_kin
     return res_o, res_e, st_o, st_e
 
 
+def replay_skipping_refused(store, req, res_e, what=""):
+    """For paths that may refuse rows (GCRA_INTERNAL: table full, residue beyond max_batch): feed the oracle `store`
+    only the rows the engine did NOT refuse, and require each of them to be bit-identical.  A refused row leaves no
+    trace in the engine, so this is exact.  Returns the indices of the refused rows."""
+    refused = np.nonzero(res_e["status"] == tc.INTERNAL)[0]
+    keep = np.ones(len(req), bool)
+    keep[refused] = False
+    res_o = store.replay(req[keep])
+    bad = first_mismatch(res_o, res_e[keep], req[keep])
+    assert bad is None, what + bad + " (%d refused rows skipped)" % len(refused)
+    return refused
+
+
 def first_mismatch(res_o, res_e, req=None):
     a = res_o.view(np.uint8).reshape(len(res_o), -1)
     b = res_e.view(np.uint8).reshape(len(res_e), -1)

@@ -29,11 +29,21 @@ def _worker(rank, world, port, n_keys, n_ticks, tick, ret, native=False):
     return _worker_impl(rank, world, port, n_keys, n_ticks, tick, ret, "native" if native else "torch")
 
 
-def _worker_p2p(rank, world, port, n_keys, n_ticks, tick, ret):
-    return _worker_impl(rank, world, port, n_keys, n_ticks, tick, ret, "p2p")
+def _worker_p2p(rank, world, port, n_keys, n_ticks, tick, ret, trace="config4"):
+    return _worker_impl(rank, world, port, n_keys, n_ticks, tick, ret, "p2p", trace)
 
 
-def _worker_impl(rank, world, port, n_keys, n_ticks, tick, ret, kind):
+def _global_trace(trace, n_keys, n_ticks, tick, world):
+    """the union trace of all ranks, tick by tick (rank r's rows of tick t: [(t world + r) tick, +tick))"""
+    import traces
+    if trace == "config4":
+        return traces.config4(n_keys=n_keys, n_ticks=n_ticks, tick_size=tick * world, hot=20)
+    # flood: every row on one key, ticks at T0, +1 ms, +1 s (tests/test_gpu_p2p_skew.py)
+    import p2p_loopback_worker as w
+    return np.concatenate([w.flood(tick * world, traces.T0 + ms * 1_000_000) for ms in (0, 1, 1000)[:n_ticks]])
+
+
+def _worker_impl(rank, world, port, n_keys, n_ticks, tick, ret, kind, trace="config4"):
     import torch.distributed as dist
     os.environ.update(MASTER_ADDR="127.0.0.1", MASTER_PORT=str(port))
     torch.cuda.set_device(rank)
@@ -43,9 +53,11 @@ def _worker_impl(rank, world, port, n_keys, n_ticks, tick, ret, kind):
     import traces
     from throttlecrab_b200.sharded import NativeShardedLimiter, PeerShardedLimiter, ShardedLimiter
     key_hash_of = tc.hash_key_ids(np.arange(n_keys, dtype=np.uint64))
-    lim = tc.RateLimiter(tc.ManualStore(capacity=n_keys, device=rank, created_ns=traces.T0, max_batch=2 * tick))
+    # (flood: table room for the 1.25 x tick rows an engine reserves per tick, so that no tick grows the table)
+    lim = tc.RateLimiter(tc.ManualStore(capacity=n_keys if trace == "config4" else 6_000_000, device=rank,
+                                        created_ns=traces.T0, max_batch=2 * tick))
     sh = {"native": NativeShardedLimiter, "torch": ShardedLimiter, "p2p": PeerShardedLimiter}[kind](lim, dist, dev)
-    glob = traces.config4(n_keys=n_keys, n_ticks=n_ticks, tick_size=tick * world, hot=20)
+    glob = _global_trace(trace, n_keys, n_ticks, tick, world)
     stream = torch.cuda.Stream(dev)
     torch.cuda.set_stream(stream)
     reqs, ress = [], []
@@ -61,7 +73,13 @@ def _worker_impl(rank, world, port, n_keys, n_ticks, tick, ret, kind):
         sh.submit(reqs[t], ress[t])            # pipelined across ticks
     sh.finish()
     torch.cuda.synchronize()
-    ret[rank] = np.concatenate([r.cpu().numpy() for r in ress]).tobytes()
+    if kind == "p2p":
+        assert sh.error() == 0, "a peer-memory wait gave up"
+    out = np.concatenate([r.cpu().numpy() for r in ress])
+    if isinstance(ret, str):                  # large runs: through a file, not the manager's pipe
+        np.save(os.path.join(ret, "rank%d.npy" % rank), out)
+    else:
+        ret[rank] = out.tobytes()
     dist.barrier()
     dist.destroy_process_group()
 
@@ -92,7 +110,7 @@ def _union_trace_check(ret, world, n_keys, n_ticks, tick, glob=None):
     import oracle
     import traces
     if glob is None:
-        glob = traces.config4(n_keys=n_keys, n_ticks=n_ticks, tick_size=tick * world, hot=20)
+        glob = _global_trace("config4", n_keys, n_ticks, tick, world)
     want = oracle.OracleStore(oracle.PERIODIC, capacity=n_keys, created_ns=traces.T0, p0=10**9).replay(glob)
     got = np.empty(len(glob), oracle.RES_DTYPE)
     for r in range(world):
@@ -105,17 +123,22 @@ def _union_trace_check(ret, world, n_keys, n_ticks, tick, glob=None):
     assert want["allowed"].sum() > 0 and (want["allowed"] == 0).sum() > 0
 
 
-@pytest.mark.timeout(600)
-def test_two_gpu_peer_memory_matches_single_oracle():
+@pytest.mark.timeout(1200)
+@pytest.mark.parametrize("trace", ["config4", "flood"])
+def test_two_gpu_peer_memory_matches_single_oracle(trace, tmp_path, k1_path):
     """gcra_p2p_*: rows stored straight into the owner's inbox over NVLink, results straight into the sender's
-    outbox; two processes, CUDA IPC windows."""
+    outbox; two processes, CUDA IPC windows.  `flood`: 3 ticks of 2 x 2^22 rows on ONE key (fresh, saturated, 1 s
+    later), so the owner's batch spans 32768 tiles, each holding the key 256 times (tests/test_gpu_p2p_skew.py)."""
     if torch.cuda.device_count() < 2:
         pytest.skip("needs 2 GPUs")
+    if trace == "flood" and k1_path != "auto":
+        pytest.skip("a segmented tick takes the index-order pipeline whatever K1 path is forced")
     world, n_keys, n_ticks, tick = 2, 50_000, 6, 1 << 16
-    mgr = mp.Manager()
-    ret = mgr.dict()
-    mp.spawn(_worker_p2p, args=(world, _free_port(), n_keys, n_ticks, tick, ret), nprocs=world, join=True)
-    _union_trace_check(ret, world, n_keys, n_ticks, tick)
+    if trace == "flood":
+        n_keys, n_ticks, tick = 1, 3, 1 << 22
+    mp.spawn(_worker_p2p, args=(world, _free_port(), n_keys, n_ticks, tick, str(tmp_path), trace), nprocs=world, join=True)
+    ret = {r: np.load(str(tmp_path / ("rank%d.npy" % r))).tobytes() for r in range(world)}
+    _union_trace_check(ret, world, n_keys, n_ticks, tick, _global_trace(trace, n_keys, n_ticks, tick, world))
 
 
 @pytest.mark.timeout(600)

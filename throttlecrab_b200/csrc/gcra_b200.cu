@@ -161,7 +161,7 @@ struct Scratch {
     // index-order pipeline (gcra_index_path.cuh)
     u32 *slot_arr = nullptr;            // [rows] slot of every row (null slot: the row failed validation)
     unsigned char *flags = nullptr;     // [rows] pass-B verdict of rows on shared slots
-    u32 *bitmap = nullptr;              // [bm_words] 16-bit occurrence counters of the batch, hashed by slot
+    u32 *bitmap = nullptr;              // [bm_words] 32-bit occurrence counters of the batch, hashed by slot
     u32 *pend = nullptr;                // [pend_words] 1 bit per entry: the PREVIOUS batch's tail owns a slot of the entry
     u64 *ctrl_block = nullptr;          // word 0: {tile ticket, residue count}; word 1: {sort barrier, -}; then one status word per tile
     uint32_t rows_alloc = 0;
@@ -640,10 +640,8 @@ static int enqueue_denied(gcra_engine *h, const BatchView &v, bool compact, cuda
 }
 
 static bool use_index_path(const gcra_engine *h, uint32_t n) {
-    // The batch counters are 16-bit fields that receive at most 2 per distinct slot and 256-row tile.  Slots that
-    // share a hashed entry add up: k slots that occur in EVERY tile reach 2 k x tiles.  Up to 2^21 rows (8192 tiles)
-    // that stays below 65536 unless four such ultra-hot keys (each > 0.4 % of the traffic) hash to one of the 2^23+
-    // entries; larger batches take the sort pipeline.
+    // A performance choice only: both pipelines are exact at any size (the index-order pipeline's batch counters
+    // hold any batch's row count, gcra_index_path.cuh).  Single batches above 2^21 rows take the sort pipeline.
     return h->index_min != 0 && n >= h->index_min && n <= (1u << 21);
 }
 
@@ -1007,15 +1005,18 @@ int32_t gcra_create(const gcra_config *cfg, gcra_engine **out) {
     const size_t mb = h->max_batch;
     const uint32_t stiles = (uint32_t)((mb + SORT_TILE - 1) / SORT_TILE);
     {
-        // index-order pipeline: hashed batch counters (16 bits) and pend bits, 8 entries per row of the largest
+        // index-order pipeline: hashed batch counters (32 bits) and pend bits, 8 entries per row of the largest
         // batch (n distinct slots share their entry with probability ~1/8), 64 K .. 16 M entries
         uint32_t lg = ceil_log2(std::max<uint64_t>(8ULL * mb, 1ULL << 16));
         if (lg > 24) lg = 24;
         h->bm_mask = (1u << lg) - 1;
-        h->bm_words = (size_t)1 << (lg - 1);      // 16-bit counters, 2 per word
+        h->bm_words = (size_t)1 << lg;            // one 32-bit counter per entry
         h->pend_words = (size_t)1 << (lg - 5);    // 1 bit per entry
         h->index_min = 32768;
         if (const char *g = getenv("GCRA_INDEX_MIN")) { h->index_min = (uint32_t)atoll(g); h->adaptive = false; }
+        // tests only: the batch epoch to count on from, so that a test can cross the 32-bit wrap (which clears every
+        // mark, enqueue_mid_index) in a few batches instead of 4 G
+        if (const char *g = getenv("GCRA_EPOCH0")) h->epoch = (uint32_t)strtoull(g, nullptr, 0);
         if (cfg->flags & GCRA_FLAG_INDEX_PATH) { h->index_min = SMALL_MAX + 1; h->adaptive = false; }
         if (cfg->flags & GCRA_FLAG_SORT_PATH) { h->index_min = 0; h->adaptive = false; }
         if (const char *g = getenv("GCRA_ADAPTIVE")) h->adaptive = atoi(g) != 0;
@@ -1870,7 +1871,7 @@ int32_t gcra_p2p_prepare(gcra_engine *h, int32_t rank, int32_t world, uint32_t c
     p->rank = rank; p->world = world;
     p->cap_shift = std::max<uint32_t>(ceil_log2(cap_rows), 10);      // whole resolve tiles per segment
     p->cap = 1u << p->cap_shift;
-    if (((uint64_t)world << p->cap_shift) >= (1ULL << 31)) { delete p; h->err = "world * cap_rows too large"; return GCRA_INTERNAL; }
+    if (((uint64_t)world << p->cap_shift) >= INDEX_MAX_ROWS) { delete p; h->err = "world * cap_rows too large"; return GCRA_INTERNAL; }
     const size_t seg_rows = (size_t)P2P_DEPTH * world * p->cap;
     p->inbox_off = align_up(sizeof(P2PHeader), 256);
     p->outbox_off = align_up(p->inbox_off + seg_rows * sizeof(gcra_request), 256);

@@ -84,18 +84,22 @@ __device__ __forceinline__ void stage_tile(unsigned char *stage, u64 *bar, const
 
 // Batch-local knowledge about slots, both hashed by (slot & mask) -- a hashed index only merges slots, and a false
 // "shared" / "pending" verdict costs time, never exactness:
-//   counters  16 bits per entry: how often the entry's slots occur in THIS batch, as far as that matters: pass A
+//   counters  32 bits per entry: how often the entry's slots occur in THIS batch, as far as that matters: pass A
 //             finds the distinct slots of every 256-row tile with a hash set in shared memory and adds
 //             min(count in the tile, 2) per distinct slot with ONE posted RED (no global atomic ever returns a
 //             value: returning atomics are throttled by the few that an SM can keep in flight).  >= 2 <=> shared.
-//             At most 2 x (number of tiles) per slot: the host keeps batches of more than 2^21 rows off this
-//             pipeline, so even several ultra-hot slots sharing one entry stay far below 65536.
+//             A tile adds at most its row count (256) to an entry, whatever slots share the entry, so an entry
+//             never exceeds the batch's rows -- below INDEX_MAX_ROWS, which a 32-bit counter holds.  (16-bit
+//             counters would wrap: one key in every row of a 2^23-row multi-GPU tick adds 2 x 32768 = 65536.)
 //   pend      1 bit per entry, written by the PREVIOUS batch's pass C: a slot of the entry still has residue
 //             requests in that batch's sorted tail, which may run concurrently with this batch's passes B and C;
 //             this batch's requests on such a slot are deferred to its own tail (tails run one after another)
+// Row ids of an index-order batch: a single batch has at most 2^21 rows (use_index_path), a multi-GPU tick spans
+// world x cap_rows < 2^31 row ids (gcra_p2p_prepare).
+constexpr u64 INDEX_MAX_ROWS = 1ULL << 31;
+static_assert(INDEX_MAX_ROWS - 1 <= 0xFFFFFFFFull, "a 32-bit batch counter holds the row count of any index-order batch");
 __device__ __forceinline__ u32 counter_of(const u32 *__restrict__ cnt, u32 mask, u32 slot) {
-    const u32 e = slot & mask;
-    return (__ldg(cnt + (e >> 1)) >> ((e & 1) * 16)) & 0xFFFF;
+    return __ldg(cnt + (slot & mask));
 }
 __device__ __forceinline__ bool pend_of(const u32 *__restrict__ pend, u32 mask, u32 slot) {
     const u32 e = slot & mask;
@@ -213,8 +217,7 @@ probe_kernel(Table t, BatchView b, const PolicyDerived *__restrict__ pol, u32 np
         for (u32 i = threadIdx.x; i < NOTE_HASH; i += TILE_THREADS) {
             const u32 sl = hkey[i];
             if (sl == 0xFFFFFFFFu) continue;
-            const u32 e = sl & bm_mask;
-            atomicAdd(counters + (e >> 1), min(hcnt[i], 2u) << ((e & 1) * 16));
+            atomicAdd(counters + (sl & bm_mask), min(hcnt[i], 2u));
             hkey[i] = 0xFFFFFFFFu;
             hcnt[i] = 0;
         }
