@@ -693,8 +693,11 @@ __device__ __forceinline__ void decide_chunk(const Table &t, const u64 *sorted, 
     }
 }
 
+// Resident threads per SM the register budget is sized for: 512 (97 registers, no spills; 2 CTAs of 256 per SM).
+// At 1024 the cap of 64 registers spilled ~200 B per thread to local memory, and on H100 the Zipf ticks ran ~5 %
+// slower (bench.py, 400 W): the run walk is latency-bound on its state loads, and spill traffic competes with them.
 #ifndef GCRA_DECIDE_MINBLOCKS
-#define GCRA_DECIDE_MINBLOCKS (1024 / GCRA_DECIDE_THREADS)
+#define GCRA_DECIDE_MINBLOCKS (512 / GCRA_DECIDE_THREADS)
 #endif
 template <bool BY_ROW>
 __global__ void __launch_bounds__(DECIDE_THREADS, GCRA_DECIDE_MINBLOCKS)
