@@ -216,6 +216,31 @@ int32_t gcra_peek(gcra_engine *h, uint64_t key_hash, int64_t *tat, int64_t *expi
  * restart); decisions after a load are identical to those of the engine that saved */
 int32_t gcra_snapshot_save(gcra_engine *h, const char *path);
 int32_t gcra_snapshot_load(gcra_engine *h, const char *path);
+/* Insert the entries of a snapshot file (gcra_snapshot_save, any geometry, any source engine) that shard `rank`
+ * of `world` owns (gcra_owner_of(key_hash, world) == rank) into this engine's table, next to what it holds.  This is
+ * how a deployment changes its GPU count: every new rank restores every old rank's file (world = 1, rank = 0 takes
+ * every entry).
+ *   - Checked before any change (else GCRA_INTERNAL, engine untouched): the path opens; world > 0 and rank < world;
+ *     the header (magic, version 2, nb_main x 4 + stash_slots <= total_lines x 4); the file length is the header +
+ *     total_lines x 4 x (8 + 16 + 8) bytes.  The file's geometry need not be one this build would choose: entries are
+ *     re-inserted, not copied.
+ *   - Carried: every slot whose key word is >= 2 and whose state is an entry (expiry = tat + off >= 0), expired but
+ *     not swept ones included; tat, off and ei verbatim.  Keys that hold no entry (swept, only ever denied) are not.
+ *   - The table stores mix64(key_hash), so ownership is decided on the unmixed key word.  The two key hashes whose
+ *     mix64 is 0 or 1 share the key words 2 and 3 with the two whose mix64 is 2 or 3 (one entry for both, in any
+ *     table); such an entry goes to the owner of the latter.
+ *   - A key that already holds an entry here keeps it and counts in *conflicts; every other key is inserted
+ *     (*restored).  The table first grows by the usual rule for the entries this shard takes from the file (not for
+ *     the file's whole len), then the keys are placed as traffic places them; a key that finds the table full is an
+ *     error.
+ *   - An engine that holds no entries (len 0) adopts the file's key-hash seed, as gcra_snapshot_load does; otherwise
+ *     the seeds must be equal.
+ *   - len, occupied slots and stash follow the inserted keys; the traffic totals and the sweep policy's state do not
+ *     change.  Memory use is bounded: the file is streamed in chunks.
+ * Waits for the engine's submitted work.  Multi-GPU callers restore between ticks, after gcra_p2p_join (or
+ * gcra_shard_join) on every rank. */
+int32_t gcra_snapshot_restore(gcra_engine *h, const char *path, uint32_t rank, uint32_t world, uint64_t *restored,
+                              uint64_t *conflicts);
 /* block until all device work of this handle has finished */
 int32_t gcra_sync(gcra_engine *h);
 /* device time (ms) of the kernels of the most recent batch call, measured with CUDA events on

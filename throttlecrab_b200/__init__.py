@@ -261,6 +261,13 @@ class _GpuStore:
     def load(self, path):
         self._check(self._L.gcra_snapshot_load(self._h, os.fsencode(path)))
 
+    def restore(self, path, rank=0, world=1):
+        """Insert the entries of a snapshot file that shard `rank` of `world` owns next to what this store holds
+        (gcra_snapshot_restore); returns (restored, conflicts)."""
+        r, c = C.c_uint64(), C.c_uint64()
+        self._check(self._L.gcra_snapshot_restore(self._h, os.fsencode(path), rank, world, C.byref(r), C.byref(c)))
+        return r.value, c.value
+
     def sync(self):
         self._check(self._L.gcra_sync(self._h))
 

@@ -104,6 +104,7 @@ SYMBOLS = {
     "gcra_peek": (_i32, [_vp, _u64, _pi64, _pi64, _pu8]),
     "gcra_snapshot_save": (_i32, [_vp, C.c_char_p]),
     "gcra_snapshot_load": (_i32, [_vp, C.c_char_p]),
+    "gcra_snapshot_restore": (_i32, [_vp, C.c_char_p, _u32, _u32, _pu64, _pu64]),
     "gcra_sync": (_i32, [_vp]),
     "gcra_last_kernel_ms": (_i32, [_vp, C.POINTER(C.c_float * 4)]),
     "gcra_last_kernel_ms_detail": (_i32, [_vp, C.POINTER(C.c_float * 7)]),

@@ -12,7 +12,10 @@
 #include <cstdlib>
 #include <dlfcn.h>
 #include <cstring>
+#include <fcntl.h>
 #include <string>
+#include <sys/stat.h>
+#include <unistd.h>
 #include <vector>
 
 #include "gcra_kernels.cuh"
@@ -1682,6 +1685,123 @@ int32_t gcra_snapshot_load(gcra_engine *h, const char *path) {
     h->seen_allowed = hd.counters[C_ALLOWED];
     h->seen_expired_hits = hd.counters[C_EXPIRED_HITS];
     for (int i = 0; i < gcra_engine::N_SNAP; i++) h->snap_used[i] = false;
+    return GCRA_OK;
+}
+
+// Streams the file through the GPU twice, in chunks of RESTORE_CHUNK slots (one staging set = SNAP_CHUNK bytes over
+// the three sections; two sets, so that reading chunk i + 1 overlaps the kernel over chunk i): a COUNT pass sizes the
+// table for the entries this shard takes, an INSERT pass inserts them.
+namespace {
+const size_t RESTORE_CHUNK = SNAP_CHUNK / (sizeof(u64) + sizeof(TatOff) + sizeof(i64));
+
+struct RestoreBuffers {
+    char *host[2] = {};                // pinned: keys | state | ei of one chunk
+    char *dev[2] = {};
+    u64 *counts = nullptr;             // [RESTORE_COUNTS]
+    cudaEvent_t done[2] = {};          // the set's copy + kernel finished: its host buffer may be refilled
+    int fd = -1;
+    ~RestoreBuffers() {
+        for (int s = 0; s < 2; s++) {
+            if (done[s]) { cudaEventSynchronize(done[s]); cudaEventDestroy(done[s]); }
+            cudaFreeHost(host[s]);
+            cudaFree(dev[s]);
+        }
+        cudaFree(counts);
+        if (fd >= 0) close(fd);
+    }
+};
+}  // namespace
+
+static bool pread_all(int fd, void *buf, size_t bytes, uint64_t off) {
+    for (size_t got = 0; got < bytes;) {
+        const ssize_t r = pread(fd, (char *)buf + got, bytes - got, (off_t)(off + got));
+        if (r <= 0) return false;
+        got += (size_t)r;
+    }
+    return true;
+}
+
+static int restore_pass(gcra_engine *h, RestoreBuffers &b, uint64_t slots, uint32_t rank, uint32_t world, bool insert) {
+    const uint64_t keys_off = sizeof(SnapshotHeader), state_off = keys_off + slots * sizeof(u64),
+                   ei_off = state_off + slots * sizeof(TatOff);
+    for (uint64_t first = 0, c = 0; first < slots; first += RESTORE_CHUNK, c++) {
+        const int s = (int)(c & 1);
+        const uint64_t n = std::min<uint64_t>(RESTORE_CHUNK, slots - first);
+        char *hk = b.host[s], *hs = hk + RESTORE_CHUNK * sizeof(u64), *he = hs + RESTORE_CHUNK * sizeof(TatOff);
+        char *dk = b.dev[s], *ds = dk + RESTORE_CHUNK * sizeof(u64), *de = ds + RESTORE_CHUNK * sizeof(TatOff);
+        CK(cudaEventSynchronize(b.done[s]));
+        if (!pread_all(b.fd, hk, n * sizeof(u64), keys_off + first * sizeof(u64)) ||
+            !pread_all(b.fd, hs, n * sizeof(TatOff), state_off + first * sizeof(TatOff)) ||
+            (insert && !pread_all(b.fd, he, n * sizeof(i64), ei_off + first * sizeof(i64)))) {
+            h->err = "snapshot restore: short read";
+            return GCRA_INTERNAL;
+        }
+        CK(cudaMemcpyAsync(dk, hk, n * sizeof(u64), cudaMemcpyHostToDevice, h->stream));
+        CK(cudaMemcpyAsync(ds, hs, n * sizeof(TatOff), cudaMemcpyHostToDevice, h->stream));
+        if (insert) CK(cudaMemcpyAsync(de, he, n * sizeof(i64), cudaMemcpyHostToDevice, h->stream));
+        const uint32_t grid = (uint32_t)std::min<uint64_t>((n + TILE_THREADS - 1) / TILE_THREADS, 8 * h->sms);
+        (insert ? restore_kernel<true> : restore_kernel<false>)<<<grid, TILE_THREADS, 0, h->stream>>>(
+            h->tab, (const u64 *)dk, (const TatOff *)ds, (const i64 *)de, n, rank, world, b.counts);
+        h->launches++;
+        CK(cudaGetLastError());
+        CK(cudaEventRecord(b.done[s], h->stream));
+    }
+    CK(cudaStreamSynchronize(h->stream));
+    return GCRA_OK;
+}
+
+int32_t gcra_snapshot_restore(gcra_engine *h, const char *path, uint32_t rank, uint32_t world, uint64_t *restored,
+                              uint64_t *conflicts) {
+    if (restored) *restored = 0;
+    if (conflicts) *conflicts = 0;
+    CK(cudaSetDevice(h->device));
+    if (world == 0 || rank >= world) { h->err = "snapshot restore: needs rank < world"; return GCRA_INTERNAL; }
+    RestoreBuffers b;
+    b.fd = open(path, O_RDONLY);
+    if (b.fd < 0) { h->err = std::string("snapshot restore: cannot open ") + path; return GCRA_INTERNAL; }
+    SnapshotHeader hd{};
+    struct stat sb;
+    if (fstat(b.fd, &sb) != 0 || !pread_all(b.fd, &hd, sizeof(hd), 0) || memcmp(hd.magic, SNAP_MAGIC, 8) != 0 ||
+        hd.version != 2) {
+        h->err = "snapshot restore: bad header";
+        return GCRA_INTERNAL;
+    }
+    const uint64_t slots = (uint64_t)hd.total_lines * 4;
+    if ((uint64_t)hd.nb_main * 4 + hd.stash_slots > slots) { h->err = "snapshot restore: bad geometry"; return GCRA_INTERNAL; }
+    if ((uint64_t)sb.st_size != sizeof(hd) + slots * (sizeof(u64) + sizeof(TatOff) + sizeof(i64))) {
+        h->err = "snapshot restore: file length does not match its header";
+        return GCRA_INTERNAL;
+    }
+    CK(cudaDeviceSynchronize());
+    RC(refresh_counters(h, true));
+    const bool adopt_seed = h->h_counters[C_REAL] == 0;
+    if (!adopt_seed && (hd.hash_seed[0] != h->hash_seed[0] || hd.hash_seed[1] != h->hash_seed[1])) {
+        h->err = "snapshot restore: the file's key-hash seed differs from that of the entries held";
+        return GCRA_INTERNAL;
+    }
+    for (int s = 0; s < 2; s++) {
+        CK(cudaMallocHost(&b.host[s], SNAP_CHUNK));
+        CK(cudaMalloc(&b.dev[s], SNAP_CHUNK));
+        CK(cudaEventCreateWithFlags(&b.done[s], cudaEventDisableTiming));
+    }
+    CK(cudaMalloc(&b.counts, RESTORE_COUNTS * sizeof(u64)));
+    CK(cudaMemsetAsync(b.counts, 0, RESTORE_COUNTS * sizeof(u64), h->stream));
+    RC(restore_pass(h, b, slots, rank, world, false));
+    u64 counts[RESTORE_COUNTS];
+    CK(cudaMemcpy(counts, b.counts, sizeof(counts), cudaMemcpyDeviceToHost));
+    RC(ensure_room(h, counts[RESTORE_OWNED]));     // may purge or grow: h->tab is read after it
+    RC(restore_pass(h, b, slots, rank, world, true));
+    CK(cudaMemcpy(counts, b.counts, sizeof(counts), cudaMemcpyDeviceToHost));
+    RC(refresh_counters(h, true));
+    h->occupied_ub = h->h_counters[C_OCCUPIED];
+    for (int i = 0; i < gcra_engine::N_SNAP; i++) h->snap_used[i] = false;
+    if (counts[RESTORE_FAILED]) {
+        h->err = "snapshot restore: table full (" + std::to_string(counts[RESTORE_FAILED]) + " entries not inserted)";
+        return GCRA_INTERNAL;
+    }
+    if (adopt_seed) { h->hash_seed[0] = hd.hash_seed[0]; h->hash_seed[1] = hd.hash_seed[1]; }
+    if (restored) *restored = counts[RESTORE_INSERTED];
+    if (conflicts) *conflicts = counts[RESTORE_CONFLICTS];
     return GCRA_OK;
 }
 

@@ -84,6 +84,16 @@ __host__ __device__ __forceinline__ u64 mix64(u64 x) {
     x ^= x >> 31;
     return x;
 }
+// inverse of mix64: the key hash a table's key word was made from (each xor-shift undone by repeating it until the
+// shift passes 64 bits, each multiplier replaced by its inverse mod 2^64)
+__host__ __device__ __forceinline__ u64 unmix64(u64 x) {
+    x ^= (x >> 31) ^ (x >> 62);
+    x *= 0x319642b2d24d8ec3ULL;
+    x ^= (x >> 27) ^ (x >> 54);
+    x *= 0x96de1b173f119089ULL;
+    x ^= (x >> 30) ^ (x >> 60);
+    return x;
+}
 __host__ __device__ __forceinline__ u64 stored_key(u64 key_hash) {
     u64 k = mix64(key_hash);
     return k < 2 ? k + 2 : k;   // 0 / 1 are the empty / tombstone marks

@@ -1270,6 +1270,59 @@ route_unpermute_kernel(const gcra_result *__restrict__ routed, const u32 *__rest
     }
 }
 
+// ---------------------------------------------------------------------------------------------
+// snapshot restore (gcra_snapshot_restore): one staged chunk of a snapshot file's key, state and ei sections
+// ---------------------------------------------------------------------------------------------
+// An entry is carried when its key word is >= 2 and its state is a real entry (expiry = tat + off >= 0, expired or
+// not, as rehash_kernel keeps them), and shard `rank` of `world` owns it: owner_of(unmix64(key word)).  The key hashes
+// whose mix64 is 0 or 1 share the key words 2 and 3 with those whose mix64 is 2 or 3 (stored_key); such a shared entry
+// goes to the owner of the unmixed key word, i.e. of the latter.
+// COUNT adds the chunk's carried entries to out[0].  INSERT claims their keys through find_or_claim (the placement
+// rule of traffic) and writes tat, off and ei verbatim -- unless the key already holds a real entry here, which
+// stays (out[2], a conflict); out[1] = inserted, out[3] = keys that found the table full.
+enum { RESTORE_OWNED = 0, RESTORE_INSERTED, RESTORE_CONFLICTS, RESTORE_FAILED, RESTORE_COUNTS };
+
+template <bool INSERT>
+__global__ void __launch_bounds__(TILE_THREADS)
+restore_kernel(Table t, const u64 *__restrict__ keys, const TatOff *__restrict__ state, const i64 *__restrict__ ei,
+               u64 n, u32 rank, u32 world, u64 *__restrict__ out) {
+    u32 owned = 0, inserted = 0, fresh_n = 0, conflicts = 0, failed = 0;
+    const u64 stride = (u64)gridDim.x * TILE_THREADS;
+    for (u64 i = (u64)blockIdx.x * TILE_THREADS + threadIdx.x; i < n; i += stride) {
+        const ulonglong2 v = ld_stream(&state[i]);
+        if ((i64)(v.x + v.y) < 0) continue;
+        const u64 k = keys[i];
+        if (k < 2 || owner_of(unmix64(k), world) != rank) continue;
+        if (!INSERT) { owned++; continue; }
+        bool fresh;
+        const u32 s = find_or_claim(t, k, fresh);
+        if (s == t.null_slot) { failed++; continue; }
+        if (!fresh) {
+            const TatOff cur = t.state[s];
+            if ((i64)((u64)cur.tat + cur.off) >= 0) { conflicts++; continue; }
+        }
+        *reinterpret_cast<ulonglong2 *>(&t.state[s]) = v;
+        t.ei[s] = ei[i];
+        inserted++;
+        fresh_n += fresh ? 1 : 0;
+    }
+    owned = __reduce_add_sync(0xffffffffu, owned);
+    inserted = __reduce_add_sync(0xffffffffu, inserted);
+    fresh_n = __reduce_add_sync(0xffffffffu, fresh_n);
+    conflicts = __reduce_add_sync(0xffffffffu, conflicts);
+    failed = __reduce_add_sync(0xffffffffu, failed);
+    if ((threadIdx.x & 31) == 0) {
+        if (owned) atomicAdd(&out[RESTORE_OWNED], (u64)owned);
+        if (inserted) {
+            atomicAdd(&out[RESTORE_INSERTED], (u64)inserted);
+            atomicAdd(&t.counters[C_REAL], (u64)inserted);
+        }
+        if (fresh_n) atomicAdd(&t.counters[C_OCCUPIED], (u64)fresh_n);
+        if (conflicts) atomicAdd(&out[RESTORE_CONFLICTS], (u64)conflicts);
+        if (failed) atomicAdd(&out[RESTORE_FAILED], (u64)failed);
+    }
+}
+
 
 // ---------------------------------------------------------------------------------------------
 // metrics bridge: denied requests per key, from the kernels' own outputs

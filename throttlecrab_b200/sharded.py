@@ -20,10 +20,35 @@ and tick i-1's results travel back.  `DEPTH` buffer sets are cycled; `finish()` 
 
 torch is plumbing only: device buffers, the NCCL process group and stream/event ordering.
 """
+import os
+
 import torch
 
 REQ_B, RES_B = 48, 32
 DEPTH = 4
+
+
+class _Snapshots:
+    """Snapshots of a sharded key space.  Every rank submits every tick, so ranks that each save after joining the
+    same tick together hold one consistent cut; any number of ranks can take it up again, whatever the world size
+    that wrote it (gcra_snapshot_restore keeps the entries each rank owns)."""
+
+    def save(self, directory):
+        """Wait for every tick submitted so far, then write this rank's table to <directory>/rank<r>.gcra."""
+        self.finish()
+        path = os.path.join(directory, "rank%d.gcra" % self.rank)
+        self.lim.store.save(path)          # gcra_snapshot_save waits for the device
+        return path
+
+    def restore(self, paths):
+        """Insert this rank's share of every snapshot file in `paths` (all files of a save(), any world size), next to
+        what the engine holds.  Call it between ticks, on every rank.  Returns (restored, conflicts) over the files."""
+        self.finish()
+        restored = conflicts = 0
+        for p in paths:
+            r, c = self.lim.store.restore(p, self.rank, self.world)
+            restored, conflicts = restored + r, conflicts + c
+        return restored, conflicts
 
 
 class CudaOps:
@@ -65,9 +90,9 @@ class _Slot:
         self.done_ev = None        # results un-permuted into the caller's buffer
 
 
-class ShardedLimiter:
+class ShardedLimiter(_Snapshots):
     def __init__(self, limiter, dist, device, ops=None, max_rows=None):
-        self.dist, self.dev = dist, device
+        self.lim, self.dist, self.dev = limiter, dist, device
         self.world, self.rank = dist.get_world_size(), dist.get_rank()
         self.ops = ops if ops is not None else CudaOps(limiter)
         self.max_rows = max_rows or limiter.store.max_batch
@@ -194,7 +219,7 @@ class ShardedLimiter:
         return n_recv
 
 
-class NativeShardedLimiter:
+class NativeShardedLimiter(_Snapshots):
     """The same pipeline driven by ONE C call per tick (gcra_shard_submit): partition, NCCL count exchange and
     all-to-alls (libnccl resolved with dlopen inside the library), the engine's pipelined kernels and the way
     back all live in libgcra_b200.so.  torch.distributed is used once, to hand the three ncclUniqueIds that
@@ -239,7 +264,7 @@ class NativeShardedLimiter:
         return "native NCCL pipeline (gcra_shard_submit: partition, count exchange, all-to-all, decide, all-to-all)"
 
 
-class PeerShardedLimiter:
+class PeerShardedLimiter(_Snapshots):
     """The sharded tick over NVLink peer memory (gcra_p2p_*, csrc/gcra_p2p.cuh): the partition kernel stores every
     request row straight into its owner's inbox, the owner's engine runs over the inbox as one batch of `world`
     segments and stores every result straight into the sender's outbox; ranks synchronise with tick numbers in peer
