@@ -51,7 +51,7 @@ def lib():
         L.ora_replay.argtypes = [vp, u64, vp, vp]
         L.ora_replay_sharded.restype = C.c_double
         L.ora_replay_sharded.argtypes = [vp, C.c_int, u64, vp, vp]
-        for f in ("ora_len", "ora_expired_count", "ora_sweeps"):
+        for f in ("ora_len", "ora_expired_count", "ora_sweeps", "ora_expired_writes"):
             getattr(L, f).restype = u64
             getattr(L, f).argtypes = [vp]
         L.ora_entry.argtypes = [vp, cp, u64, C.POINTER(i64), C.POINTER(i64)]
@@ -128,6 +128,11 @@ class OracleStore:
 
     def sweeps(self):
         return int(lib().ora_sweeps(self._h))
+
+    def expired_writes(self):
+        """Writes over an existing, expired entry since creation, for every store kind (the engine's
+        expired_hits)."""
+        return int(lib().ora_expired_writes(self._h))
 
     def entry(self, key):
         k = _kb(key)

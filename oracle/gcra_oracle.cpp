@@ -165,6 +165,7 @@ struct ora_store {
     uint64_t last_removed = 0, last_total = 0;
     uint64_t ops_count = 0, cleanup_modulo = 0;   /* probabilistic */
     uint64_t sweeps = 0;
+    uint64_t expired_writes = 0;                  /* not a reference field: see ora_expired_writes */
 };
 
 /* adaptive_cleanup.rs:138-171 */
@@ -271,6 +272,7 @@ extern "C" int ora_set_nx(ora_store *s, const char *key, uint64_t len, int64_t v
     Entry *e = s->data.find(key, len, h);
     if (e && e->expiry > now) return 0;
     if (e && s->kind == ORA_ADAPTIVE) s->expired_count++;           /* :267 */
+    if (e) s->expired_writes++;
     std::string owned(key, len);                       /* key.to_string() :269,274 */
     s->data.insert(std::move(owned), h, value, now + (i128)ttl_ns);
     return 1;
@@ -400,6 +402,7 @@ extern "C" double ora_replay_sharded(ora_store **stores, int threads, uint64_t n
 extern "C" uint64_t ora_len(ora_store *s) { return s->data.items; }
 extern "C" uint64_t ora_expired_count(ora_store *s) { return s->expired_count; }
 extern "C" uint64_t ora_sweeps(ora_store *s) { return s->sweeps; }
+extern "C" uint64_t ora_expired_writes(ora_store *s) { return s->expired_writes; }
 extern "C" int ora_entry(ora_store *s, const char *key, uint64_t len, int64_t *tat, int64_t *expiry_sat) {
     Entry *e = s->data.find(key, len, hash_bytes(key, len));
     if (!e) return 0;

@@ -92,6 +92,9 @@ double ora_replay_sharded(ora_store **stores, int threads, uint64_t n,
 uint64_t ora_len(ora_store *s);
 uint64_t ora_expired_count(ora_store *s);
 uint64_t ora_sweeps(ora_store *s);
+/* writes over an existing, expired entry (set_if_not_exists_with_ttl that found one), every store kind, never reset:
+ * what the engine counts as expired_hits */
+uint64_t ora_expired_writes(ora_store *s);
 /* returns 1 and fills tat / expiry (saturated to INT64_MAX) when the key has an entry */
 int ora_entry(ora_store *s, const char *key, uint64_t len, int64_t *tat, int64_t *expiry_sat);
 /* force retain(expiry > now) regardless of policy; returns removed */

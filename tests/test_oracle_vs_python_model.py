@@ -33,6 +33,7 @@ def derive(max_burst, count, period):
 class Model:
     def __init__(self):
         self.t = {}                                            # key -> (tat, expiry as unbounded int)
+        self.expired_writes = 0                                # allowed writes over an existing, expired entry
 
     def rate_limit(self, key, max_burst, count, period, q, now):
         if q < 0:
@@ -49,6 +50,7 @@ class Model:
         allow_at = clamp(new_tat - dvt)
         allowed = now >= allow_at
         if allowed:
+            self.expired_writes += e is not None and not live
             ttl = clamp(clamp(new_tat - now) + dvt) % U64     # `as u64`
             self.t[key] = (new_tat, now + ttl)
         cur = new_tat if allowed else tat
@@ -89,6 +91,29 @@ def test_oracle_matches_python_model(steps):
         assert (ent is None) == (me is None)
         if me is not None:
             assert ent == (me[0], min(me[1], I64_MAX))
+        assert orc.expired_writes() == mod.expired_writes
+
+
+def test_expired_writes_count_every_write_over_an_expired_entry():
+    """The oracle's expired-write total (the engine's expired_hits) on hand-picked boundaries: a write exactly at
+    expiry counts, one a nanosecond before does not, denied requests and a swept entry never count, and it is
+    counted for every store kind."""
+    b, c, p = 2, 120, 60                                         # P5: ei = dvt = 0.5 s
+    _, ei, dvt = derive(b, c, p)
+    # (all clocks stay below the adaptive store's first cleanup at created + 5 s, so no store sweeps on its own)
+    steps = [("a", 1, T0), ("a", 1, T0 + dvt - 1), ("a", 1, T0 + 4 * 10**9),   # written, live, expired: counts
+             ("b", 0, T0), ("b", 0, T0),                                       # a zero TTL: expiry == now counts
+             ("c", b + 1, T0), ("c", 1, T0 + 4 * 10**9)]                       # denied: no entry, then a fresh one
+    for kind in (oracle.PERIODIC, oracle.PROBABILISTIC, oracle.ADAPTIVE):
+        orc = oracle.OracleStore(kind, capacity=100, created_ns=T0, p0=10**9, p1=10**9, p2=10**9)
+        mod = Model()
+        for key, q, now in steps:
+            assert orc.rate_limit(key, b, c, p, q, now) == mod.rate_limit(key, b, c, p, q, now)
+        assert orc.sweeps() == 0
+        assert orc.expired_writes() == mod.expired_writes == 2, (kind, orc.expired_writes(), mod.expired_writes)
+        orc.force_sweep(T0 + 10**13)                             # a swept entry is gone: the next write is fresh
+        orc.rate_limit("a", b, c, p, 1, T0 + 10**13)
+        assert orc.expired_writes() == 2
 
 
 @settings(max_examples=300, deadline=None)
