@@ -95,6 +95,15 @@ typedef struct {
     int64_t max_burst, count_per_period, period;
 } gcra_policy;
 
+/* 16-byte result of a compact request: what rate_limiter.rs:208 calls `cur`, plus status and allowed.
+ * gcra_expand_results16 turns it into the gcra_result the 32-byte path returns, bit for bit. */
+typedef struct {
+    int64_t cur_tat_ns;   /* allowed ? new_tat : the tat the request started from; 0 when status != GCRA_OK */
+    int32_t status;
+    uint8_t allowed;
+    uint8_t pad[3];
+} gcra_result16;
+
 typedef struct {
     uint64_t len;             /* entries holding state, like HashMap::len() (periodic.rs:113-116) */
     uint64_t occupied_slots;  /* slots whose key word is taken: len + keys without an entry (swept, or only ever denied) */
@@ -181,13 +190,34 @@ int32_t gcra_rate_limit_batch16(gcra_engine *h, uint64_t n, const gcra_request16
                                 int64_t now_ns, gcra_result *res);
 int32_t gcra_rate_limit_batch16_device(gcra_engine *h, uint64_t n, const gcra_request16 *d_req,
                                        int64_t now_ns, gcra_result *d_res, void *stream);
+/* compact requests, 16-byte results: the same decisions, table updates, counters and sweeps as the two calls above
+ * (same chunking by max_batch, same sweep policy before every chunk), but every result row is a gcra_result16 --
+ * half the device-to-host bytes, and no kernel computes remaining / reset_after / retry_after.
+ * gcra_expand_results16 derives them on the host. */
+int32_t gcra_rate_limit_batch16_r16(gcra_engine *h, uint64_t n, const gcra_request16 *req, int64_t now_ns,
+                                    gcra_result16 *res);
+int32_t gcra_rate_limit_batch16_r16_device(gcra_engine *h, uint64_t n, const gcra_request16 *d_req, int64_t now_ns,
+                                           gcra_result16 *d_res, void *stream);
+/* Host only: no handle, no device work, thread-safe, works without a GPU.  out[i] = the gcra_result the 32-byte path
+ * returns for row i of a compact batch decided at now_ns, derived from in[i] (rate_limiter.rs:208-238 from cur, the
+ * request's quantity and its policy, each policy derived once).  A row with status != GCRA_OK becomes
+ * {0, 0, 0, status, 0} without reading the table.  Bit-exact ONLY with the policy table that was registered
+ * (gcra_set_policies) when the batch ran: a caller that changes its table keeps the old one until the results of the
+ * batches decided under it have been expanded.  Returns GCRA_INTERNAL (and writes status GCRA_INTERNAL into such rows)
+ * when an OK row names a policy the table lacks or one that is invalid -- i.e. not the batch's table. */
+int32_t gcra_expand_results16(uint64_t n, const gcra_request16 *req, int64_t now_ns, const gcra_policy *policies,
+                              uint32_t npol, const gcra_result16 *in, gcra_result *out);
 
 /* ---- pinned host ring: fill a slot in place, submit, collect ---------------------------- */
 /* replaces the actor's mpsc channel hand-off (actor.rs:68-82,217-236) for batched callers.
- * Slots are processed strictly in submission order. compact != 0 -> slots hold gcra_request16. */
-int32_t gcra_ring_create(gcra_engine *h, uint32_t slots, uint32_t slot_capacity, int32_t compact);
+ * Slots are processed strictly in submission order.  mode: 0 -> slots hold gcra_request / gcra_result; 2 -> slots
+ * hold gcra_request16 / gcra_result16 (gcra_ring_results16; the D2H copy moves n x 16 bytes); any other value ->
+ * gcra_request16 / gcra_result.  Pipelining, the sweep policy on submit and the counters read-back are the same in
+ * every mode. */
+int32_t gcra_ring_create(gcra_engine *h, uint32_t slots, uint32_t slot_capacity, int32_t mode);
 void *gcra_ring_requests(gcra_engine *h, uint32_t slot);        /* pinned, caller fills */
-gcra_result *gcra_ring_results(gcra_engine *h, uint32_t slot);  /* pinned, valid after wait */
+gcra_result *gcra_ring_results(gcra_engine *h, uint32_t slot);  /* pinned, valid after wait; NULL in mode 2 */
+gcra_result16 *gcra_ring_results16(gcra_engine *h, uint32_t slot);  /* pinned, valid after wait; NULL unless mode 2 */
 int32_t gcra_ring_submit(gcra_engine *h, uint32_t slot, uint32_t n, int64_t now_ns);
 int32_t gcra_ring_wait(gcra_engine *h, uint32_t slot);
 int32_t gcra_ring_poll(gcra_engine *h, uint32_t slot, int32_t *done);

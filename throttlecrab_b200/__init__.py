@@ -20,12 +20,13 @@ from dataclasses import dataclass
 import numpy as np
 
 from . import _native
-from ._native import (REQ_DTYPE, RES_DTYPE, REQ16_DTYPE, POLICY_DTYPE, OK, NEGATIVE_QUANTITY,
+from ._native import (REQ_DTYPE, RES_DTYPE, REQ16_DTYPE, RES16_DTYPE, POLICY_DTYPE, OK, NEGATIVE_QUANTITY,
                       INVALID_RATE_LIMIT, INTERNAL)
 
 __all__ = ["RateLimiter", "RateLimitResult", "Rate", "CellError", "NegativeQuantity", "InvalidRateLimit",
            "Internal", "AdaptiveStore", "PeriodicStore", "ProbabilisticStore", "ManualStore",
-           "hash_key", "derive_params", "REQ_DTYPE", "RES_DTYPE", "REQ16_DTYPE", "POLICY_DTYPE"]
+           "hash_key", "derive_params", "expand_results16", "REQ_DTYPE", "RES_DTYPE", "REQ16_DTYPE", "RES16_DTYPE",
+           "POLICY_DTYPE"]
 
 NS = 1_000_000_000
 
@@ -98,6 +99,23 @@ def derive_params(max_burst, count_per_period, period):
     ei, dvt = C.c_int64(), C.c_int64()
     st = _native.lib().gcra_derive_params(max_burst, count_per_period, period, C.byref(ei), C.byref(dvt))
     return st, ei.value, dvt.value
+
+
+def expand_results16(req16, now, policies, res16, out=None):
+    """RES_DTYPE results of a compact batch from its RES16_DTYPE results (gcra_expand_results16: host only, no GPU).
+    Bit-exact with the 32-byte path when `policies` is the table that was registered when the batch ran; raises
+    Internal when an OK row names a policy that table does not have (or an invalid one)."""
+    req = np.ascontiguousarray(req16, REQ16_DTYPE)
+    res = np.ascontiguousarray(res16, RES16_DTYPE)
+    pol = np.ascontiguousarray(policies, POLICY_DTYPE)
+    if len(req) != len(res):
+        raise ValueError("req16 and res16 differ in length")
+    out = np.empty(len(req), RES_DTYPE) if out is None else out
+    rc = _native.lib().gcra_expand_results16(len(req), req.ctypes.data, _ns(now), pol.ctypes.data, len(pol),
+                                            res.ctypes.data, out.ctypes.data)
+    if rc != OK:
+        raise Internal("gcra_expand_results16: a row names a policy outside the given table, or an invalid one")
+    return out
 
 
 class Rate:
@@ -401,8 +419,15 @@ class RateLimiter:
         pol = np.ascontiguousarray(policies, POLICY_DTYPE)
         self.store._check(self._L.gcra_set_policies(self._h, len(pol), pol.ctypes.data))
 
-    def rate_limit_batch16(self, requests, now, out=None):
+    def rate_limit_batch16(self, requests, now, out=None, compact_results=False):
+        """REQ16_DTYPE requests against the registered policy table; RES_DTYPE results, or with compact_results
+        RES16_DTYPE results (16 bytes: cur_tat_ns, status, allowed -- expand_results16 derives the rest)."""
         req = np.ascontiguousarray(requests, REQ16_DTYPE)
+        if compact_results:
+            res = np.empty(len(req), RES16_DTYPE) if out is None else out
+            self.store._check(self._L.gcra_rate_limit_batch16_r16(self._h, len(req), req.ctypes.data, _ns(now),
+                                                                  res.ctypes.data))
+            return res
         res = np.empty(len(req), RES_DTYPE) if out is None else out
         self.store._check(self._L.gcra_rate_limit_batch16(self._h, len(req), req.ctypes.data, _ns(now),
                                                           res.ctypes.data))
@@ -419,27 +444,33 @@ class RateLimiter:
     def join(self, stream=None):
         self.store._check(self._L.gcra_pipeline_join(self._h, stream))
 
-    def rate_limit_batch16_device(self, n, d_req_ptr, now, d_res_ptr, stream=None):
-        self.store._check(self._L.gcra_rate_limit_batch16_device(self._h, n, d_req_ptr, _ns(now), d_res_ptr, stream))
+    def rate_limit_batch16_device(self, n, d_req_ptr, now, d_res_ptr, stream=None, compact_results=False):
+        """compact_results: d_res_ptr receives n RES16_DTYPE rows instead of RES_DTYPE rows."""
+        fn = self._L.gcra_rate_limit_batch16_r16_device if compact_results else self._L.gcra_rate_limit_batch16_device
+        self.store._check(fn(self._h, n, d_req_ptr, _ns(now), d_res_ptr, stream))
 
 
 class Ring:
-    """Pinned host ring (gcra_ring_*): fill a slot in place, submit, wait, read results in place."""
+    """Pinned host ring (gcra_ring_*): fill a slot in place, submit, wait, read results in place.
+    compact: False = REQ_DTYPE / RES_DTYPE slots, True = REQ16_DTYPE / RES_DTYPE, 2 = REQ16_DTYPE / RES16_DTYPE."""
 
     def __init__(self, limiter, slots, slot_capacity, compact=False):
         self.lim, self.store = limiter, limiter.store
         self._L, self._h = limiter._L, limiter._h
         self.slots, self.cap, self.compact = slots, slot_capacity, compact
-        self.store._check(self._L.gcra_ring_create(self._h, slots, slot_capacity, 1 if compact else 0))
-        dt = REQ16_DTYPE if compact else REQ_DTYPE
+        mode = 2 if (compact == 2 and compact is not True) else (1 if compact else 0)
+        self.store._check(self._L.gcra_ring_create(self._h, slots, slot_capacity, mode))
+        dt = REQ16_DTYPE if mode else REQ_DTYPE
+        rdt = RES16_DTYPE if mode == 2 else RES_DTYPE
+        results = self._L.gcra_ring_results16 if mode == 2 else self._L.gcra_ring_results
         self.req, self.res = [], []
         for s in range(slots):
             rp = self._L.gcra_ring_requests(self._h, s)
-            sp = self._L.gcra_ring_results(self._h, s)
+            sp = results(self._h, s)
             rb = (C.c_char * (slot_capacity * dt.itemsize)).from_address(rp)
-            sb = (C.c_char * (slot_capacity * RES_DTYPE.itemsize)).from_address(sp)
+            sb = (C.c_char * (slot_capacity * rdt.itemsize)).from_address(sp)
             self.req.append(np.frombuffer(rb, dtype=dt))
-            self.res.append(np.frombuffer(sb, dtype=RES_DTYPE))
+            self.res.append(np.frombuffer(sb, dtype=rdt))
 
     def submit(self, slot, n, now=0):
         self.store._check(self._L.gcra_ring_submit(self._h, slot, n, _ns(now)))

@@ -23,8 +23,10 @@ REQ_DTYPE = np.dtype([("key_hash", "<u8"), ("max_burst", "<i8"), ("count_per_per
 RES_DTYPE = np.dtype([("remaining", "<i8"), ("reset_after_ns", "<i8"), ("retry_after_ns", "<i8"),
                       ("status", "<i4"), ("allowed", "u1"), ("pad", "u1", (3,))])
 REQ16_DTYPE = np.dtype([("key_hash", "<u8"), ("quantity", "<i4"), ("policy", "<u4")])
+RES16_DTYPE = np.dtype([("cur_tat_ns", "<i8"), ("status", "<i4"), ("allowed", "u1"), ("pad", "u1", (3,))])
 POLICY_DTYPE = np.dtype([("max_burst", "<i8"), ("count_per_period", "<i8"), ("period", "<i8")])
 assert REQ_DTYPE.itemsize == 48 and RES_DTYPE.itemsize == 32 and REQ16_DTYPE.itemsize == 16
+assert RES16_DTYPE.itemsize == 16
 
 OK, NEGATIVE_QUANTITY, INVALID_RATE_LIMIT, INTERNAL = 0, 1, 2, 3
 STORE_PERIODIC, STORE_PROBABILISTIC, STORE_ADAPTIVE, STORE_MANUAL = 0, 1, 2, 3
@@ -89,9 +91,13 @@ SYMBOLS = {
     "gcra_set_policies": (_i32, [_vp, _u32, _vp]),
     "gcra_rate_limit_batch16": (_i32, [_vp, _u64, _vp, _i64, _vp]),
     "gcra_rate_limit_batch16_device": (_i32, [_vp, _u64, _vp, _i64, _vp, _vp]),
+    "gcra_rate_limit_batch16_r16": (_i32, [_vp, _u64, _vp, _i64, _vp]),
+    "gcra_rate_limit_batch16_r16_device": (_i32, [_vp, _u64, _vp, _i64, _vp, _vp]),
+    "gcra_expand_results16": (_i32, [_u64, _vp, _i64, _vp, _u32, _vp, _vp]),
     "gcra_ring_create": (_i32, [_vp, _u32, _u32, _i32]),
     "gcra_ring_requests": (_vp, [_vp, _u32]),
     "gcra_ring_results": (_vp, [_vp, _u32]),
+    "gcra_ring_results16": (_vp, [_vp, _u32]),
     "gcra_ring_submit": (_i32, [_vp, _u32, _u32, _i64]),
     "gcra_ring_wait": (_i32, [_vp, _u32]),
     "gcra_ring_poll": (_i32, [_vp, _u32, C.POINTER(_i32)]),

@@ -44,9 +44,9 @@ const __int128 NS_PER_S = 1000000000;
 
 struct RingSlot {
     void *h_req = nullptr;
-    gcra_result *h_res = nullptr;
+    void *h_res = nullptr;           // gcra_result, or gcra_result16 rows in ring mode 2
     void *d_req = nullptr;
-    gcra_result *d_res = nullptr;
+    void *d_res = nullptr;
     cudaEvent_t ev_in = nullptr, ev_comp = nullptr, ev_done = nullptr;
     bool in_flight = false;
 };
@@ -236,7 +236,7 @@ struct gcra_engine {
     uint32_t index_min = 0;          // batches of at least this many rows take the index-order pipeline (0: never)
     int prefetch_state = 0;
     uint32_t max_tiles = 0;
-    uint32_t grid_probe[2] = {}, grid_decide[2] = {};   // resident CTAs of the persistent kernels [compact]
+    uint32_t grid_probe[3] = {}, grid_decide[3] = {};   // resident CTAs of the persistent kernels [RowFmt]
     uint32_t dbg = 0;                // timing experiments only (gcra_debug_set): skips parts of pass B
     uint32_t last_nres = 0, last_nres_rows = 0;   // newest residue size that has reached the host (and its batch's rows)
     bool adaptive = true;            // choose the pipeline from the residue feedback (off when a test / env forces one)
@@ -247,7 +247,7 @@ struct gcra_engine {
     // ring
     std::vector<RingSlot> ring;
     uint32_t ring_cap = 0;
-    bool ring_compact = false;
+    int ring_mode = 0;               // gcra_ring_create: 0, 1 or 2 = the slots' RowFmt
     // denied requests per key (gcra_track_denied): device table, updated by a pass over every finished batch
     DeniedTable denied{};
     uint32_t denied_max = 0, denied_cap = 0;
@@ -510,7 +510,7 @@ static int apply_policy(gcra_engine *h, int64_t now_ns) {
 }
 
 // the cluster kernel: cluster dimension given at launch (cudaLaunchKernelEx)
-template <bool BY_ROW>
+template <bool BY_ROW, bool R16>
 static int launch_giant(gcra_engine *h, Scratch &sc, const u64 *src, const OutMap &om, cudaStream_t st) {
     cudaLaunchConfig_t cfg = {};
     cfg.gridDim = dim3((128 / CLUSTER_CTAS) * CLUSTER_CTAS);
@@ -525,9 +525,9 @@ static int launch_giant(gcra_engine *h, Scratch &sc, const u64 *src, const OutMa
     cfg.numAttrs = 1;
     if (CLUSTER_CTAS > 8) {
         static bool once = false;
-        if (!once) { cudaFuncSetAttribute(decide_runs_kernel<CLUSTER_CTAS, BY_ROW>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1); once = true; }
+        if (!once) { cudaFuncSetAttribute(decide_runs_kernel<CLUSTER_CTAS, BY_ROW, R16>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1); once = true; }
     }
-    CK(cudaLaunchKernelEx(&cfg, decide_runs_kernel<CLUSTER_CTAS, BY_ROW>, h->tab, (const u64 *)src, (const Req *)sc.drec, om,
+    CK(cudaLaunchKernelEx(&cfg, decide_runs_kernel<CLUSTER_CTAS, BY_ROW, R16>, h->tab, (const u64 *)src, (const Req *)sc.drec, om,
                           (const LongRun *)sc.giant_runs, (const u32 *)(sc.long_count + 1)));
     return GCRA_OK;
 }
@@ -576,7 +576,7 @@ static int enqueue_sort(gcra_engine *h, Scratch &sc, uint32_t n_max, const u32 *
     return GCRA_OK;
 }
 
-template <bool BY_ROW>
+template <bool BY_ROW, bool R16>
 static int enqueue_decide_sorted_t(gcra_engine *h, Scratch &sc, uint32_t n_max, const u32 *n_dev, const u64 *src,
                                    const OutMap &om, cudaStream_t st) {
     // (sort pipeline: the work-list counters were cleared at the end of the front half, off this stream)
@@ -584,7 +584,7 @@ static int enqueue_decide_sorted_t(gcra_engine *h, Scratch &sc, uint32_t n_max, 
     const uint32_t warps = (n_max + 31) / 32;
     uint32_t grid = (warps + DECIDE_THREADS / 32 - 1) / (DECIDE_THREADS / 32);
     if (n_dev) grid = std::min<uint32_t>(grid, 4 * h->sms);
-    decide_kernel<BY_ROW><<<grid, DECIDE_THREADS, 0, st>>>(h->tab, src, sc.drec, n_max, n_dev, om, sc.long_runs, sc.giant_runs,
+    decide_kernel<BY_ROW, R16><<<grid, DECIDE_THREADS, 0, st>>>(h->tab, src, sc.drec, n_max, n_dev, om, sc.long_runs, sc.giant_runs,
                                                            sc.long_count, 0);
     h->launches++;
     if (n_max >= GIANT_RUN_MIN) {
@@ -592,23 +592,26 @@ static int enqueue_decide_sorted_t(gcra_engine *h, Scratch &sc, uint32_t n_max, 
         // stream and overlaps the cluster kernel (fork/join with events)
         CK(cudaEventRecord(sc.ev_fork, st));
         CK(cudaStreamWaitEvent(h->aux_stream, sc.ev_fork, 0));
-        decide_runs_kernel<1, BY_ROW><<<h->sms, LONG_THREADS, 0, h->aux_stream>>>(h->tab, src, sc.drec, om, sc.long_runs, sc.long_count);
+        decide_runs_kernel<1, BY_ROW, R16><<<h->sms, LONG_THREADS, 0, h->aux_stream>>>(h->tab, src, sc.drec, om, sc.long_runs, sc.long_count);
         CK(cudaEventRecord(sc.ev_join, h->aux_stream));
-        RC(launch_giant<BY_ROW>(h, sc, src, om, st));   // hottest keys: one cluster per run
+        RC((launch_giant<BY_ROW, R16>(h, sc, src, om, st)));   // hottest keys: one cluster per run
         CK(cudaStreamWaitEvent(st, sc.ev_join, 0));
         h->launches += 2;
     } else if (n_max >= LONG_RUN_MIN) {
-        decide_runs_kernel<1, BY_ROW><<<h->sms, LONG_THREADS, 0, st>>>(h->tab, src, sc.drec, om, sc.long_runs, sc.long_count);
+        decide_runs_kernel<1, BY_ROW, R16><<<h->sms, LONG_THREADS, 0, st>>>(h->tab, src, sc.drec, om, sc.long_runs, sc.long_count);
         h->launches++;
     }
     return GCRA_OK;
 }
 
-// the warp-cooperative compare-and-update over sorted keys + the hot-run kernels
+// the warp-cooperative compare-and-update over sorted keys + the hot-run kernels; r16: 16-byte results (FMT_16_16)
 static int enqueue_decide_sorted(gcra_engine *h, Scratch &sc, uint32_t n_max, const u32 *n_dev, const u64 *src,
-                                 const OutMap &om, cudaStream_t st) {
-    return om.by_row ? enqueue_decide_sorted_t<true>(h, sc, n_max, n_dev, src, om, st)
-                     : enqueue_decide_sorted_t<false>(h, sc, n_max, n_dev, src, om, st);
+                                 const OutMap &om, bool r16, cudaStream_t st) {
+    if (r16)
+        return om.by_row ? enqueue_decide_sorted_t<true, true>(h, sc, n_max, n_dev, src, om, st)
+                         : enqueue_decide_sorted_t<false, true>(h, sc, n_max, n_dev, src, om, st);
+    return om.by_row ? enqueue_decide_sorted_t<true, false>(h, sc, n_max, n_dev, src, om, st)
+                     : enqueue_decide_sorted_t<false, false>(h, sc, n_max, n_dev, src, om, st);
 }
 
 // per-set buffers of the index-order pipeline for batches of up to `rows` row ids
@@ -632,11 +635,12 @@ static int alloc_index_scratch(gcra_engine *h, Scratch &sc, uint32_t rows) {
 }
 
 // metrics bridge: count this batch's denied rows per key (single-segment batches: request and result rows local)
-static int enqueue_denied(gcra_engine *h, const BatchView &v, bool compact, cudaStream_t st) {
+static int enqueue_denied(gcra_engine *h, const BatchView &v, int fmt, cudaStream_t st) {
     if (!h->denied_max || v.nseg != 1 || v.n == 0) return GCRA_OK;
     const uint32_t tiles = (v.n + TILE_THREADS - 1) / TILE_THREADS;
-    if (compact) denied_count_kernel<true><<<tiles, TILE_THREADS, 0, st>>>(v.req0, v.res0, v.n, h->denied);
-    else denied_count_kernel<false><<<tiles, TILE_THREADS, 0, st>>>(v.req0, v.res0, v.n, h->denied);
+    if (fmt == FMT_16_16) denied_count_kernel<FMT_16_16><<<tiles, TILE_THREADS, 0, st>>>(v.req0, v.res0, v.n, h->denied);
+    else if (fmt == FMT_16_32) denied_count_kernel<FMT_16_32><<<tiles, TILE_THREADS, 0, st>>>(v.req0, v.res0, v.n, h->denied);
+    else denied_count_kernel<FMT_48_32><<<tiles, TILE_THREADS, 0, st>>>(v.req0, v.res0, v.n, h->denied);
     h->launches++;
     CK(cudaGetLastError());
     return GCRA_OK;
@@ -654,21 +658,24 @@ static uint32_t view_max_rows(const BatchView &v) { return v.nseg == 1 ? v.n : (
 // the keys array; it never touches the state array), which no earlier batch's decide kernels touch.
 //   sort pipeline         ingest (validate, derive, probe/claim) + stable sort by slot
 //   index-order pipeline  pass A (probe) + pass A' (batch bitmap)
-static int enqueue_front(gcra_engine *h, Scratch &sc, const BatchView &v, bool index_path, bool compact, int64_t now_batch,
+static int enqueue_front(gcra_engine *h, Scratch &sc, const BatchView &v, bool index_path, int fmt, int64_t now_batch,
                          cudaStream_t st, bool timed, u64 **sorted_out) {
     if (timed) CK(cudaEventRecord(h->ev[0], st));
     *sorted_out = nullptr;
     if (index_path) {
         const uint32_t rows = view_max_rows(v);
         const uint32_t tiles = (rows + TILE_THREADS - 1) / TILE_THREADS;
-        const uint32_t grid = std::min<uint32_t>(tiles, h->grid_probe[compact ? 1 : 0]);    // persistent, software-pipelined CTAs
+        const uint32_t grid = std::min<uint32_t>(tiles, h->grid_probe[fmt]);    // persistent, software-pipelined CTAs
         CK(cudaMemsetAsync(sc.ctrl_block, 0, ((size_t)h->max_tiles + 2) * sizeof(u64), st));
         if (timed) CK(cudaEventRecord(h->evd[0], st));
-        if (compact)
-            probe_kernel<true><<<grid, TILE_THREADS, 0, st>>>(h->tab, v, h->d_pol, h->npol, now_batch, sc.slot_arr, sc.bitmap,
-                                                              h->bm_mask, h->prefetch_state);
+        if (fmt == FMT_16_16)
+            probe_kernel<FMT_16_16><<<grid, TILE_THREADS, 0, st>>>(h->tab, v, h->d_pol, h->npol, now_batch, sc.slot_arr,
+                                                                   sc.bitmap, h->bm_mask, h->prefetch_state);
+        else if (fmt == FMT_16_32)
+            probe_kernel<FMT_16_32><<<grid, TILE_THREADS, 0, st>>>(h->tab, v, h->d_pol, h->npol, now_batch, sc.slot_arr,
+                                                                   sc.bitmap, h->bm_mask, h->prefetch_state);
         else
-            probe_kernel<false><<<grid, TILE_THREADS, 0, st>>>(h->tab, v, nullptr, 0, 0, sc.slot_arr, sc.bitmap, h->bm_mask,
+            probe_kernel<FMT_48_32><<<grid, TILE_THREADS, 0, st>>>(h->tab, v, nullptr, 0, 0, sc.slot_arr, sc.bitmap, h->bm_mask,
                                                                h->prefetch_state);
         if (timed) CK(cudaEventRecord(h->evd[1], st));
         h->launches += 1;
@@ -677,11 +684,14 @@ static int enqueue_front(gcra_engine *h, Scratch &sc, const BatchView &v, bool i
     }
     const uint32_t n = v.n;
     const uint32_t tiles = (n + TILE_THREADS - 1) / TILE_THREADS;
-    if (compact)
-        ingest_kernel<true><<<tiles, TILE_THREADS, 0, st>>>(h->tab, v.req0, h->d_pol, h->npol, now_batch, n,
-                                                            sc.drec, sc.keys_a, v.res0);
+    if (fmt == FMT_16_16)
+        ingest_kernel<FMT_16_16><<<tiles, TILE_THREADS, 0, st>>>(h->tab, v.req0, h->d_pol, h->npol, now_batch, n,
+                                                                 sc.drec, sc.keys_a, v.res0);
+    else if (fmt == FMT_16_32)
+        ingest_kernel<FMT_16_32><<<tiles, TILE_THREADS, 0, st>>>(h->tab, v.req0, h->d_pol, h->npol, now_batch, n,
+                                                                 sc.drec, sc.keys_a, v.res0);
     else
-        ingest_kernel<false><<<tiles, TILE_THREADS, 0, st>>>(h->tab, v.req0, nullptr, 0, 0, n, sc.drec,
+        ingest_kernel<FMT_48_32><<<tiles, TILE_THREADS, 0, st>>>(h->tab, v.req0, nullptr, 0, 0, n, sc.drec,
                                                              sc.keys_a, v.res0);
     h->launches++;
     if (timed) CK(cudaEventRecord(h->ev[1], st));
@@ -694,7 +704,7 @@ static int enqueue_front(gcra_engine *h, Scratch &sc, const BatchView &v, bool i
 // Stage 2 of an index-order batch: pass B (decide in batch order) + pass C (resolve).  Batches' stages 2 run
 // strictly in submission order.  `next` is the scratch set the NEXT batch will use: pass C leaves the PEND bits
 // of this batch's residue keys in its bitmap.  This set's own bitmap is cleared for its next use afterwards.
-static int enqueue_mid_index(gcra_engine *h, Scratch &sc, Scratch &next, const BatchView &v, bool compact, int64_t now_batch,
+static int enqueue_mid_index(gcra_engine *h, Scratch &sc, Scratch &next, const BatchView &v, int fmt, int64_t now_batch,
                              bool honour_pend, cudaStream_t st, bool timed) {
     const u32 hp = honour_pend ? 1u : 0u;
     if (++h->epoch == 0) {
@@ -703,22 +713,31 @@ static int enqueue_mid_index(gcra_engine *h, Scratch &sc, Scratch &next, const B
         h->epoch = 1;
     }
     const uint32_t rows = view_max_rows(v);
-    const uint32_t grid = std::min<uint32_t>((rows + TILE_THREADS - 1) / TILE_THREADS, h->grid_decide[compact ? 1 : 0]);   // persistent CTAs
+    const uint32_t grid = std::min<uint32_t>((rows + TILE_THREADS - 1) / TILE_THREADS, h->grid_decide[fmt]);   // persistent CTAs
     const uint32_t rgrid = std::min<uint32_t>((rows + RES_TILE - 1) / RES_TILE + v.nseg, 6 * h->sms);
     u32 *ctrl = reinterpret_cast<u32 *>(sc.ctrl_block);
     u64 *status = sc.ctrl_block + 2;
-    if (compact) {
-        decide_index_kernel<true><<<grid, TILE_THREADS, 0, st>>>(h->tab, v, h->d_pol, h->npol, now_batch, sc.slot_arr,
-                                                                 sc.bitmap, sc.pend, h->bm_mask, sc.flags, h->epoch, hp, h->dbg);
+    if (fmt == FMT_16_16) {
+        decide_index_kernel<FMT_16_16><<<grid, TILE_THREADS, 0, st>>>(h->tab, v, h->d_pol, h->npol, now_batch, sc.slot_arr,
+                                                                      sc.bitmap, sc.pend, h->bm_mask, sc.flags, h->epoch, hp,
+                                                                      h->dbg);
         if (timed) CK(cudaEventRecord(h->evd[3], st));
-        resolve_kernel<true><<<rgrid, TILE_THREADS, 0, st>>>(h->tab, v, h->d_pol, h->npol, now_batch, sc.slot_arr,
-                                                             h->bm_mask, sc.flags, h->epoch, ctrl, status, sc.keys_a,
-                                                             next.pend, sc.h_nres, h->max_batch);
+        resolve_kernel<FMT_16_16><<<rgrid, TILE_THREADS, 0, st>>>(h->tab, v, h->d_pol, h->npol, now_batch, sc.slot_arr,
+                                                                  h->bm_mask, sc.flags, h->epoch, ctrl, status, sc.keys_a,
+                                                                  next.pend, sc.h_nres, h->max_batch);
+    } else if (fmt == FMT_16_32) {
+        decide_index_kernel<FMT_16_32><<<grid, TILE_THREADS, 0, st>>>(h->tab, v, h->d_pol, h->npol, now_batch, sc.slot_arr,
+                                                                      sc.bitmap, sc.pend, h->bm_mask, sc.flags, h->epoch, hp,
+                                                                      h->dbg);
+        if (timed) CK(cudaEventRecord(h->evd[3], st));
+        resolve_kernel<FMT_16_32><<<rgrid, TILE_THREADS, 0, st>>>(h->tab, v, h->d_pol, h->npol, now_batch, sc.slot_arr,
+                                                                  h->bm_mask, sc.flags, h->epoch, ctrl, status, sc.keys_a,
+                                                                  next.pend, sc.h_nres, h->max_batch);
     } else {
-        decide_index_kernel<false><<<grid, TILE_THREADS, 0, st>>>(h->tab, v, nullptr, 0, 0, sc.slot_arr, sc.bitmap, sc.pend,
+        decide_index_kernel<FMT_48_32><<<grid, TILE_THREADS, 0, st>>>(h->tab, v, nullptr, 0, 0, sc.slot_arr, sc.bitmap, sc.pend,
                                                                   h->bm_mask, sc.flags, h->epoch, hp, h->dbg);
         if (timed) CK(cudaEventRecord(h->evd[3], st));
-        resolve_kernel<false><<<rgrid, TILE_THREADS, 0, st>>>(h->tab, v, nullptr, 0, 0, sc.slot_arr, h->bm_mask,
+        resolve_kernel<FMT_48_32><<<rgrid, TILE_THREADS, 0, st>>>(h->tab, v, nullptr, 0, 0, sc.slot_arr, h->bm_mask,
                                                               sc.flags, h->epoch, ctrl, status, sc.keys_a,
                                                               next.pend, sc.h_nres, h->max_batch);
     }
@@ -737,7 +756,7 @@ static int enqueue_mid_index(gcra_engine *h, Scratch &sc, Scratch &next, const B
 // Stage 3 of an index-order batch: the residue (requests behind the first state change of their key, and
 // requests deferred because the previous batch's tail still owned their key) through the sort pipeline; its
 // size only exists on the device.  Tails run strictly in submission order.
-static int enqueue_tail_index(gcra_engine *h, Scratch &sc, const BatchView &v, bool compact, int64_t now_batch, cudaStream_t st,
+static int enqueue_tail_index(gcra_engine *h, Scratch &sc, const BatchView &v, int fmt, int64_t now_batch, cudaStream_t st,
                               bool timed) {
     const u32 *n_res = reinterpret_cast<const u32 *>(sc.ctrl_block) + RC_NRES;
     const uint32_t n_max = std::min<uint32_t>(view_max_rows(v), h->max_batch);
@@ -752,39 +771,41 @@ static int enqueue_tail_index(gcra_engine *h, Scratch &sc, const BatchView &v, b
     OutMap om{};
     om.out = nullptr;
     om.by_row = 1;
-    om.compact = compact ? 1 : 0;
+    om.compact = fmt != FMT_48_32 ? 1 : 0;
     om.view = v;
     om.pol = h->d_pol;
     om.npol = h->npol;
     om.now_batch = now_batch;
-    RC(enqueue_decide_sorted(h, sc, n_max, n_res, rs, om, st));
+    RC(enqueue_decide_sorted(h, sc, n_max, n_res, rs, om, fmt == FMT_16_16, st));
     if (timed) { CK(cudaEventRecord(h->ev[3], st)); h->ev_valid = true; CK(cudaEventRecord(h->evd[7], st)); h->evd_valid = true; }
     CK(cudaGetLastError());
     return GCRA_OK;
 }
 
 // Stage 2 of a sort-pipeline batch: the compare-and-update kernels over the sorted keys
-static int enqueue_back_sorted(gcra_engine *h, Scratch &sc, const BatchView &v, const u64 *sorted, cudaStream_t st, bool timed) {
+static int enqueue_back_sorted(gcra_engine *h, Scratch &sc, const BatchView &v, int fmt, const u64 *sorted, cudaStream_t st,
+                               bool timed) {
     OutMap om{};
     om.out = v.res0;
     om.by_row = 0;
-    RC(enqueue_decide_sorted(h, sc, v.n, nullptr, sorted, om, st));
+    RC(enqueue_decide_sorted(h, sc, v.n, nullptr, sorted, om, fmt == FMT_16_16, st));
     if (timed) { CK(cudaEventRecord(h->ev[3], st)); h->ev_valid = true; }
     CK(cudaGetLastError());
     return GCRA_OK;
 }
 
-static int check_batch(gcra_engine *h, uint32_t n, bool compact) {
+static int check_batch(gcra_engine *h, uint32_t n, int fmt) {
     if (n > h->max_batch) { h->err = "batch larger than max_batch"; return GCRA_INTERNAL; }
-    if (compact && h->npol == 0) { h->err = "no policy table registered"; return GCRA_INTERNAL; }
+    if (fmt != FMT_48_32 && h->npol == 0) { h->err = "no policy table registered"; return GCRA_INTERNAL; }
     return ensure_room(h, n);
 }
 
 // ---- one batch, everything on the caller's stream ------------------------------------------------
-static int launch_batch(gcra_engine *h, uint32_t n, const void *d_req, bool compact, int64_t now_batch,
-                        gcra_result *d_res, cudaStream_t st, bool timed) {
+static int launch_batch(gcra_engine *h, uint32_t n, const void *d_req, int fmt, int64_t now_batch,
+                        void *d_res_rows, cudaStream_t st, bool timed) {
     if (n == 0) return GCRA_OK;
-    RC(check_batch(h, n, compact));
+    RC(check_batch(h, n, fmt));
+    gcra_result *d_res = (gcra_result *)d_res_rows;     // (gcra_result16 rows for FMT_16_16: see BatchView::res16_at)
     const uint32_t k = h->scr_next;
     Scratch &sc = h->scr[k];
     h->scr_next = (h->scr_next + 1) % gcra_engine::N_SCR;
@@ -797,10 +818,12 @@ static int launch_batch(gcra_engine *h, uint32_t n, const void *d_req, bool comp
         // small batch (a single rate_limit call, a lightly loaded actor): one CTA does ingest, ordering and
         // the compare-and-update in a single launch
         if (timed) { CK(cudaEventRecord(h->ev[0], st)); CK(cudaEventRecord(h->ev[1], st)); CK(cudaEventRecord(h->ev[2], st)); }
-        if (compact)
-            small_batch_kernel<true><<<1, TILE_THREADS, 0, st>>>(h->tab, d_req, h->d_pol, h->npol, now_batch, n, sc.drec, d_res);
+        if (fmt == FMT_16_16)
+            small_batch_kernel<FMT_16_16><<<1, TILE_THREADS, 0, st>>>(h->tab, d_req, h->d_pol, h->npol, now_batch, n, sc.drec, d_res);
+        else if (fmt == FMT_16_32)
+            small_batch_kernel<FMT_16_32><<<1, TILE_THREADS, 0, st>>>(h->tab, d_req, h->d_pol, h->npol, now_batch, n, sc.drec, d_res);
         else
-            small_batch_kernel<false><<<1, TILE_THREADS, 0, st>>>(h->tab, d_req, nullptr, 0, 0, n, sc.drec, d_res);
+            small_batch_kernel<FMT_48_32><<<1, TILE_THREADS, 0, st>>>(h->tab, d_req, nullptr, 0, 0, n, sc.drec, d_res);
         h->launches++;
         if (timed) { CK(cudaEventRecord(h->ev[3], st)); h->ev_valid = true; }
         CK(cudaGetLastError());
@@ -808,18 +831,18 @@ static int launch_batch(gcra_engine *h, uint32_t n, const void *d_req, bool comp
         u64 *sorted = nullptr;
         const BatchView v = single_view(d_req, d_res, n);
         const bool ip = use_index_path(h, n);
-        RC(enqueue_front(h, sc, v, ip, compact, now_batch, st, timed, &sorted));
+        RC(enqueue_front(h, sc, v, ip, fmt, now_batch, st, timed, &sorted));
         if (ip) {
-            RC(enqueue_mid_index(h, sc, next, v, compact, now_batch, false, st, timed));
+            RC(enqueue_mid_index(h, sc, next, v, fmt, now_batch, false, st, timed));
             CK(cudaEventRecord(sc.ev_mid, st));
             sc.mid_recorded = true;
-            RC(enqueue_tail_index(h, sc, v, compact, now_batch, st, timed));
+            RC(enqueue_tail_index(h, sc, v, fmt, now_batch, st, timed));
         } else {
-            RC(enqueue_back_sorted(h, sc, v, sorted, st, timed));
+            RC(enqueue_back_sorted(h, sc, v, fmt, sorted, st, timed));
             sc.mid_recorded = false;
         }
     }
-    RC(enqueue_denied(h, single_view(d_req, d_res, n), compact, st));
+    RC(enqueue_denied(h, single_view(d_req, d_res, n), fmt, st));
     CK(cudaEventRecord(sc.ev_back, st));
     sc.back_recorded = true;
     h->pend_set = -1;          // everything of this batch is ordered on `st`: the next batch waits for all of it
@@ -833,9 +856,11 @@ static int launch_batch(gcra_engine *h, uint32_t n, const void *d_req, bool comp
 // ingest + sort, stage 2 = decide, after every earlier batch has completely finished.
 // `ready` (may be null) is an event after which the requests may be read; `*done` is set to an event after which
 // the results are complete.
-static int launch_pipelined_view(gcra_engine *h, const BatchView &v, uint32_t n_rows, bool compact, int64_t now_batch,
+static int launch_pipelined_view(gcra_engine *h, const BatchView &v, uint32_t n_rows, int fmt, int64_t now_batch,
                                  cudaEvent_t ready, cudaEvent_t *done) {
-    RC(check_batch(h, n_rows, compact));
+    // 16-byte results are a single-GPU format: the multi-GPU ticks return 32-byte rows into peers' outboxes
+    if (fmt == FMT_16_16 && v.nseg != 1) { h->err = "16-byte results need a single-segment batch"; return GCRA_INTERNAL; }
+    RC(check_batch(h, n_rows, fmt));
     const uint32_t k = h->scr_next;
     Scratch &sc = h->scr[k];
     h->scr_next = (h->scr_next + 1) % gcra_engine::N_SCR;
@@ -866,7 +891,7 @@ static int launch_pipelined_view(gcra_engine *h, const BatchView &v, uint32_t n_
             h->sort_hold = 31; h->last_nres = 0; h->last_nres_rows = 0; ip = false; h->n_path_switches++;
         }
     }
-    RC(enqueue_front(h, sc, v, ip, compact, now_batch, fs, false, &sorted));
+    RC(enqueue_front(h, sc, v, ip, fmt, now_batch, fs, false, &sorted));
     CK(cudaEventRecord(sc.ev_front, fs));
     cudaStream_t ms = h->back_stream;
     CK(cudaStreamWaitEvent(ms, sc.ev_front, 0));
@@ -889,21 +914,21 @@ static int launch_pipelined_view(gcra_engine *h, const BatchView &v, uint32_t n_
         CK(cudaStreamWaitEvent(ms, os.ev_back, 0));
     }
     if (ip) {
-        RC(enqueue_mid_index(h, sc, h->scr[kn], v, compact, now_batch, overlap, ms, false));
+        RC(enqueue_mid_index(h, sc, h->scr[kn], v, fmt, now_batch, overlap, ms, false));
         CK(cudaEventRecord(sc.ev_mid, ms));
         sc.mid_recorded = true;
         cudaStream_t ts = h->tail_stream;
         CK(cudaStreamWaitEvent(ts, sc.ev_mid, 0));
-        RC(enqueue_tail_index(h, sc, v, compact, now_batch, ts, false));
-        RC(enqueue_denied(h, v, compact, ts));
+        RC(enqueue_tail_index(h, sc, v, fmt, now_batch, ts, false));
+        RC(enqueue_denied(h, v, fmt, ts));
         CK(cudaEventRecord(sc.ev_back, ts));
         sc.back_recorded = true;
         h->pend_set = (int)kn;
         if (done) *done = sc.ev_back;
         return snapshot_async(h, n_rows, ts);
     }
-    RC(enqueue_back_sorted(h, sc, v, sorted, ms, false));
-    RC(enqueue_denied(h, v, compact, ms));
+    RC(enqueue_back_sorted(h, sc, v, fmt, sorted, ms, false));
+    RC(enqueue_denied(h, v, fmt, ms));
     sc.mid_recorded = false;   // (no residue count from this batch)
     CK(cudaEventRecord(sc.ev_back, ms));
     sc.back_recorded = true;
@@ -912,10 +937,10 @@ static int launch_pipelined_view(gcra_engine *h, const BatchView &v, uint32_t n_
     return snapshot_async(h, n_rows, ms);
 }
 
-static int launch_pipelined(gcra_engine *h, uint32_t n, const void *d_req, bool compact, int64_t now_batch,
-                            gcra_result *d_res, cudaEvent_t ready, cudaEvent_t *done) {
+static int launch_pipelined(gcra_engine *h, uint32_t n, const void *d_req, int fmt, int64_t now_batch,
+                            void *d_res, cudaEvent_t ready, cudaEvent_t *done) {
     if (n == 0) { if (done) *done = nullptr; return GCRA_OK; }
-    return launch_pipelined_view(h, single_view(d_req, d_res, n), n, compact, now_batch, ready, done);
+    return launch_pipelined_view(h, single_view(d_req, (gcra_result *)d_res, n), n, fmt, now_batch, ready, done);
 }
 
 // CUDA loads a kernel's code lazily, at its FIRST launch, and that load may wait for running kernels.  The
@@ -928,20 +953,23 @@ static void preload(K kernel) {
 }
 
 static void preload_kernels() {
-    preload(ingest_kernel<false>); preload(ingest_kernel<true>);
-    preload(small_batch_kernel<false>); preload(small_batch_kernel<true>);
+    preload(ingest_kernel<FMT_48_32>); preload(ingest_kernel<FMT_16_32>); preload(ingest_kernel<FMT_16_16>);
+    preload(small_batch_kernel<FMT_48_32>); preload(small_batch_kernel<FMT_16_32>); preload(small_batch_kernel<FMT_16_16>);
     preload(sort_hist_kernel); preload(sort_rowscan_kernel); preload(sort_scatter_kernel); preload(sort_pass_fused_kernel);
-    preload(decide_kernel<false>); preload(decide_kernel<true>);
-    preload(decide_runs_kernel<1, false>); preload(decide_runs_kernel<CLUSTER_CTAS, false>);
-    preload(decide_runs_kernel<1, true>); preload(decide_runs_kernel<CLUSTER_CTAS, true>);
-    preload(probe_kernel<false>); preload(probe_kernel<true>);
-    preload(decide_index_kernel<false>); preload(decide_index_kernel<true>);
-    preload(resolve_kernel<false>); preload(resolve_kernel<true>);
+    preload(decide_kernel<false, false>); preload(decide_kernel<true, false>);
+    preload(decide_kernel<false, true>); preload(decide_kernel<true, true>);
+    preload(decide_runs_kernel<1, false, false>); preload(decide_runs_kernel<CLUSTER_CTAS, false, false>);
+    preload(decide_runs_kernel<1, true, false>); preload(decide_runs_kernel<CLUSTER_CTAS, true, false>);
+    preload(decide_runs_kernel<1, false, true>); preload(decide_runs_kernel<CLUSTER_CTAS, false, true>);
+    preload(decide_runs_kernel<1, true, true>); preload(decide_runs_kernel<CLUSTER_CTAS, true, true>);
+    preload(probe_kernel<FMT_48_32>); preload(probe_kernel<FMT_16_32>); preload(probe_kernel<FMT_16_16>);
+    preload(decide_index_kernel<FMT_48_32>); preload(decide_index_kernel<FMT_16_32>); preload(decide_index_kernel<FMT_16_16>);
+    preload(resolve_kernel<FMT_48_32>); preload(resolve_kernel<FMT_16_32>); preload(resolve_kernel<FMT_16_16>);
     preload(sweep_kernel); preload(purge_kernel); preload(clear_slots_kernel); preload(rehash_kernel); preload(store_op_kernel);
     preload(route_count_kernel); preload(route_scan_kernel); preload(route_scatter_kernel); preload(route_unpermute_kernel);
     preload(p2p_scan_kernel); preload(p2p_scatter_kernel); preload(p2p_signal_req_kernel); preload(p2p_signal_res_kernel);
     preload(p2p_wait_kernel); preload(p2p_unpermute_kernel);
-    preload(denied_count_kernel<false>); preload(denied_count_kernel<true>);
+    preload(denied_count_kernel<FMT_48_32>); preload(denied_count_kernel<FMT_16_32>); preload(denied_count_kernel<FMT_16_16>);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -1026,15 +1054,17 @@ int32_t gcra_create(const gcra_config *cfg, gcra_engine **out) {
         h->prefetch_state = 0;
         if (const char *g = getenv("GCRA_PREFETCH")) h->prefetch_state = atoi(g);
         int nb = 0;
-        h->grid_probe[0] = h->grid_probe[1] = 4 * h->sms;      // used when the occupancy query fails
-        h->grid_decide[0] = h->grid_decide[1] = 3 * h->sms;
-        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, probe_kernel<false>, TILE_THREADS, 0) == cudaSuccess && nb > 0) h->grid_probe[0] = (uint32_t)(nb * sms);
-        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, probe_kernel<true>, TILE_THREADS, 0) == cudaSuccess && nb > 0) h->grid_probe[1] = (uint32_t)(nb * sms);
-        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, decide_index_kernel<false>, TILE_THREADS, 0) == cudaSuccess && nb > 0) h->grid_decide[0] = (uint32_t)(nb * sms);
-        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, decide_index_kernel<true>, TILE_THREADS, 0) == cudaSuccess && nb > 0) h->grid_decide[1] = (uint32_t)(nb * sms);
+        h->grid_probe[0] = h->grid_probe[1] = h->grid_probe[2] = 4 * h->sms;      // used when the occupancy query fails
+        h->grid_decide[0] = h->grid_decide[1] = h->grid_decide[2] = 3 * h->sms;
+        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, probe_kernel<FMT_48_32>, TILE_THREADS, 0) == cudaSuccess && nb > 0) h->grid_probe[0] = (uint32_t)(nb * sms);
+        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, probe_kernel<FMT_16_32>, TILE_THREADS, 0) == cudaSuccess && nb > 0) h->grid_probe[1] = (uint32_t)(nb * sms);
+        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, probe_kernel<FMT_16_16>, TILE_THREADS, 0) == cudaSuccess && nb > 0) h->grid_probe[2] = (uint32_t)(nb * sms);
+        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, decide_index_kernel<FMT_48_32>, TILE_THREADS, 0) == cudaSuccess && nb > 0) h->grid_decide[0] = (uint32_t)(nb * sms);
+        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, decide_index_kernel<FMT_16_32>, TILE_THREADS, 0) == cudaSuccess && nb > 0) h->grid_decide[1] = (uint32_t)(nb * sms);
+        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, decide_index_kernel<FMT_16_16>, TILE_THREADS, 0) == cudaSuccess && nb > 0) h->grid_decide[2] = (uint32_t)(nb * sms);
         // tuning: CTAs per SM of the persistent kernels (fewer leave room for the other stages' kernels)
-        if (const char *g = getenv("GCRA_CTAS_PROBE")) { uint32_t c = (uint32_t)atoi(g) * sms; if (c) { h->grid_probe[0] = std::min(h->grid_probe[0], c); h->grid_probe[1] = std::min(h->grid_probe[1], c); } }
-        if (const char *g = getenv("GCRA_CTAS_DECIDE")) { uint32_t c = (uint32_t)atoi(g) * sms; if (c) { h->grid_decide[0] = std::min(h->grid_decide[0], c); h->grid_decide[1] = std::min(h->grid_decide[1], c); } }
+        if (const char *g = getenv("GCRA_CTAS_PROBE")) { uint32_t c = (uint32_t)atoi(g) * sms; if (c) for (auto &x : h->grid_probe) x = std::min(x, c); }
+        if (const char *g = getenv("GCRA_CTAS_DECIDE")) { uint32_t c = (uint32_t)atoi(g) * sms; if (c) for (auto &x : h->grid_decide) x = std::min(x, c); }
     }
     bool ok = cudaMalloc(&h->d_req, mb * sizeof(gcra_request)) == cudaSuccess &&
               cudaMalloc(&h->d_res, mb * sizeof(gcra_result)) == cudaSuccess &&
@@ -1277,13 +1307,19 @@ int32_t gcra_store_set_nx(gcra_engine *h, const void *key, uint64_t len, int64_t
 int32_t gcra_rate_limit_batch_device(gcra_engine *h, uint64_t n, const gcra_request *d_req, gcra_result *d_res,
                                      void *stream) {
     CK(cudaSetDevice(h->device));
-    return launch_batch(h, (uint32_t)n, d_req, false, 0, d_res, stream ? (cudaStream_t)stream : h->stream, true);
+    return launch_batch(h, (uint32_t)n, d_req, FMT_48_32, 0, d_res, stream ? (cudaStream_t)stream : h->stream, true);
 }
 
 int32_t gcra_rate_limit_batch16_device(gcra_engine *h, uint64_t n, const gcra_request16 *d_req, int64_t now_ns,
                                        gcra_result *d_res, void *stream) {
     CK(cudaSetDevice(h->device));
-    return launch_batch(h, (uint32_t)n, d_req, true, now_ns, d_res, stream ? (cudaStream_t)stream : h->stream, true);
+    return launch_batch(h, (uint32_t)n, d_req, FMT_16_32, now_ns, d_res, stream ? (cudaStream_t)stream : h->stream, true);
+}
+
+int32_t gcra_rate_limit_batch16_r16_device(gcra_engine *h, uint64_t n, const gcra_request16 *d_req, int64_t now_ns,
+                                           gcra_result16 *d_res, void *stream) {
+    CK(cudaSetDevice(h->device));
+    return launch_batch(h, (uint32_t)n, d_req, FMT_16_16, now_ns, d_res, stream ? (cudaStream_t)stream : h->stream, true);
 }
 
 int32_t gcra_rate_limit_batch_device_pipelined(gcra_engine *h, uint64_t n, const gcra_request *d_req,
@@ -1294,7 +1330,7 @@ int32_t gcra_rate_limit_batch_device_pipelined(gcra_engine *h, uint64_t n, const
         CK(cudaEventRecord(h->ev_ready, (cudaStream_t)ready_stream));
         ready = h->ev_ready;
     }
-    return launch_pipelined(h, (uint32_t)n, d_req, false, 0, d_res, ready, nullptr);
+    return launch_pipelined(h, (uint32_t)n, d_req, FMT_48_32, 0, d_res, ready, nullptr);
 }
 
 int32_t gcra_pipeline_join(gcra_engine *h, void *stream) {
@@ -1307,9 +1343,11 @@ int32_t gcra_pipeline_join(gcra_engine *h, void *stream) {
     return GCRA_OK;
 }
 
-static int host_batch(gcra_engine *h, uint64_t n, const void *req, size_t rsz, bool compact, int64_t now_batch,
-                      gcra_result *res) {
+static int host_batch(gcra_engine *h, uint64_t n, const void *req, int fmt, int64_t now_batch, void *res) {
     CK(cudaSetDevice(h->device));
+    const bool compact = fmt != FMT_48_32;
+    const size_t rsz = compact ? sizeof(gcra_request16) : sizeof(gcra_request);
+    const size_t ressz = fmt == FMT_16_16 ? sizeof(gcra_result16) : sizeof(gcra_result);
     uint64_t done = 0;
     while (done < n) {
         uint32_t m = (uint32_t)std::min<uint64_t>(n - done, h->max_batch);
@@ -1320,9 +1358,9 @@ static int host_batch(gcra_engine *h, uint64_t n, const void *req, size_t rsz, b
         int rc = apply_policy(h, now_hint);
         if (rc) return rc;
         CK(cudaMemcpyAsync(h->d_req, src, (size_t)m * rsz, cudaMemcpyHostToDevice, h->stream));
-        rc = launch_batch(h, m, h->d_req, compact, now_batch, h->d_res, h->stream, true);
+        rc = launch_batch(h, m, h->d_req, fmt, now_batch, h->d_res, h->stream, true);
         if (rc) return rc;
-        CK(cudaMemcpyAsync(res + done, h->d_res, (size_t)m * sizeof(gcra_result), cudaMemcpyDeviceToHost, h->stream));
+        CK(cudaMemcpyAsync((unsigned char *)res + done * ressz, h->d_res, (size_t)m * ressz, cudaMemcpyDeviceToHost, h->stream));
         RC(refresh_counters(h, false));
         CK(cudaStreamSynchronize(h->stream));
         done += m;
@@ -1331,27 +1369,32 @@ static int host_batch(gcra_engine *h, uint64_t n, const void *req, size_t rsz, b
 }
 
 int32_t gcra_rate_limit_batch(gcra_engine *h, uint64_t n, const gcra_request *req, gcra_result *res) {
-    return host_batch(h, n, req, sizeof(gcra_request), false, 0, res);
+    return host_batch(h, n, req, FMT_48_32, 0, res);
 }
 
 int32_t gcra_rate_limit_batch16(gcra_engine *h, uint64_t n, const gcra_request16 *req, int64_t now_ns,
                                 gcra_result *res) {
-    return host_batch(h, n, req, sizeof(gcra_request16), true, now_ns, res);
+    return host_batch(h, n, req, FMT_16_32, now_ns, res);
+}
+
+int32_t gcra_rate_limit_batch16_r16(gcra_engine *h, uint64_t n, const gcra_request16 *req, int64_t now_ns,
+                                    gcra_result16 *res) {
+    return host_batch(h, n, req, FMT_16_16, now_ns, res);
 }
 
 int32_t gcra_rate_limit(gcra_engine *h, const void *key, uint64_t len, int64_t max_burst, int64_t count_per_period,
                         int64_t period, int64_t quantity, int64_t now_ns, gcra_result *out) {
     gcra_request r = {engine_hash(h, key, len), max_burst, count_per_period, period, quantity, now_ns};
     gcra_result tmp;
-    int rc = host_batch(h, 1, &r, sizeof(r), false, 0, &tmp);
+    int rc = host_batch(h, 1, &r, FMT_48_32, 0, &tmp);
     if (rc) { if (out) { memset(out, 0, sizeof(*out)); out->status = GCRA_INTERNAL; } return rc; }
     if (out) *out = tmp;
     if (tmp.status == GCRA_INTERNAL) h->err = "rate_limit: internal (duration overflow, pre-epoch time or table full)";
     return tmp.status;
 }
 
-int32_t gcra_set_policies(gcra_engine *h, uint32_t n, const gcra_policy *policies) {
-    CK(cudaSetDevice(h->device));
+// validation (rate_limiter.rs:115-117) + derivation of every policy of a table, once
+static std::vector<PolicyDerived> derive_policies(uint32_t n, const gcra_policy *policies) {
     std::vector<PolicyDerived> pd(n);
     for (uint32_t i = 0; i < n; i++) {
         const gcra_policy &p = policies[i];
@@ -1359,6 +1402,12 @@ int32_t gcra_set_policies(gcra_engine *h, uint32_t n, const gcra_policy *policie
         if (p.max_burst <= 0 || p.count_per_period <= 0 || p.period <= 0) pd[i].status = GCRA_INVALID_RATE_LIMIT;
         else pd[i].status = derive_params(p.max_burst, p.count_per_period, p.period, &pd[i].ei, &pd[i].dvt);
     }
+    return pd;
+}
+
+int32_t gcra_set_policies(gcra_engine *h, uint32_t n, const gcra_policy *policies) {
+    CK(cudaSetDevice(h->device));
+    std::vector<PolicyDerived> pd = derive_policies(n, policies);
     CK(cudaStreamSynchronize(h->stream));
     cudaFree(h->d_pol);
     h->d_pol = nullptr;
@@ -1371,22 +1420,55 @@ int32_t gcra_set_policies(gcra_engine *h, uint32_t n, const gcra_policy *policie
     return GCRA_OK;
 }
 
+// Host only, no handle: the 32-byte results of a compact batch from its 16-byte results.  The same outputs_from_cur the
+// kernels' outputs_of goes through (gcra_device.cuh), so the rows equal the 32-byte path's bit for bit -- given the
+// policy table the batch ran with.
+int32_t gcra_expand_results16(uint64_t n, const gcra_request16 *req, int64_t now_ns, const gcra_policy *policies,
+                              uint32_t npol, const gcra_result16 *in, gcra_result *out) {
+    const std::vector<PolicyDerived> pd = derive_policies(npol, policies);
+    int32_t rc = GCRA_OK;
+    for (uint64_t i = 0; i < n; i++) {
+        gcra_result o;
+        memset(&o, 0, sizeof(o));
+        o.status = in[i].status;
+        if (o.status == GCRA_OK) {
+            const uint32_t p = req[i].policy;
+            if (p >= npol || pd[p].status != GCRA_OK || now_ns < 0 || req[i].quantity < 0) {
+                // the engine cannot have decided this row with this table: not the table the batch ran with
+                o.status = GCRA_INTERNAL;
+                rc = GCRA_INTERNAL;
+            } else {
+                const Req r = {now_ns, pd[p].ei, pd[p].dvt, req[i].quantity};
+                const Outputs x = outputs_from_cur(in[i].cur_tat_ns, in[i].allowed != 0, r);
+                o.remaining = x.remaining;
+                o.reset_after_ns = x.reset_after;
+                o.retry_after_ns = x.retry_after;
+                o.allowed = in[i].allowed;
+            }
+        }
+        out[i] = o;
+    }
+    return rc;
+}
+
 // ---- ring --------------------------------------------------------------------------------------
-int32_t gcra_ring_create(gcra_engine *h, uint32_t slots, uint32_t slot_capacity, int32_t compact) {
+int32_t gcra_ring_create(gcra_engine *h, uint32_t slots, uint32_t slot_capacity, int32_t mode) {
     CK(cudaSetDevice(h->device));
     if (!h->ring.empty()) { h->err = "ring already created"; return GCRA_INTERNAL; }
     if (slot_capacity == 0 || slot_capacity > h->max_batch) { h->err = "slot_capacity must be in 1..max_batch"; return GCRA_INTERNAL; }
     h->ring_cap = slot_capacity;
-    h->ring_compact = compact != 0;
-    size_t rsz = compact ? sizeof(gcra_request16) : sizeof(gcra_request);
+    // 0: 48-byte requests, 32-byte results; any other value but 2: 16-byte requests, 32-byte results; 2: 16 / 16
+    h->ring_mode = mode == 0 ? FMT_48_32 : mode == 2 ? FMT_16_16 : FMT_16_32;
+    const size_t rsz = h->ring_mode != FMT_48_32 ? sizeof(gcra_request16) : sizeof(gcra_request);
+    const size_t ressz = h->ring_mode == FMT_16_16 ? sizeof(gcra_result16) : sizeof(gcra_result);
     h->ring.resize(slots);
     for (auto &s : h->ring) {
         // request slots are only WRITTEN by the host: optionally write-combined pinned memory (GCRA_RING_WC=1)
         CK(cudaHostAlloc(&s.h_req, slot_capacity * rsz,
                          getenv("GCRA_RING_WC") && atoi(getenv("GCRA_RING_WC")) ? cudaHostAllocWriteCombined : cudaHostAllocDefault));
-        CK(cudaMallocHost(&s.h_res, slot_capacity * sizeof(gcra_result)));
+        CK(cudaMallocHost(&s.h_res, slot_capacity * ressz));
         CK(cudaMalloc(&s.d_req, slot_capacity * rsz));
-        CK(cudaMalloc(&s.d_res, slot_capacity * sizeof(gcra_result)));
+        CK(cudaMalloc(&s.d_res, slot_capacity * ressz));
         CK(cudaEventCreateWithFlags(&s.ev_in, cudaEventDisableTiming));
         CK(cudaEventCreateWithFlags(&s.ev_comp, cudaEventDisableTiming));
         CK(cudaEventCreateWithFlags(&s.ev_done, cudaEventDisableTiming));
@@ -1395,7 +1477,12 @@ int32_t gcra_ring_create(gcra_engine *h, uint32_t slots, uint32_t slot_capacity,
 }
 
 void *gcra_ring_requests(gcra_engine *h, uint32_t slot) { return slot < h->ring.size() ? h->ring[slot].h_req : nullptr; }
-gcra_result *gcra_ring_results(gcra_engine *h, uint32_t slot) { return slot < h->ring.size() ? h->ring[slot].h_res : nullptr; }
+gcra_result *gcra_ring_results(gcra_engine *h, uint32_t slot) {
+    return slot < h->ring.size() && h->ring_mode != FMT_16_16 ? (gcra_result *)h->ring[slot].h_res : nullptr;
+}
+gcra_result16 *gcra_ring_results16(gcra_engine *h, uint32_t slot) {
+    return slot < h->ring.size() && h->ring_mode == FMT_16_16 ? (gcra_result16 *)h->ring[slot].h_res : nullptr;
+}
 
 int32_t gcra_ring_submit(gcra_engine *h, uint32_t slot, uint32_t n, int64_t now_ns) {
     CK(cudaSetDevice(h->device));
@@ -1404,17 +1491,18 @@ int32_t gcra_ring_submit(gcra_engine *h, uint32_t slot, uint32_t n, int64_t now_
     if (s.in_flight) { h->err = "ring slot still in flight"; return GCRA_INTERNAL; }
     // sweep policy with the counters of the batches finished so far (no stall)
     if (cudaEventQuery(h->ev_counters) == cudaSuccess) { int rc = apply_policy(h, now_ns); if (rc) return rc; }
-    size_t rsz = h->ring_compact ? sizeof(gcra_request16) : sizeof(gcra_request);
+    const size_t rsz = h->ring_mode != FMT_48_32 ? sizeof(gcra_request16) : sizeof(gcra_request);
+    const size_t ressz = h->ring_mode == FMT_16_16 ? sizeof(gcra_result16) : sizeof(gcra_result);
     CK(cudaMemcpyAsync(s.d_req, s.h_req, (size_t)n * rsz, cudaMemcpyHostToDevice, h->in_stream));
     CK(cudaEventRecord(s.ev_in, h->in_stream));
     // front half (ingest + order) of this slot overlaps the back half (decide) of the previous one
     cudaEvent_t done = nullptr;
-    int rc = launch_pipelined(h, n, s.d_req, h->ring_compact, now_ns, s.d_res, s.ev_in, &done);
+    int rc = launch_pipelined(h, n, s.d_req, h->ring_mode, now_ns, s.d_res, s.ev_in, &done);
     if (rc) return rc;
     if (done) CK(cudaStreamWaitEvent(h->out_stream, done, 0));
     CK(cudaMemcpyAsync(h->h_counters, h->tab.counters, C_COUNT * sizeof(u64), cudaMemcpyDeviceToHost, h->out_stream));
     CK(cudaEventRecord(h->ev_counters, h->out_stream));
-    CK(cudaMemcpyAsync(s.h_res, s.d_res, (size_t)n * sizeof(gcra_result), cudaMemcpyDeviceToHost, h->out_stream));
+    CK(cudaMemcpyAsync(s.h_res, s.d_res, (size_t)n * ressz, cudaMemcpyDeviceToHost, h->out_stream));
     CK(cudaEventRecord(s.ev_done, h->out_stream));
     s.in_flight = true;
     return GCRA_OK;
@@ -1872,7 +1960,7 @@ static int shard_issue_decide_return(gcra_engine *h) {
     for (uint32_t a = 0; a < sl.n_recv || a == 0; a += h->max_batch) {
         const uint32_t m = std::min<uint32_t>(sl.n_recv - a, h->max_batch);
         cudaEvent_t dn = nullptr;
-        RC(launch_pipelined(h, m, sl.recv_req + a, false, 0, sl.recv_res + a, sl.ev_routed, &dn));
+        RC(launch_pipelined(h, m, sl.recv_req + a, FMT_48_32, 0, sl.recv_res + a, sl.ev_routed, &dn));
         if (dn) { done = dn; CK(cudaStreamWaitEvent(sh->s_return, dn, 0)); }
         if (sl.n_recv == 0) break;
     }
@@ -2136,7 +2224,7 @@ int32_t gcra_p2p_submit_finish(gcra_engine *h, gcra_result *d_res) {
     // find_or_claim always does; the next tick's check then sees the real occupancy and grows the table.
     const uint32_t n_rows = (uint32_t)std::min<uint64_t>((uint64_t)sl.n + sl.n / 4 + 4096, std::min<uint64_t>((uint64_t)W << p->cap_shift, h->max_batch));
     if (p->timed) CK(cudaEventRecord(p->ev_t[2], p->s_wait));
-    RC(launch_pipelined_view(h, v, n_rows, false, 0, sl.ev_wait, &done));
+    RC(launch_pipelined_view(h, v, n_rows, FMT_48_32, 0, sl.ev_wait, &done));
     CK(cudaStreamWaitEvent(p->s_sig, done, 0));
     if (p->timed) CK(cudaEventRecord(p->ev_t[3], p->s_sig));
     p2p_signal_res_kernel<<<1, 32, 0, p->s_sig>>>(p->peers_dev, W, me, tick);

@@ -59,23 +59,28 @@ struct Table {
 };
 
 // ------------------------------------------------------------------ exact i64 arithmetic
-__device__ __forceinline__ i64 sat_add(i64 a, i64 b) {
+// (host and device: the host expands 16-byte results with the same outputs_from as the kernels)
+__host__ __device__ __forceinline__ i64 sat_add(i64 a, i64 b) {
     i64 r = (i64)((u64)a + (u64)b);
     if (((a ^ r) & (b ^ r)) < 0) r = a < 0 ? I64_MIN : I64_MAX;
     return r;
 }
-__device__ __forceinline__ i64 sat_sub(i64 a, i64 b) {
+__host__ __device__ __forceinline__ i64 sat_sub(i64 a, i64 b) {
     i64 r = (i64)((u64)a - (u64)b);
     if (((a ^ b) & (a ^ r)) < 0) r = a < 0 ? I64_MIN : I64_MAX;
     return r;
 }
-__device__ __forceinline__ i64 sat_mul(i64 a, i64 b) {
+__host__ __device__ __forceinline__ i64 sat_mul(i64 a, i64 b) {
     i64 lo = (i64)((u64)a * (u64)b);
+#ifdef __CUDA_ARCH__
     i64 hi = __mul64hi(a, b);
+#else
+    i64 hi = (i64)(((__int128)a * b) >> 64);
+#endif
     if (hi != (lo >> 63)) lo = ((a < 0) != (b < 0)) ? I64_MIN : I64_MAX;
     return lo;
 }
-__device__ __forceinline__ i64 wrap_add(i64 a, i64 b) { return (i64)((u64)a + (u64)b); }
+__host__ __device__ __forceinline__ i64 wrap_add(i64 a, i64 b) { return (i64)((u64)a + (u64)b); }
 
 // bijective mixer (splitmix64 finaliser): caller hashes may be poorly mixed
 __host__ __device__ __forceinline__ u64 mix64(u64 x) {
@@ -180,10 +185,11 @@ __device__ __forceinline__ Decision decide(i64 s_tat, i64 s_exp, const Req &r) {
 
 struct Outputs { i64 remaining, reset_after, retry_after; };
 
-// rate_limiter.rs:208-238
-__device__ __forceinline__ Outputs outputs_of(const Decision &d, const Req &r) {
+// rate_limiter.rs:208-238: the three outputs of a decision from `cur` (:208: new_tat if allowed, else the tat the
+// request started from), the verdict, allow_at (:174, read only when denied) and the request.  The ONE definition:
+// the kernels call it through outputs_of, the host through outputs_from_cur (gcra_expand_results16).
+__host__ __device__ __forceinline__ Outputs outputs_from(i64 cur, bool allowed, i64 allow_at, const Req &r) {
     Outputs o;
-    i64 cur = d.allowed ? d.new_tat : d.tat;
     // ordinary magnitudes (see ordinary_request; cur is then within +-2^62): nothing below saturates
 #ifdef GCRA_NO_FASTPATH
     const bool plain = false;
@@ -191,11 +197,12 @@ __device__ __forceinline__ Outputs outputs_of(const Decision &d, const Req &r) {
     const bool plain = ((((u64)r.now >> 61) | ((u64)r.dvt >> 60)) == 0) && cur > -(1LL << 62) && cur < (1LL << 62);
 #endif
     i64 room = plain ? (r.now + r.dvt) - cur : sat_sub(wrap_add(r.now, r.dvt), cur);
-    // remaining = max(room / ei, 0) for ei > 0 (truncating).  room <= 0 gives 0.  Both operands below 2^53
-    // (always, away from saturation corners): one IEEE double division, exact after a +-1 correction;
-    // otherwise the 64-bit integer division.
+    // remaining = max(room / ei, 0) for ei > 0 (truncating).  room <= 0 gives 0.  Device: both operands below 2^53
+    // (always, away from saturation corners): one IEEE double division, exact after a +-1 correction; otherwise the
+    // 64-bit integer division.  Host: the integer division (the same exact quotient).
     i64 rem = 0;
     if (r.ei > 0 && room > 0) {
+#ifdef __CUDA_ARCH__
         if ((u64)(room | r.ei) < (1ULL << 53)) {
             i64 q = (i64)__ddiv_rn(__ll2double_rn(room), __ll2double_rn(r.ei));
             i64 rr = room - q * r.ei;
@@ -204,18 +211,32 @@ __device__ __forceinline__ Outputs outputs_of(const Decision &d, const Req &r) {
         } else {
             rem = room / r.ei;
         }
+#else
+        rem = room / r.ei;
+#endif
     }
     o.remaining = rem;
     i64 reset = plain ? (cur - r.now) + r.dvt : sat_add(sat_sub(cur, r.now), r.dvt);
     o.reset_after = reset < 0 ? 0 : reset;
     i64 retry = 0;
-    if (!d.allowed) {
+    if (!allowed) {
         // allow_at = new_tat - dvt stays within +-2^63 on the plain path (|new_tat| < 2^62 + 2^60)
-        retry = (plain && d.allow_at > -(1LL << 62) && d.allow_at < (1LL << 62)) ? d.allow_at - r.now : sat_sub(d.allow_at, r.now);
+        retry = (plain && allow_at > -(1LL << 62) && allow_at < (1LL << 62)) ? allow_at - r.now : sat_sub(allow_at, r.now);
         if (retry < 0) retry = 0;
     }
     o.retry_after = retry;
     return o;
+}
+
+// The same from `cur` alone.  A denied request left the state alone, so cur is the tat it started from and
+// allow_at = (cur + ei * q) - dvt (rate_limiter.rs:170-174), saturating as decide() computes it.
+__host__ __device__ __forceinline__ Outputs outputs_from_cur(i64 cur, bool allowed, const Req &r) {
+    const i64 allow_at = allowed ? 0 : sat_sub(sat_add(cur, sat_mul(r.ei, r.q)), r.dvt);
+    return outputs_from(cur, allowed, allow_at, r);
+}
+
+__device__ __forceinline__ Outputs outputs_of(const Decision &d, const Req &r) {
+    return outputs_from(d.allowed ? d.new_tat : d.tat, d.allowed, d.allow_at, r);
 }
 
 // ------------------------------------------------------------------ key -> slot

@@ -146,10 +146,11 @@ __device__ __forceinline__ void issue_tile(unsigned char *stage, u64 *bar, const
     bulk_g2s(stage, tr.req, tr.cnt * rsz, bar);
 }
 
-template <bool COMPACT>
+template <int FMT>
 __global__ void __launch_bounds__(TILE_THREADS)
 probe_kernel(Table t, BatchView b, const PolicyDerived *__restrict__ pol, u32 npol, i64 now_batch,
              u32 *__restrict__ slot_arr, u32 *__restrict__ counters, u32 bm_mask, int prefetch_state) {
+    constexpr bool COMPACT = FMT != FMT_48_32;
     constexpr u32 RSZ = COMPACT ? sizeof(gcra_request16) : sizeof(gcra_request);
     __shared__ __align__(128) unsigned char stage[2][TILE_THREADS * RSZ];
     __shared__ __align__(8) u64 bar[2];
@@ -200,7 +201,11 @@ probe_kernel(Table t, BatchView b, const PolicyDerived *__restrict__ pol, u32 np
                 if (slot == t.null_slot) status = GCRA_INTERNAL;   // table full
             }
             slot_arr[row] = slot;
-            if (status != 0) { write_result(b.res_at(row), 0, 0, 0, status, 0); n_err++; }
+            if (status != 0) {
+                if (FMT == FMT_16_16) write_result16(b.res16_at(row), 0, status, 0);
+                else write_result(b.res_at(row), 0, 0, 0, status, 0);
+                n_err++;
+            }
             else {
                 // the state pair is what pass B touches next: optionally pull its sector into L2 now
                 if (prefetch_state) asm volatile("prefetch.global.L2 [%0];" ::"l"(&t.state[slot]));
@@ -276,18 +281,20 @@ __device__ __forceinline__ u64 mark_value(u32 epoch, u32 row) { return ((u64)(~e
 #endif
 // Persistent CTAs, software-pipelined: while tile t is decided, tile t+1's requests sit in the second stage buffer,
 // its rows' state pairs, counters and pend bits are in flight into registers, and tile t+2's slots are being read.
-template <bool COMPACT>
+template <int FMT>
 __global__ void __launch_bounds__(TILE_THREADS, GCRA_B_MINBLOCKS)
 decide_index_kernel(Table t, BatchView b, const PolicyDerived *__restrict__ pol, u32 npol, i64 now_batch,
                     const u32 *__restrict__ slot_arr, const u32 *__restrict__ counters, const u32 *__restrict__ pend,
                     u32 bm_mask, unsigned char *__restrict__ flags, u32 epoch, u32 honour_pend, u32 dbg) {
+    constexpr bool COMPACT = FMT != FMT_48_32, R16 = FMT == FMT_16_16;
     constexpr u32 RSZ = COMPACT ? sizeof(gcra_request16) : sizeof(gcra_request);
+    constexpr u32 PIECES = R16 ? 1 : 2;          // 16-byte pieces per result row
     __shared__ __align__(128) unsigned char stage[2][TILE_THREADS * RSZ];
     __shared__ __align__(8) u64 bar[2];
-    // results leave through shared memory: a tile's 256 results are written out as 512 consecutive 16-byte pieces
-    // (a warp store covers 512 contiguous bytes).  A segment's result array may be a peer GPU's outbox: a lane
-    // storing the two halves of its own row would put 16-byte packets on NVLink.
-    __shared__ __align__(16) longlong2 rstage[2][TILE_THREADS * 2];
+    // results leave through shared memory: a tile's 256 results are written out as 256 x PIECES consecutive 16-byte
+    // pieces (a warp store covers 512 contiguous bytes: 16 rows of 32 bytes, 32 rows of 16).  A segment's result array
+    // may be a peer GPU's outbox: a lane storing the two halves of its own row would put 16-byte packets on NVLink.
+    __shared__ __align__(16) longlong2 rstage[2][TILE_THREADS * PIECES];
     __shared__ unsigned char rwrite[2][TILE_THREADS];
     if (threadIdx.x == 0) {
         mbar_init(&bar[0], 1);
@@ -348,10 +355,14 @@ decide_index_kernel(Table t, BatchView b, const PolicyDerived *__restrict__ pol,
             Decision d;
             Outputs o;
             if (dbg & 8) { d.allowed = (r.q & 1) != 0; d.live = true; d.new_tat = r.now; d.new_exp = r.now + r.dvt; d.tat = s.tat; d.allow_at = 0; o.remaining = r.q; o.reset_after = r.ei; o.retry_after = 0; }
-            else { d = decide(s.tat, s.exp, r); o = outputs_of(d, r); }
+            else { d = decide(s.tat, s.exp, r); if (!R16) o = outputs_of(d, r); }
             if (!(dbg & 2)) {
-                rstage[buf][threadIdx.x * 2] = make_longlong2(o.remaining, o.reset_after);
-                rstage[buf][threadIdx.x * 2 + 1] = make_longlong2(o.retry_after, (i64)(u32)0 | ((i64)(d.allowed ? 1 : 0) << 32));
+                if (R16) {
+                    rstage[buf][threadIdx.x] = make_longlong2(d.allowed ? d.new_tat : d.tat, (i64)(u32)0 | ((i64)(d.allowed ? 1 : 0) << 32));
+                } else {
+                    rstage[buf][threadIdx.x * 2] = make_longlong2(o.remaining, o.reset_after);
+                    rstage[buf][threadIdx.x * 2 + 1] = make_longlong2(o.retry_after, (i64)(u32)0 | ((i64)(d.allowed ? 1 : 0) << 32));
+                }
                 rwrite[buf][threadIdx.x] = 1;
             }
             const bool mut = d.allowed && ((d.new_tat != s.tat) | (d.new_exp != s.exp));
@@ -384,11 +395,11 @@ decide_index_kernel(Table t, BatchView b, const PolicyDerived *__restrict__ pol,
         {
             // rows that failed validation (pass A wrote their error) or were deferred (the tail will write them) keep
             // their place: only staged rows are stored
-            longlong2 *dst = reinterpret_cast<longlong2 *>(b.res_at(cur.row0));
+            longlong2 *dst = R16 ? reinterpret_cast<longlong2 *>(b.res16_at(cur.row0)) : reinterpret_cast<longlong2 *>(b.res_at(cur.row0));
 #pragma unroll
-            for (int k = 0; k < 2; k++) {
+            for (int k = 0; k < (int)PIECES; k++) {
                 const u32 c = threadIdx.x + k * TILE_THREADS;
-                if (rwrite[buf][c >> 1]) dst[c] = rstage[buf][c];
+                if (rwrite[buf][c / PIECES]) dst[c] = rstage[buf][c];
             }
         }
         if (!has_nxt) break;
@@ -447,13 +458,14 @@ __device__ __forceinline__ u32 lookback(volatile u64 *__restrict__ status, u32 t
     return base;
 }
 
-template <bool COMPACT>
+template <int FMT>
 __global__ void __launch_bounds__(TILE_THREADS)
 resolve_kernel(Table t, BatchView b, const PolicyDerived *__restrict__ pol, u32 npol, i64 now_batch,
                const u32 *__restrict__ slot_arr, u32 bm_mask,
                const unsigned char *__restrict__ flags, u32 epoch, u32 *__restrict__ ctrl,
                volatile u64 *__restrict__ tile_status, u64 *__restrict__ res_keys,
                u32 *__restrict__ next_pend, volatile u32 *__restrict__ host_nres, u32 res_cap) {
+    constexpr bool COMPACT = FMT != FMT_48_32;
     constexpr u32 RSZ = COMPACT ? sizeof(gcra_request16) : sizeof(gcra_request);
     __shared__ u32 part[TILE_THREADS / 32];
     __shared__ u32 sm_tile, sm_base;
@@ -548,7 +560,8 @@ resolve_kernel(Table t, BatchView b, const PolicyDerived *__restrict__ pol, u32 
             if (p >= res_cap) {
                 // more residue than the engine's batch capacity (a multi-GPU tick far beyond max_batch): the row
                 // is answered with an internal error instead of overrunning the sort buffers
-                write_result(b.res_at(row), 0, 0, 0, GCRA_INTERNAL, 0);
+                if (FMT == FMT_16_16) write_result16(b.res16_at(row), 0, GCRA_INTERNAL, 0);
+                else write_result(b.res_at(row), 0, 0, 0, GCRA_INTERNAL, 0);
                 atomicAdd(&t.counters[C_ERRORS], 1ULL);
                 continue;
             }

@@ -71,6 +71,23 @@ __device__ __forceinline__ void write_result(gcra_result *out, i64 remaining, i6
     reinterpret_cast<longlong2 *>(out)[1] = b;
 }
 
+// 16-byte result of a compact request: `cur` (rate_limiter.rs:208) instead of the three outputs derived from it;
+// the host expands it (gcra_expand_results16 -> outputs_from_cur)
+__device__ __forceinline__ void write_result16(gcra_result16 *out, i64 cur, int status, int allowed) {
+    *reinterpret_cast<longlong2 *>(out) = make_longlong2(cur, (i64)(u32)status | ((i64)(allowed & 0xff) << 32));
+}
+
+// Row format of a batch, request bytes / result bytes.  16-byte results exist for compact requests only (the host
+// re-derives the outputs from the policy table), and only for single-segment batches.
+enum RowFmt { FMT_48_32 = 0, FMT_16_32 = 1, FMT_16_16 = 2 };
+
+// an error row (validation failed, table full, refused residue) in the batch's result format
+template <int FMT>
+__device__ __forceinline__ void write_error(gcra_result *out, u32 i, int status) {
+    if (FMT == FMT_16_16) write_result16(reinterpret_cast<gcra_result16 *>(out) + i, 0, status, 0);
+    else write_result(out + i, 0, 0, 0, status, 0);
+}
+
 // validation (rate_limiter.rs:111-117) + parameter derivation of ONE request record (shared or global memory):
 // returns the status the reference would return before touching the store, fills the key hash and the
 // derived request.
@@ -116,10 +133,11 @@ __device__ __forceinline__ int parse_request(const unsigned char *rec, const Pol
 // validation, parameter derivation, key probe/claim for ONE request whose record sits at `rec` (shared or
 // global memory).  Writes the derived request, the error result if any, and returns the sort key
 // (slot << 32 | i).  Must be called by all 32 lanes of a warp (warp-aggregated counters).
-template <bool COMPACT>
+template <int FMT>
 __device__ __forceinline__ u64 ingest_one(const Table &t, const unsigned char *rec, bool in_range,
                                           const PolicyDerived *__restrict__ pol, u32 npol, i64 now_batch, u32 i,
                                           Req *__restrict__ drec, gcra_result *__restrict__ out) {
+    constexpr bool COMPACT = FMT != FMT_48_32;
     int status = 0;
     u64 key_hash = 0;
     Req r = {0, 0, 0, 0};
@@ -133,7 +151,7 @@ __device__ __forceinline__ u64 ingest_one(const Table &t, const unsigned char *r
     if (in_range) {
         reinterpret_cast<longlong2 *>(drec + i)[0] = make_longlong2(r.now, r.ei);
         reinterpret_cast<longlong2 *>(drec + i)[1] = make_longlong2(r.dvt, r.q);
-        if (status != 0) write_result(out + i, 0, 0, 0, status, 0);
+        if (status != 0) write_error<FMT>(out, i, status);
     }
     // warp-aggregated counters
     u32 mf = __ballot_sync(0xffffffffu, fresh);
@@ -145,12 +163,12 @@ __device__ __forceinline__ u64 ingest_one(const Table &t, const unsigned char *r
     return ((u64)slot << 32) | i;
 }
 
-template <bool COMPACT>
+template <int FMT>
 __global__ void __launch_bounds__(TILE_THREADS)
 ingest_kernel(Table t, const void *__restrict__ req_base, const PolicyDerived *__restrict__ pol,
               u32 npol, i64 now_batch, u32 n, Req *__restrict__ drec, u64 *__restrict__ sortkeys,
               gcra_result *__restrict__ out) {
-    constexpr u32 RSZ = COMPACT ? sizeof(gcra_request16) : sizeof(gcra_request);
+    constexpr u32 RSZ = FMT != FMT_48_32 ? sizeof(gcra_request16) : sizeof(gcra_request);
     __shared__ __align__(128) unsigned char stage[TILE_THREADS * RSZ];
     __shared__ __align__(8) u64 bar;
 
@@ -169,7 +187,7 @@ ingest_kernel(Table t, const void *__restrict__ req_base, const PolicyDerived *_
 
     const u32 i = base + threadIdx.x;
     const bool in_range = threadIdx.x < cnt;
-    const u64 key = ingest_one<COMPACT>(t, stage + (size_t)threadIdx.x * RSZ, in_range, pol, npol, now_batch, i, drec, out);
+    const u64 key = ingest_one<FMT>(t, stage + (size_t)threadIdx.x * RSZ, in_range, pol, npol, now_batch, i, drec, out);
     if (in_range) sortkeys[i] = key;
 }
 
@@ -388,6 +406,8 @@ struct BatchView {
         if (nseg == 1) return res0 + i;
         return (gcra_result *)__ldg((const u64 *)&segs[i >> cap_shift].res) + (i & ((1u << cap_shift) - 1));
     }
+    // FMT_16_16 batches (always one segment): res0 holds gcra_result16 rows
+    __device__ __forceinline__ gcra_result16 *res16_at(u32 i) const { return reinterpret_cast<gcra_result16 *>(res0) + i; }
     __device__ __forceinline__ const unsigned char *req_at(u32 i, u32 rsz) const {
         if (nseg == 1) return req0 + (size_t)i * rsz;
         return (const unsigned char *)__ldg((const u64 *)&segs[i >> cap_shift].req) + (size_t)(i & ((1u << cap_shift) - 1)) * rsz;
@@ -407,6 +427,21 @@ struct OutMap {
     i64 now_batch;
     template <bool BY_ROW>
     __device__ __forceinline__ gcra_result *at(u32 i) const { return BY_ROW ? view.res_at(i) : out + i; }
+    template <bool BY_ROW>
+    __device__ __forceinline__ gcra_result16 *at16(u32 i) const {
+        return BY_ROW ? view.res16_at(i) : reinterpret_cast<gcra_result16 *>(out) + i;
+    }
+
+    // the result row of a finished decision: R16 (FMT_16_16 batches) stores `cur` alone, else the 32-byte result
+    template <bool BY_ROW, bool R16>
+    __device__ __forceinline__ void write(u32 i, const Decision &d, const Req &r) const {
+        if (R16) {
+            write_result16(at16<BY_ROW>(i), d.allowed ? d.new_tat : d.tat, 0, d.allowed ? 1 : 0);
+        } else {
+            const Outputs o = outputs_of(d, r);
+            write_result(at<BY_ROW>(i), o.remaining, o.reset_after, o.retry_after, 0, d.allowed ? 1 : 0);
+        }
+    }
 };
 
 // ---------------------------------------------------------------------------------------------
@@ -529,8 +564,8 @@ __device__ __forceinline__ void store_state(const Table &t, u32 slot, const RunS
 constexpr int DECIDE_THREADS = GCRA_DECIDE_THREADS;   // warps are independent: the CTA size only sets scheduling granularity
 
 // one warp, one chunk of 32 sorted positions (see the comment above run_chunk); BY_ROW: the sorted payload is a row
-// id of the batch (residue of the index-order pipeline), else a batch index into drec / out
-template <bool BY_ROW>
+// id of the batch (residue of the index-order pipeline), else a batch index into drec / out; R16: 16-byte results
+template <bool BY_ROW, bool R16>
 __device__ __forceinline__ void decide_chunk(const Table &t, const u64 *sorted, const Req *__restrict__ drec, u32 n,
                                              const OutMap &out, LongRun *__restrict__ long_runs,
                                              LongRun *__restrict__ giant_runs, u32 *__restrict__ long_count,
@@ -609,8 +644,7 @@ __device__ __forceinline__ void decide_chunk(const Table &t, const u64 *sorted, 
 
     u32 n_allowed = 0, n_denied = 0;
     if (mine) {
-        Outputs o = outputs_of(fin, r);
-        write_result(out.template at<BY_ROW>(idx), o.remaining, o.reset_after, o.retry_after, 0, fin.allowed ? 1 : 0);
+        out.template write<BY_ROW, R16>(idx, fin, r);
         n_allowed += fin.allowed ? 1 : 0;
         n_denied += fin.allowed ? 0 : 1;
     }
@@ -661,8 +695,7 @@ __device__ __forceinline__ void decide_chunk(const Table &t, const u64 *sorted, 
             bool ch2 = false;
             run_chunk(lane, in_run, rm, r2, s2, f2, ch2, exp_hits);
             if (in_run) {
-                Outputs o = outputs_of(f2, r2);
-                write_result(out.template at<BY_ROW>((u32)e2), o.remaining, o.reset_after, o.retry_after, 0, f2.allowed ? 1 : 0);
+                out.template write<BY_ROW, R16>((u32)e2, f2, r2);
                 n_allowed += f2.allowed ? 1 : 0;
                 n_denied += f2.allowed ? 0 : 1;
             }
@@ -699,7 +732,7 @@ __device__ __forceinline__ void decide_chunk(const Table &t, const u64 *sorted, 
 #ifndef GCRA_DECIDE_MINBLOCKS
 #define GCRA_DECIDE_MINBLOCKS (512 / GCRA_DECIDE_THREADS)
 #endif
-template <bool BY_ROW>
+template <bool BY_ROW, bool R16>
 __global__ void __launch_bounds__(DECIDE_THREADS, GCRA_DECIDE_MINBLOCKS)
 decide_kernel(Table t, const u64 *__restrict__ sorted, const Req *__restrict__ drec, u32 n_host,
               const u32 *__restrict__ n_dev, OutMap out, LongRun *__restrict__ long_runs,
@@ -707,7 +740,7 @@ decide_kernel(Table t, const u64 *__restrict__ sorted, const Req *__restrict__ d
     const u32 n = sort_count(n_host, n_dev);
     const u32 warps_total = gridDim.x * (DECIDE_THREADS / 32);
     for (u32 wg = (blockIdx.x * DECIDE_THREADS + threadIdx.x) >> 5; wg * 32 < n; wg += warps_total)
-        decide_chunk<BY_ROW>(t, sorted, drec, n, out, long_runs, giant_runs, long_count, wg, threadIdx.x & 31, mode);
+        decide_chunk<BY_ROW, R16>(t, sorted, drec, n, out, long_runs, giant_runs, long_count, wg, threadIdx.x & 31, mode);
 }
 
 // Small batches (n < LONG_RUN_MIN, e.g. one RateLimiter::rate_limit call or a lightly loaded actor): ONE CTA
@@ -716,15 +749,15 @@ decide_kernel(Table t, const u64 *__restrict__ sorted, const Req *__restrict__ d
 constexpr u32 SMALL_MAX = 255;
 static_assert(SMALL_MAX < GCRA_LONG_MIN && SMALL_MAX < TILE_THREADS, "small path must not create long runs");
 
-template <bool COMPACT>
+template <int FMT>
 __global__ void __launch_bounds__(TILE_THREADS)
 small_batch_kernel(Table t, const void *__restrict__ req_base, const PolicyDerived *__restrict__ pol, u32 npol,
                    i64 now_batch, u32 n, Req *__restrict__ drec, gcra_result *__restrict__ out) {
-    constexpr u32 RSZ = COMPACT ? sizeof(gcra_request16) : sizeof(gcra_request);
+    constexpr u32 RSZ = FMT != FMT_48_32 ? sizeof(gcra_request16) : sizeof(gcra_request);
     __shared__ u64 keys[TILE_THREADS];
     const u32 tid = threadIdx.x;
     const bool in_range = tid < n;
-    const u64 key = ingest_one<COMPACT>(t, (const unsigned char *)req_base + (size_t)(in_range ? tid : 0) * RSZ, in_range,
+    const u64 key = ingest_one<FMT>(t, (const unsigned char *)req_base + (size_t)(in_range ? tid : 0) * RSZ, in_range,
                                         pol, npol, now_batch, tid, drec, out);
     keys[tid] = in_range ? key : ~0ULL;
     __syncthreads();
@@ -744,7 +777,7 @@ small_batch_kernel(Table t, const void *__restrict__ req_base, const PolicyDeriv
     OutMap om;
     om.out = out;
     om.by_row = 0;
-    decide_chunk<false>(t, keys, drec, n, om, nullptr, nullptr, nullptr, tid >> 5, tid & 31);
+    decide_chunk<false, FMT == FMT_16_16>(t, keys, drec, n, om, nullptr, nullptr, nullptr, tid >> 5, tid & 31);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -801,7 +834,7 @@ struct Cands {
 
 struct PubState { i64 tat, exp; };
 
-template <int CTAS, bool BY_ROW>
+template <int CTAS, bool BY_ROW, bool R16>
 __global__ void __launch_bounds__(LONG_THREADS, 1)
 decide_runs_kernel(Table t, const u64 *__restrict__ sorted, const Req *__restrict__ drec,
                    OutMap out, const LongRun *__restrict__ runs,
@@ -937,8 +970,7 @@ decide_runs_kernel(Table t, const u64 *__restrict__ sorted, const Req *__restric
                     i64 ct, ce;
                     cd.get(in_idx, ct, ce);
                     const Decision d = decide(ct, ce, r);
-                    const Outputs o = outputs_of(d, r);
-                    write_result(out.template at<BY_ROW>(idx), o.remaining, o.reset_after, o.retry_after, 0, d.allowed ? 1 : 0);
+                    out.template write<BY_ROW, R16>(idx, d, r);
                     n_allowed += d.allowed ? 1 : 0;
                     n_denied += d.allowed ? 0 : 1;
                     if (d.allowed && !d.live && ce >= 0) exp_hits++;
@@ -1340,17 +1372,19 @@ struct DeniedTable {
 };
 constexpr u32 DENIED_HASH = 512;
 
-template <bool COMPACT>
+template <int FMT>
 __global__ void __launch_bounds__(TILE_THREADS)
 denied_count_kernel(const unsigned char *__restrict__ req, const gcra_result *__restrict__ res, u32 n, DeniedTable t) {
-    constexpr u32 RSZ = COMPACT ? sizeof(gcra_request16) : sizeof(gcra_request);
+    constexpr u32 RSZ = FMT != FMT_48_32 ? sizeof(gcra_request16) : sizeof(gcra_request);
     __shared__ u64 hkey[DENIED_HASH];
     __shared__ u32 hcnt[DENIED_HASH];
     for (u32 i = threadIdx.x; i < DENIED_HASH; i += TILE_THREADS) { hkey[i] = 0; hcnt[i] = 0; }
     __syncthreads();
     const u32 i = blockIdx.x * TILE_THREADS + threadIdx.x;
     if (i < n) {
-        const longlong2 tail = reinterpret_cast<const longlong2 *>(res + i)[1];      // retry_after, status | allowed << 32
+        // (retry_after | cur_tat_ns), status | allowed << 32: the second half of a 32-byte row, a whole 16-byte row
+        const longlong2 tail = FMT == FMT_16_16 ? reinterpret_cast<const longlong2 *>(res)[i]
+                                                : reinterpret_cast<const longlong2 *>(res + i)[1];
         const bool denied = (u32)tail.y == GCRA_OK && ((tail.y >> 32) & 0xff) == 0;
         if (denied) {
             u64 k = *reinterpret_cast<const u64 *>(req + (size_t)i * RSZ);
