@@ -236,7 +236,9 @@ int32_t gcra_get_stats(gcra_engine *h, gcra_stats *out);
  * max_keys > 0) a pass over every finished single-GPU batch counts its denied requests per key hash in a device
  * table; gcra_top_denied returns the k most denied (hash, count) pairs, most denied first, and prunes the table to
  * its max_keys top entries once more than 3 x max_keys keys have accumulated (the reference's cleanup rule).  Keys
- * are hashes here -- the caller of the batch entry points owns the strings.  max_keys = 0 switches tracking off. */
+ * are hashes here -- the caller of the batch entry points owns the strings.  max_keys = 0 switches tracking off.
+ * max_keys is at most 2^27 (the table holds 16 entries per key, at most 2^31); a larger value, or a failed
+ * allocation, returns GCRA_INTERNAL and leaves the previous setting and its counts as they were. */
 int32_t gcra_track_denied(gcra_engine *h, uint32_t max_keys);
 int32_t gcra_top_denied(gcra_engine *h, uint32_t k, uint64_t *key_hashes, uint64_t *counts, uint32_t *n_out,
                         uint64_t *dropped);

@@ -13,6 +13,7 @@
 #include <dlfcn.h>
 #include <cstring>
 #include <fcntl.h>
+#include <memory>
 #include <string>
 #include <sys/stat.h>
 #include <unistd.h>
@@ -21,14 +22,17 @@
 #include "gcra_kernels.cuh"
 #include "gcra_index_path.cuh"
 #include "gcra_p2p.cuh"
+#include "gcra_owned.cuh"
 
 using namespace gcra;
 
+// (reported through h->err; cudaGetLastError clears the runtime's record, so that no later launch check reports it)
 #define CK(call)                                                                         \
     do {                                                                                 \
         cudaError_t e_ = (call);                                                         \
         if (e_ != cudaSuccess) {                                                         \
             h->err = std::string(#call) + ": " + cudaGetErrorString(e_);                 \
+            cudaGetLastError();                                                          \
             return GCRA_INTERNAL;                                                        \
         }                                                                                \
     } while (0)
@@ -43,11 +47,10 @@ namespace {
 const __int128 NS_PER_S = 1000000000;
 
 struct RingSlot {
-    void *h_req = nullptr;
-    void *h_res = nullptr;           // gcra_result, or gcra_result16 rows in ring mode 2
-    void *d_req = nullptr;
-    void *d_res = nullptr;
-    cudaEvent_t ev_in = nullptr, ev_comp = nullptr, ev_done = nullptr;
+    PinnedBuf<unsigned char> h_req;
+    PinnedBuf<unsigned char> h_res;  // gcra_result, or gcra_result16 rows in ring mode 2
+    DevBuf<unsigned char> d_req, d_res;
+    Event ev_in, ev_done;
     bool in_flight = false;
 };
 }  // namespace
@@ -98,14 +101,21 @@ static bool load() {
 const int kUint8 = 1, kUint32 = 3;
 }  // namespace nccl_rt
 
+inline void release_comm(nccl_rt::Comm c) { nccl_rt::g_api.CommDestroy(c); }
+
+struct NcclComm : Owned<nccl_rt::Comm, release_comm> {   // (make returns an NCCL result code)
+    int make(int world, nccl_rt::UniqueId id, int rank) { reset(); return took(nccl_rt::g_api.CommInitRank(&h_, world, id, rank)); }
+    nccl_rt::Comm get() const { return h_; }
+};
+
 // one tick in flight through the sharded pipeline
 struct ShardSlot {
-    gcra_request *routed = nullptr, *recv_req = nullptr;
-    gcra_result *recv_res = nullptr, *back_res = nullptr;
-    u32 *src_index = nullptr;
-    u32 *counts_dev = nullptr;     // [2*W]: rows I send to every peer, rows every peer sends me
-    u32 *counts_host = nullptr;    // pinned copy
-    cudaEvent_t ev_ready = nullptr, ev_counts = nullptr, ev_routed = nullptr, ev_done = nullptr;
+    DevBuf<gcra_request> routed, recv_req;
+    DevBuf<gcra_result> recv_res, back_res;
+    DevBuf<u32> src_index;
+    DevBuf<u32> counts_dev;        // [2*W]: rows I send to every peer, rows every peer sends me
+    PinnedBuf<u32> counts_host;    // pinned copy
+    Event ev_ready, ev_counts, ev_routed, ev_done;
     bool used = false;
     uint32_t n = 0, n_recv = 0;
     gcra_result *d_res_user = nullptr;
@@ -116,20 +126,20 @@ struct Shard {
     static const int DEPTH = 4;
     int rank = 0, world = 0;
     uint32_t max_rows = 0;
-    nccl_rt::Comm comm_counts = nullptr, comm_req = nullptr, comm_res = nullptr;
-    cudaStream_t s_part = nullptr, s_route = nullptr, s_return = nullptr;   // partition+counts | request all-to-all | way back
+    Stream s_part, s_route, s_return;   // partition+counts | request all-to-all | way back
+    NcclComm comm_counts, comm_req, comm_res;
     ShardSlot slots[DEPTH];
     uint32_t next = 0;
     int pending = -1;              // slot whose decide + return stages have not been issued yet
-    cudaEvent_t ev_tmp = nullptr;
+    Event ev_tmp;
 };
 
 // ---- multi-GPU over NVLink peer memory (gcra_p2p.cuh) ------------------------------------------------------
 struct P2PSlot {
-    u32 *res_loc = nullptr;            // [cap] where the result of my row i arrives in my outbox
-    u32 *counts_dev = nullptr;         // [world] rows I routed to every owner in this tick
-    SegDesc *segs_dev = nullptr;       // [world] segment r of this inbox slot: sender r's rows, sender r's outbox
-    cudaEvent_t ev_ready = nullptr, ev_wait = nullptr, ev_done = nullptr;
+    DevBuf<u32> res_loc;               // [cap] where the result of my row i arrives in my outbox
+    DevBuf<u32> counts_dev;            // [world] rows I routed to every owner in this tick
+    DevBuf<SegDesc> segs_dev;          // [world] segment r of this inbox slot: sender r's rows, sender r's outbox
+    Event ev_ready, ev_wait, ev_done;
     bool used = false;
     uint32_t n = 0;
 };
@@ -137,46 +147,52 @@ struct P2PSlot {
 struct P2P {
     int rank = 0, world = 0;
     uint32_t cap = 0, cap_shift = 0;
-    void *window = nullptr;
+    DevBuf<unsigned char> window;
     size_t window_bytes = 0, inbox_off = 0, outbox_off = 0;
-    void *peer_base[P2P_MAX_WORLD] = {};
-    bool opened[P2P_MAX_WORLD] = {};
+    IpcMapping peer_map[P2P_MAX_WORLD];    // the windows of other processes' ranks (gcra_p2p_connect with IPC handles)
     bool connected = false, routed_pending = false;
-    P2PPeers *peers_dev = nullptr;
-    u32 *tile_counts = nullptr;
-    cudaStream_t s_part = nullptr, s_wait = nullptr, s_sig = nullptr, s_return = nullptr;
+    DevBuf<P2PPeers> peers_dev;
+    DevBuf<u32> tile_counts;
+    Stream s_part, s_wait, s_sig, s_return;
     P2PSlot slots[P2P_DEPTH];
     uint64_t next_tick = 0;
     bool timed = false, timed_valid = false;
-    cudaEvent_t ev_t[6] = {};
+    Event ev_t[6];
 };
 
 // per-batch scratch; several sets so that the front halves of the next batches can overlap the back half of
 // the current one
 struct Scratch {
-    Req *drec = nullptr;
-    u64 *keys_a = nullptr, *keys_b = nullptr;
-    u32 *hist = nullptr, *tot = nullptr;
-    LongRun *long_runs = nullptr, *giant_runs = nullptr;
-    u32 *long_count = nullptr;
-    cudaEvent_t ev_front = nullptr, ev_mid = nullptr, ev_back = nullptr, ev_fork = nullptr, ev_join = nullptr, ev_join2 = nullptr;
+    DevBuf<Req> drec;
+    DevBuf<u64> keys_a, keys_b;
+    DevBuf<u32> hist, tot;
+    DevBuf<LongRun> long_runs, giant_runs;
+    DevBuf<u32> long_count;
+    Event ev_front, ev_mid, ev_back, ev_fork, ev_join;
     bool back_recorded = false;
     // index-order pipeline (gcra_index_path.cuh)
-    u32 *slot_arr = nullptr;            // [rows] slot of every row (null slot: the row failed validation)
-    unsigned char *flags = nullptr;     // [rows] pass-B verdict of rows on shared slots
-    u32 *bitmap = nullptr;              // [bm_words] 32-bit occurrence counters of the batch, hashed by slot
-    u32 *pend = nullptr;                // [pend_words] 1 bit per entry: the PREVIOUS batch's tail owns a slot of the entry
-    u64 *ctrl_block = nullptr;          // word 0: {tile ticket, residue count}; word 1: {sort barrier, -}; then one status word per tile
+    DevBuf<u32> slot_arr;               // [rows] slot of every row (null slot: the row failed validation)
+    DevBuf<unsigned char> flags;        // [rows] pass-B verdict of rows on shared slots
+    DevBuf<u32> bitmap;                 // [bm_words] 32-bit occurrence counters of the batch, hashed by slot
+    DevBuf<u32> pend;                   // [pend_words] 1 bit per entry: the PREVIOUS batch's tail owns a slot of the entry
+    DevBuf<u64> ctrl_block;             // word 0: {tile ticket, residue count}; word 1: {sort barrier, -}; then one status word per tile
     uint32_t rows_alloc = 0;
-    u32 *h_nres = nullptr;              // pinned: residue size of the set's latest index-order batch (valid after ev_mid)
+    PinnedBuf<u32> h_nres;              // pinned: residue size of the set's latest index-order batch (valid after ev_mid)
     bool mid_recorded = false, nres_counted = true;
     uint32_t nres_rows = 0;             // rows of that batch
 };
 
+// the arrays of the table and of the denied-key table: gcra_engine::tab and ::denied are the views the kernels take
+struct TableArrays { DevBuf<u64> keys, mark; DevBuf<TatOff> state; DevBuf<i64> ei; };
+struct DeniedArrays { DevBuf<u64> keys, counts, dropped; };
+
+// Members are released in reverse declaration order, after gcra_destroy has synchronized the device: no release waits.
 struct gcra_engine {
     int device = 0;
     uint32_t sms = 0;                // streaming multiprocessors of the device: sizes the grids of the streaming kernels
-    cudaStream_t stream = nullptr, in_stream = nullptr, out_stream = nullptr, aux_stream = nullptr, aux2_stream = nullptr;
+    Stream stream, in_stream, out_stream, aux_stream, aux2_stream;
+    DevBuf<u64> counters;            // the table's counters: replaced by grow, kept by gcra_snapshot_load
+    TableArrays tab_arrays;
     Table tab{};
     uint32_t total_lines = 0;
     uint64_t capacity = 0;
@@ -191,29 +207,32 @@ struct gcra_engine {
     uint32_t scr_next = 0;
     // pipelined submission: three stages on three streams (front: probe | mid: decide + resolve | tail: the
     // sorted residue); the sort pipeline uses front (ingest + sort) and mid (decide)
-    cudaStream_t front_stream[N_SCR] = {}, back_stream = nullptr, tail_stream = nullptr;
+    // (ONE front stream shared by all scratch sets: front halves run one after another; since ingest only CASes
+    // the keys array they could overlap as well -- not measured yet)
+    Stream front_stream, back_stream, tail_stream;
     int pend_set = -1;               // scratch set whose bitmap holds the PEND bits of the batch submitted last (-1: none)
-    cudaEvent_t ev_ready = nullptr;
-    void *d_req = nullptr;
-    gcra_result *d_res = nullptr;
-    u32 *route_counts = nullptr;
-    PolicyDerived *d_pol = nullptr;
+    Event ev_ready;
+    DevBuf<gcra_request> d_req;      // (16-byte rows in the compact formats)
+    DevBuf<gcra_result> d_res;
+    DevBuf<u32> route_counts;
+    DevBuf<PolicyDerived> d_pol;
     uint32_t npol = 0;
-    StoreOpResult *d_op = nullptr, *h_op = nullptr;
-    u64 *h_counters = nullptr;       // pinned snapshot, refreshed after every batch
-    cudaEvent_t ev_counters = nullptr;
-    cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};
-    cudaEvent_t evd[8] = {};         // index-order pipeline, serial timed batch: after each kernel group
+    DevBuf<StoreOpResult> d_op;
+    PinnedBuf<StoreOpResult> h_op;
+    PinnedBuf<u64> h_counters;       // pinned snapshot, refreshed after every batch
+    Event ev_counters;
+    Event ev[4];
+    Event evd[8];                    // index-order pipeline, serial timed batch: after each kernel group
     bool evd_valid = false;
-    cudaEvent_t ev_sweep[2] = {nullptr, nullptr};
+    Event ev_sweep[2];
     bool sweep_timed = false;
     bool ev_valid = false;
     uint64_t launches = 0;
     uint64_t occupied_ub = 0;        // host-side upper bound of claimed slots
     // asynchronous occupancy snapshots: counters copied after every batch, read when their event is done
     static const int N_SNAP = 8;
-    u64 *h_snap = nullptr;           // pinned [N_SNAP][C_COUNT]
-    cudaEvent_t ev_snap[N_SNAP] = {};
+    PinnedBuf<u64> h_snap;           // pinned [N_SNAP][C_COUNT]
+    Event ev_snap[N_SNAP];
     uint64_t snap_rows_after[N_SNAP] = {};   // rows launched up to and including the snapshot's batch
     bool snap_used[N_SNAP] = {};
     uint32_t snap_next = 0;
@@ -227,8 +246,8 @@ struct gcra_engine {
     uint64_t ops_count = 0, cleanup_modulo = 0;
     uint64_t seen_allowed = 0, seen_expired_hits = 0;
     uint64_t n_sweeps = 0, n_grows = 0, n_purges = 0;
-    Shard *shard = nullptr;          // multi-GPU: native NCCL pipeline (gcra_shard_*)
-    P2P *p2p = nullptr;              // multi-GPU: NVLink peer-memory pipeline (gcra_p2p_*)
+    std::unique_ptr<Shard> shard;    // multi-GPU: native NCCL pipeline (gcra_shard_*)
+    std::unique_ptr<P2P> p2p;        // multi-GPU: NVLink peer-memory pipeline (gcra_p2p_*)
     // index-order pipeline
     uint32_t epoch = 0;              // batch epoch of the slot marks (never 0)
     uint32_t bm_mask = 0;            // bitmap entries - 1
@@ -249,13 +268,13 @@ struct gcra_engine {
     uint32_t ring_cap = 0;
     int ring_mode = 0;               // gcra_ring_create: 0, 1 or 2 = the slots' RowFmt
     // denied requests per key (gcra_track_denied): device table, updated by a pass over every finished batch
+    DeniedArrays denied_arrays;
     DeniedTable denied{};
-    uint32_t denied_max = 0, denied_cap = 0;
+    uint32_t denied_max = 0;
+    uint64_t denied_cap = 0;
     uint64_t hash_seed[2] = {0, 0};  // SipHash key of the string-keyed entry points ((0,0): the unkeyed gcra_hash_key)
     std::string err;
 };
-
-static int alloc_index_scratch(gcra_engine *h, Scratch &sc, uint32_t rows);
 
 static uint32_t ceil_log2(uint64_t x) {
     uint32_t b = 0;
@@ -272,22 +291,24 @@ static void table_geometry(uint64_t capacity, bool tight, uint32_t &total_lines,
     stash_slots = (ns - 1) * 4;   // the last line is reserved (null slot)
 }
 
-static int alloc_table(gcra_engine *h, uint64_t capacity, Table &t, uint32_t &total_lines, u64 *counters) {
+// a new table in `a`, `t` its view
+static int alloc_table(gcra_engine *h, uint64_t capacity, TableArrays &a, Table &t, uint32_t &total_lines, u64 *counters) {
     uint32_t nb, ss;
     table_geometry(capacity, h->tight, total_lines, nb, ss);
     const size_t slots = (size_t)total_lines * 4;
-    CK(cudaMalloc(&t.keys, slots * sizeof(u64)));
-    CK(cudaMalloc(&t.state, slots * sizeof(TatOff)));
-    CK(cudaMalloc(&t.ei, slots * sizeof(i64)));
-    CK(cudaMalloc(&t.mark, slots * sizeof(u64)));
-    CK(cudaMemsetAsync(t.mark, 0xff, slots * sizeof(u64), h->stream));   // no batch epoch matches
+    CK(a.keys.make(slots));
+    CK(a.state.make(slots));
+    CK(a.ei.make(slots));
+    CK(a.mark.make(slots));
+    t.keys = a.keys.get(); t.state = a.state.get(); t.ei = a.ei.get(); t.mark = a.mark.get();
+    CK(cudaMemsetAsync(t.mark, 0xff, slots * sizeof(u64), h->stream.get()));   // no batch epoch matches
     t.nb_main = nb;
     t.stash_slots = ss;
     t.null_slot = total_lines * 4 - 1;
     t.slot_bits = ceil_log2((uint64_t)total_lines * 4);
     t.counters = counters;
     uint32_t grid = (uint32_t)std::min<size_t>((slots + TILE_THREADS - 1) / TILE_THREADS, 16 * h->sms);
-    clear_slots_kernel<<<grid, TILE_THREADS, 0, h->stream>>>(t, 0, slots);
+    clear_slots_kernel<<<grid, TILE_THREADS, 0, h->stream.get()>>>(t, 0, slots);
     h->launches++;
     CK(cudaGetLastError());
     return GCRA_OK;
@@ -306,9 +327,9 @@ static uint64_t load_limit_for(uint64_t capacity, bool tight) {
 }
 
 static int refresh_counters(gcra_engine *h, bool wait) {
-    CK(cudaMemcpyAsync(h->h_counters, h->tab.counters, C_COUNT * sizeof(u64), cudaMemcpyDeviceToHost, h->stream));
-    CK(cudaEventRecord(h->ev_counters, h->stream));
-    if (wait) CK(cudaEventSynchronize(h->ev_counters));
+    CK(cudaMemcpyAsync(h->h_counters.get(), h->tab.counters, C_COUNT * sizeof(u64), cudaMemcpyDeviceToHost, h->stream.get()));
+    CK(cudaEventRecord(h->ev_counters.get(), h->stream.get()));
+    if (wait) CK(cudaEventSynchronize(h->ev_counters.get()));
     return GCRA_OK;
 }
 
@@ -316,20 +337,20 @@ static int do_sweep(gcra_engine *h, int64_t now_ns, uint64_t *removed) {
     CK(cudaSetDevice(h->device));
     CK(cudaDeviceSynchronize());   // the sweep is exclusive: batches may be in flight on caller streams
     RC(refresh_counters(h, true));
-    uint64_t before = h->h_counters[C_SWEPT];
+    uint64_t before = h->h_counters.get()[C_SWEPT];
     uint32_t grid = (uint32_t)std::min<uint64_t>(((uint64_t)h->total_lines * 2 + TILE_THREADS * SWEEP_UNROLL - 1) / (TILE_THREADS * SWEEP_UNROLL), 16 * h->sms);
-    CK(cudaEventRecord(h->ev_sweep[0], h->stream));
+    CK(cudaEventRecord(h->ev_sweep[0].get(), h->stream.get()));
     static const int sweep_mode = getenv("GCRA_SWEEP_MODE") ? atoi(getenv("GCRA_SWEEP_MODE")) : 0;
-    sweep_kernel<<<grid, TILE_THREADS, 0, h->stream>>>(h->tab, (u64)h->total_lines * 4, now_ns, sweep_mode);
-    CK(cudaEventRecord(h->ev_sweep[1], h->stream));
+    sweep_kernel<<<grid, TILE_THREADS, 0, h->stream.get()>>>(h->tab, (u64)h->total_lines * 4, now_ns, sweep_mode);
+    CK(cudaEventRecord(h->ev_sweep[1].get(), h->stream.get()));
     h->sweep_timed = true;
     h->launches++;
     CK(cudaGetLastError());
     RC(refresh_counters(h, true));
-    h->occupied_ub = h->h_counters[C_OCCUPIED];
+    h->occupied_ub = h->h_counters.get()[C_OCCUPIED];
     for (int i = 0; i < gcra_engine::N_SNAP; i++) h->snap_used[i] = false;
     h->n_sweeps++;
-    if (removed) *removed = h->h_counters[C_SWEPT] - before;
+    if (removed) *removed = h->h_counters.get()[C_SWEPT] - before;
     return GCRA_OK;
 }
 
@@ -338,19 +359,19 @@ static int purge(gcra_engine *h) {
     CK(cudaDeviceSynchronize());
     const uint64_t slots = (uint64_t)h->total_lines * 4;
     uint32_t grid = (uint32_t)std::min<uint64_t>((slots + TILE_THREADS - 1) / TILE_THREADS, 16 * h->sms);
-    purge_kernel<<<grid, TILE_THREADS, 0, h->stream>>>(h->tab, slots);
+    purge_kernel<<<grid, TILE_THREADS, 0, h->stream.get()>>>(h->tab, slots);
     h->launches++;
     CK(cudaGetLastError());
     RC(refresh_counters(h, true));
-    if (h->h_counters[C_STASH] == 0) {
+    if (h->h_counters.get()[C_STASH] == 0) {
         // no key lives in the stash any more: drop its tombstones
         uint64_t first = (uint64_t)h->tab.nb_main * 4, cnt = slots - first;
-        clear_slots_kernel<<<(uint32_t)((cnt + TILE_THREADS - 1) / TILE_THREADS), TILE_THREADS, 0, h->stream>>>(
+        clear_slots_kernel<<<(uint32_t)((cnt + TILE_THREADS - 1) / TILE_THREADS), TILE_THREADS, 0, h->stream.get()>>>(
             h->tab, first, cnt);
         h->launches++;
         CK(cudaGetLastError());
     }
-    h->occupied_ub = h->h_counters[C_OCCUPIED];
+    h->occupied_ub = h->h_counters.get()[C_OCCUPIED];
     for (int i = 0; i < gcra_engine::N_SNAP; i++) h->snap_used[i] = false;
     h->n_purges++;
     return GCRA_OK;
@@ -358,35 +379,36 @@ static int purge(gcra_engine *h) {
 
 // HashMap growth: rebuild into a table twice the size
 static int grow(gcra_engine *h, uint64_t need) {
-    CK(cudaStreamSynchronize(h->stream));
+    CK(cudaStreamSynchronize(h->stream.get()));
     uint64_t newcap = std::max<uint64_t>(h->capacity * 2, 256);
     while (load_limit_for(newcap, h->tight) < need) newcap *= 2;
+    TableArrays na;
     Table nt{};
     uint32_t nl = 0;
-    u64 *ncounters = nullptr;
-    CK(cudaMalloc(&ncounters, C_COUNT * sizeof(u64)));
-    CK(cudaMemsetAsync(ncounters, 0, C_COUNT * sizeof(u64), h->stream));
-    int rc = alloc_table(h, newcap, nt, nl, ncounters);
-    if (rc) return rc;
+    DevBuf<u64> nc;
+    CK(nc.make(C_COUNT));
+    u64 *ncounters = nc.get();
+    CK(cudaMemsetAsync(ncounters, 0, C_COUNT * sizeof(u64), h->stream.get()));
+    RC(alloc_table(h, newcap, na, nt, nl, ncounters));
     uint32_t grid = std::min<uint32_t>((h->total_lines + TILE_THREADS - 1) / TILE_THREADS, 8 * h->sms);
-    rehash_kernel<<<grid, TILE_THREADS, 0, h->stream>>>(h->tab, (u64)h->total_lines * 4, nt);
+    rehash_kernel<<<grid, TILE_THREADS, 0, h->stream.get()>>>(h->tab, (u64)h->total_lines * 4, nt);
     h->launches++;
     CK(cudaGetLastError());
     // carry the running totals over
     RC(refresh_counters(h, true));
     u64 keep[C_COUNT];
-    memcpy(keep, h->h_counters, sizeof(keep));
+    memcpy(keep, h->h_counters.get(), sizeof(keep));
     u64 fresh[C_COUNT];
-    CK(cudaMemcpyAsync(fresh, ncounters, sizeof(fresh), cudaMemcpyDeviceToHost, h->stream));
-    CK(cudaStreamSynchronize(h->stream));
+    CK(cudaMemcpyAsync(fresh, ncounters, sizeof(fresh), cudaMemcpyDeviceToHost, h->stream.get()));
+    CK(cudaStreamSynchronize(h->stream.get()));
     if (fresh[C_INSERT_FAIL]) { h->err = "table growth lost entries"; return GCRA_INTERNAL; }
     keep[C_OCCUPIED] = fresh[C_OCCUPIED];
     keep[C_REAL] = fresh[C_REAL];
     keep[C_STASH] = fresh[C_STASH];
-    CK(cudaMemcpyAsync(ncounters, keep, sizeof(keep), cudaMemcpyHostToDevice, h->stream));
-    CK(cudaStreamSynchronize(h->stream));
-    cudaFree(h->tab.keys); cudaFree(h->tab.state); cudaFree(h->tab.ei); cudaFree(h->tab.mark);
-    cudaFree(h->tab.counters);
+    CK(cudaMemcpyAsync(ncounters, keep, sizeof(keep), cudaMemcpyHostToDevice, h->stream.get()));
+    CK(cudaStreamSynchronize(h->stream.get()));
+    h->tab_arrays = std::move(na);
+    h->counters = std::move(nc);
     h->tab = nt;
     h->total_lines = nl;
     h->capacity = newcap;
@@ -403,8 +425,8 @@ static int ensure_room(gcra_engine *h, uint64_t n) {
     for (int back = 1; back <= gcra_engine::N_SNAP; back++) {
         int k = (int)((h->snap_next + gcra_engine::N_SNAP - back) % gcra_engine::N_SNAP);
         if (!h->snap_used[k]) break;
-        if (cudaEventQuery(h->ev_snap[k]) != cudaSuccess) continue;
-        uint64_t ub = h->h_snap[(size_t)k * C_COUNT + C_OCCUPIED] + (h->rows_launched - h->snap_rows_after[k]);
+        if (cudaEventQuery(h->ev_snap[k].get()) != cudaSuccess) continue;
+        uint64_t ub = h->h_snap.get()[(size_t)k * C_COUNT + C_OCCUPIED] + (h->rows_launched - h->snap_rows_after[k]);
         if (ub < h->occupied_ub) h->occupied_ub = ub;
         break;
     }
@@ -414,8 +436,8 @@ static int ensure_room(gcra_engine *h, uint64_t n) {
     CK(cudaDeviceSynchronize());   // batches may be in flight on caller streams
     rc = refresh_counters(h, true);
     if (rc) return rc;
-    h->occupied_ub = h->h_counters[C_OCCUPIED];
-    if (h->occupied_ub + n > load_limit(h) && h->h_counters[C_OCCUPIED] > h->h_counters[C_REAL]) {
+    h->occupied_ub = h->h_counters.get()[C_OCCUPIED];
+    if (h->occupied_ub + n > load_limit(h) && h->h_counters.get()[C_OCCUPIED] > h->h_counters.get()[C_REAL]) {
         // crowded: first give back the slots of keys that hold no entry (swept or only ever denied)
         rc = purge(h);
         if (rc) return rc;
@@ -432,8 +454,8 @@ static int snapshot_async(gcra_engine *h, uint64_t n, cudaStream_t st) {
     h->rows_launched += n;
     int k = (int)h->snap_next;
     h->snap_next = (h->snap_next + 1) % gcra_engine::N_SNAP;
-    CK(cudaMemcpyAsync(h->h_snap + (size_t)k * C_COUNT, h->tab.counters, C_COUNT * sizeof(u64), cudaMemcpyDeviceToHost, st));
-    CK(cudaEventRecord(h->ev_snap[k], st));
+    CK(cudaMemcpyAsync(h->h_snap.get() + (size_t)k * C_COUNT, h->tab.counters, C_COUNT * sizeof(u64), cudaMemcpyDeviceToHost, st));
+    CK(cudaEventRecord(h->ev_snap[k].get(), st));
     h->snap_rows_after[k] = h->rows_launched;
     h->snap_used[k] = true;
     return GCRA_OK;
@@ -455,7 +477,7 @@ static bool adaptive_should_clean(const gcra_engine *h, __int128 now, uint64_t l
 // called at batch boundaries with the counters of the batches finished so far
 static int apply_policy(gcra_engine *h, int64_t now_ns) {
     if (h->kind == GCRA_STORE_MANUAL) return GCRA_OK;
-    uint64_t allowed = h->h_counters[C_ALLOWED], hits = h->h_counters[C_EXPIRED_HITS];
+    uint64_t allowed = h->h_counters.get()[C_ALLOWED], hits = h->h_counters.get()[C_EXPIRED_HITS];
     uint64_t d_ops = allowed - h->seen_allowed, d_hits = hits - h->seen_expired_hits;
     h->seen_allowed = allowed;
     h->seen_expired_hits = hits;
@@ -488,7 +510,7 @@ static int apply_policy(gcra_engine *h, int64_t now_ns) {
     } else {                                                    // adaptive_cleanup.rs:205-211
         h->ops_since_cleanup += d_ops;
         h->expired_count += d_hits;
-        uint64_t len = h->h_counters[C_REAL];
+        uint64_t len = h->h_counters.get()[C_REAL];
         if (adaptive_should_clean(h, now, len)) {               // cleanup(): :173-203
             int rc = do_sweep(h, now_ns, &removed);
             if (rc) return rc;
@@ -527,8 +549,8 @@ static int launch_giant(gcra_engine *h, Scratch &sc, const u64 *src, const OutMa
         static bool once = false;
         if (!once) { cudaFuncSetAttribute(decide_runs_kernel<CLUSTER_CTAS, BY_ROW, R16>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1); once = true; }
     }
-    CK(cudaLaunchKernelEx(&cfg, decide_runs_kernel<CLUSTER_CTAS, BY_ROW, R16>, h->tab, (const u64 *)src, (const Req *)sc.drec, om,
-                          (const LongRun *)sc.giant_runs, (const u32 *)(sc.long_count + 1)));
+    CK(cudaLaunchKernelEx(&cfg, decide_runs_kernel<CLUSTER_CTAS, BY_ROW, R16>, h->tab, (const u64 *)src, (const Req *)sc.drec.get(), om,
+                          (const LongRun *)sc.giant_runs.get(), (const u32 *)(sc.long_count.get() + 1)));
     return GCRA_OK;
 }
 
@@ -554,19 +576,19 @@ static int enqueue_sort(gcra_engine *h, Scratch &sc, uint32_t n_max, const u32 *
         const uint32_t guess = (uint32_t)std::min<uint64_t>(std::max<uint64_t>(2ULL * h->last_nres, n_max / 8) + 8 * SORT_TILE, n_max);
         stiles = std::max<uint32_t>(std::min<uint32_t>((guess + SORT_TILE - 1) / SORT_TILE, 2 * h->sms), 8);
     }
-    u64 *src = sc.keys_a, *dst = sc.keys_b;
+    u64 *src = sc.keys_a.get(), *dst = sc.keys_b.get();
     uint32_t shift = 32;
     for (uint32_t p = 0; p < passes; p++) {
         uint32_t pb = bits / passes + (p < bits % passes ? 1 : 0);
         if (n_dev) {
             // device-side count (the residue): one launch per pass, grid barriers between its phases
-            u32 *bar_cnt = reinterpret_cast<u32 *>(sc.ctrl_block + 1);
-            sort_pass_fused_kernel<<<stiles, TILE_THREADS, 0, st>>>(src, dst, n_dev, shift, pb, sc.hist, sc.tot, bar_cnt, p);
+            u32 *bar_cnt = reinterpret_cast<u32 *>(sc.ctrl_block.get() + 1);
+            sort_pass_fused_kernel<<<stiles, TILE_THREADS, 0, st>>>(src, dst, n_dev, shift, pb, sc.hist.get(), sc.tot.get(), bar_cnt, p);
             h->launches++;
         } else {
-            sort_hist_kernel<<<stiles, TILE_THREADS, 0, st>>>(src, n_max, n_dev, shift, pb, sc.hist);
-            sort_rowscan_kernel<<<1u << pb, TILE_THREADS, 0, st>>>(sc.hist, n_max, n_dev, sc.tot);
-            sort_scatter_kernel<<<stiles, TILE_THREADS, 0, st>>>(src, dst, n_max, n_dev, shift, pb, sc.hist, sc.tot);
+            sort_hist_kernel<<<stiles, TILE_THREADS, 0, st>>>(src, n_max, n_dev, shift, pb, sc.hist.get());
+            sort_rowscan_kernel<<<1u << pb, TILE_THREADS, 0, st>>>(sc.hist.get(), n_max, n_dev, sc.tot.get());
+            sort_scatter_kernel<<<stiles, TILE_THREADS, 0, st>>>(src, dst, n_max, n_dev, shift, pb, sc.hist.get(), sc.tot.get());
             h->launches += 3;
         }
         std::swap(src, dst);
@@ -580,25 +602,25 @@ template <bool BY_ROW, bool R16>
 static int enqueue_decide_sorted_t(gcra_engine *h, Scratch &sc, uint32_t n_max, const u32 *n_dev, const u64 *src,
                                    const OutMap &om, cudaStream_t st) {
     // (sort pipeline: the work-list counters were cleared at the end of the front half, off this stream)
-    if (BY_ROW) CK(cudaMemsetAsync(sc.long_count, 0, 2 * sizeof(u32), st));
+    if (BY_ROW) CK(cudaMemsetAsync(sc.long_count.get(), 0, 2 * sizeof(u32), st));
     const uint32_t warps = (n_max + 31) / 32;
     uint32_t grid = (warps + DECIDE_THREADS / 32 - 1) / (DECIDE_THREADS / 32);
     if (n_dev) grid = std::min<uint32_t>(grid, 4 * h->sms);
-    decide_kernel<BY_ROW, R16><<<grid, DECIDE_THREADS, 0, st>>>(h->tab, src, sc.drec, n_max, n_dev, om, sc.long_runs, sc.giant_runs,
-                                                           sc.long_count, 0);
+    decide_kernel<BY_ROW, R16><<<grid, DECIDE_THREADS, 0, st>>>(h->tab, src, sc.drec.get(), n_max, n_dev, om, sc.long_runs.get(), sc.giant_runs.get(),
+                                                           sc.long_count.get(), 0);
     h->launches++;
     if (n_max >= GIANT_RUN_MIN) {
         // the two hot-run kernels work on disjoint runs: the one-CTA-per-run kernel goes to a side
         // stream and overlaps the cluster kernel (fork/join with events)
-        CK(cudaEventRecord(sc.ev_fork, st));
-        CK(cudaStreamWaitEvent(h->aux_stream, sc.ev_fork, 0));
-        decide_runs_kernel<1, BY_ROW, R16><<<h->sms, LONG_THREADS, 0, h->aux_stream>>>(h->tab, src, sc.drec, om, sc.long_runs, sc.long_count);
-        CK(cudaEventRecord(sc.ev_join, h->aux_stream));
+        CK(cudaEventRecord(sc.ev_fork.get(), st));
+        CK(cudaStreamWaitEvent(h->aux_stream.get(), sc.ev_fork.get(), 0));
+        decide_runs_kernel<1, BY_ROW, R16><<<h->sms, LONG_THREADS, 0, h->aux_stream.get()>>>(h->tab, src, sc.drec.get(), om, sc.long_runs.get(), sc.long_count.get());
+        CK(cudaEventRecord(sc.ev_join.get(), h->aux_stream.get()));
         RC((launch_giant<BY_ROW, R16>(h, sc, src, om, st)));   // hottest keys: one cluster per run
-        CK(cudaStreamWaitEvent(st, sc.ev_join, 0));
+        CK(cudaStreamWaitEvent(st, sc.ev_join.get(), 0));
         h->launches += 2;
     } else if (n_max >= LONG_RUN_MIN) {
-        decide_runs_kernel<1, BY_ROW, R16><<<h->sms, LONG_THREADS, 0, st>>>(h->tab, src, sc.drec, om, sc.long_runs, sc.long_count);
+        decide_runs_kernel<1, BY_ROW, R16><<<h->sms, LONG_THREADS, 0, st>>>(h->tab, src, sc.drec.get(), om, sc.long_runs.get(), sc.long_count.get());
         h->launches++;
     }
     return GCRA_OK;
@@ -614,23 +636,25 @@ static int enqueue_decide_sorted(gcra_engine *h, Scratch &sc, uint32_t n_max, co
                      : enqueue_decide_sorted_t<false, false>(h, sc, n_max, n_dev, src, om, st);
 }
 
-// per-set buffers of the index-order pipeline for batches of up to `rows` row ids
-static int alloc_index_scratch(gcra_engine *h, Scratch &sc, uint32_t rows) {
-    cudaFree(sc.slot_arr); cudaFree(sc.flags); cudaFree(sc.ctrl_block);
-    sc.slot_arr = nullptr; sc.flags = nullptr; sc.ctrl_block = nullptr;
-    const uint32_t tiles = (rows + TILE_THREADS - 1) / TILE_THREADS;
-    if (tiles > h->max_tiles) h->max_tiles = tiles;
-    CK(cudaMalloc(&sc.slot_arr, (size_t)rows * sizeof(u32)));
-    CK(cudaMalloc(&sc.flags, (size_t)rows));
-    CK(cudaMalloc(&sc.ctrl_block, ((size_t)h->max_tiles + 2) * sizeof(u64)));
-    if (!sc.h_nres) { CK(cudaMallocHost(&sc.h_nres, sizeof(u32))); *sc.h_nres = 0; }
-    if (!sc.bitmap) {
-        CK(cudaMalloc(&sc.bitmap, h->bm_words * sizeof(u32)));
-        CK(cudaMalloc(&sc.pend, h->pend_words * sizeof(u32)));
-        CK(cudaMemsetAsync(sc.bitmap, 0, h->bm_words * sizeof(u32), h->stream));   // from then on cleared after every use
-        CK(cudaMemsetAsync(sc.pend, 0, h->pend_words * sizeof(u32), h->stream));
+// every set's per-row buffers of the index-order pipeline, for batches of up to `rows` row ids (never shrinking), made
+// for all sets before any set's are replaced.  The caller makes sure that no batch in flight uses the old ones.
+static int alloc_index_scratch(gcra_engine *h, uint32_t rows) {
+    if (rows <= h->scr[0].rows_alloc) return GCRA_OK;
+    const uint32_t max_tiles = std::max<uint32_t>(h->max_tiles, (rows + TILE_THREADS - 1) / TILE_THREADS);
+    struct { DevBuf<u32> slot_arr; DevBuf<unsigned char> flags; DevBuf<u64> ctrl_block; } fresh[gcra_engine::N_SCR];
+    for (auto &f : fresh) {
+        CK(f.slot_arr.make(rows));
+        CK(f.flags.make(rows));
+        CK(f.ctrl_block.make((size_t)max_tiles + 2));
     }
-    sc.rows_alloc = rows;
+    for (int k = 0; k < gcra_engine::N_SCR; k++) {
+        Scratch &sc = h->scr[k];
+        sc.slot_arr = std::move(fresh[k].slot_arr);
+        sc.flags = std::move(fresh[k].flags);
+        sc.ctrl_block = std::move(fresh[k].ctrl_block);
+        sc.rows_alloc = rows;
+    }
+    h->max_tiles = max_tiles;
     return GCRA_OK;
 }
 
@@ -660,44 +684,44 @@ static uint32_t view_max_rows(const BatchView &v) { return v.nseg == 1 ? v.n : (
 //   index-order pipeline  pass A (probe) + pass A' (batch bitmap)
 static int enqueue_front(gcra_engine *h, Scratch &sc, const BatchView &v, bool index_path, int fmt, int64_t now_batch,
                          cudaStream_t st, bool timed, u64 **sorted_out) {
-    if (timed) CK(cudaEventRecord(h->ev[0], st));
+    if (timed) CK(cudaEventRecord(h->ev[0].get(), st));
     *sorted_out = nullptr;
     if (index_path) {
         const uint32_t rows = view_max_rows(v);
         const uint32_t tiles = (rows + TILE_THREADS - 1) / TILE_THREADS;
         const uint32_t grid = std::min<uint32_t>(tiles, h->grid_probe[fmt]);    // persistent, software-pipelined CTAs
-        CK(cudaMemsetAsync(sc.ctrl_block, 0, ((size_t)h->max_tiles + 2) * sizeof(u64), st));
-        if (timed) CK(cudaEventRecord(h->evd[0], st));
+        CK(cudaMemsetAsync(sc.ctrl_block.get(), 0, ((size_t)h->max_tiles + 2) * sizeof(u64), st));
+        if (timed) CK(cudaEventRecord(h->evd[0].get(), st));
         if (fmt == FMT_16_16)
-            probe_kernel<FMT_16_16><<<grid, TILE_THREADS, 0, st>>>(h->tab, v, h->d_pol, h->npol, now_batch, sc.slot_arr,
-                                                                   sc.bitmap, h->bm_mask, h->prefetch_state);
+            probe_kernel<FMT_16_16><<<grid, TILE_THREADS, 0, st>>>(h->tab, v, h->d_pol.get(), h->npol, now_batch, sc.slot_arr.get(),
+                                                                   sc.bitmap.get(), h->bm_mask, h->prefetch_state);
         else if (fmt == FMT_16_32)
-            probe_kernel<FMT_16_32><<<grid, TILE_THREADS, 0, st>>>(h->tab, v, h->d_pol, h->npol, now_batch, sc.slot_arr,
-                                                                   sc.bitmap, h->bm_mask, h->prefetch_state);
+            probe_kernel<FMT_16_32><<<grid, TILE_THREADS, 0, st>>>(h->tab, v, h->d_pol.get(), h->npol, now_batch, sc.slot_arr.get(),
+                                                                   sc.bitmap.get(), h->bm_mask, h->prefetch_state);
         else
-            probe_kernel<FMT_48_32><<<grid, TILE_THREADS, 0, st>>>(h->tab, v, nullptr, 0, 0, sc.slot_arr, sc.bitmap, h->bm_mask,
+            probe_kernel<FMT_48_32><<<grid, TILE_THREADS, 0, st>>>(h->tab, v, nullptr, 0, 0, sc.slot_arr.get(), sc.bitmap.get(), h->bm_mask,
                                                                h->prefetch_state);
-        if (timed) CK(cudaEventRecord(h->evd[1], st));
+        if (timed) CK(cudaEventRecord(h->evd[1].get(), st));
         h->launches += 1;
-        if (timed) { CK(cudaEventRecord(h->ev[1], st)); CK(cudaEventRecord(h->evd[2], st)); }
+        if (timed) { CK(cudaEventRecord(h->ev[1].get(), st)); CK(cudaEventRecord(h->evd[2].get(), st)); }
         return GCRA_OK;
     }
     const uint32_t n = v.n;
     const uint32_t tiles = (n + TILE_THREADS - 1) / TILE_THREADS;
     if (fmt == FMT_16_16)
-        ingest_kernel<FMT_16_16><<<tiles, TILE_THREADS, 0, st>>>(h->tab, v.req0, h->d_pol, h->npol, now_batch, n,
-                                                                 sc.drec, sc.keys_a, v.res0);
+        ingest_kernel<FMT_16_16><<<tiles, TILE_THREADS, 0, st>>>(h->tab, v.req0, h->d_pol.get(), h->npol, now_batch, n,
+                                                                 sc.drec.get(), sc.keys_a.get(), v.res0);
     else if (fmt == FMT_16_32)
-        ingest_kernel<FMT_16_32><<<tiles, TILE_THREADS, 0, st>>>(h->tab, v.req0, h->d_pol, h->npol, now_batch, n,
-                                                                 sc.drec, sc.keys_a, v.res0);
+        ingest_kernel<FMT_16_32><<<tiles, TILE_THREADS, 0, st>>>(h->tab, v.req0, h->d_pol.get(), h->npol, now_batch, n,
+                                                                 sc.drec.get(), sc.keys_a.get(), v.res0);
     else
-        ingest_kernel<FMT_48_32><<<tiles, TILE_THREADS, 0, st>>>(h->tab, v.req0, nullptr, 0, 0, n, sc.drec,
-                                                             sc.keys_a, v.res0);
+        ingest_kernel<FMT_48_32><<<tiles, TILE_THREADS, 0, st>>>(h->tab, v.req0, nullptr, 0, 0, n, sc.drec.get(),
+                                                             sc.keys_a.get(), v.res0);
     h->launches++;
-    if (timed) CK(cudaEventRecord(h->ev[1], st));
+    if (timed) CK(cudaEventRecord(h->ev[1].get(), st));
     RC(enqueue_sort(h, sc, n, nullptr, st, sorted_out));
-    if (timed) CK(cudaEventRecord(h->ev[2], st));
-    CK(cudaMemsetAsync(sc.long_count, 0, 2 * sizeof(u32), st));   // hot-run work lists of this batch's decide kernels
+    if (timed) CK(cudaEventRecord(h->ev[2].get(), st));
+    CK(cudaMemsetAsync(sc.long_count.get(), 0, 2 * sizeof(u32), st));   // hot-run work lists of this batch's decide kernels
     return GCRA_OK;
 }
 
@@ -715,40 +739,40 @@ static int enqueue_mid_index(gcra_engine *h, Scratch &sc, Scratch &next, const B
     const uint32_t rows = view_max_rows(v);
     const uint32_t grid = std::min<uint32_t>((rows + TILE_THREADS - 1) / TILE_THREADS, h->grid_decide[fmt]);   // persistent CTAs
     const uint32_t rgrid = std::min<uint32_t>((rows + RES_TILE - 1) / RES_TILE + v.nseg, 6 * h->sms);
-    u32 *ctrl = reinterpret_cast<u32 *>(sc.ctrl_block);
-    u64 *status = sc.ctrl_block + 2;
+    u32 *ctrl = reinterpret_cast<u32 *>(sc.ctrl_block.get());
+    u64 *status = sc.ctrl_block.get() + 2;
     if (fmt == FMT_16_16) {
-        decide_index_kernel<FMT_16_16><<<grid, TILE_THREADS, 0, st>>>(h->tab, v, h->d_pol, h->npol, now_batch, sc.slot_arr,
-                                                                      sc.bitmap, sc.pend, h->bm_mask, sc.flags, h->epoch, hp,
+        decide_index_kernel<FMT_16_16><<<grid, TILE_THREADS, 0, st>>>(h->tab, v, h->d_pol.get(), h->npol, now_batch, sc.slot_arr.get(),
+                                                                      sc.bitmap.get(), sc.pend.get(), h->bm_mask, sc.flags.get(), h->epoch, hp,
                                                                       h->dbg);
-        if (timed) CK(cudaEventRecord(h->evd[3], st));
-        resolve_kernel<FMT_16_16><<<rgrid, TILE_THREADS, 0, st>>>(h->tab, v, h->d_pol, h->npol, now_batch, sc.slot_arr,
-                                                                  h->bm_mask, sc.flags, h->epoch, ctrl, status, sc.keys_a,
-                                                                  next.pend, sc.h_nres, h->max_batch);
+        if (timed) CK(cudaEventRecord(h->evd[3].get(), st));
+        resolve_kernel<FMT_16_16><<<rgrid, TILE_THREADS, 0, st>>>(h->tab, v, h->d_pol.get(), h->npol, now_batch, sc.slot_arr.get(),
+                                                                  h->bm_mask, sc.flags.get(), h->epoch, ctrl, status, sc.keys_a.get(),
+                                                                  next.pend.get(), sc.h_nres.get(), h->max_batch);
     } else if (fmt == FMT_16_32) {
-        decide_index_kernel<FMT_16_32><<<grid, TILE_THREADS, 0, st>>>(h->tab, v, h->d_pol, h->npol, now_batch, sc.slot_arr,
-                                                                      sc.bitmap, sc.pend, h->bm_mask, sc.flags, h->epoch, hp,
+        decide_index_kernel<FMT_16_32><<<grid, TILE_THREADS, 0, st>>>(h->tab, v, h->d_pol.get(), h->npol, now_batch, sc.slot_arr.get(),
+                                                                      sc.bitmap.get(), sc.pend.get(), h->bm_mask, sc.flags.get(), h->epoch, hp,
                                                                       h->dbg);
-        if (timed) CK(cudaEventRecord(h->evd[3], st));
-        resolve_kernel<FMT_16_32><<<rgrid, TILE_THREADS, 0, st>>>(h->tab, v, h->d_pol, h->npol, now_batch, sc.slot_arr,
-                                                                  h->bm_mask, sc.flags, h->epoch, ctrl, status, sc.keys_a,
-                                                                  next.pend, sc.h_nres, h->max_batch);
+        if (timed) CK(cudaEventRecord(h->evd[3].get(), st));
+        resolve_kernel<FMT_16_32><<<rgrid, TILE_THREADS, 0, st>>>(h->tab, v, h->d_pol.get(), h->npol, now_batch, sc.slot_arr.get(),
+                                                                  h->bm_mask, sc.flags.get(), h->epoch, ctrl, status, sc.keys_a.get(),
+                                                                  next.pend.get(), sc.h_nres.get(), h->max_batch);
     } else {
-        decide_index_kernel<FMT_48_32><<<grid, TILE_THREADS, 0, st>>>(h->tab, v, nullptr, 0, 0, sc.slot_arr, sc.bitmap, sc.pend,
-                                                                  h->bm_mask, sc.flags, h->epoch, hp, h->dbg);
-        if (timed) CK(cudaEventRecord(h->evd[3], st));
-        resolve_kernel<FMT_48_32><<<rgrid, TILE_THREADS, 0, st>>>(h->tab, v, nullptr, 0, 0, sc.slot_arr, h->bm_mask,
-                                                              sc.flags, h->epoch, ctrl, status, sc.keys_a,
-                                                              next.pend, sc.h_nres, h->max_batch);
+        decide_index_kernel<FMT_48_32><<<grid, TILE_THREADS, 0, st>>>(h->tab, v, nullptr, 0, 0, sc.slot_arr.get(), sc.bitmap.get(), sc.pend.get(),
+                                                                  h->bm_mask, sc.flags.get(), h->epoch, hp, h->dbg);
+        if (timed) CK(cudaEventRecord(h->evd[3].get(), st));
+        resolve_kernel<FMT_48_32><<<rgrid, TILE_THREADS, 0, st>>>(h->tab, v, nullptr, 0, 0, sc.slot_arr.get(), h->bm_mask,
+                                                              sc.flags.get(), h->epoch, ctrl, status, sc.keys_a.get(),
+                                                              next.pend.get(), sc.h_nres.get(), h->max_batch);
     }
     h->launches += 2;
     h->n_index_batches++;
-    if (timed) CK(cudaEventRecord(h->evd[4], st));
-    // (pass C wrote the residue size of this batch to sc.h_nres, mapped pinned host memory: read, once ev_mid has
+    if (timed) CK(cudaEventRecord(h->evd[4].get(), st));
+    // (pass C wrote the residue size of this batch to sc.h_nres.get(), mapped pinned host memory: read, once ev_mid has
     // completed, when later batches are submitted)
     sc.nres_rows = std::min<uint32_t>(rows, h->max_batch);
     sc.nres_counted = false;
-    if (timed) CK(cudaEventRecord(h->ev[2], st));
+    if (timed) CK(cudaEventRecord(h->ev[2].get(), st));
     CK(cudaGetLastError());
     return GCRA_OK;
 }
@@ -758,26 +782,26 @@ static int enqueue_mid_index(gcra_engine *h, Scratch &sc, Scratch &next, const B
 // size only exists on the device.  Tails run strictly in submission order.
 static int enqueue_tail_index(gcra_engine *h, Scratch &sc, const BatchView &v, int fmt, int64_t now_batch, cudaStream_t st,
                               bool timed) {
-    const u32 *n_res = reinterpret_cast<const u32 *>(sc.ctrl_block) + RC_NRES;
+    const u32 *n_res = reinterpret_cast<const u32 *>(sc.ctrl_block.get()) + RC_NRES;
     const uint32_t n_max = std::min<uint32_t>(view_max_rows(v), h->max_batch);
     u64 *rs = nullptr;
     // this set's bitmap has been read for the last time (pass C): cleared here, off stage 2's stream, for its next
     // use (pass A' of the batch that takes this set again, and the PEND bits the batch before that one leaves)
-    CK(cudaMemsetAsync(sc.bitmap, 0, h->bm_words * sizeof(u32), st));
-    CK(cudaMemsetAsync(sc.pend, 0, h->pend_words * sizeof(u32), st));   // (the bits the previous batch left: read by pass B)
-    if (timed) CK(cudaEventRecord(h->evd[5], st));
+    CK(cudaMemsetAsync(sc.bitmap.get(), 0, h->bm_words * sizeof(u32), st));
+    CK(cudaMemsetAsync(sc.pend.get(), 0, h->pend_words * sizeof(u32), st));   // (the bits the previous batch left: read by pass B)
+    if (timed) CK(cudaEventRecord(h->evd[5].get(), st));
     RC(enqueue_sort(h, sc, n_max, n_res, st, &rs));
-    if (timed) CK(cudaEventRecord(h->evd[6], st));
+    if (timed) CK(cudaEventRecord(h->evd[6].get(), st));
     OutMap om{};
     om.out = nullptr;
     om.by_row = 1;
     om.compact = fmt != FMT_48_32 ? 1 : 0;
     om.view = v;
-    om.pol = h->d_pol;
+    om.pol = h->d_pol.get();
     om.npol = h->npol;
     om.now_batch = now_batch;
     RC(enqueue_decide_sorted(h, sc, n_max, n_res, rs, om, fmt == FMT_16_16, st));
-    if (timed) { CK(cudaEventRecord(h->ev[3], st)); h->ev_valid = true; CK(cudaEventRecord(h->evd[7], st)); h->evd_valid = true; }
+    if (timed) { CK(cudaEventRecord(h->ev[3].get(), st)); h->ev_valid = true; CK(cudaEventRecord(h->evd[7].get(), st)); h->evd_valid = true; }
     CK(cudaGetLastError());
     return GCRA_OK;
 }
@@ -789,7 +813,7 @@ static int enqueue_back_sorted(gcra_engine *h, Scratch &sc, const BatchView &v, 
     om.out = v.res0;
     om.by_row = 0;
     RC(enqueue_decide_sorted(h, sc, v.n, nullptr, sorted, om, fmt == FMT_16_16, st));
-    if (timed) { CK(cudaEventRecord(h->ev[3], st)); h->ev_valid = true; }
+    if (timed) { CK(cudaEventRecord(h->ev[3].get(), st)); h->ev_valid = true; }
     CK(cudaGetLastError());
     return GCRA_OK;
 }
@@ -812,20 +836,20 @@ static int launch_batch(gcra_engine *h, uint32_t n, const void *d_req, int fmt, 
     Scratch &next = h->scr[h->scr_next];
     // order after every earlier batch (they may have been submitted pipelined on the engine's streams),
     // which also frees this scratch set
-    for (auto &o : h->scr) if (o.back_recorded) CK(cudaStreamWaitEvent(st, o.ev_back, 0));
+    for (auto &o : h->scr) if (o.back_recorded) CK(cudaStreamWaitEvent(st, o.ev_back.get(), 0));
     static const bool no_small = getenv("GCRA_NO_SMALL") && atoi(getenv("GCRA_NO_SMALL"));   // A/B switch for tools/latency_probe.py
     if (n <= SMALL_MAX && !no_small) {
         // small batch (a single rate_limit call, a lightly loaded actor): one CTA does ingest, ordering and
         // the compare-and-update in a single launch
-        if (timed) { CK(cudaEventRecord(h->ev[0], st)); CK(cudaEventRecord(h->ev[1], st)); CK(cudaEventRecord(h->ev[2], st)); }
+        if (timed) { CK(cudaEventRecord(h->ev[0].get(), st)); CK(cudaEventRecord(h->ev[1].get(), st)); CK(cudaEventRecord(h->ev[2].get(), st)); }
         if (fmt == FMT_16_16)
-            small_batch_kernel<FMT_16_16><<<1, TILE_THREADS, 0, st>>>(h->tab, d_req, h->d_pol, h->npol, now_batch, n, sc.drec, d_res);
+            small_batch_kernel<FMT_16_16><<<1, TILE_THREADS, 0, st>>>(h->tab, d_req, h->d_pol.get(), h->npol, now_batch, n, sc.drec.get(), d_res);
         else if (fmt == FMT_16_32)
-            small_batch_kernel<FMT_16_32><<<1, TILE_THREADS, 0, st>>>(h->tab, d_req, h->d_pol, h->npol, now_batch, n, sc.drec, d_res);
+            small_batch_kernel<FMT_16_32><<<1, TILE_THREADS, 0, st>>>(h->tab, d_req, h->d_pol.get(), h->npol, now_batch, n, sc.drec.get(), d_res);
         else
-            small_batch_kernel<FMT_48_32><<<1, TILE_THREADS, 0, st>>>(h->tab, d_req, nullptr, 0, 0, n, sc.drec, d_res);
+            small_batch_kernel<FMT_48_32><<<1, TILE_THREADS, 0, st>>>(h->tab, d_req, nullptr, 0, 0, n, sc.drec.get(), d_res);
         h->launches++;
-        if (timed) { CK(cudaEventRecord(h->ev[3], st)); h->ev_valid = true; }
+        if (timed) { CK(cudaEventRecord(h->ev[3].get(), st)); h->ev_valid = true; }
         CK(cudaGetLastError());
     } else {
         u64 *sorted = nullptr;
@@ -834,7 +858,7 @@ static int launch_batch(gcra_engine *h, uint32_t n, const void *d_req, int fmt, 
         RC(enqueue_front(h, sc, v, ip, fmt, now_batch, st, timed, &sorted));
         if (ip) {
             RC(enqueue_mid_index(h, sc, next, v, fmt, now_batch, false, st, timed));
-            CK(cudaEventRecord(sc.ev_mid, st));
+            CK(cudaEventRecord(sc.ev_mid.get(), st));
             sc.mid_recorded = true;
             RC(enqueue_tail_index(h, sc, v, fmt, now_batch, st, timed));
         } else {
@@ -843,7 +867,7 @@ static int launch_batch(gcra_engine *h, uint32_t n, const void *d_req, int fmt, 
         }
     }
     RC(enqueue_denied(h, single_view(d_req, d_res, n), fmt, st));
-    CK(cudaEventRecord(sc.ev_back, st));
+    CK(cudaEventRecord(sc.ev_back.get(), st));
     sc.back_recorded = true;
     h->pend_set = -1;          // everything of this batch is ordered on `st`: the next batch waits for all of it
     return snapshot_async(h, n, st);
@@ -865,19 +889,19 @@ static int launch_pipelined_view(gcra_engine *h, const BatchView &v, uint32_t n_
     Scratch &sc = h->scr[k];
     h->scr_next = (h->scr_next + 1) % gcra_engine::N_SCR;
     const uint32_t kn = h->scr_next;
-    cudaStream_t fs = h->front_stream[k];                  // (all sets share one front stream, see gcra_create)
+    cudaStream_t fs = h->front_stream.get();                  // (all sets share one front stream, see gcra_create)
     if (ready) CK(cudaStreamWaitEvent(fs, ready, 0));
-    if (sc.back_recorded) CK(cudaStreamWaitEvent(fs, sc.ev_back, 0));   // scratch set free again
+    if (sc.back_recorded) CK(cudaStreamWaitEvent(fs, sc.ev_back.get(), 0));   // scratch set free again
     u64 *sorted = nullptr;
     // residue feedback: the newest pass-C count that has reached the host
     bool residue_large = false;
     for (int back = 1; back < gcra_engine::N_SCR; back++) {
         Scratch &os = h->scr[(k + gcra_engine::N_SCR - back) % gcra_engine::N_SCR];
-        if (!os.mid_recorded || cudaEventQuery(os.ev_mid) != cudaSuccess) continue;
-        if (!os.nres_counted) { h->residue_seen += *os.h_nres; h->residue_batches_seen++; os.nres_counted = true; }
-        h->last_nres = *os.h_nres;
+        if (!os.mid_recorded || cudaEventQuery(os.ev_mid.get()) != cudaSuccess) continue;
+        if (!os.nres_counted) { h->residue_seen += *os.h_nres.get(); h->residue_batches_seen++; os.nres_counted = true; }
+        h->last_nres = *os.h_nres.get();
         h->last_nres_rows = os.nres_rows;
-        residue_large = (uint64_t)*os.h_nres * 8 > os.nres_rows;
+        residue_large = (uint64_t)*os.h_nres.get() * 8 > os.nres_rows;
         break;
     }
     bool ip = v.nseg > 1 || use_index_path(h, n_rows);
@@ -892,9 +916,9 @@ static int launch_pipelined_view(gcra_engine *h, const BatchView &v, uint32_t n_
         }
     }
     RC(enqueue_front(h, sc, v, ip, fmt, now_batch, fs, false, &sorted));
-    CK(cudaEventRecord(sc.ev_front, fs));
-    cudaStream_t ms = h->back_stream;
-    CK(cudaStreamWaitEvent(ms, sc.ev_front, 0));
+    CK(cudaEventRecord(sc.ev_front.get(), fs));
+    cudaStream_t ms = h->back_stream.get();
+    CK(cudaStreamWaitEvent(ms, sc.ev_front.get(), 0));
     // May stage 2 of this batch overlap the tail of the batch submitted just before?  Only if that batch left its
     // PEND bits in this set's pend bitmap.  Keys the tail owns stay deferred for as long as they keep appearing
     // (their requests go from tail to tail), so the overlap is given up -- stage 2 waits for every tail and ignores
@@ -911,29 +935,29 @@ static int launch_pipelined_view(gcra_engine *h, const BatchView &v, uint32_t n_
         if (o == (int)k || !os.back_recorded) continue;
         const bool is_prev = o == (int)((k + gcra_engine::N_SCR - 1) % gcra_engine::N_SCR);
         if (overlap && is_prev) continue;
-        CK(cudaStreamWaitEvent(ms, os.ev_back, 0));
+        CK(cudaStreamWaitEvent(ms, os.ev_back.get(), 0));
     }
     if (ip) {
         RC(enqueue_mid_index(h, sc, h->scr[kn], v, fmt, now_batch, overlap, ms, false));
-        CK(cudaEventRecord(sc.ev_mid, ms));
+        CK(cudaEventRecord(sc.ev_mid.get(), ms));
         sc.mid_recorded = true;
-        cudaStream_t ts = h->tail_stream;
-        CK(cudaStreamWaitEvent(ts, sc.ev_mid, 0));
+        cudaStream_t ts = h->tail_stream.get();
+        CK(cudaStreamWaitEvent(ts, sc.ev_mid.get(), 0));
         RC(enqueue_tail_index(h, sc, v, fmt, now_batch, ts, false));
         RC(enqueue_denied(h, v, fmt, ts));
-        CK(cudaEventRecord(sc.ev_back, ts));
+        CK(cudaEventRecord(sc.ev_back.get(), ts));
         sc.back_recorded = true;
         h->pend_set = (int)kn;
-        if (done) *done = sc.ev_back;
+        if (done) *done = sc.ev_back.get();
         return snapshot_async(h, n_rows, ts);
     }
     RC(enqueue_back_sorted(h, sc, v, fmt, sorted, ms, false));
     RC(enqueue_denied(h, v, fmt, ms));
     sc.mid_recorded = false;   // (no residue count from this batch)
-    CK(cudaEventRecord(sc.ev_back, ms));
+    CK(cudaEventRecord(sc.ev_back.get(), ms));
     sc.back_recorded = true;
     h->pend_set = -1;
-    if (done) *done = sc.ev_back;
+    if (done) *done = sc.ev_back.get();
     return snapshot_async(h, n_rows, ms);
 }
 
@@ -977,38 +1001,26 @@ static void preload_kernels() {
 // ---------------------------------------------------------------------------------------------
 extern "C" {
 
-int32_t gcra_create(const gcra_config *cfg, gcra_engine **out) {
-    if (!cfg || !out) return GCRA_INTERNAL;
-    *out = nullptr;
-    gcra_engine *h = new gcra_engine();
-    auto fail = [&](const char *what, cudaError_t e) {
-        fprintf(stderr, "gcra_create: %s: %s\n", what, cudaGetErrorString(e));
-        delete h;
-        return (int32_t)GCRA_INTERNAL;
-    };
+// everything gcra_create makes; on failure h->err says what failed and deleting `h` releases what was made
+static int init_engine(gcra_engine *h, const gcra_config *cfg) {
     int ndev = 0;
-    cudaError_t e = cudaGetDeviceCount(&ndev);
-    if (e != cudaSuccess || ndev == 0) return fail("no CUDA device (this engine has no CPU path)", e);
-    if (cfg->device < 0 || cfg->device >= ndev) return fail("bad device ordinal", cudaErrorInvalidDevice);
+    CK(cudaGetDeviceCount(&ndev));        // (this engine has no CPU path)
+    if (cfg->device < 0 || cfg->device >= ndev) { h->err = "bad device ordinal"; return GCRA_INTERNAL; }
     h->device = cfg->device;
-    if ((e = cudaSetDevice(h->device)) != cudaSuccess) return fail("cudaSetDevice", e);
+    CK(cudaSetDevice(h->device));
     int sms = 0;
-    if ((e = cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, h->device)) != cudaSuccess || sms <= 0)
-        return fail("cudaDevAttrMultiProcessorCount", e);
+    CK(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, h->device));
+    if (sms <= 0) { h->err = "no streaming multiprocessors"; return GCRA_INTERNAL; }
     h->sms = (uint32_t)sms;
     if (const char *g = getenv("GCRA_L2_FETCH")) cudaDeviceSetLimit(cudaLimitMaxL2FetchGranularity, (size_t)atoi(g));
-    if ((e = cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking)) != cudaSuccess) return fail("stream", e);
-    cudaStreamCreateWithFlags(&h->in_stream, cudaStreamNonBlocking);
-    cudaStreamCreateWithFlags(&h->out_stream, cudaStreamNonBlocking);
-    cudaStreamCreateWithFlags(&h->aux_stream, cudaStreamNonBlocking);
-    cudaStreamCreateWithFlags(&h->aux2_stream, cudaStreamNonBlocking);
-    // ONE front stream shared by all scratch sets (front halves run one after another; since ingest only CASes
-    // the keys array they could overlap as well -- not measured yet)
-    cudaStreamCreateWithFlags(&h->front_stream[0], cudaStreamNonBlocking);
-    for (int k = 1; k < gcra_engine::N_SCR; k++) h->front_stream[k] = h->front_stream[0];
-    cudaStreamCreateWithFlags(&h->back_stream, cudaStreamNonBlocking);
-    cudaStreamCreateWithFlags(&h->tail_stream, cudaStreamNonBlocking);
-    cudaEventCreateWithFlags(&h->ev_ready, cudaEventDisableTiming);
+    for (Stream *s : {&h->stream, &h->in_stream, &h->out_stream, &h->aux_stream, &h->aux2_stream, &h->front_stream,
+                      &h->back_stream, &h->tail_stream})
+        CK(s->make());
+    for (Event *e : {&h->ev_ready, &h->ev_counters}) CK(e->make(cudaEventDisableTiming));
+    for (Event &e : h->ev_snap) CK(e.make(cudaEventDisableTiming));
+    for (Event &e : h->ev) CK(e.make(cudaEventDefault));         // (timed)
+    for (Event &e : h->evd) CK(e.make(cudaEventDefault));
+    for (Event &e : h->ev_sweep) CK(e.make(cudaEventDefault));
     h->capacity = cfg->capacity ? cfg->capacity : 1000;      // DEFAULT_CAPACITY adaptive_cleanup.rs:10
     h->max_batch = cfg->max_batch ? cfg->max_batch : (1u << 20);
     h->tight = (cfg->flags & GCRA_FLAG_TIGHT_TABLE) != 0;
@@ -1016,23 +1028,14 @@ int32_t gcra_create(const gcra_config *cfg, gcra_engine **out) {
     h->hash_seed[1] = cfg->hash_seed[1];
     if (cfg->flags & GCRA_FLAG_RANDOM_SEED) {
         FILE *ur = fopen("/dev/urandom", "rb");
-        if (!ur || fread(h->hash_seed, sizeof(h->hash_seed), 1, ur) != 1) {
-            if (ur) fclose(ur);
-            fprintf(stderr, "gcra_create: cannot read /dev/urandom for the hash seed\n");
-            delete h;
-            return GCRA_INTERNAL;
-        }
-        fclose(ur);
+        const bool got = ur && fread(h->hash_seed, sizeof(h->hash_seed), 1, ur) == 1;
+        if (ur) fclose(ur);
+        if (!got) { h->err = "cannot read /dev/urandom for the hash seed"; return GCRA_INTERNAL; }
         h->hash_seed[0] |= 1;      // never (0, 0)
     }
-    u64 *counters = nullptr;
-    if ((e = cudaMalloc(&counters, C_COUNT * sizeof(u64))) != cudaSuccess) return fail("counters", e);
-    cudaMemsetAsync(counters, 0, C_COUNT * sizeof(u64), h->stream);
-    if (alloc_table(h, h->capacity, h->tab, h->total_lines, counters)) {
-        fprintf(stderr, "gcra_create: %s\n", h->err.c_str());
-        delete h;
-        return GCRA_INTERNAL;
-    }
+    CK(h->counters.make(C_COUNT));
+    CK(cudaMemsetAsync(h->counters.get(), 0, C_COUNT * sizeof(u64), h->stream.get()));
+    RC(alloc_table(h, h->capacity, h->tab_arrays, h->tab, h->total_lines, h->counters.get()));
     const size_t mb = h->max_batch;
     const uint32_t stiles = (uint32_t)((mb + SORT_TILE - 1) / SORT_TILE);
     {
@@ -1066,39 +1069,33 @@ int32_t gcra_create(const gcra_config *cfg, gcra_engine **out) {
         if (const char *g = getenv("GCRA_CTAS_PROBE")) { uint32_t c = (uint32_t)atoi(g) * sms; if (c) for (auto &x : h->grid_probe) x = std::min(x, c); }
         if (const char *g = getenv("GCRA_CTAS_DECIDE")) { uint32_t c = (uint32_t)atoi(g) * sms; if (c) for (auto &x : h->grid_decide) x = std::min(x, c); }
     }
-    bool ok = cudaMalloc(&h->d_req, mb * sizeof(gcra_request)) == cudaSuccess &&
-              cudaMalloc(&h->d_res, mb * sizeof(gcra_result)) == cudaSuccess &&
-              cudaMalloc(&h->route_counts, (size_t)ROUTE_MAX_SHARDS * ((mb + TILE_THREADS - 1) / TILE_THREADS) * sizeof(u32)) == cudaSuccess &&
-              cudaMalloc(&h->d_op, 2 * sizeof(StoreOpResult)) == cudaSuccess &&
-              cudaMallocHost(&h->h_op, 2 * sizeof(StoreOpResult)) == cudaSuccess &&
-              cudaMallocHost(&h->h_counters, C_COUNT * sizeof(u64)) == cudaSuccess &&
-              cudaMallocHost(&h->h_snap, (size_t)gcra_engine::N_SNAP * C_COUNT * sizeof(u64)) == cudaSuccess;
-    for (int k = 0; k < gcra_engine::N_SCR && ok; k++) {
-        Scratch &sc = h->scr[k];
-        ok = cudaMalloc(&sc.drec, mb * sizeof(Req)) == cudaSuccess &&
-             cudaMalloc(&sc.keys_a, mb * sizeof(u64)) == cudaSuccess &&
-             cudaMalloc(&sc.keys_b, mb * sizeof(u64)) == cudaSuccess &&
-             cudaMalloc(&sc.hist, (size_t)SORT_MAX_DIGITS * stiles * sizeof(u32)) == cudaSuccess &&
-             cudaMalloc(&sc.tot, SORT_MAX_DIGITS * sizeof(u32)) == cudaSuccess &&
-             cudaMalloc(&sc.long_runs, (mb / LONG_RUN_MIN + 1) * sizeof(LongRun)) == cudaSuccess &&
-             cudaMalloc(&sc.giant_runs, (mb / GIANT_RUN_MIN + 1) * sizeof(LongRun)) == cudaSuccess &&
-             cudaMalloc(&sc.long_count, 2 * sizeof(u32)) == cudaSuccess &&
-             cudaEventCreateWithFlags(&sc.ev_front, cudaEventDisableTiming) == cudaSuccess &&
-             cudaEventCreateWithFlags(&sc.ev_back, cudaEventDisableTiming) == cudaSuccess &&
-             cudaEventCreateWithFlags(&sc.ev_mid, cudaEventDisableTiming) == cudaSuccess &&
-             cudaEventCreateWithFlags(&sc.ev_fork, cudaEventDisableTiming) == cudaSuccess &&
-             cudaEventCreateWithFlags(&sc.ev_join, cudaEventDisableTiming) == cudaSuccess &&
-             cudaEventCreateWithFlags(&sc.ev_join2, cudaEventDisableTiming) == cudaSuccess;
-        ok = ok && alloc_index_scratch(h, sc, h->max_batch) == GCRA_OK;
+    CK(h->d_req.make(mb));
+    CK(h->d_res.make(mb));
+    CK(h->route_counts.make((size_t)ROUTE_MAX_SHARDS * ((mb + TILE_THREADS - 1) / TILE_THREADS)));
+    CK(h->d_op.make(2));
+    CK(h->h_op.make(2));
+    CK(h->h_counters.make(C_COUNT));
+    CK(h->h_snap.make((size_t)gcra_engine::N_SNAP * C_COUNT));
+    for (Scratch &sc : h->scr) {
+        CK(sc.drec.make(mb));
+        CK(sc.keys_a.make(mb));
+        CK(sc.keys_b.make(mb));
+        CK(sc.hist.make((size_t)SORT_MAX_DIGITS * stiles));
+        CK(sc.tot.make(SORT_MAX_DIGITS));
+        CK(sc.long_runs.make(mb / LONG_RUN_MIN + 1));
+        CK(sc.giant_runs.make(mb / GIANT_RUN_MIN + 1));
+        CK(sc.long_count.make(2));
+        for (Event *e : {&sc.ev_front, &sc.ev_back, &sc.ev_mid, &sc.ev_fork, &sc.ev_join})
+            CK(e->make(cudaEventDisableTiming));
+        CK(sc.h_nres.make(1));
+        *sc.h_nres.get() = 0;
+        CK(sc.bitmap.make(h->bm_words));
+        CK(sc.pend.make(h->pend_words));
+        CK(cudaMemsetAsync(sc.bitmap.get(), 0, h->bm_words * sizeof(u32), h->stream.get()));   // from then on cleared after every use
+        CK(cudaMemsetAsync(sc.pend.get(), 0, h->pend_words * sizeof(u32), h->stream.get()));
     }
-    if (!ok) return fail("scratch allocation", cudaGetLastError());
-    memset(h->h_counters, 0, C_COUNT * sizeof(u64));
-    cudaEventCreateWithFlags(&h->ev_counters, cudaEventDisableTiming);
-    for (int i = 0; i < gcra_engine::N_SNAP; i++) cudaEventCreateWithFlags(&h->ev_snap[i], cudaEventDisableTiming);
-    for (int i = 0; i < 4; i++) cudaEventCreate(&h->ev[i]);
-    for (int i = 0; i < 8; i++) cudaEventCreate(&h->evd[i]);
-    cudaEventCreate(&h->ev_sweep[0]);
-    cudaEventCreate(&h->ev_sweep[1]);
+    RC(alloc_index_scratch(h, h->max_batch));
+    memset(h->h_counters.get(), 0, C_COUNT * sizeof(u64));
     // store policy, defaults as in the reference constructors
     h->kind = cfg->store_kind;
     __int128 created = cfg->created_ns;
@@ -1115,61 +1112,27 @@ int32_t gcra_create(const gcra_config *cfg, gcra_engine **out) {
         h->next_cleanup = created + 5 * NS_PER_S;
     }
     preload_kernels();
-    if ((e = cudaStreamSynchronize(h->stream)) != cudaSuccess) return fail("init", e);
-    *out = h;
+    CK(cudaStreamSynchronize(h->stream.get()));
     return GCRA_OK;
 }
 
+int32_t gcra_create(const gcra_config *cfg, gcra_engine **out) {
+    if (!cfg || !out) return GCRA_INTERNAL;
+    *out = nullptr;
+    std::unique_ptr<gcra_engine> h(new gcra_engine());
+    if (init_engine(h.get(), cfg) != GCRA_OK) {
+        fprintf(stderr, "gcra_create: %s\n", h->err.c_str());
+        return GCRA_INTERNAL;
+    }
+    *out = h.release();
+    return GCRA_OK;
+}
+
+// the synchronize comes first: no member is released under work still running
 void gcra_destroy(gcra_engine *h) {
     if (!h) return;
     cudaSetDevice(h->device);
     cudaDeviceSynchronize();
-    if (h->shard) {
-        Shard *sh = h->shard;
-        for (auto &sl : sh->slots) {
-            cudaFree(sl.routed); cudaFree(sl.recv_req); cudaFree(sl.recv_res); cudaFree(sl.back_res); cudaFree(sl.src_index);
-            cudaFree(sl.counts_dev); cudaFreeHost(sl.counts_host);
-            cudaEventDestroy(sl.ev_ready); cudaEventDestroy(sl.ev_counts); cudaEventDestroy(sl.ev_routed); cudaEventDestroy(sl.ev_done);
-        }
-        if (nccl_rt::g_api.CommDestroy) { nccl_rt::g_api.CommDestroy(sh->comm_counts); nccl_rt::g_api.CommDestroy(sh->comm_req); nccl_rt::g_api.CommDestroy(sh->comm_res); }
-        cudaStreamDestroy(sh->s_part); cudaStreamDestroy(sh->s_route); cudaStreamDestroy(sh->s_return); cudaEventDestroy(sh->ev_tmp);
-        delete sh;
-    }
-    if (h->p2p) {
-        P2P *p = h->p2p;
-        for (int r = 0; r < p->world; r++) if (p->opened[r]) cudaIpcCloseMemHandle(p->peer_base[r]);
-        for (auto &sl : p->slots) {
-            cudaFree(sl.res_loc); cudaFree(sl.counts_dev); cudaFree(sl.segs_dev);
-            cudaEventDestroy(sl.ev_ready); cudaEventDestroy(sl.ev_wait); cudaEventDestroy(sl.ev_done);
-        }
-        for (auto &e : p->ev_t) cudaEventDestroy(e);
-        cudaFree(p->peers_dev); cudaFree(p->tile_counts); cudaFree(p->window);
-        cudaStreamDestroy(p->s_part); cudaStreamDestroy(p->s_wait); cudaStreamDestroy(p->s_sig); cudaStreamDestroy(p->s_return);
-        delete p;
-    }
-    for (auto &s : h->ring) {
-        cudaFreeHost(s.h_req); cudaFreeHost(s.h_res); cudaFree(s.d_req); cudaFree(s.d_res);
-        cudaEventDestroy(s.ev_in); cudaEventDestroy(s.ev_comp); cudaEventDestroy(s.ev_done);
-    }
-    cudaFree(h->tab.keys); cudaFree(h->tab.state); cudaFree(h->tab.ei); cudaFree(h->tab.mark); cudaFree(h->tab.counters);
-    for (auto &sc : h->scr) {
-        cudaFree(sc.drec); cudaFree(sc.keys_a); cudaFree(sc.keys_b); cudaFree(sc.hist); cudaFree(sc.tot);
-        cudaFree(sc.long_runs); cudaFree(sc.giant_runs); cudaFree(sc.long_count);
-        cudaFree(sc.slot_arr); cudaFree(sc.flags); cudaFree(sc.bitmap); cudaFree(sc.pend); cudaFree(sc.ctrl_block);
-        cudaFreeHost(sc.h_nres);
-        cudaEventDestroy(sc.ev_front); cudaEventDestroy(sc.ev_mid); cudaEventDestroy(sc.ev_back); cudaEventDestroy(sc.ev_fork); cudaEventDestroy(sc.ev_join); cudaEventDestroy(sc.ev_join2);
-    }
-    cudaFree(h->denied.keys); cudaFree(h->denied.counts); cudaFree(h->denied.dropped);
-    cudaFree(h->d_req); cudaFree(h->d_res); cudaFree(h->route_counts); cudaFree(h->d_pol); cudaFree(h->d_op);
-    cudaFreeHost(h->h_op); cudaFreeHost(h->h_counters); cudaFreeHost(h->h_snap);
-    for (int i = 0; i < gcra_engine::N_SNAP; i++) cudaEventDestroy(h->ev_snap[i]);
-    cudaEventDestroy(h->ev_counters);
-    for (int i = 0; i < 4; i++) cudaEventDestroy(h->ev[i]);
-    for (int i = 0; i < 8; i++) cudaEventDestroy(h->evd[i]);
-    cudaEventDestroy(h->ev_sweep[0]); cudaEventDestroy(h->ev_sweep[1]);
-    cudaStreamDestroy(h->stream); cudaStreamDestroy(h->in_stream); cudaStreamDestroy(h->out_stream); cudaStreamDestroy(h->aux_stream); cudaStreamDestroy(h->aux2_stream);
-    cudaStreamDestroy(h->front_stream[0]);
-    cudaStreamDestroy(h->back_stream); cudaStreamDestroy(h->tail_stream); cudaEventDestroy(h->ev_ready);
     delete h;
 }
 
@@ -1259,11 +1222,11 @@ static int store_op(gcra_engine *h, int op, uint64_t key_hash, int64_t a, int64_
     if (op == 2) { int rc = ensure_room(h, 1); if (rc) return rc; }
     // a Store-trait call reads / writes a slot's state: after every batch still in flight on the engine's or a
     // caller's stream (launch_batch orders itself the same way)
-    for (auto &o : h->scr) if (o.back_recorded) CK(cudaStreamWaitEvent(h->stream, o.ev_back, 0));
-    store_op_kernel<<<1, 1, 0, h->stream>>>(h->tab, op, stored_key(key_hash), a, b, ttl, now, h->d_op);
+    for (auto &o : h->scr) if (o.back_recorded) CK(cudaStreamWaitEvent(h->stream.get(), o.ev_back.get(), 0));
+    store_op_kernel<<<1, 1, 0, h->stream.get()>>>(h->tab, op, stored_key(key_hash), a, b, ttl, now, h->d_op.get());
     h->launches++;
-    CK(cudaMemcpyAsync(h->h_op, h->d_op, 2 * sizeof(StoreOpResult), cudaMemcpyDeviceToHost, h->stream));
-    CK(cudaStreamSynchronize(h->stream));
+    CK(cudaMemcpyAsync(h->h_op.get(), h->d_op.get(), 2 * sizeof(StoreOpResult), cudaMemcpyDeviceToHost, h->stream.get()));
+    CK(cudaStreamSynchronize(h->stream.get()));
     return GCRA_OK;
 }
 
@@ -1278,8 +1241,8 @@ int32_t gcra_store_get(gcra_engine *h, const void *key, uint64_t len, int64_t no
                        uint8_t *found) {
     int rc = store_op(h, 0, engine_hash(h, key, len), 0, 0, 0, now_ns);
     if (rc) return rc;
-    if (found) *found = (uint8_t)h->h_op[0].flag;
-    if (value) *value = h->h_op[0].value;
+    if (found) *found = (uint8_t)h->h_op.get()[0].flag;
+    if (value) *value = h->h_op.get()[0].value;
     return GCRA_OK;
 }
 
@@ -1289,7 +1252,7 @@ int32_t gcra_store_cas(gcra_engine *h, const void *key, uint64_t len, int64_t ol
     if (rc) return rc;
     rc = store_op(h, 1, engine_hash(h, key, len), old_value, new_value, ttl_ns, now_ns);
     if (rc) return rc;
-    if (swapped) *swapped = (uint8_t)h->h_op[0].flag;
+    if (swapped) *swapped = (uint8_t)h->h_op.get()[0].flag;
     return GCRA_OK;
 }
 
@@ -1299,27 +1262,27 @@ int32_t gcra_store_set_nx(gcra_engine *h, const void *key, uint64_t len, int64_t
     if (rc) return rc;
     rc = store_op(h, 2, engine_hash(h, key, len), value, 0, ttl_ns, now_ns);
     if (rc) return rc;
-    if (h->h_op[0].status) { h->err = "table full"; return GCRA_INTERNAL; }
-    if (stored) *stored = (uint8_t)h->h_op[0].flag;
+    if (h->h_op.get()[0].status) { h->err = "table full"; return GCRA_INTERNAL; }
+    if (stored) *stored = (uint8_t)h->h_op.get()[0].flag;
     return GCRA_OK;
 }
 
 int32_t gcra_rate_limit_batch_device(gcra_engine *h, uint64_t n, const gcra_request *d_req, gcra_result *d_res,
                                      void *stream) {
     CK(cudaSetDevice(h->device));
-    return launch_batch(h, (uint32_t)n, d_req, FMT_48_32, 0, d_res, stream ? (cudaStream_t)stream : h->stream, true);
+    return launch_batch(h, (uint32_t)n, d_req, FMT_48_32, 0, d_res, stream ? (cudaStream_t)stream : h->stream.get(), true);
 }
 
 int32_t gcra_rate_limit_batch16_device(gcra_engine *h, uint64_t n, const gcra_request16 *d_req, int64_t now_ns,
                                        gcra_result *d_res, void *stream) {
     CK(cudaSetDevice(h->device));
-    return launch_batch(h, (uint32_t)n, d_req, FMT_16_32, now_ns, d_res, stream ? (cudaStream_t)stream : h->stream, true);
+    return launch_batch(h, (uint32_t)n, d_req, FMT_16_32, now_ns, d_res, stream ? (cudaStream_t)stream : h->stream.get(), true);
 }
 
 int32_t gcra_rate_limit_batch16_r16_device(gcra_engine *h, uint64_t n, const gcra_request16 *d_req, int64_t now_ns,
                                            gcra_result16 *d_res, void *stream) {
     CK(cudaSetDevice(h->device));
-    return launch_batch(h, (uint32_t)n, d_req, FMT_16_16, now_ns, d_res, stream ? (cudaStream_t)stream : h->stream, true);
+    return launch_batch(h, (uint32_t)n, d_req, FMT_16_16, now_ns, d_res, stream ? (cudaStream_t)stream : h->stream.get(), true);
 }
 
 int32_t gcra_rate_limit_batch_device_pipelined(gcra_engine *h, uint64_t n, const gcra_request *d_req,
@@ -1327,8 +1290,8 @@ int32_t gcra_rate_limit_batch_device_pipelined(gcra_engine *h, uint64_t n, const
     CK(cudaSetDevice(h->device));
     cudaEvent_t ready = nullptr;
     if (ready_stream) {
-        CK(cudaEventRecord(h->ev_ready, (cudaStream_t)ready_stream));
-        ready = h->ev_ready;
+        CK(cudaEventRecord(h->ev_ready.get(), (cudaStream_t)ready_stream));
+        ready = h->ev_ready.get();
     }
     return launch_pipelined(h, (uint32_t)n, d_req, FMT_48_32, 0, d_res, ready, nullptr);
 }
@@ -1337,8 +1300,8 @@ int32_t gcra_pipeline_join(gcra_engine *h, void *stream) {
     CK(cudaSetDevice(h->device));
     for (auto &o : h->scr) {
         if (!o.back_recorded) continue;
-        if (stream) CK(cudaStreamWaitEvent((cudaStream_t)stream, o.ev_back, 0));
-        else CK(cudaEventSynchronize(o.ev_back));
+        if (stream) CK(cudaStreamWaitEvent((cudaStream_t)stream, o.ev_back.get(), 0));
+        else CK(cudaEventSynchronize(o.ev_back.get()));
     }
     return GCRA_OK;
 }
@@ -1357,12 +1320,12 @@ static int host_batch(gcra_engine *h, uint64_t n, const void *req, int fmt, int6
         int64_t now_hint = compact ? now_batch : ((const gcra_request *)req)[done].now_ns;
         int rc = apply_policy(h, now_hint);
         if (rc) return rc;
-        CK(cudaMemcpyAsync(h->d_req, src, (size_t)m * rsz, cudaMemcpyHostToDevice, h->stream));
-        rc = launch_batch(h, m, h->d_req, fmt, now_batch, h->d_res, h->stream, true);
+        CK(cudaMemcpyAsync(h->d_req.get(), src, (size_t)m * rsz, cudaMemcpyHostToDevice, h->stream.get()));
+        rc = launch_batch(h, m, h->d_req.get(), fmt, now_batch, h->d_res.get(), h->stream.get(), true);
         if (rc) return rc;
-        CK(cudaMemcpyAsync((unsigned char *)res + done * ressz, h->d_res, (size_t)m * ressz, cudaMemcpyDeviceToHost, h->stream));
+        CK(cudaMemcpyAsync((unsigned char *)res + done * ressz, h->d_res.get(), (size_t)m * ressz, cudaMemcpyDeviceToHost, h->stream.get()));
         RC(refresh_counters(h, false));
-        CK(cudaStreamSynchronize(h->stream));
+        CK(cudaStreamSynchronize(h->stream.get()));
         done += m;
     }
     return GCRA_OK;
@@ -1408,15 +1371,14 @@ static std::vector<PolicyDerived> derive_policies(uint32_t n, const gcra_policy 
 int32_t gcra_set_policies(gcra_engine *h, uint32_t n, const gcra_policy *policies) {
     CK(cudaSetDevice(h->device));
     std::vector<PolicyDerived> pd = derive_policies(n, policies);
-    CK(cudaStreamSynchronize(h->stream));
-    cudaFree(h->d_pol);
-    h->d_pol = nullptr;
-    h->npol = 0;
+    CK(cudaStreamSynchronize(h->stream.get()));
+    DevBuf<PolicyDerived> d_pol;      // (a failed call keeps the registered table)
     if (n) {
-        CK(cudaMalloc(&h->d_pol, n * sizeof(PolicyDerived)));
-        CK(cudaMemcpy(h->d_pol, pd.data(), n * sizeof(PolicyDerived), cudaMemcpyHostToDevice));
-        h->npol = n;
+        CK(d_pol.make(n));
+        CK(cudaMemcpy(d_pol.get(), pd.data(), n * sizeof(PolicyDerived), cudaMemcpyHostToDevice));
     }
+    h->d_pol = std::move(d_pol);
+    h->npol = n;
     return GCRA_OK;
 }
 
@@ -1456,32 +1418,32 @@ int32_t gcra_ring_create(gcra_engine *h, uint32_t slots, uint32_t slot_capacity,
     CK(cudaSetDevice(h->device));
     if (!h->ring.empty()) { h->err = "ring already created"; return GCRA_INTERNAL; }
     if (slot_capacity == 0 || slot_capacity > h->max_batch) { h->err = "slot_capacity must be in 1..max_batch"; return GCRA_INTERNAL; }
-    h->ring_cap = slot_capacity;
     // 0: 48-byte requests, 32-byte results; any other value but 2: 16-byte requests, 32-byte results; 2: 16 / 16
-    h->ring_mode = mode == 0 ? FMT_48_32 : mode == 2 ? FMT_16_16 : FMT_16_32;
-    const size_t rsz = h->ring_mode != FMT_48_32 ? sizeof(gcra_request16) : sizeof(gcra_request);
-    const size_t ressz = h->ring_mode == FMT_16_16 ? sizeof(gcra_result16) : sizeof(gcra_result);
-    h->ring.resize(slots);
-    for (auto &s : h->ring) {
+    const int fmt = mode == 0 ? FMT_48_32 : mode == 2 ? FMT_16_16 : FMT_16_32;
+    const size_t rsz = fmt != FMT_48_32 ? sizeof(gcra_request16) : sizeof(gcra_request);
+    const size_t ressz = fmt == FMT_16_16 ? sizeof(gcra_result16) : sizeof(gcra_result);
+    std::vector<RingSlot> ring(slots);    // (a failed call leaves no ring)
+    for (auto &s : ring) {
         // request slots are only WRITTEN by the host: optionally write-combined pinned memory (GCRA_RING_WC=1)
-        CK(cudaHostAlloc(&s.h_req, slot_capacity * rsz,
-                         getenv("GCRA_RING_WC") && atoi(getenv("GCRA_RING_WC")) ? cudaHostAllocWriteCombined : cudaHostAllocDefault));
-        CK(cudaMallocHost(&s.h_res, slot_capacity * ressz));
-        CK(cudaMalloc(&s.d_req, slot_capacity * rsz));
-        CK(cudaMalloc(&s.d_res, slot_capacity * ressz));
-        CK(cudaEventCreateWithFlags(&s.ev_in, cudaEventDisableTiming));
-        CK(cudaEventCreateWithFlags(&s.ev_comp, cudaEventDisableTiming));
-        CK(cudaEventCreateWithFlags(&s.ev_done, cudaEventDisableTiming));
+        CK(s.h_req.make(slot_capacity * rsz,
+                        getenv("GCRA_RING_WC") && atoi(getenv("GCRA_RING_WC")) ? cudaHostAllocWriteCombined : cudaHostAllocDefault));
+        CK(s.h_res.make(slot_capacity * ressz));
+        CK(s.d_req.make(slot_capacity * rsz));
+        CK(s.d_res.make(slot_capacity * ressz));
+        for (Event *e : {&s.ev_in, &s.ev_done}) CK(e->make(cudaEventDisableTiming));
     }
+    h->ring = std::move(ring);
+    h->ring_cap = slot_capacity;
+    h->ring_mode = fmt;
     return GCRA_OK;
 }
 
-void *gcra_ring_requests(gcra_engine *h, uint32_t slot) { return slot < h->ring.size() ? h->ring[slot].h_req : nullptr; }
+void *gcra_ring_requests(gcra_engine *h, uint32_t slot) { return slot < h->ring.size() ? h->ring[slot].h_req.get() : nullptr; }
 gcra_result *gcra_ring_results(gcra_engine *h, uint32_t slot) {
-    return slot < h->ring.size() && h->ring_mode != FMT_16_16 ? (gcra_result *)h->ring[slot].h_res : nullptr;
+    return slot < h->ring.size() && h->ring_mode != FMT_16_16 ? (gcra_result *)h->ring[slot].h_res.get() : nullptr;
 }
 gcra_result16 *gcra_ring_results16(gcra_engine *h, uint32_t slot) {
-    return slot < h->ring.size() && h->ring_mode == FMT_16_16 ? (gcra_result16 *)h->ring[slot].h_res : nullptr;
+    return slot < h->ring.size() && h->ring_mode == FMT_16_16 ? (gcra_result16 *)h->ring[slot].h_res.get() : nullptr;
 }
 
 int32_t gcra_ring_submit(gcra_engine *h, uint32_t slot, uint32_t n, int64_t now_ns) {
@@ -1490,20 +1452,20 @@ int32_t gcra_ring_submit(gcra_engine *h, uint32_t slot, uint32_t n, int64_t now_
     RingSlot &s = h->ring[slot];
     if (s.in_flight) { h->err = "ring slot still in flight"; return GCRA_INTERNAL; }
     // sweep policy with the counters of the batches finished so far (no stall)
-    if (cudaEventQuery(h->ev_counters) == cudaSuccess) { int rc = apply_policy(h, now_ns); if (rc) return rc; }
+    if (cudaEventQuery(h->ev_counters.get()) == cudaSuccess) { int rc = apply_policy(h, now_ns); if (rc) return rc; }
     const size_t rsz = h->ring_mode != FMT_48_32 ? sizeof(gcra_request16) : sizeof(gcra_request);
     const size_t ressz = h->ring_mode == FMT_16_16 ? sizeof(gcra_result16) : sizeof(gcra_result);
-    CK(cudaMemcpyAsync(s.d_req, s.h_req, (size_t)n * rsz, cudaMemcpyHostToDevice, h->in_stream));
-    CK(cudaEventRecord(s.ev_in, h->in_stream));
+    CK(cudaMemcpyAsync(s.d_req.get(), s.h_req.get(), (size_t)n * rsz, cudaMemcpyHostToDevice, h->in_stream.get()));
+    CK(cudaEventRecord(s.ev_in.get(), h->in_stream.get()));
     // front half (ingest + order) of this slot overlaps the back half (decide) of the previous one
     cudaEvent_t done = nullptr;
-    int rc = launch_pipelined(h, n, s.d_req, h->ring_mode, now_ns, s.d_res, s.ev_in, &done);
+    int rc = launch_pipelined(h, n, s.d_req.get(), h->ring_mode, now_ns, s.d_res.get(), s.ev_in.get(), &done);
     if (rc) return rc;
-    if (done) CK(cudaStreamWaitEvent(h->out_stream, done, 0));
-    CK(cudaMemcpyAsync(h->h_counters, h->tab.counters, C_COUNT * sizeof(u64), cudaMemcpyDeviceToHost, h->out_stream));
-    CK(cudaEventRecord(h->ev_counters, h->out_stream));
-    CK(cudaMemcpyAsync(s.h_res, s.d_res, (size_t)n * ressz, cudaMemcpyDeviceToHost, h->out_stream));
-    CK(cudaEventRecord(s.ev_done, h->out_stream));
+    if (done) CK(cudaStreamWaitEvent(h->out_stream.get(), done, 0));
+    CK(cudaMemcpyAsync(h->h_counters.get(), h->tab.counters, C_COUNT * sizeof(u64), cudaMemcpyDeviceToHost, h->out_stream.get()));
+    CK(cudaEventRecord(h->ev_counters.get(), h->out_stream.get()));
+    CK(cudaMemcpyAsync(s.h_res.get(), s.d_res.get(), (size_t)n * ressz, cudaMemcpyDeviceToHost, h->out_stream.get()));
+    CK(cudaEventRecord(s.ev_done.get(), h->out_stream.get()));
     s.in_flight = true;
     return GCRA_OK;
 }
@@ -1512,7 +1474,7 @@ int32_t gcra_ring_wait(gcra_engine *h, uint32_t slot) {
     if (slot >= h->ring.size()) { h->err = "bad ring slot"; return GCRA_INTERNAL; }
     RingSlot &s = h->ring[slot];
     if (!s.in_flight) return GCRA_OK;
-    CK(cudaEventSynchronize(s.ev_done));
+    CK(cudaEventSynchronize(s.ev_done.get()));
     s.in_flight = false;
     return GCRA_OK;
 }
@@ -1521,7 +1483,7 @@ int32_t gcra_ring_poll(gcra_engine *h, uint32_t slot, int32_t *done) {
     if (slot >= h->ring.size()) { h->err = "bad ring slot"; return GCRA_INTERNAL; }
     RingSlot &s = h->ring[slot];
     if (!s.in_flight) { *done = 1; return GCRA_OK; }
-    cudaError_t e = cudaEventQuery(s.ev_done);
+    cudaError_t e = cudaEventQuery(s.ev_done.get());
     if (e == cudaSuccess) { s.in_flight = false; *done = 1; return GCRA_OK; }
     if (e == cudaErrorNotReady) { *done = 0; return GCRA_OK; }
     h->err = cudaGetErrorString(e);
@@ -1539,25 +1501,25 @@ int32_t gcra_policy_tick(gcra_engine *h, int64_t now_ns, uint64_t *swept) {
     CK(cudaSetDevice(h->device));
     if (swept) *swept = 0;
     if (h->kind == GCRA_STORE_MANUAL) return GCRA_OK;
-    for (auto &o : h->scr) if (o.back_recorded) CK(cudaEventSynchronize(o.ev_back));
+    for (auto &o : h->scr) if (o.back_recorded) CK(cudaEventSynchronize(o.ev_back.get()));
     RC(refresh_counters(h, true));
-    const uint64_t before = h->h_counters[C_SWEPT];
+    const uint64_t before = h->h_counters.get()[C_SWEPT];
     RC(apply_policy(h, now_ns));
-    if (swept) { RC(refresh_counters(h, true)); *swept = h->h_counters[C_SWEPT] - before; }
+    if (swept) { RC(refresh_counters(h, true)); *swept = h->h_counters.get()[C_SWEPT] - before; }
     return GCRA_OK;
 }
 
 uint64_t gcra_len(gcra_engine *h) {
     cudaSetDevice(h->device);
     if (refresh_counters(h, true)) return 0;
-    return h->h_counters[C_REAL];
+    return h->h_counters.get()[C_REAL];
 }
 
 int32_t gcra_get_stats(gcra_engine *h, gcra_stats *out) {
     CK(cudaSetDevice(h->device));
     int rc = refresh_counters(h, true);
     if (rc) return rc;
-    const u64 *c = h->h_counters;
+    const u64 *c = h->h_counters.get();
     out->len = c[C_REAL];
     out->occupied_slots = c[C_OCCUPIED];
     out->table_slots = (uint64_t)h->total_lines * 4;
@@ -1581,28 +1543,31 @@ int32_t gcra_get_stats(gcra_engine *h, gcra_stats *out) {
 int32_t gcra_peek(gcra_engine *h, uint64_t key_hash, int64_t *tat, int64_t *expiry_ns, uint8_t *found) {
     int rc = store_op(h, 3, key_hash, 0, 0, 0, 0);
     if (rc) return rc;
-    *found = (uint8_t)h->h_op[0].flag;
-    if (*found) { *tat = h->h_op[0].value; *expiry_ns = h->h_op[1].value; }
+    *found = (uint8_t)h->h_op.get()[0].flag;
+    if (*found) { *tat = h->h_op.get()[0].value; *expiry_ns = h->h_op.get()[1].value; }
     return GCRA_OK;
 }
 
 // ---- metrics bridge: top denied keys (throttlecrab-server/src/metrics.rs:24-64,162-173) --------------------------
 int32_t gcra_track_denied(gcra_engine *h, uint32_t max_keys) {
     CK(cudaSetDevice(h->device));
+    // the table holds 16 entries per tracked key: at most 2^31
+    if (max_keys > (1u << 27)) { h->err = "track_denied: max_keys must be at most 2^27"; return GCRA_INTERNAL; }
     CK(cudaDeviceSynchronize());
-    cudaFree(h->denied.keys); cudaFree(h->denied.counts); cudaFree(h->denied.dropped);
-    h->denied = DeniedTable{};
+    DeniedArrays a;
+    const uint64_t cap = max_keys ? 1ULL << ceil_log2(std::max<uint64_t>(16ULL * max_keys, 1024)) : 0;
+    if (max_keys) {
+        CK(a.keys.make(cap));
+        CK(a.counts.make(cap));
+        CK(a.dropped.make(1));
+        CK(cudaMemset(a.keys.get(), 0, cap * sizeof(u64)));
+        CK(cudaMemset(a.counts.get(), 0, cap * sizeof(u64)));
+        CK(cudaMemset(a.dropped.get(), 0, sizeof(u64)));
+    }
+    h->denied = max_keys ? DeniedTable{a.keys.get(), a.counts.get(), (u32)(cap - 1), a.dropped.get()} : DeniedTable{};
+    h->denied_arrays = std::move(a);
     h->denied_max = max_keys;
-    h->denied_cap = 0;
-    if (!max_keys) return GCRA_OK;
-    h->denied_cap = 1u << ceil_log2(std::max<uint64_t>(16ULL * max_keys, 1024));
-    CK(cudaMalloc(&h->denied.keys, (size_t)h->denied_cap * sizeof(u64)));
-    CK(cudaMalloc(&h->denied.counts, (size_t)h->denied_cap * sizeof(u64)));
-    CK(cudaMalloc(&h->denied.dropped, sizeof(u64)));
-    CK(cudaMemset(h->denied.keys, 0, (size_t)h->denied_cap * sizeof(u64)));
-    CK(cudaMemset(h->denied.counts, 0, (size_t)h->denied_cap * sizeof(u64)));
-    CK(cudaMemset(h->denied.dropped, 0, sizeof(u64)));
-    h->denied.mask = h->denied_cap - 1;
+    h->denied_cap = cap;
     return GCRA_OK;
 }
 
@@ -1613,7 +1578,7 @@ int32_t gcra_top_denied(gcra_engine *h, uint32_t k, uint64_t *key_hashes, uint64
     CK(cudaSetDevice(h->device));
     if (n_out) *n_out = 0;
     if (!h->denied_max) { h->err = "gcra_track_denied first"; return GCRA_INTERNAL; }
-    for (auto &o : h->scr) if (o.back_recorded) CK(cudaEventSynchronize(o.ev_back));
+    for (auto &o : h->scr) if (o.back_recorded) CK(cudaEventSynchronize(o.ev_back.get()));
     std::vector<u64> keys(h->denied_cap), cnts(h->denied_cap);
     CK(cudaMemcpy(keys.data(), h->denied.keys, keys.size() * sizeof(u64), cudaMemcpyDeviceToHost));
     CK(cudaMemcpy(cnts.data(), h->denied.counts, cnts.size() * sizeof(u64), cudaMemcpyDeviceToHost));
@@ -1643,31 +1608,31 @@ int32_t gcra_top_denied(gcra_engine *h, uint32_t k, uint64_t *key_hashes, uint64
 
 int32_t gcra_sync(gcra_engine *h) {
     CK(cudaSetDevice(h->device));
-    CK(cudaStreamSynchronize(h->in_stream));
-    CK(cudaStreamSynchronize(h->front_stream[0]));
-    CK(cudaStreamSynchronize(h->back_stream));
-    CK(cudaStreamSynchronize(h->tail_stream));
-    CK(cudaStreamSynchronize(h->aux_stream));
-    CK(cudaStreamSynchronize(h->aux2_stream));
-    CK(cudaStreamSynchronize(h->stream));
-    CK(cudaStreamSynchronize(h->out_stream));
+    CK(cudaStreamSynchronize(h->in_stream.get()));
+    CK(cudaStreamSynchronize(h->front_stream.get()));
+    CK(cudaStreamSynchronize(h->back_stream.get()));
+    CK(cudaStreamSynchronize(h->tail_stream.get()));
+    CK(cudaStreamSynchronize(h->aux_stream.get()));
+    CK(cudaStreamSynchronize(h->aux2_stream.get()));
+    CK(cudaStreamSynchronize(h->stream.get()));
+    CK(cudaStreamSynchronize(h->out_stream.get()));
     return GCRA_OK;
 }
 
 int32_t gcra_last_kernel_ms(gcra_engine *h, float out[4]) {
     if (!h->ev_valid) { h->err = "no timed batch yet"; return GCRA_INTERNAL; }
-    CK(cudaEventSynchronize(h->ev[3]));
-    CK(cudaEventElapsedTime(&out[0], h->ev[0], h->ev[3]));
-    CK(cudaEventElapsedTime(&out[1], h->ev[0], h->ev[1]));
-    CK(cudaEventElapsedTime(&out[2], h->ev[1], h->ev[2]));
-    CK(cudaEventElapsedTime(&out[3], h->ev[2], h->ev[3]));
+    CK(cudaEventSynchronize(h->ev[3].get()));
+    CK(cudaEventElapsedTime(&out[0], h->ev[0].get(), h->ev[3].get()));
+    CK(cudaEventElapsedTime(&out[1], h->ev[0].get(), h->ev[1].get()));
+    CK(cudaEventElapsedTime(&out[2], h->ev[1].get(), h->ev[2].get()));
+    CK(cudaEventElapsedTime(&out[3], h->ev[2].get(), h->ev[3].get()));
     return GCRA_OK;
 }
 
 int32_t gcra_last_kernel_ms_detail(gcra_engine *h, float out[7]) {
     if (!h->evd_valid) { h->err = "no timed index-order batch yet"; return GCRA_INTERNAL; }
-    CK(cudaEventSynchronize(h->evd[7]));
-    for (int i = 0; i < 7; i++) CK(cudaEventElapsedTime(&out[i], h->evd[i], h->evd[i + 1]));
+    CK(cudaEventSynchronize(h->evd[7].get()));
+    for (int i = 0; i < 7; i++) CK(cudaEventElapsedTime(&out[i], h->evd[i].get(), h->evd[i + 1].get()));
     return GCRA_OK;
 }
 
@@ -1675,8 +1640,8 @@ void gcra_debug_set(gcra_engine *h, uint32_t mask) { h->dbg = mask; }
 
 int32_t gcra_last_sweep_ms(gcra_engine *h, float *ms) {
     if (!h->sweep_timed) { h->err = "no sweep yet"; return GCRA_INTERNAL; }
-    CK(cudaEventSynchronize(h->ev_sweep[1]));
-    CK(cudaEventElapsedTime(ms, h->ev_sweep[0], h->ev_sweep[1]));
+    CK(cudaEventSynchronize(h->ev_sweep[1].get()));
+    CK(cudaEventElapsedTime(ms, h->ev_sweep[0].get(), h->ev_sweep[1].get()));
     return GCRA_OK;
 }
 
@@ -1751,12 +1716,13 @@ int32_t gcra_snapshot_load(gcra_engine *h, const char *path) {
         if (tl != hd.total_lines || nb != hd.nb_main || ss != hd.stash_slots) {
             fclose(f); h->err = "snapshot: geometry not reproducible with this build/flags"; return GCRA_INTERNAL;
         }
+        TableArrays na;
         Table nt{};
         uint32_t nl = 0;
-        rc = alloc_table(h, hd.capacity, nt, nl, h->tab.counters);
+        rc = alloc_table(h, hd.capacity, na, nt, nl, h->tab.counters);
         if (rc) { fclose(f); return rc; }
-        CK(cudaStreamSynchronize(h->stream));
-        cudaFree(h->tab.keys); cudaFree(h->tab.state); cudaFree(h->tab.ei); cudaFree(h->tab.mark);
+        CK(cudaStreamSynchronize(h->stream.get()));
+        h->tab_arrays = std::move(na);
         h->tab = nt; h->total_lines = nl; h->capacity = hd.capacity;
     }
     std::vector<char> buf(SNAP_CHUNK);
@@ -1783,20 +1749,11 @@ namespace {
 const size_t RESTORE_CHUNK = SNAP_CHUNK / (sizeof(u64) + sizeof(TatOff) + sizeof(i64));
 
 struct RestoreBuffers {
-    char *host[2] = {};                // pinned: keys | state | ei of one chunk
-    char *dev[2] = {};
-    u64 *counts = nullptr;             // [RESTORE_COUNTS]
-    cudaEvent_t done[2] = {};          // the set's copy + kernel finished: its host buffer may be refilled
+    PinnedBuf<char> host[2];           // keys | state | ei of one chunk
+    DevBuf<char> dev[2];
+    DevBuf<u64> counts;                // [RESTORE_COUNTS]
+    Event done[2];                     // the set's copy + kernel finished: its host buffer may be refilled
     int fd = -1;
-    ~RestoreBuffers() {
-        for (int s = 0; s < 2; s++) {
-            if (done[s]) { cudaEventSynchronize(done[s]); cudaEventDestroy(done[s]); }
-            cudaFreeHost(host[s]);
-            cudaFree(dev[s]);
-        }
-        cudaFree(counts);
-        if (fd >= 0) close(fd);
-    }
 };
 }  // namespace
 
@@ -1815,38 +1772,31 @@ static int restore_pass(gcra_engine *h, RestoreBuffers &b, uint64_t slots, uint3
     for (uint64_t first = 0, c = 0; first < slots; first += RESTORE_CHUNK, c++) {
         const int s = (int)(c & 1);
         const uint64_t n = std::min<uint64_t>(RESTORE_CHUNK, slots - first);
-        char *hk = b.host[s], *hs = hk + RESTORE_CHUNK * sizeof(u64), *he = hs + RESTORE_CHUNK * sizeof(TatOff);
-        char *dk = b.dev[s], *ds = dk + RESTORE_CHUNK * sizeof(u64), *de = ds + RESTORE_CHUNK * sizeof(TatOff);
-        CK(cudaEventSynchronize(b.done[s]));
+        char *hk = b.host[s].get(), *hs = hk + RESTORE_CHUNK * sizeof(u64), *he = hs + RESTORE_CHUNK * sizeof(TatOff);
+        char *dk = b.dev[s].get(), *ds = dk + RESTORE_CHUNK * sizeof(u64), *de = ds + RESTORE_CHUNK * sizeof(TatOff);
+        CK(cudaEventSynchronize(b.done[s].get()));
         if (!pread_all(b.fd, hk, n * sizeof(u64), keys_off + first * sizeof(u64)) ||
             !pread_all(b.fd, hs, n * sizeof(TatOff), state_off + first * sizeof(TatOff)) ||
             (insert && !pread_all(b.fd, he, n * sizeof(i64), ei_off + first * sizeof(i64)))) {
             h->err = "snapshot restore: short read";
             return GCRA_INTERNAL;
         }
-        CK(cudaMemcpyAsync(dk, hk, n * sizeof(u64), cudaMemcpyHostToDevice, h->stream));
-        CK(cudaMemcpyAsync(ds, hs, n * sizeof(TatOff), cudaMemcpyHostToDevice, h->stream));
-        if (insert) CK(cudaMemcpyAsync(de, he, n * sizeof(i64), cudaMemcpyHostToDevice, h->stream));
+        CK(cudaMemcpyAsync(dk, hk, n * sizeof(u64), cudaMemcpyHostToDevice, h->stream.get()));
+        CK(cudaMemcpyAsync(ds, hs, n * sizeof(TatOff), cudaMemcpyHostToDevice, h->stream.get()));
+        if (insert) CK(cudaMemcpyAsync(de, he, n * sizeof(i64), cudaMemcpyHostToDevice, h->stream.get()));
         const uint32_t grid = (uint32_t)std::min<uint64_t>((n + TILE_THREADS - 1) / TILE_THREADS, 8 * h->sms);
-        (insert ? restore_kernel<true> : restore_kernel<false>)<<<grid, TILE_THREADS, 0, h->stream>>>(
-            h->tab, (const u64 *)dk, (const TatOff *)ds, (const i64 *)de, n, rank, world, b.counts);
+        (insert ? restore_kernel<true> : restore_kernel<false>)<<<grid, TILE_THREADS, 0, h->stream.get()>>>(
+            h->tab, (const u64 *)dk, (const TatOff *)ds, (const i64 *)de, n, rank, world, b.counts.get());
         h->launches++;
         CK(cudaGetLastError());
-        CK(cudaEventRecord(b.done[s], h->stream));
+        CK(cudaEventRecord(b.done[s].get(), h->stream.get()));
     }
-    CK(cudaStreamSynchronize(h->stream));
+    CK(cudaStreamSynchronize(h->stream.get()));
     return GCRA_OK;
 }
 
-int32_t gcra_snapshot_restore(gcra_engine *h, const char *path, uint32_t rank, uint32_t world, uint64_t *restored,
-                              uint64_t *conflicts) {
-    if (restored) *restored = 0;
-    if (conflicts) *conflicts = 0;
-    CK(cudaSetDevice(h->device));
-    if (world == 0 || rank >= world) { h->err = "snapshot restore: needs rank < world"; return GCRA_INTERNAL; }
-    RestoreBuffers b;
-    b.fd = open(path, O_RDONLY);
-    if (b.fd < 0) { h->err = std::string("snapshot restore: cannot open ") + path; return GCRA_INTERNAL; }
+static int restore_file(gcra_engine *h, RestoreBuffers &b, uint32_t rank, uint32_t world, uint64_t *restored,
+                        uint64_t *conflicts) {
     SnapshotHeader hd{};
     struct stat sb;
     if (fstat(b.fd, &sb) != 0 || !pread_all(b.fd, &hd, sizeof(hd), 0) || memcmp(hd.magic, SNAP_MAGIC, 8) != 0 ||
@@ -1862,26 +1812,26 @@ int32_t gcra_snapshot_restore(gcra_engine *h, const char *path, uint32_t rank, u
     }
     CK(cudaDeviceSynchronize());
     RC(refresh_counters(h, true));
-    const bool adopt_seed = h->h_counters[C_REAL] == 0;
+    const bool adopt_seed = h->h_counters.get()[C_REAL] == 0;
     if (!adopt_seed && (hd.hash_seed[0] != h->hash_seed[0] || hd.hash_seed[1] != h->hash_seed[1])) {
         h->err = "snapshot restore: the file's key-hash seed differs from that of the entries held";
         return GCRA_INTERNAL;
     }
     for (int s = 0; s < 2; s++) {
-        CK(cudaMallocHost(&b.host[s], SNAP_CHUNK));
-        CK(cudaMalloc(&b.dev[s], SNAP_CHUNK));
-        CK(cudaEventCreateWithFlags(&b.done[s], cudaEventDisableTiming));
+        CK(b.host[s].make(SNAP_CHUNK));
+        CK(b.dev[s].make(SNAP_CHUNK));
+        CK(b.done[s].make(cudaEventDisableTiming));
     }
-    CK(cudaMalloc(&b.counts, RESTORE_COUNTS * sizeof(u64)));
-    CK(cudaMemsetAsync(b.counts, 0, RESTORE_COUNTS * sizeof(u64), h->stream));
+    CK(b.counts.make(RESTORE_COUNTS));
+    CK(cudaMemsetAsync(b.counts.get(), 0, RESTORE_COUNTS * sizeof(u64), h->stream.get()));
     RC(restore_pass(h, b, slots, rank, world, false));
     u64 counts[RESTORE_COUNTS];
-    CK(cudaMemcpy(counts, b.counts, sizeof(counts), cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(counts, b.counts.get(), sizeof(counts), cudaMemcpyDeviceToHost));
     RC(ensure_room(h, counts[RESTORE_OWNED]));     // may purge or grow: h->tab is read after it
     RC(restore_pass(h, b, slots, rank, world, true));
-    CK(cudaMemcpy(counts, b.counts, sizeof(counts), cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(counts, b.counts.get(), sizeof(counts), cudaMemcpyDeviceToHost));
     RC(refresh_counters(h, true));
-    h->occupied_ub = h->h_counters[C_OCCUPIED];
+    h->occupied_ub = h->h_counters.get()[C_OCCUPIED];
     for (int i = 0; i < gcra_engine::N_SNAP; i++) h->snap_used[i] = false;
     if (counts[RESTORE_FAILED]) {
         h->err = "snapshot restore: table full (" + std::to_string(counts[RESTORE_FAILED]) + " entries not inserted)";
@@ -1891,6 +1841,22 @@ int32_t gcra_snapshot_restore(gcra_engine *h, const char *path, uint32_t rank, u
     if (restored) *restored = counts[RESTORE_INSERTED];
     if (conflicts) *conflicts = counts[RESTORE_CONFLICTS];
     return GCRA_OK;
+}
+
+int32_t gcra_snapshot_restore(gcra_engine *h, const char *path, uint32_t rank, uint32_t world, uint64_t *restored,
+                              uint64_t *conflicts) {
+    if (restored) *restored = 0;
+    if (conflicts) *conflicts = 0;
+    CK(cudaSetDevice(h->device));
+    if (world == 0 || rank >= world) { h->err = "snapshot restore: needs rank < world"; return GCRA_INTERNAL; }
+    RestoreBuffers b;
+    b.fd = open(path, O_RDONLY);
+    if (b.fd < 0) { h->err = std::string("snapshot restore: cannot open ") + path; return GCRA_INTERNAL; }
+    const int rc = restore_file(h, b, rank, world, restored, conflicts);
+    // copies still in flight read the pinned staging buffers: wait for them before `b` releases them
+    for (Event &e : b.done) if (e.get()) cudaEventSynchronize(e.get());
+    close(b.fd);
+    return rc;
 }
 
 
@@ -1917,40 +1883,35 @@ int32_t gcra_shard_init(gcra_engine *h, int32_t rank, int32_t world, const void 
     if (world < 1 || world > ROUTE_MAX_SHARDS || rank < 0 || rank >= world) { h->err = "bad rank / world"; return GCRA_INTERNAL; }
     if (max_rows == 0 || max_rows > h->max_batch) { h->err = "max_rows must be in 1..max_batch"; return GCRA_INTERNAL; }
     if (!nccl_rt::load()) { h->err = "libnccl.so.2 not found"; return GCRA_INTERNAL; }
-    Shard *sh = new Shard();
+    std::unique_ptr<Shard> sh(new Shard());    // (assigned to the engine only once complete)
     sh->rank = rank; sh->world = world; sh->max_rows = max_rows;
     const nccl_rt::UniqueId *ids = (const nccl_rt::UniqueId *)ids_3x128;
     // one communicator per stage: NCCL runs the operations of ONE communicator in issue order
-    NK(nccl_rt::g_api.CommInitRank(&sh->comm_counts, world, ids[0], rank));
-    NK(nccl_rt::g_api.CommInitRank(&sh->comm_req, world, ids[1], rank));
-    NK(nccl_rt::g_api.CommInitRank(&sh->comm_res, world, ids[2], rank));
-    CK(cudaStreamCreateWithFlags(&sh->s_part, cudaStreamNonBlocking));
-    CK(cudaStreamCreateWithFlags(&sh->s_route, cudaStreamNonBlocking));
-    CK(cudaStreamCreateWithFlags(&sh->s_return, cudaStreamNonBlocking));
-    CK(cudaEventCreateWithFlags(&sh->ev_tmp, cudaEventDisableTiming));
+    NK(sh->comm_counts.make(world, ids[0], rank));
+    NK(sh->comm_req.make(world, ids[1], rank));
+    NK(sh->comm_res.make(world, ids[2], rank));
+    for (Stream *s : {&sh->s_part, &sh->s_route, &sh->s_return}) CK(s->make());
+    CK(sh->ev_tmp.make(cudaEventDisableTiming));
     for (auto &sl : sh->slots) {
-        CK(cudaMalloc(&sl.routed, (size_t)max_rows * sizeof(gcra_request)));
+        CK(sl.routed.make(max_rows));
         // a shard can receive up to world x max_rows rows in one tick (every rank's whole tick): sized for that, so
         // no rank ever has to bail out of a tick its peers have already posted their sends for
-        CK(cudaMalloc(&sl.recv_req, (size_t)world * max_rows * sizeof(gcra_request)));
-        CK(cudaMalloc(&sl.recv_res, (size_t)world * max_rows * sizeof(gcra_result)));
-        CK(cudaMalloc(&sl.back_res, (size_t)max_rows * sizeof(gcra_result)));
-        CK(cudaMalloc(&sl.src_index, (size_t)max_rows * sizeof(u32)));
-        CK(cudaMalloc(&sl.counts_dev, 2 * ROUTE_MAX_SHARDS * sizeof(u32)));
-        CK(cudaMallocHost(&sl.counts_host, 2 * ROUTE_MAX_SHARDS * sizeof(u32)));
-        CK(cudaEventCreateWithFlags(&sl.ev_ready, cudaEventDisableTiming));
-        CK(cudaEventCreateWithFlags(&sl.ev_counts, cudaEventDisableTiming));
-        CK(cudaEventCreateWithFlags(&sl.ev_routed, cudaEventDisableTiming));
-        CK(cudaEventCreateWithFlags(&sl.ev_done, cudaEventDisableTiming));
+        CK(sl.recv_req.make((size_t)world * max_rows));
+        CK(sl.recv_res.make((size_t)world * max_rows));
+        CK(sl.back_res.make(max_rows));
+        CK(sl.src_index.make(max_rows));
+        CK(sl.counts_dev.make(2 * ROUTE_MAX_SHARDS));
+        CK(sl.counts_host.make(2 * ROUTE_MAX_SHARDS));
+        for (Event *e : {&sl.ev_ready, &sl.ev_counts, &sl.ev_routed, &sl.ev_done}) CK(e->make(cudaEventDisableTiming));
         sl.send.resize(world); sl.recv.resize(world); sl.send_off.resize(world); sl.recv_off.resize(world);
     }
-    h->shard = sh;
+    h->shard = std::move(sh);
     return GCRA_OK;
 }
 
 // stages 3+4 of a tick: the engine's kernels (pipelined inside the engine) and the way back
 static int shard_issue_decide_return(gcra_engine *h) {
-    Shard *sh = h->shard;
+    Shard *sh = h->shard.get();
     if (sh->pending < 0) return GCRA_OK;
     ShardSlot &sl = sh->slots[sh->pending];
     sh->pending = -1;
@@ -1960,31 +1921,31 @@ static int shard_issue_decide_return(gcra_engine *h) {
     for (uint32_t a = 0; a < sl.n_recv || a == 0; a += h->max_batch) {
         const uint32_t m = std::min<uint32_t>(sl.n_recv - a, h->max_batch);
         cudaEvent_t dn = nullptr;
-        RC(launch_pipelined(h, m, sl.recv_req + a, FMT_48_32, 0, sl.recv_res + a, sl.ev_routed, &dn));
-        if (dn) { done = dn; CK(cudaStreamWaitEvent(sh->s_return, dn, 0)); }
+        RC(launch_pipelined(h, m, sl.recv_req.get() + a, FMT_48_32, 0, sl.recv_res.get() + a, sl.ev_routed.get(), &dn));
+        if (dn) { done = dn; CK(cudaStreamWaitEvent(sh->s_return.get(), dn, 0)); }
         if (sl.n_recv == 0) break;
     }
-    if (!done) CK(cudaStreamWaitEvent(sh->s_return, sl.ev_routed, 0));
+    if (!done) CK(cudaStreamWaitEvent(sh->s_return.get(), sl.ev_routed.get(), 0));
     NK(nccl_rt::g_api.GroupStart());
     for (int p = 0; p < W; p++) {
         // results of the rows peer p sent me go back to p; my own rows' results arrive in partition order
-        NK(nccl_rt::g_api.Send(sl.recv_res + sl.recv_off[p], sl.recv[p] * sizeof(gcra_result), nccl_rt::kUint8, p, sh->comm_res, sh->s_return));
-        NK(nccl_rt::g_api.Recv(sl.back_res + sl.send_off[p], sl.send[p] * sizeof(gcra_result), nccl_rt::kUint8, p, sh->comm_res, sh->s_return));
+        NK(nccl_rt::g_api.Send(sl.recv_res.get() + sl.recv_off[p], sl.recv[p] * sizeof(gcra_result), nccl_rt::kUint8, p, sh->comm_res.get(), sh->s_return.get()));
+        NK(nccl_rt::g_api.Recv(sl.back_res.get() + sl.send_off[p], sl.send[p] * sizeof(gcra_result), nccl_rt::kUint8, p, sh->comm_res.get(), sh->s_return.get()));
     }
     NK(nccl_rt::g_api.GroupEnd());
     if (sl.n) {
-        route_unpermute_kernel<<<(sl.n + TILE_THREADS - 1) / TILE_THREADS, TILE_THREADS, 0, sh->s_return>>>(
-            sl.back_res, sl.src_index, sl.n, sl.d_res_user);
+        route_unpermute_kernel<<<(sl.n + TILE_THREADS - 1) / TILE_THREADS, TILE_THREADS, 0, sh->s_return.get()>>>(
+            sl.back_res.get(), sl.src_index.get(), sl.n, sl.d_res_user);
         h->launches++;
     }
-    CK(cudaEventRecord(sl.ev_done, sh->s_return));
+    CK(cudaEventRecord(sl.ev_done.get(), sh->s_return.get()));
     CK(cudaGetLastError());
     return GCRA_OK;
 }
 
 int32_t gcra_shard_submit(gcra_engine *h, uint64_t n64, const gcra_request *d_req, gcra_result *d_res, void *ready_stream) {
     CK(cudaSetDevice(h->device));
-    Shard *sh = h->shard;
+    Shard *sh = h->shard.get();
     if (!sh) { h->err = "gcra_shard_init first"; return GCRA_INTERNAL; }
     if (n64 > sh->max_rows) { h->err = "tick larger than max_rows"; return GCRA_INTERNAL; }
     const uint32_t n = (uint32_t)n64;
@@ -1992,50 +1953,50 @@ int32_t gcra_shard_submit(gcra_engine *h, uint64_t n64, const gcra_request *d_re
     const int k = (int)(sh->next++ % Shard::DEPTH);
     ShardSlot &sl = sh->slots[k];
     if ((int)sh->pending == k) RC(shard_issue_decide_return(h));
-    if (sl.used) CK(cudaStreamWaitEvent(sh->s_part, sl.ev_done, 0));     // the slot's buffers are free again
+    if (sl.used) CK(cudaStreamWaitEvent(sh->s_part.get(), sl.ev_done.get(), 0));     // the slot's buffers are free again
     sl.used = true; sl.n = n; sl.d_res_user = d_res;
     if (ready_stream) {
-        CK(cudaEventRecord(sl.ev_ready, (cudaStream_t)ready_stream));
-        CK(cudaStreamWaitEvent(sh->s_part, sl.ev_ready, 0));
+        CK(cudaEventRecord(sl.ev_ready.get(), (cudaStream_t)ready_stream));
+        CK(cudaStreamWaitEvent(sh->s_part.get(), sl.ev_ready.get(), 0));
     }
     // stage 1: stable partition by owner + count exchange
     if (n) {
         uint32_t tiles = (n + TILE_THREADS - 1) / TILE_THREADS;
-        route_count_kernel<<<tiles, TILE_THREADS, 0, sh->s_part>>>(d_req, n, (u32)W, tiles, h->route_counts);
-        route_scan_kernel<<<1, TILE_THREADS, 0, sh->s_part>>>(h->route_counts, (u32)W, tiles, sl.counts_dev);
-        route_scatter_kernel<<<tiles, TILE_THREADS, 0, sh->s_part>>>(d_req, n, (u32)W, tiles, h->route_counts, sl.routed, sl.src_index);
+        route_count_kernel<<<tiles, TILE_THREADS, 0, sh->s_part.get()>>>(d_req, n, (u32)W, tiles, h->route_counts.get());
+        route_scan_kernel<<<1, TILE_THREADS, 0, sh->s_part.get()>>>(h->route_counts.get(), (u32)W, tiles, sl.counts_dev.get());
+        route_scatter_kernel<<<tiles, TILE_THREADS, 0, sh->s_part.get()>>>(d_req, n, (u32)W, tiles, h->route_counts.get(), sl.routed.get(), sl.src_index.get());
         h->launches += 3;
     } else {
-        CK(cudaMemsetAsync(sl.counts_dev, 0, W * sizeof(u32), sh->s_part));
+        CK(cudaMemsetAsync(sl.counts_dev.get(), 0, W * sizeof(u32), sh->s_part.get()));
     }
     NK(nccl_rt::g_api.GroupStart());
     for (int p = 0; p < W; p++) {
-        NK(nccl_rt::g_api.Send(sl.counts_dev + p, 1, nccl_rt::kUint32, p, sh->comm_counts, sh->s_part));
-        NK(nccl_rt::g_api.Recv(sl.counts_dev + W + p, 1, nccl_rt::kUint32, p, sh->comm_counts, sh->s_part));
+        NK(nccl_rt::g_api.Send(sl.counts_dev.get() + p, 1, nccl_rt::kUint32, p, sh->comm_counts.get(), sh->s_part.get()));
+        NK(nccl_rt::g_api.Recv(sl.counts_dev.get() + W + p, 1, nccl_rt::kUint32, p, sh->comm_counts.get(), sh->s_part.get()));
     }
     NK(nccl_rt::g_api.GroupEnd());
-    CK(cudaMemcpyAsync(sl.counts_host, sl.counts_dev, 2 * W * sizeof(u32), cudaMemcpyDeviceToHost, sh->s_part));
-    CK(cudaEventRecord(sl.ev_counts, sh->s_part));
+    CK(cudaMemcpyAsync(sl.counts_host.get(), sl.counts_dev.get(), 2 * W * sizeof(u32), cudaMemcpyDeviceToHost, sh->s_part.get()));
+    CK(cudaEventRecord(sl.ev_counts.get(), sh->s_part.get()));
     // while this runs, enqueue the previous tick's engine kernels and its way back
     RC(shard_issue_decide_return(h));
     // stage 2: request all-to-all on its own stream (the partition + count exchange of the NEXT tick overlap
     // it); the counts are the only thing the host waits for
-    CK(cudaEventSynchronize(sl.ev_counts));
-    CK(cudaStreamWaitEvent(sh->s_route, sl.ev_counts, 0));
+    CK(cudaEventSynchronize(sl.ev_counts.get()));
+    CK(cudaStreamWaitEvent(sh->s_route.get(), sl.ev_counts.get(), 0));
     size_t so = 0, ro = 0;
     for (int p = 0; p < W; p++) {
-        sl.send[p] = sl.counts_host[p]; sl.recv[p] = sl.counts_host[W + p];
+        sl.send[p] = sl.counts_host.get()[p]; sl.recv[p] = sl.counts_host.get()[W + p];
         sl.send_off[p] = so; sl.recv_off[p] = ro;
         so += sl.send[p]; ro += sl.recv[p];
     }
     sl.n_recv = (uint32_t)ro;             // <= world x max_rows, which the buffers hold
     NK(nccl_rt::g_api.GroupStart());
     for (int p = 0; p < W; p++) {
-        NK(nccl_rt::g_api.Send(sl.routed + sl.send_off[p], sl.send[p] * sizeof(gcra_request), nccl_rt::kUint8, p, sh->comm_req, sh->s_route));
-        NK(nccl_rt::g_api.Recv(sl.recv_req + sl.recv_off[p], sl.recv[p] * sizeof(gcra_request), nccl_rt::kUint8, p, sh->comm_req, sh->s_route));
+        NK(nccl_rt::g_api.Send(sl.routed.get() + sl.send_off[p], sl.send[p] * sizeof(gcra_request), nccl_rt::kUint8, p, sh->comm_req.get(), sh->s_route.get()));
+        NK(nccl_rt::g_api.Recv(sl.recv_req.get() + sl.recv_off[p], sl.recv[p] * sizeof(gcra_request), nccl_rt::kUint8, p, sh->comm_req.get(), sh->s_route.get()));
     }
     NK(nccl_rt::g_api.GroupEnd());
-    CK(cudaEventRecord(sl.ev_routed, sh->s_route));
+    CK(cudaEventRecord(sl.ev_routed.get(), sh->s_route.get()));
     CK(cudaGetLastError());
     sh->pending = k;
     return GCRA_OK;
@@ -2045,23 +2006,23 @@ int32_t gcra_shard_submit(gcra_engine *h, uint64_t n64, const gcra_request *d_re
 // only the last DEPTH-1 ticks can be addressed
 int32_t gcra_shard_wait_tick(gcra_engine *h, uint32_t ticks_back, void *stream) {
     CK(cudaSetDevice(h->device));
-    Shard *sh = h->shard;
+    Shard *sh = h->shard.get();
     if (!sh || ticks_back >= (uint32_t)Shard::DEPTH - 1 || ticks_back >= sh->next) { h->err = "bad tick"; return GCRA_INTERNAL; }
     const int k = (int)((sh->next - 1 - ticks_back) % Shard::DEPTH);
     if (sh->pending == k) RC(shard_issue_decide_return(h));
-    if (stream) CK(cudaStreamWaitEvent((cudaStream_t)stream, sh->slots[k].ev_done, 0));
-    else CK(cudaEventSynchronize(sh->slots[k].ev_done));
+    if (stream) CK(cudaStreamWaitEvent((cudaStream_t)stream, sh->slots[k].ev_done.get(), 0));
+    else CK(cudaEventSynchronize(sh->slots[k].ev_done.get()));
     return GCRA_OK;
 }
 
 int32_t gcra_shard_join(gcra_engine *h, void *stream) {
     CK(cudaSetDevice(h->device));
-    Shard *sh = h->shard;
+    Shard *sh = h->shard.get();
     if (!sh) { h->err = "gcra_shard_init first"; return GCRA_INTERNAL; }
     RC(shard_issue_decide_return(h));
-    CK(cudaEventRecord(sh->ev_tmp, sh->s_return));
-    if (stream) CK(cudaStreamWaitEvent((cudaStream_t)stream, sh->ev_tmp, 0));
-    else CK(cudaEventSynchronize(sh->ev_tmp));
+    CK(cudaEventRecord(sh->ev_tmp.get(), sh->s_return.get()));
+    if (stream) CK(cudaStreamWaitEvent((cudaStream_t)stream, sh->ev_tmp.get(), 0));
+    else CK(cudaEventSynchronize(sh->ev_tmp.get()));
     return GCRA_OK;
 }
 
@@ -2075,43 +2036,38 @@ int32_t gcra_p2p_prepare(gcra_engine *h, int32_t rank, int32_t world, uint32_t c
     if (h->p2p) { h->err = "p2p already prepared"; return GCRA_INTERNAL; }
     if (world < 1 || world > P2P_MAX_WORLD || rank < 0 || rank >= world) { h->err = "bad rank / world"; return GCRA_INTERNAL; }
     if (cap_rows == 0 || cap_rows > (1u << 24)) { h->err = "cap_rows must be in 1..2^24"; return GCRA_INTERNAL; }
-    P2P *p = new P2P();
+    std::unique_ptr<P2P> p(new P2P());    // (assigned to the engine only once complete)
     p->rank = rank; p->world = world;
     p->cap_shift = std::max<uint32_t>(ceil_log2(cap_rows), 10);      // whole resolve tiles per segment
     p->cap = 1u << p->cap_shift;
-    if (((uint64_t)world << p->cap_shift) >= INDEX_MAX_ROWS) { delete p; h->err = "world * cap_rows too large"; return GCRA_INTERNAL; }
+    if (((uint64_t)world << p->cap_shift) >= INDEX_MAX_ROWS) { h->err = "world * cap_rows too large"; return GCRA_INTERNAL; }
     const size_t seg_rows = (size_t)P2P_DEPTH * world * p->cap;
     p->inbox_off = align_up(sizeof(P2PHeader), 256);
     p->outbox_off = align_up(p->inbox_off + seg_rows * sizeof(gcra_request), 256);
     p->window_bytes = align_up(p->outbox_off + seg_rows * sizeof(gcra_result), 256);
-    CK(cudaMalloc(&p->window, p->window_bytes));
-    CK(cudaMemset(p->window, 0, p->inbox_off));
+    CK(p->window.make(p->window_bytes));
+    CK(cudaMemset(p->window.get(), 0, p->inbox_off));
     if (ipc_handle_out_64) {
         cudaIpcMemHandle_t hd;
-        CK(cudaIpcGetMemHandle(&hd, p->window));
+        CK(cudaIpcGetMemHandle(&hd, p->window.get()));
         static_assert(sizeof(hd) == 64, "cudaIpcMemHandle_t is 64 bytes");
         memcpy(ipc_handle_out_64, &hd, 64);
     }
-    if (window_out) *window_out = p->window;
-    CK(cudaStreamCreateWithFlags(&p->s_part, cudaStreamNonBlocking));
-    CK(cudaStreamCreateWithFlags(&p->s_wait, cudaStreamNonBlocking));
-    CK(cudaStreamCreateWithFlags(&p->s_sig, cudaStreamNonBlocking));
-    CK(cudaStreamCreateWithFlags(&p->s_return, cudaStreamNonBlocking));
-    for (auto &e : p->ev_t) CK(cudaEventCreate(&e));
-    CK(cudaMalloc(&p->peers_dev, sizeof(P2PPeers)));
-    CK(cudaMalloc(&p->tile_counts, (size_t)ROUTE_MAX_SHARDS * ((p->cap + TILE_THREADS - 1) / TILE_THREADS) * sizeof(u32)));
+    if (window_out) *window_out = p->window.get();
+    for (Stream *s : {&p->s_part, &p->s_wait, &p->s_sig, &p->s_return}) CK(s->make());
+    for (Event &e : p->ev_t) CK(e.make(cudaEventDefault));
+    CK(p->peers_dev.make(1));
+    CK(p->tile_counts.make((size_t)ROUTE_MAX_SHARDS * ((p->cap + TILE_THREADS - 1) / TILE_THREADS)));
     for (auto &sl : p->slots) {
-        CK(cudaMalloc(&sl.res_loc, (size_t)p->cap * sizeof(u32)));
-        CK(cudaMalloc(&sl.counts_dev, P2P_MAX_WORLD * sizeof(u32)));
-        CK(cudaMalloc(&sl.segs_dev, P2P_MAX_WORLD * sizeof(SegDesc)));
-        CK(cudaEventCreateWithFlags(&sl.ev_ready, cudaEventDisableTiming));
-        CK(cudaEventCreateWithFlags(&sl.ev_wait, cudaEventDisableTiming));
-        CK(cudaEventCreateWithFlags(&sl.ev_done, cudaEventDisableTiming));
+        CK(sl.res_loc.make(p->cap));
+        CK(sl.counts_dev.make(P2P_MAX_WORLD));
+        CK(sl.segs_dev.make(P2P_MAX_WORLD));
+        for (Event *e : {&sl.ev_ready, &sl.ev_wait, &sl.ev_done}) CK(e->make(cudaEventDisableTiming));
     }
     // the engine's per-row buffers now span the row-id space of a whole inbox slot
     CK(cudaDeviceSynchronize());
-    for (auto &sc : h->scr) RC(alloc_index_scratch(h, sc, (uint32_t)world << p->cap_shift));
-    h->p2p = p;
+    RC(alloc_index_scratch(h, (uint32_t)world << p->cap_shift));
+    h->p2p = std::move(p);
     return GCRA_OK;
 }
 
@@ -2119,26 +2075,25 @@ int32_t gcra_p2p_prepare(gcra_engine *h, int32_t rank, int32_t world, uint32_t c
 // process: engines that share a process, e.g. the single-GPU loop-back test)
 int32_t gcra_p2p_connect(gcra_engine *h, const void *ipc_handles, void *const *windows) {
     CK(cudaSetDevice(h->device));
-    P2P *p = h->p2p;
+    P2P *p = h->p2p.get();
     if (!p) { h->err = "gcra_p2p_prepare first"; return GCRA_INTERNAL; }
     if (!ipc_handles && !windows) { h->err = "need ipc handles or window pointers"; return GCRA_INTERNAL; }
     P2PPeers peers{};
     for (int r = 0; r < p->world; r++) {
         void *base = nullptr;
-        if (r == p->rank) base = p->window;
+        if (r == p->rank) base = p->window.get();
         else if (windows) base = windows[r];
         else {
             cudaIpcMemHandle_t hd;
             memcpy(&hd, (const char *)ipc_handles + 64 * r, 64);
-            CK(cudaIpcOpenMemHandle(&base, hd, cudaIpcMemLazyEnablePeerAccess));
-            p->opened[r] = true;
+            CK(p->peer_map[r].make(hd));
+            base = p->peer_map[r].get();
         }
-        p->peer_base[r] = base;
         peers.hdr[r] = (P2PHeader *)base;
         peers.inbox[r] = (unsigned char *)base + p->inbox_off;
         peers.outbox[r] = (unsigned char *)base + p->outbox_off;
     }
-    CK(cudaMemcpy(p->peers_dev, &peers, sizeof(peers), cudaMemcpyHostToDevice));
+    CK(cudaMemcpy(p->peers_dev.get(), &peers, sizeof(peers), cudaMemcpyHostToDevice));
     for (int d = 0; d < P2P_DEPTH; d++) {
         SegDesc segs[P2P_MAX_WORLD] = {};
         for (int r = 0; r < p->world; r++) {
@@ -2147,7 +2102,7 @@ int32_t gcra_p2p_connect(gcra_engine *h, const void *ipc_handles, void *const *w
             segs[r].req = peers.inbox[p->rank] + (((size_t)d * p->world + r) << p->cap_shift) * sizeof(gcra_request);
             segs[r].res = (gcra_result *)(peers.outbox[r] + (((size_t)d * p->world + p->rank) << p->cap_shift) * sizeof(gcra_result));
         }
-        CK(cudaMemcpy(p->slots[d].segs_dev, segs, sizeof(segs), cudaMemcpyHostToDevice));
+        CK(cudaMemcpy(p->slots[d].segs_dev.get(), segs, sizeof(segs), cudaMemcpyHostToDevice));
     }
     p->connected = true;
     return GCRA_OK;
@@ -2156,7 +2111,7 @@ int32_t gcra_p2p_connect(gcra_engine *h, const void *ipc_handles, void *const *w
 // first half of a tick: the sender's side (partition + transfer + flags)
 int32_t gcra_p2p_submit_route(gcra_engine *h, uint64_t n64, const gcra_request *d_req, void *ready_stream) {
     CK(cudaSetDevice(h->device));
-    P2P *p = h->p2p;
+    P2P *p = h->p2p.get();
     if (!p || !p->connected) { h->err = "gcra_p2p_prepare / gcra_p2p_connect first"; return GCRA_INTERNAL; }
     if (p->routed_pending) { h->err = "gcra_p2p_submit_finish the previous tick first"; return GCRA_INTERNAL; }
     if (n64 > p->cap) { h->err = "tick larger than cap_rows"; return GCRA_INTERNAL; }
@@ -2167,26 +2122,26 @@ int32_t gcra_p2p_submit_route(gcra_engine *h, uint64_t n64, const gcra_request *
     P2PSlot &sl = p->slots[d];
     // slot d again: its previous tick has been un-permuted here, i.e. every owner is through with my rows of that
     // tick and with my outbox slot
-    if (sl.used) CK(cudaStreamWaitEvent(p->s_part, sl.ev_done, 0));
+    if (sl.used) CK(cudaStreamWaitEvent(p->s_part.get(), sl.ev_done.get(), 0));
     sl.used = true; sl.n = n;
     if (ready_stream) {
-        CK(cudaEventRecord(sl.ev_ready, (cudaStream_t)ready_stream));
-        CK(cudaStreamWaitEvent(p->s_part, sl.ev_ready, 0));
+        CK(cudaEventRecord(sl.ev_ready.get(), (cudaStream_t)ready_stream));
+        CK(cudaStreamWaitEvent(p->s_part.get(), sl.ev_ready.get(), 0));
     }
     // stable partition by owner, rows stored straight into the owners' inboxes, then the flags
     const uint32_t tiles = (n + TILE_THREADS - 1) / TILE_THREADS;
-    if (p->timed) CK(cudaEventRecord(p->ev_t[0], p->s_part));
+    if (p->timed) CK(cudaEventRecord(p->ev_t[0].get(), p->s_part.get()));
     if (n) {
-        route_count_kernel<<<tiles, TILE_THREADS, 0, p->s_part>>>(d_req, n, W, tiles, p->tile_counts);
-        p2p_scan_kernel<<<W, TILE_THREADS, 0, p->s_part>>>(p->tile_counts, tiles, sl.counts_dev);
-        p2p_scatter_kernel<<<tiles, TILE_THREADS, 0, p->s_part>>>(d_req, n, W, me, d, p->cap_shift, tiles, p->tile_counts,
-                                                                 p->peers_dev, sl.res_loc);
+        route_count_kernel<<<tiles, TILE_THREADS, 0, p->s_part.get()>>>(d_req, n, W, tiles, p->tile_counts.get());
+        p2p_scan_kernel<<<W, TILE_THREADS, 0, p->s_part.get()>>>(p->tile_counts.get(), tiles, sl.counts_dev.get());
+        p2p_scatter_kernel<<<tiles, TILE_THREADS, 0, p->s_part.get()>>>(d_req, n, W, me, d, p->cap_shift, tiles, p->tile_counts.get(),
+                                                                 p->peers_dev.get(), sl.res_loc.get());
         h->launches += 3;
     } else {
-        CK(cudaMemsetAsync(sl.counts_dev, 0, W * sizeof(u32), p->s_part));
+        CK(cudaMemsetAsync(sl.counts_dev.get(), 0, W * sizeof(u32), p->s_part.get()));
     }
-    p2p_signal_req_kernel<<<1, 32, 0, p->s_part>>>(p->peers_dev, sl.counts_dev, W, me, d, tick);
-    if (p->timed) CK(cudaEventRecord(p->ev_t[1], p->s_part));
+    p2p_signal_req_kernel<<<1, 32, 0, p->s_part.get()>>>(p->peers_dev.get(), sl.counts_dev.get(), W, me, d, tick);
+    if (p->timed) CK(cudaEventRecord(p->ev_t[1].get(), p->s_part.get()));
     h->launches++;
     CK(cudaGetLastError());
     p->routed_pending = true;
@@ -2197,21 +2152,21 @@ int32_t gcra_p2p_submit_route(gcra_engine *h, uint64_t n64, const gcra_request *
 // way back (wait for every owner, results into input order)
 int32_t gcra_p2p_submit_finish(gcra_engine *h, gcra_result *d_res) {
     CK(cudaSetDevice(h->device));
-    P2P *p = h->p2p;
+    P2P *p = h->p2p.get();
     if (!p || !p->routed_pending) { h->err = "gcra_p2p_submit_route first"; return GCRA_INTERNAL; }
     p->routed_pending = false;
     const uint32_t W = (uint32_t)p->world, me = (uint32_t)p->rank;
     const uint64_t tick = p->next_tick;
     const uint32_t d = (uint32_t)((tick - 1) % P2P_DEPTH);
     P2PSlot &sl = p->slots[d];
-    P2PHeader *hdr = (P2PHeader *)p->window;
+    P2PHeader *hdr = (P2PHeader *)p->window.get();
     // owner: wait for every sender's rows of this tick, then the engine over the inbox slot as one batch of W
     // segments (row counts in the header); its kernels store the results into the senders' outboxes
-    p2p_wait_kernel<<<1, 32, 0, p->s_wait>>>(hdr, 0, W, tick);
-    CK(cudaEventRecord(sl.ev_wait, p->s_wait));
+    p2p_wait_kernel<<<1, 32, 0, p->s_wait.get()>>>(hdr, 0, W, tick);
+    CK(cudaEventRecord(sl.ev_wait.get(), p->s_wait.get()));
     BatchView v{};
     v.req0 = nullptr; v.res0 = nullptr;
-    v.segs = sl.segs_dev;
+    v.segs = sl.segs_dev.get();
     v.dev_counts = &hdr->counts[d][0];
     v.n = 0;
     v.nseg = W;
@@ -2223,22 +2178,22 @@ int32_t gcra_p2p_submit_finish(gcra_engine *h, gcra_result *d_res) {
     // NEW keys than the table has room for, the surplus rows are answered with GCRA_INTERNAL ("table full"), as
     // find_or_claim always does; the next tick's check then sees the real occupancy and grows the table.
     const uint32_t n_rows = (uint32_t)std::min<uint64_t>((uint64_t)sl.n + sl.n / 4 + 4096, std::min<uint64_t>((uint64_t)W << p->cap_shift, h->max_batch));
-    if (p->timed) CK(cudaEventRecord(p->ev_t[2], p->s_wait));
-    RC(launch_pipelined_view(h, v, n_rows, FMT_48_32, 0, sl.ev_wait, &done));
-    CK(cudaStreamWaitEvent(p->s_sig, done, 0));
-    if (p->timed) CK(cudaEventRecord(p->ev_t[3], p->s_sig));
-    p2p_signal_res_kernel<<<1, 32, 0, p->s_sig>>>(p->peers_dev, W, me, tick);
+    if (p->timed) CK(cudaEventRecord(p->ev_t[2].get(), p->s_wait.get()));
+    RC(launch_pipelined_view(h, v, n_rows, FMT_48_32, 0, sl.ev_wait.get(), &done));
+    CK(cudaStreamWaitEvent(p->s_sig.get(), done, 0));
+    if (p->timed) CK(cudaEventRecord(p->ev_t[3].get(), p->s_sig.get()));
+    p2p_signal_res_kernel<<<1, 32, 0, p->s_sig.get()>>>(p->peers_dev.get(), W, me, tick);
     // sender again: every owner's results of this tick are in my outbox -> input order, into the caller's buffer
-    p2p_wait_kernel<<<1, 32, 0, p->s_return>>>(hdr, 1, W, tick);
-    if (p->timed) CK(cudaEventRecord(p->ev_t[4], p->s_return));
+    p2p_wait_kernel<<<1, 32, 0, p->s_return.get()>>>(hdr, 1, W, tick);
+    if (p->timed) CK(cudaEventRecord(p->ev_t[4].get(), p->s_return.get()));
     if (sl.n) {
         const uint32_t tiles = (sl.n + TILE_THREADS - 1) / TILE_THREADS;
-        p2p_unpermute_kernel<<<tiles, TILE_THREADS, 0, p->s_return>>>((const unsigned char *)p->window + p->outbox_off, sl.res_loc,
+        p2p_unpermute_kernel<<<tiles, TILE_THREADS, 0, p->s_return.get()>>>((const unsigned char *)p->window.get() + p->outbox_off, sl.res_loc.get(),
                                                                      sl.n, W, d, p->cap_shift, d_res);
         h->launches++;
     }
-    CK(cudaEventRecord(sl.ev_done, p->s_return));
-    if (p->timed) { CK(cudaEventRecord(p->ev_t[5], p->s_return)); p->timed_valid = true; }
+    CK(cudaEventRecord(sl.ev_done.get(), p->s_return.get()));
+    if (p->timed) { CK(cudaEventRecord(p->ev_t[5].get(), p->s_return.get())); p->timed_valid = true; }
     h->launches += 3;
     CK(cudaGetLastError());
     return GCRA_OK;
@@ -2249,7 +2204,7 @@ int32_t gcra_p2p_submit_finish(gcra_engine *h, gcra_result *d_res) {
 // here (includes the other ranks' skew), [2] the engine over the inbox, [3] until every owner's results are here,
 // [4] un-permutation
 int32_t gcra_p2p_set_timing(gcra_engine *h, int32_t on) {
-    P2P *p = h->p2p;
+    P2P *p = h->p2p.get();
     if (!p) { h->err = "gcra_p2p_prepare first"; return GCRA_INTERNAL; }
     p->timed = on != 0;
     return GCRA_OK;
@@ -2257,10 +2212,10 @@ int32_t gcra_p2p_set_timing(gcra_engine *h, int32_t on) {
 
 int32_t gcra_p2p_last_tick_ms(gcra_engine *h, float out[5]) {
     CK(cudaSetDevice(h->device));
-    P2P *p = h->p2p;
+    P2P *p = h->p2p.get();
     if (!p || !p->timed_valid) { h->err = "no timed tick yet"; return GCRA_INTERNAL; }
-    CK(cudaEventSynchronize(p->ev_t[5]));
-    for (int i = 0; i < 5; i++) CK(cudaEventElapsedTime(&out[i], p->ev_t[i], p->ev_t[i + 1]));
+    CK(cudaEventSynchronize(p->ev_t[5].get()));
+    for (int i = 0; i < 5; i++) CK(cudaEventElapsedTime(&out[i], p->ev_t[i].get(), p->ev_t[i + 1].get()));
     return GCRA_OK;
 }
 
@@ -2272,22 +2227,22 @@ int32_t gcra_p2p_submit(gcra_engine *h, uint64_t n, const gcra_request *d_req, g
 // make `stream` wait for the results of the tick submitted `ticks_back` submissions ago (0 = the latest, < DEPTH)
 int32_t gcra_p2p_wait_tick(gcra_engine *h, uint32_t ticks_back, void *stream) {
     CK(cudaSetDevice(h->device));
-    P2P *p = h->p2p;
+    P2P *p = h->p2p.get();
     if (!p || ticks_back >= (uint32_t)P2P_DEPTH || ticks_back >= p->next_tick) { h->err = "bad tick"; return GCRA_INTERNAL; }
     P2PSlot &sl = p->slots[(p->next_tick - 1 - ticks_back) % P2P_DEPTH];
-    if (stream) CK(cudaStreamWaitEvent((cudaStream_t)stream, sl.ev_done, 0));
-    else CK(cudaEventSynchronize(sl.ev_done));
+    if (stream) CK(cudaStreamWaitEvent((cudaStream_t)stream, sl.ev_done.get(), 0));
+    else CK(cudaEventSynchronize(sl.ev_done.get()));
     return GCRA_OK;
 }
 
 int32_t gcra_p2p_join(gcra_engine *h, void *stream) {
     CK(cudaSetDevice(h->device));
-    P2P *p = h->p2p;
+    P2P *p = h->p2p.get();
     if (!p) { h->err = "gcra_p2p_prepare first"; return GCRA_INTERNAL; }
     for (auto &sl : p->slots) {
         if (!sl.used) continue;
-        if (stream) CK(cudaStreamWaitEvent((cudaStream_t)stream, sl.ev_done, 0));
-        else CK(cudaEventSynchronize(sl.ev_done));
+        if (stream) CK(cudaStreamWaitEvent((cudaStream_t)stream, sl.ev_done.get(), 0));
+        else CK(cudaEventSynchronize(sl.ev_done.get()));
     }
     return GCRA_OK;
 }
@@ -2295,9 +2250,9 @@ int32_t gcra_p2p_join(gcra_engine *h, void *stream) {
 // 1 when a wait on this rank gave up (a peer never delivered a tick): results since then are not to be trusted
 int32_t gcra_p2p_error(gcra_engine *h, uint32_t *error) {
     CK(cudaSetDevice(h->device));
-    P2P *p = h->p2p;
+    P2P *p = h->p2p.get();
     if (!p) { h->err = "gcra_p2p_prepare first"; return GCRA_INTERNAL; }
-    CK(cudaMemcpy(error, (const char *)p->window + offsetof(P2PHeader, error), sizeof(u32), cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(error, (const char *)p->window.get() + offsetof(P2PHeader, error), sizeof(u32), cudaMemcpyDeviceToHost));
     return GCRA_OK;
 }
 
@@ -2308,12 +2263,12 @@ int32_t gcra_route_partition(gcra_engine *h, uint64_t n, const gcra_request *d_r
                              gcra_request *d_out, uint32_t *d_src_index, uint32_t *d_counts, void *stream) {
     CK(cudaSetDevice(h->device));
     if (n_shards == 0 || n_shards > ROUTE_MAX_SHARDS || n > h->max_batch) { h->err = "bad shard count / batch size"; return GCRA_INTERNAL; }
-    cudaStream_t st = stream ? (cudaStream_t)stream : h->stream;
+    cudaStream_t st = stream ? (cudaStream_t)stream : h->stream.get();
     if (n == 0) { CK(cudaMemsetAsync(d_counts, 0, n_shards * sizeof(u32), st)); return GCRA_OK; }
     uint32_t tiles = (uint32_t)((n + TILE_THREADS - 1) / TILE_THREADS);
-    route_count_kernel<<<tiles, TILE_THREADS, 0, st>>>(d_req, (u32)n, n_shards, tiles, h->route_counts);
-    route_scan_kernel<<<1, TILE_THREADS, 0, st>>>(h->route_counts, n_shards, tiles, d_counts);
-    route_scatter_kernel<<<tiles, TILE_THREADS, 0, st>>>(d_req, (u32)n, n_shards, tiles, h->route_counts, d_out, d_src_index);
+    route_count_kernel<<<tiles, TILE_THREADS, 0, st>>>(d_req, (u32)n, n_shards, tiles, h->route_counts.get());
+    route_scan_kernel<<<1, TILE_THREADS, 0, st>>>(h->route_counts.get(), n_shards, tiles, d_counts);
+    route_scatter_kernel<<<tiles, TILE_THREADS, 0, st>>>(d_req, (u32)n, n_shards, tiles, h->route_counts.get(), d_out, d_src_index);
     h->launches += 3;
     CK(cudaGetLastError());
     return GCRA_OK;
@@ -2323,7 +2278,7 @@ int32_t gcra_route_unpermute(gcra_engine *h, uint64_t n, const gcra_result *d_re
                              gcra_result *d_res, void *stream) {
     CK(cudaSetDevice(h->device));
     if (n == 0) return GCRA_OK;
-    cudaStream_t st = stream ? (cudaStream_t)stream : h->stream;
+    cudaStream_t st = stream ? (cudaStream_t)stream : h->stream.get();
     route_unpermute_kernel<<<(uint32_t)((n + TILE_THREADS - 1) / TILE_THREADS), TILE_THREADS, 0, st>>>(
         d_res_routed, d_src_index, (u32)n, d_res);
     h->launches++;
