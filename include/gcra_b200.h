@@ -57,7 +57,7 @@ typedef struct {
     int32_t store_kind;   /* GCRA_STORE_* */
     uint64_t p0, p1, p2;  /* policy parameters, 0 = the reference's library default */
     int64_t created_ns;   /* stands in for SystemTime::now() in the constructors (adaptive_cleanup.rs:94) */
-    uint32_t max_batch;   /* largest number of requests one kernel pass carries (0 -> 1<<20) */
+    uint32_t max_batch;   /* largest number of requests one kernel pass carries (0 -> 1<<20; below 1<<30) */
     uint32_t flags;       /* GCRA_FLAG_* */
     uint64_t hash_seed[2]; /* SipHash key of the string-keyed entry points; (0,0) = the unkeyed gcra_hash_key */
 } gcra_config;

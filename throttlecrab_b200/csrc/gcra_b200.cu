@@ -165,7 +165,7 @@ struct P2P {
 struct Scratch {
     DevBuf<Req> drec;
     DevBuf<u64> keys_a, keys_b;
-    DevBuf<u32> hist, tot;
+    DevBuf<u32> sort_ws;                // enqueue_sort: tickets, digit counts, status words (sort_ws_words)
     DevBuf<LongRun> long_runs, giant_runs;
     DevBuf<u32> long_count;
     Event ev_front, ev_mid, ev_back, ev_fork, ev_join;
@@ -175,7 +175,7 @@ struct Scratch {
     DevBuf<unsigned char> flags;        // [rows] pass-B verdict of rows on shared slots
     DevBuf<u32> bitmap;                 // [bm_words] 32-bit occurrence counters of the batch, hashed by slot
     DevBuf<u32> pend;                   // [pend_words] 1 bit per entry: the PREVIOUS batch's tail owns a slot of the entry
-    DevBuf<u64> ctrl_block;             // word 0: {tile ticket, residue count}; word 1: {sort barrier, -}; then one status word per tile
+    DevBuf<u64> ctrl_block;             // word 0: {tile ticket, residue count}; then one status word per tile
     uint32_t rows_alloc = 0;
     PinnedBuf<u32> h_nres;              // pinned: residue size of the set's latest index-order batch (valid after ev_mid)
     bool mid_recorded = false, nres_counted = true;
@@ -565,32 +565,29 @@ static BatchView single_view(const void *d_req, gcra_result *d_res, uint32_t n) 
 }
 
 // stable LSD radix sort of `n` (host count) or `*n_dev` (device count) keys on the slot bits; returns the buffer
-// that holds the sorted keys
+// that holds the sorted keys.  One digit-count launch, then one sweep launch per pass.
 static int enqueue_sort(gcra_engine *h, Scratch &sc, uint32_t n_max, const u32 *n_dev, cudaStream_t st, u64 **sorted_out) {
     const uint32_t bits = h->tab.slot_bits;
     const uint32_t passes = (bits + SORT_MAX_BITS - 1) / SORT_MAX_BITS;
-    uint32_t stiles = (n_max + SORT_TILE - 1) / SORT_TILE;
-    if (n_dev) {
-        // fixed grid, all CTAs resident (grid barriers), the kernels loop over the tiles: sized for about twice the
-        // residue the host saw last (a barrier over few CTAs is cheaper), any size is correct
-        const uint32_t guess = (uint32_t)std::min<uint64_t>(std::max<uint64_t>(2ULL * h->last_nres, n_max / 8) + 8 * SORT_TILE, n_max);
-        stiles = std::max<uint32_t>(std::min<uint32_t>((guess + SORT_TILE - 1) / SORT_TILE, 2 * h->sms), 8);
-    }
+    const uint32_t tiles = (n_max + SORT_TILE - 1) / SORT_TILE;
+    // With a device count (the residue of the index-order pipeline, usually a small part of n_max) both grids are
+    // fixed at one CTA per SM: the sweep CTAs take tiles until the count's run out, and the kernels leave room for
+    // the other stages' kernels that run beside the tail.  An empty count leaves the keys where they are and makes no
+    // CTA wait.
+    const uint32_t cap = n_dev ? h->sms : 2 * h->sms;
+    const uint32_t sgrid = std::max<uint32_t>(n_dev ? std::min(tiles, h->sms) : tiles, 1);
+    const uint32_t hgrid = std::max<uint32_t>(std::min<uint32_t>((n_max + 8 * TILE_THREADS - 1) / (8 * TILE_THREADS), cap), 1);
+    u32 *ws = sc.sort_ws.get();
+    CK(cudaMemsetAsync(ws, 0, sort_ws_words(passes, tiles) * sizeof(u32), st));
+    sort_digits_kernel<<<hgrid, TILE_THREADS, 0, st>>>(sc.keys_a.get(), n_max, n_dev, bits, passes, ws);
+    h->launches++;
     u64 *src = sc.keys_a.get(), *dst = sc.keys_b.get();
     uint32_t shift = 32;
     for (uint32_t p = 0; p < passes; p++) {
-        uint32_t pb = bits / passes + (p < bits % passes ? 1 : 0);
-        if (n_dev) {
-            // device-side count (the residue): one launch per pass, grid barriers between its phases
-            u32 *bar_cnt = reinterpret_cast<u32 *>(sc.ctrl_block.get() + 1);
-            sort_pass_fused_kernel<<<stiles, TILE_THREADS, 0, st>>>(src, dst, n_dev, shift, pb, sc.hist.get(), sc.tot.get(), bar_cnt, p);
-            h->launches++;
-        } else {
-            sort_hist_kernel<<<stiles, TILE_THREADS, 0, st>>>(src, n_max, n_dev, shift, pb, sc.hist.get());
-            sort_rowscan_kernel<<<1u << pb, TILE_THREADS, 0, st>>>(sc.hist.get(), n_max, n_dev, sc.tot.get());
-            sort_scatter_kernel<<<stiles, TILE_THREADS, 0, st>>>(src, dst, n_max, n_dev, shift, pb, sc.hist.get(), sc.tot.get());
-            h->launches += 3;
-        }
+        const uint32_t pb = sort_pass_bits(bits, passes, p);
+        sort_sweep_kernel<<<sgrid, TILE_THREADS, 0, st>>>(src, dst, n_max, n_dev, shift, pb, ws + SW_HIST + p * SORT_MAX_DIGITS,
+                                                          ws + SW_TICKETS + p, ws + SW_STATUS + (size_t)p * tiles * SORT_MAX_DIGITS);
+        h->launches++;
         std::swap(src, dst);
         shift += pb;
     }
@@ -645,7 +642,7 @@ static int alloc_index_scratch(gcra_engine *h, uint32_t rows) {
     for (auto &f : fresh) {
         CK(f.slot_arr.make(rows));
         CK(f.flags.make(rows));
-        CK(f.ctrl_block.make((size_t)max_tiles + 2));
+        CK(f.ctrl_block.make((size_t)max_tiles + 1));
     }
     for (int k = 0; k < gcra_engine::N_SCR; k++) {
         Scratch &sc = h->scr[k];
@@ -690,7 +687,7 @@ static int enqueue_front(gcra_engine *h, Scratch &sc, const BatchView &v, bool i
         const uint32_t rows = view_max_rows(v);
         const uint32_t tiles = (rows + TILE_THREADS - 1) / TILE_THREADS;
         const uint32_t grid = std::min<uint32_t>(tiles, h->grid_probe[fmt]);    // persistent, software-pipelined CTAs
-        CK(cudaMemsetAsync(sc.ctrl_block.get(), 0, ((size_t)h->max_tiles + 2) * sizeof(u64), st));
+        CK(cudaMemsetAsync(sc.ctrl_block.get(), 0, ((size_t)h->max_tiles + 1) * sizeof(u64), st));
         if (timed) CK(cudaEventRecord(h->evd[0].get(), st));
         if (fmt == FMT_16_16)
             probe_kernel<FMT_16_16><<<grid, TILE_THREADS, 0, st>>>(h->tab, v, h->d_pol.get(), h->npol, now_batch, sc.slot_arr.get(),
@@ -740,7 +737,7 @@ static int enqueue_mid_index(gcra_engine *h, Scratch &sc, Scratch &next, const B
     const uint32_t grid = std::min<uint32_t>((rows + TILE_THREADS - 1) / TILE_THREADS, h->grid_decide[fmt]);   // persistent CTAs
     const uint32_t rgrid = std::min<uint32_t>((rows + RES_TILE - 1) / RES_TILE + v.nseg, 6 * h->sms);
     u32 *ctrl = reinterpret_cast<u32 *>(sc.ctrl_block.get());
-    u64 *status = sc.ctrl_block.get() + 2;
+    u64 *status = sc.ctrl_block.get() + 1;
     if (fmt == FMT_16_16) {
         decide_index_kernel<FMT_16_16><<<grid, TILE_THREADS, 0, st>>>(h->tab, v, h->d_pol.get(), h->npol, now_batch, sc.slot_arr.get(),
                                                                       sc.bitmap.get(), sc.pend.get(), h->bm_mask, sc.flags.get(), h->epoch, hp,
@@ -979,7 +976,7 @@ static void preload(K kernel) {
 static void preload_kernels() {
     preload(ingest_kernel<FMT_48_32>); preload(ingest_kernel<FMT_16_32>); preload(ingest_kernel<FMT_16_16>);
     preload(small_batch_kernel<FMT_48_32>); preload(small_batch_kernel<FMT_16_32>); preload(small_batch_kernel<FMT_16_16>);
-    preload(sort_hist_kernel); preload(sort_rowscan_kernel); preload(sort_scatter_kernel); preload(sort_pass_fused_kernel);
+    preload(sort_digits_kernel); preload(sort_sweep_kernel);
     preload(decide_kernel<false, false>); preload(decide_kernel<true, false>);
     preload(decide_kernel<false, true>); preload(decide_kernel<true, true>);
     preload(decide_runs_kernel<1, false, false>); preload(decide_runs_kernel<CLUSTER_CTAS, false, false>);
@@ -1037,7 +1034,6 @@ static int init_engine(gcra_engine *h, const gcra_config *cfg) {
     CK(cudaMemsetAsync(h->counters.get(), 0, C_COUNT * sizeof(u64), h->stream.get()));
     RC(alloc_table(h, h->capacity, h->tab_arrays, h->tab, h->total_lines, h->counters.get()));
     const size_t mb = h->max_batch;
-    const uint32_t stiles = (uint32_t)((mb + SORT_TILE - 1) / SORT_TILE);
     {
         // index-order pipeline: hashed batch counters (32 bits) and pend bits, 8 entries per row of the largest
         // batch (n distinct slots share their entry with probability ~1/8), 64 K .. 16 M entries
@@ -1076,12 +1072,12 @@ static int init_engine(gcra_engine *h, const gcra_config *cfg) {
     CK(h->h_op.make(2));
     CK(h->h_counters.make(C_COUNT));
     CK(h->h_snap.make((size_t)gcra_engine::N_SNAP * C_COUNT));
+    if (h->max_batch > SORT_MAX_COUNT) { h->err = "max_batch must be below 2^30"; return GCRA_INTERNAL; }   // (the sort's 30-bit counts)
     for (Scratch &sc : h->scr) {
         CK(sc.drec.make(mb));
         CK(sc.keys_a.make(mb));
         CK(sc.keys_b.make(mb));
-        CK(sc.hist.make((size_t)SORT_MAX_DIGITS * stiles));
-        CK(sc.tot.make(SORT_MAX_DIGITS));
+        CK(sc.sort_ws.make(sort_ws_words(SORT_MAX_PASSES, (uint32_t)((mb + SORT_TILE - 1) / SORT_TILE))));
         CK(sc.long_runs.make(mb / LONG_RUN_MIN + 1));
         CK(sc.giant_runs.make(mb / GIANT_RUN_MIN + 1));
         CK(sc.long_count.make(2));

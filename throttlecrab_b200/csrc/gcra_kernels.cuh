@@ -192,15 +192,38 @@ ingest_kernel(Table t, const void *__restrict__ req_base, const PolicyDerived *_
 }
 
 // ---------------------------------------------------------------------------------------------
-// K1b: stable LSD radix sort on the slot bits of (slot << 32 | index)
+// K1b: stable LSD radix sort on the slot bits of (slot << 32 | index), one sweep per pass
 // ---------------------------------------------------------------------------------------------
+// One launch counts the digits of every pass (the multiset of digits of a pass does not depend on the order the
+// earlier passes leave), then one launch per pass ranks a tile of keys, takes the tile's global offset of each
+// digit from the tiles before it (decoupled look-back on per-(tile, digit) status words) and writes the tile back
+// in digit order: 1 + passes launches, one read of the keys for the counts and one read + one write per pass.
 #ifndef GCRA_SORT_ITEMS
-#define GCRA_SORT_ITEMS 4
+#define GCRA_SORT_ITEMS 16
 #endif
 constexpr int SORT_ITEMS = GCRA_SORT_ITEMS;                // items per thread
-constexpr int SORT_TILE = TILE_THREADS * SORT_ITEMS;       // 1024 keys per CTA
+constexpr int SORT_TILE = TILE_THREADS * SORT_ITEMS;       // 4096 keys per tile
 constexpr int SORT_MAX_BITS = 9;
 constexpr int SORT_MAX_DIGITS = 1 << SORT_MAX_BITS;
+constexpr int SORT_MAX_PASSES = (32 + SORT_MAX_BITS - 1) / SORT_MAX_BITS;   // slot ids are 32 bits
+static_assert(SORT_MAX_DIGITS == 2 * TILE_THREADS, "the sweep handles two digits per thread");
+
+// Work space of one sort, zeroed once per batch: the tile tickets of the passes, the digit counts of every pass,
+// then one status word per (pass, tile, digit); a pass's tiles are `status_tiles` apart (the tiles of the largest
+// count the batch can sort).
+constexpr u32 SW_TICKETS = 0, SW_HIST = 32, SW_STATUS = SW_HIST + SORT_MAX_PASSES * SORT_MAX_DIGITS;
+__host__ __device__ constexpr size_t sort_ws_words(u32 passes, u32 status_tiles) {
+    return SW_STATUS + (size_t)passes * status_tiles * SORT_MAX_DIGITS;
+}
+
+// digit bits of pass p when `bits` slot bits are sorted in `passes` passes (the low passes take the odd bits)
+__host__ __device__ constexpr u32 sort_pass_bits(u32 bits, u32 passes, u32 p) { return bits / passes + (p < bits % passes ? 1 : 0); }
+
+// status word of one (tile, digit): 0 = not yet published, else a flag and a count of keys (< 2^30, max_batch is
+// at most that): AGG = this tile's keys of the digit, INC = those of this tile and of every tile before it, plus
+// the keys of all smaller digits (the digit's base in the output)
+constexpr u32 SS_AGG = 1u << 30, SS_INC = 2u << 30, SS_COUNT = SS_AGG - 1;
+constexpr u32 SORT_MAX_COUNT = SS_COUNT;
 
 // block-wide exclusive scan of one value per thread (warp shuffles + one shared-memory hop);
 // returns the exclusive prefix, the block total in *total
@@ -229,156 +252,187 @@ __device__ __forceinline__ u32 block_exclusive_scan(u32 v, u32 *part, u32 *total
     return before + inc - v;
 }
 
-// All three kernels loop over the tiles (grid-stride), and take the element count either from the host
-// (`n`) or -- when `n_dev` is given -- from device memory: the residue of the index-order pipeline is only
-// known on the device, its kernels are launched with a fixed grid.
+// Both kernels take the element count either from the host (`n`) or -- when `n_dev` is given -- from device
+// memory: the residue of the index-order pipeline is only known on the device, its sort has a fixed grid.
 __device__ __forceinline__ u32 sort_count(u32 n, const u32 *__restrict__ n_dev) { return n_dev ? *n_dev : n; }
 
-// the three phases of one pass; hist / tot are read through L2 (__ldcg): the fused kernel below reads what
-// OTHER CTAs of the same launch wrote a phase earlier
-__device__ __forceinline__ void sort_hist_body(u32 *h, const u64 *__restrict__ in, u32 n, u32 shift, u32 bits,
-                                               u32 *__restrict__ hist) {
-    const u32 num_tiles = (n + SORT_TILE - 1) / SORT_TILE;
-    const u32 nd = 1u << bits, mask = nd - 1;
-    for (u32 tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
-        for (u32 d = threadIdx.x; d < nd; d += TILE_THREADS) h[d] = 0;
-        __syncthreads();
-        const u32 base = tile * SORT_TILE;
-#pragma unroll
-        for (int k = 0; k < SORT_ITEMS; k++) {
-            u32 i = base + k * TILE_THREADS + threadIdx.x;
-            if (i < n) atomicAdd(&h[(u32)(in[i] >> shift) & mask], 1u);
-        }
-        __syncthreads();
-        for (u32 d = threadIdx.x; d < nd; d += TILE_THREADS) hist[(size_t)d * num_tiles + tile] = h[d];
-        __syncthreads();
-    }
-}
-
-// exclusive scan of digit `digit`'s per-tile counts, digit total to tot[digit] (the whole CTA works on it)
-__device__ __forceinline__ void sort_rowscan_body(u32 *part, u32 *__restrict__ hist, u32 n, u32 digit, u32 *__restrict__ tot) {
-    const u32 num_tiles = (n + SORT_TILE - 1) / SORT_TILE;
-    u32 *row = hist + (size_t)digit * num_tiles;
-    const u32 per = (num_tiles + TILE_THREADS - 1) / TILE_THREADS;
-    const u32 lo = min(threadIdx.x * per, num_tiles), hi = min(lo + per, num_tiles);
+// digit counts of all passes: shared-memory bins, then one posted add per nonzero bin per CTA (persistent grid)
+__global__ void __launch_bounds__(TILE_THREADS)
+sort_digits_kernel(const u64 *__restrict__ in, u32 n_host, const u32 *__restrict__ n_dev, u32 bits, u32 passes,
+                   u32 *__restrict__ ws) {
+    __shared__ u32 h[SORT_MAX_PASSES * SORT_MAX_DIGITS];
+    for (u32 d = threadIdx.x; d < passes * SORT_MAX_DIGITS; d += TILE_THREADS) h[d] = 0;
+    __syncthreads();
+    const u32 n = sort_count(n_host, n_dev);
+    u32 shift[SORT_MAX_PASSES], mask[SORT_MAX_PASSES];
     u32 s = 0;
-    for (u32 i = lo; i < hi; i++) s += __ldcg(&row[i]);
-    u32 total;
-    u32 acc = block_exclusive_scan(s, part, &total);
-    for (u32 i = lo; i < hi; i++) { u32 v = __ldcg(&row[i]); row[i] = acc; acc += v; }
-    if (threadIdx.x == 0) tot[digit] = total;
-    __syncthreads();   // `part` is reused by the next call
+#pragma unroll
+    for (int p = 0; p < SORT_MAX_PASSES; p++) {
+        const u32 pb = (u32)p < passes ? sort_pass_bits(bits, passes, p) : 0;
+        shift[p] = s;
+        mask[p] = (1u << pb) - 1;
+        s += pb;
+    }
+    const u32 stride = gridDim.x * TILE_THREADS;
+#pragma unroll 4
+    for (u32 i = blockIdx.x * TILE_THREADS + threadIdx.x; i < n; i += stride) {
+        const u32 slot = (u32)(in[i] >> 32);
+#pragma unroll
+        for (int p = 0; p < SORT_MAX_PASSES; p++)
+            if ((u32)p < passes) atomicAdd(&h[p * SORT_MAX_DIGITS + ((slot >> shift[p]) & mask[p])], 1u);
+    }
+    __syncthreads();
+    for (u32 d = threadIdx.x; d < passes * SORT_MAX_DIGITS; d += TILE_THREADS)
+        if (h[d]) atomicAdd(&ws[SW_HIST + d], h[d]);
 }
 
-struct SortScatterSmem {
-    u32 cnt[TILE_THREADS / 32][SORT_MAX_DIGITS];   // per-warp digit counters -> per-warp offsets
-    u32 gbase[SORT_MAX_DIGITS];                    // global base of (digit, this tile)
+// the status words of digits d and d + 1 (d even) of one tile, in one 8-byte access
+__device__ __forceinline__ uint2 ld_status2(const u32 *p) {
+    uint2 v;
+    asm volatile("ld.volatile.v2.u32 {%0, %1}, [%2];" : "=r"(v.x), "=r"(v.y) : "l"(p) : "memory");
+    return v;
+}
+__device__ __forceinline__ void st_status2(u32 *p, u32 a, u32 b) {
+    asm volatile("st.volatile.v2.u32 [%0], {%1, %2};" ::"l"(p), "r"(a), "r"(b) : "memory");
+}
+
+// Exclusive prefixes of digits d and d + 1 (d even) over the tiles before `tile`, digit bases included: walks back
+// from tile - 1, LB tiles per round trip, until each digit meets an inclusive prefix (tile 0 publishes them at once).
+// Every earlier tile was handed to a CTA that runs already (ticket), so each wait ends.
+__device__ __forceinline__ uint2 sort_lookback2(const u32 *status, u32 tile, u32 d) {
+    constexpr int LB = 8;
+    u32 sum0 = 0, sum1 = 0;
+    bool open0 = true, open1 = true;
+    for (int j = (int)tile - 1; open0 || open1; j -= LB) {
+        uint2 v[LB];
+#pragma unroll
+        for (int i = 0; i < LB; i++)
+            v[i] = j - i >= 0 ? ld_status2(status + (size_t)(j - i) * SORT_MAX_DIGITS + d) : make_uint2(SS_INC, SS_INC);
+#pragma unroll
+        for (int i = 0; i < LB; i++) {
+            while ((open0 && v[i].x == 0) || (open1 && v[i].y == 0)) v[i] = ld_status2(status + (size_t)(j - i) * SORT_MAX_DIGITS + d);
+            if (open0) { sum0 += v[i].x & SS_COUNT; open0 = !(v[i].x & SS_INC); }
+            if (open1) { sum1 += v[i].y & SS_COUNT; open1 = !(v[i].y & SS_INC); }
+        }
+    }
+    return make_uint2(sum0, sum1);
+}
+
+struct SortSweepSmem {
+    union {
+        u32 cnt[TILE_THREADS / 32][SORT_MAX_DIGITS];   // per-warp digit counters -> per-warp offsets
+        u64 keys[SORT_TILE];                           // the tile in digit order
+    } x;
+    u32 tile_ex[SORT_MAX_DIGITS];                      // first position of each digit in the tile
+    u32 gofs[SORT_MAX_DIGITS];                         // output position - tile position, per digit
     u32 part[TILE_THREADS / 32];
+    u32 tile;
 };
 
-__device__ __forceinline__ void sort_scatter_body(SortScatterSmem &sm, const u64 *__restrict__ in, u64 *__restrict__ outk,
-                                                  u32 n, u32 shift, u32 bits, const u32 *__restrict__ hist,
-                                                  const u32 *__restrict__ tot) {
+// One pass.  CTAs take tiles by ticket until the tiles of the count run out.  Warp w ranks tile elements
+// [w * 32 ITEMS, (w + 1) * 32 ITEMS) in index order (item k, lane l -> w * 32 ITEMS + 32 k + l), so equal digits
+// keep their order: within a warp by MATCH.ANY, across warps and tiles by the prefix sums.
+__global__ void __launch_bounds__(TILE_THREADS)
+sort_sweep_kernel(const u64 *__restrict__ in, u64 *__restrict__ outk, u32 n_host, const u32 *__restrict__ n_dev,
+                  u32 shift, u32 bits, const u32 *__restrict__ hist, u32 *__restrict__ ticket,
+                  u32 *__restrict__ status) {
     constexpr int NW = TILE_THREADS / 32;
+    __shared__ SortSweepSmem sm;
+    const u32 n = sort_count(n_host, n_dev);
     const u32 num_tiles = (n + SORT_TILE - 1) / SORT_TILE;
-    if (blockIdx.x >= num_tiles) return;       // uniform over the CTA
     const u32 nd = 1u << bits, mask = nd - 1;
     const u32 w = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    // exclusive scan of the digit totals (nd <= 512: two consecutive digits per thread), once per CTA
-    const u32 d0 = 2 * threadIdx.x, d1 = d0 + 1;
-    const u32 t0 = d0 < nd ? __ldcg(&tot[d0]) : 0, t1 = d1 < nd ? __ldcg(&tot[d1]) : 0;
-    u32 total;
-    const u32 ex = block_exclusive_scan(t0 + t1, sm.part, &total);
     const u32 lt = (1u << lane) - 1;
-    for (u32 tile = blockIdx.x; tile < num_tiles; tile += gridDim.x) {
+    const u32 d0 = 2 * threadIdx.x, d1 = d0 + 1;       // this thread's digits in the per-digit steps
+    if (blockIdx.x >= num_tiles) return;               // (the CTAs below take every tile)
+    for (;;) {
+        if (threadIdx.x == 0) sm.tile = atomicAdd(ticket, 1u);
         for (u32 d = threadIdx.x; d < nd; d += TILE_THREADS) {
 #pragma unroll
-            for (int x = 0; x < NW; x++) sm.cnt[x][d] = 0;
+            for (int x = 0; x < NW; x++) sm.x.cnt[x][d] = 0;
         }
-        if (d0 < nd) sm.gbase[d0] = ex + __ldcg(&hist[(size_t)d0 * num_tiles + tile]);
-        if (d1 < nd) sm.gbase[d1] = ex + t0 + __ldcg(&hist[(size_t)d1 * num_tiles + tile]);
         __syncthreads();
-        // warp w owns tile elements [w*128, w*128+128): item k, lane l -> w*128 + k*32 + l (index order)
-        const u32 base = tile * SORT_TILE + w * (32 * SORT_ITEMS);
+        const u32 tile = sm.tile;
+        if (tile >= num_tiles) break;                  // uniform over the CTA
+        const u32 tile0 = tile * SORT_TILE;
+        const u32 tcount = min((u32)SORT_TILE, n - tile0);
+        const u32 base = tile0 + w * (32 * SORT_ITEMS);
         u64 key[SORT_ITEMS];
-        u32 dig[SORT_ITEMS], rank[SORT_ITEMS];
 #pragma unroll
         for (int k = 0; k < SORT_ITEMS; k++) {
-            u32 i = base + k * 32 + lane;
-            bool valid = i < n;
-            key[k] = valid ? in[i] : 0;
-            dig[k] = (u32)(key[k] >> shift) & mask;
-            u32 peers = __match_any_sync(0xffffffffu, valid ? dig[k] : (0x80000000u | lane));
-            u32 before = valid ? sm.cnt[w][dig[k]] : 0;
+            const u32 i = base + k * 32 + lane;
+            key[k] = i < n ? in[i] : 0;
+        }
+        u32 rank[SORT_ITEMS];
+#pragma unroll
+        for (int k = 0; k < SORT_ITEMS; k++) {
+            const bool valid = base + k * 32 + lane < n;
+            const u32 dig = (u32)(key[k] >> shift) & mask;
+            const u32 peers = __match_any_sync(0xffffffffu, valid ? dig : (0x80000000u | lane));
+            const u32 before = valid ? sm.x.cnt[w][dig] : 0;
             rank[k] = before + __popc(peers & lt);
             __syncwarp();
-            if (valid && (peers & lt) == 0) sm.cnt[w][dig[k]] = before + __popc(peers);
+            if (valid && (peers & lt) == 0) sm.x.cnt[w][dig] = before + __popc(peers);
             __syncwarp();
         }
         __syncthreads();
-        // per digit: exclusive scan over the warps
-        for (u32 d = threadIdx.x; d < nd; d += TILE_THREADS) {
-            u32 acc = 0;
+        // per digit: exclusive scan over the warps -> the tile's count of the digit
+        u32 t0 = 0, t1 = 0;
+        if (d1 < nd) {                                 // (nd is even: a thread has both digits or none)
 #pragma unroll
-            for (int x = 0; x < NW; x++) { u32 v = sm.cnt[x][d]; sm.cnt[x][d] = acc; acc += v; }
+            for (int x = 0; x < NW; x++) {
+                const u32 a = sm.x.cnt[x][d0], b = sm.x.cnt[x][d1];
+                sm.x.cnt[x][d0] = t0;
+                sm.x.cnt[x][d1] = t1;
+                t0 += a;
+                t1 += b;
+            }
+            if (tile > 0) st_status2(status + (size_t)tile * SORT_MAX_DIGITS + d0, SS_AGG | t0, SS_AGG | t1);
+        }
+        u32 total;
+        const u32 ex = block_exclusive_scan(t0 + t1, sm.part, &total);
+        u32 g0, g1;                                    // output position of the tile's first key of d0 / d1
+        if (tile == 0) {
+            // the digit bases: exclusive scan of the pass's digit counts, once per pass
+            const u32 h0 = d1 < nd ? hist[d0] : 0, h1 = d1 < nd ? hist[d1] : 0;
+            __syncthreads();                           // (part is reused)
+            g0 = block_exclusive_scan(h0 + h1, sm.part, &total);
+            g1 = g0 + h0;
+        } else {
+            const uint2 g = d1 < nd ? sort_lookback2(status, tile, d0) : make_uint2(0, 0);
+            g0 = g.x;
+            g1 = g.y;
+        }
+        if (d1 < nd) {
+            st_status2(status + (size_t)tile * SORT_MAX_DIGITS + d0, SS_INC | (g0 + t0), SS_INC | (g1 + t1));
+            sm.tile_ex[d0] = ex;
+            sm.tile_ex[d1] = ex + t0;
+            sm.gofs[d0] = g0 - ex;
+            sm.gofs[d1] = g1 - ex - t0;
         }
         __syncthreads();
+        u32 pos[SORT_ITEMS];
 #pragma unroll
         for (int k = 0; k < SORT_ITEMS; k++) {
-            u32 i = base + k * 32 + lane;
-            if (i < n) outk[sm.gbase[dig[k]] + sm.cnt[w][dig[k]] + rank[k]] = key[k];
+            const u32 dig = (u32)(key[k] >> shift) & mask;
+            pos[k] = sm.tile_ex[dig] + sm.x.cnt[w][dig] + rank[k];
         }
+        __syncthreads();                               // (the counters and the keys share memory)
+#pragma unroll
+        for (int k = 0; k < SORT_ITEMS; k++)
+            if (base + k * 32 + lane < n) sm.x.keys[pos[k]] = key[k];
         __syncthreads();
+        // consecutive threads write consecutive positions of one digit's range
+#pragma unroll
+        for (int k = 0; k < SORT_ITEMS; k++) {
+            const u32 j = k * TILE_THREADS + threadIdx.x;
+            if (j < tcount) {
+                const u64 v = sm.x.keys[j];
+                outk[sm.gofs[(u32)(v >> shift) & mask] + j] = v;
+            }
+        }
+        __syncthreads();                               // the shared memory is reused by the next tile
     }
-}
-
-__global__ void __launch_bounds__(TILE_THREADS)
-sort_hist_kernel(const u64 *__restrict__ in, u32 n_host, const u32 *__restrict__ n_dev, u32 shift, u32 bits,
-                 u32 *__restrict__ hist) {
-    __shared__ u32 h[SORT_MAX_DIGITS];
-    sort_hist_body(h, in, sort_count(n_host, n_dev), shift, bits, hist);
-}
-
-// one CTA per digit
-__global__ void __launch_bounds__(TILE_THREADS)
-sort_rowscan_kernel(u32 *__restrict__ hist, u32 n_host, const u32 *__restrict__ n_dev, u32 *__restrict__ tot) {
-    __shared__ u32 part[TILE_THREADS / 32];
-    sort_rowscan_body(part, hist, sort_count(n_host, n_dev), blockIdx.x, tot);
-}
-
-__global__ void __launch_bounds__(TILE_THREADS)
-sort_scatter_kernel(const u64 *__restrict__ in, u64 *__restrict__ outk, u32 n_host, const u32 *__restrict__ n_dev,
-                    u32 shift, u32 bits, const u32 *__restrict__ hist, const u32 *__restrict__ tot) {
-    __shared__ SortScatterSmem sm;
-    sort_scatter_body(sm, in, outk, sort_count(n_host, n_dev), shift, bits, hist, tot);
-}
-
-// One radix pass in ONE launch for small inputs (the residue of the index-order pipeline: its nine launches of a
-// few microseconds each were pure launch latency).  All CTAs are resident (the host launches at most what fits),
-// the phases are separated by a grid-wide barrier on a counter that the host zeroes once per batch: the barrier
-// after phase p of pass q is complete when the counter reaches (2 q + p + 1) * gridDim.x.
-__device__ __forceinline__ void grid_barrier(u32 *cnt, u32 target) {
-    __syncthreads();
-    if (threadIdx.x == 0) {
-        __threadfence();
-        atomicAdd(cnt, 1u);
-        while (*reinterpret_cast<volatile u32 *>(cnt) < target) { }
-        __threadfence();
-    }
-    __syncthreads();
-}
-
-__global__ void __launch_bounds__(TILE_THREADS)
-sort_pass_fused_kernel(const u64 *__restrict__ in, u64 *__restrict__ outk, const u32 *__restrict__ n_dev, u32 shift,
-                       u32 bits, u32 *__restrict__ hist, u32 *__restrict__ tot, u32 *__restrict__ bar_cnt, u32 pass) {
-    __shared__ SortScatterSmem sm;
-    const u32 n = *n_dev;
-    if (n == 0) return;                                   // uniform over the grid: nobody enters a barrier
-    sort_hist_body(sm.gbase, in, n, shift, bits, hist);   // (gbase doubles as the histogram of phase 1)
-    grid_barrier(bar_cnt, (2 * pass + 1) * gridDim.x);
-    for (u32 d = blockIdx.x; d < (1u << bits); d += gridDim.x) sort_rowscan_body(sm.part, hist, n, d, tot);
-    grid_barrier(bar_cnt, (2 * pass + 2) * gridDim.x);
-    sort_scatter_body(sm, in, outk, n, shift, bits, hist, tot);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -745,7 +799,7 @@ decide_kernel(Table t, const u64 *__restrict__ sorted, const Req *__restrict__ d
 
 // Small batches (n < LONG_RUN_MIN, e.g. one RateLimiter::rate_limit call or a lightly loaded actor): ONE CTA
 // does everything -- ingest, a bitonic sort of the (slot, index) keys in shared memory, and the warp-chunk
-// compare-and-update -- instead of 13 launches.  No run can reach LONG_RUN_MIN, so no work list is produced.
+// compare-and-update -- instead of the sort pipeline's 4-7 launches and 2 memsets.  No run can reach LONG_RUN_MIN, so no work list is produced.
 constexpr u32 SMALL_MAX = 255;
 static_assert(SMALL_MAX < GCRA_LONG_MIN && SMALL_MAX < TILE_THREADS, "small path must not create long runs");
 
