@@ -112,10 +112,11 @@ def new_engine(capacity, max_batch, flags=0):
     return st, lim
 
 
-def expand(batches, res16):
+def expand(batches, res16, table=None):
+    table = policies() if table is None else table
     out, a = [], 0
     for b in batches:
-        out.append(tc.expand_results16(b.req16, b.now, policies(), res16[a:a + len(b.key)]))
+        out.append(tc.expand_results16(b.req16, b.now, table, res16[a:a + len(b.key)]))
         a += len(b.key)
     return np.concatenate(out)
 
@@ -127,9 +128,10 @@ def first_bad(a, b):
     return None if len(bad) == 0 else int(bad[0])
 
 
-def assert_pair(batches, want, cur, res32, res16, st32, st16, ora, sample_keys, stat_fields=STAT_BLOCKING):
+def assert_pair(batches, want, cur, res32, res16, st32, st16, ora, sample_keys, stat_fields=STAT_BLOCKING, table=None):
     """16-byte rows == the oracle's (cur, status, allowed); expanded rows == the 32-byte engine's == the oracle's;
-    the two engines' tables, counters and top denied keys agree (and the tables with the oracle's entries)."""
+    the two engines' tables, counters and top denied keys agree (and the tables with the oracle's entries).
+    `table`: the policy table both engines ran with (default: this file's)."""
     assert len(res16) == len(res32) == len(want)
     got = np.stack([res16["cur_tat_ns"], res16["status"].astype(np.int64), res16["allowed"].astype(np.int64)], 1)
     exp = np.stack([cur, want["status"].astype(np.int64), want["allowed"].astype(np.int64)], 1)
@@ -137,7 +139,7 @@ def assert_pair(batches, want, cur, res32, res16, st32, st16, ora, sample_keys, 
     assert len(bad) == 0, "16-byte row %d: engine %s, oracle (cur, status, allowed) %s" % (bad[0], got[bad[0]], exp[bad[0]])
     i = first_bad(want, res32)
     assert i is None, "32-byte row %d: oracle %s engine %s" % (i, want[i], res32[i])
-    full = expand(batches, res16)
+    full = expand(batches, res16, table)
     i = first_bad(res32, full)
     assert i is None, "expanded row %d: 32-byte engine %s expanded %s" % (i, res32[i], full[i])
     s32, s16 = st32.stats(), st16.stats()

@@ -1213,7 +1213,7 @@ int32_t gcra_derive_params(int64_t max_burst, int64_t count, int64_t period, int
 
 static int store_op(gcra_engine *h, int op, uint64_t key_hash, int64_t a, int64_t b, uint64_t ttl, int64_t now) {
     CK(cudaSetDevice(h->device));
-    // the table encodes 'no state' as a negative expiry: times before the epoch are outside its domain
+    // the table encodes 'no state' as a negative expiry (has_state): times before the epoch are outside its domain
     if (op != 3 && now < 0) { h->err = "pre-epoch time is not supported"; return GCRA_INTERNAL; }
     if (op == 2) { int rc = ensure_room(h, 1); if (rc) return rc; }
     // a Store-trait call reads / writes a slot's state: after every batch still in flight on the engine's or a

@@ -17,13 +17,18 @@ constexpr u64 KEY_TOMB = 1;    // swept stash slot (stash probing continues past
 constexpr i64 EXP_EMPTY = -1;  // (tat=0, off=-1): the slot holds no state (free slot, or a key without an entry)
 constexpr i64 I64_MAX = 0x7fffffffffffffffLL;
 constexpr i64 I64_MIN = (-0x7fffffffffffffffLL - 1);
+// An entry's expiry is now + ttl, kept exact in the reference (SystemTime + Duration).  Past I64_MAX it never expires:
+// stored as I64_MAX.  Exactly I64_MAX (live up to I64_MAX - 1) has the code EXP_AT_MAX instead, the one negative expiry
+// that is an entry; every other negative expiry is "no state".  All readers go through has_state / live_at.
+constexpr i64 EXP_AT_MAX = I64_MIN;
 
 // Structure of arrays, one element per slot; a bucket = 4 consecutive slots:
 //   keys[slot]   u64   mixed key hash (0 empty, 1 stash tombstone); a bucket's four keys are one
 //                      32-byte sector, compared after two 128-bit loads
 //   state[slot]  16 B  (tat_ns, burst_offset) -- always read and written together, so one decision is
 //                      ONE 128-bit load + ONE 128-bit store, and the sweep streams this array densely
-//                      (16 B per slot, coalesced 128-bit loads).  expiry = tat + off (wrapping).
+//                      (16 B per slot, coalesced 128-bit loads).  expiry code = tat + off (wrapping, see
+//                      EXP_AT_MAX).
 //   ei[slot]     i64   emission interval (ns) of the request that created the entry (informational)
 // Layout history (profiles/r01_k1_summary.md): v1 kept all four columns of a bucket in one 128-byte
 // line; ncu showed 64-byte DRAM fetch granules and a 44-54 %-of-peak sweep, and the probe (ingest
@@ -132,6 +137,20 @@ __host__ __device__ __forceinline__ int derive_params(i64 max_burst, i64 count, 
     return hi >= 1000000000ULL ? 3 : 0;
 }
 
+// ------------------------------------------------------------------ expiry codes
+__host__ __device__ __forceinline__ bool has_state(i64 exp) { return exp >= 0 || exp == EXP_AT_MAX; }
+// Store::get shows the entry at `now` (adaptive_cleanup.rs:248: expiry > now); now >= 0
+__host__ __device__ __forceinline__ bool live_at(i64 exp, i64 now) {
+    return exp > now || exp == I64_MAX || (exp == EXP_AT_MAX && now != I64_MAX);
+}
+// the expiry code of now + ttl (now >= 0; a negative ttl has wrapped to a huge u64)
+__host__ __device__ __forceinline__ i64 expiry_code(i64 now, u64 ttl) {
+    const u64 e = (u64)now + ttl;
+    return (e < ttl || e > (u64)I64_MAX) ? I64_MAX : e == (u64)I64_MAX ? EXP_AT_MAX : (i64)e;
+}
+// the expiry an entry reports (gcra_peek), clamped to I64_MAX as the oracle reports it
+__host__ __device__ __forceinline__ i64 expiry_value(i64 exp) { return exp == EXP_AT_MAX ? I64_MAX : exp; }
+
 // ------------------------------------------------------------------ the decision
 struct Req { i64 now, ei, dvt, q; };   // 32 bytes: the derived request the decide kernel gathers
 
@@ -139,7 +158,7 @@ struct Decision {
     i64 tat;       // TAT the request starts from (rate_limiter.rs:158-166)
     i64 new_tat;   // :171
     i64 allow_at;  // :174
-    i64 new_exp;   // now + ttl, saturated to I64_MAX (adaptive_cleanup.rs:237,268,273)
+    i64 new_exp;   // expiry code of now + ttl (adaptive_cleanup.rs:237,268,273)
     bool allowed;  // :175
     bool live;     // stored entry visible to Store::get (adaptive_cleanup.rs:248)
 };
@@ -156,7 +175,7 @@ __device__ __forceinline__ bool ordinary_request(const Req &r, i64 *inc) {
 
 __device__ __forceinline__ Decision decide(i64 s_tat, i64 s_exp, const Req &r) {
     Decision d;
-    d.live = s_exp > r.now;
+    d.live = live_at(s_exp, r.now);
     i64 inc;
 #ifdef GCRA_NO_FASTPATH
     if (false) {
@@ -169,8 +188,7 @@ __device__ __forceinline__ Decision decide(i64 s_tat, i64 s_exp, const Req &r) {
         d.allow_at = d.new_tat - r.dvt;
         d.allowed = r.now >= d.allow_at;
         const u64 ttl = (u64)((d.new_tat - r.now) + r.dvt);          // negative wraps (:179-183)
-        const u64 e = (u64)r.now + ttl;
-        d.new_exp = (e < ttl || e > (u64)I64_MAX) ? I64_MAX : (i64)e;
+        d.new_exp = expiry_code(r.now, ttl);
         return d;
     }
     d.tat = d.live ? max(s_tat, sat_sub(r.now, r.dvt)) : sat_sub(r.now, r.ei);
@@ -178,8 +196,7 @@ __device__ __forceinline__ Decision decide(i64 s_tat, i64 s_exp, const Req &r) {
     d.allow_at = sat_sub(d.new_tat, r.dvt);
     d.allowed = r.now >= d.allow_at;
     u64 ttl = (u64)sat_add(sat_sub(d.new_tat, r.now), r.dvt);   // negative wraps (:179-183)
-    u64 e = (u64)r.now + ttl;
-    d.new_exp = (e < ttl || e > (u64)I64_MAX) ? I64_MAX : (i64)e;
+    d.new_exp = expiry_code(r.now, ttl);
     return d;
 }
 

@@ -367,12 +367,12 @@ decide_index_kernel(Table t, BatchView b, const PolicyDerived *__restrict__ pol,
             }
             const bool mut = d.allowed && ((d.new_tat != s.tat) | (d.new_exp != s.exp));
             // a write over an entry that exists but is expired (adaptive_cleanup.rs:233,267)
-            const bool hit = d.allowed && !d.live && s.exp >= 0;
+            const bool hit = d.allowed && !d.live && has_state(s.exp);
             if (!(bits & F_SHARED)) {
                 // the only request of the batch on this key: final, and its write is the key's only write
                 flags[row] = 0;
                 if (mut && !(dbg & 1)) {
-                    const bool created = s.exp < 0;
+                    const bool created = !has_state(s.exp);
                     RunState ns = {d.new_tat, d.new_exp, r.ei};
                     store_state(t, slot, ns, created);
                     real_inc += created ? 1 : 0;
@@ -527,7 +527,7 @@ resolve_kernel(Table t, BatchView b, const PolicyDerived *__restrict__ pol, u32 
                         RunState s;
                         load_state(t, slot[k], s);
                         const Decision d = decide(s.tat, s.exp, r);
-                        const bool created = s.exp < 0;
+                        const bool created = !has_state(s.exp);
                         RunState ns = {d.new_tat, d.new_exp, r.ei};
                         store_state(t, slot[k], ns, created);
                         real_inc += created ? 1 : 0;

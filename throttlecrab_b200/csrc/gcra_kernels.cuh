@@ -538,7 +538,7 @@ __device__ __forceinline__ void run_chunk(u32 lane, bool mine, u32 gmask, const 
         if (final_now) {
             fin = d;
             // a write over an entry that exists but is expired (adaptive_cleanup.rs:233,267)
-            if (d.allowed && !d.live && s.exp >= 0) n_exp_hits++;
+            if (d.allowed && !d.live && has_state(s.exp)) n_exp_hits++;
             if (mut) { s.tat = so_tat; s.exp = so_exp; mflag = true; }
             pending = false;
         }
@@ -689,7 +689,7 @@ __device__ __forceinline__ void decide_chunk(const Table &t, const u64 *sorted, 
     if (head && mine) load_state(t, slot, s);
     s.tat = __shfl_sync(0xffffffffu, s.tat, hl);
     s.exp = __shfl_sync(0xffffffffu, s.exp, hl);
-    const bool was_phantom = s.exp < 0;              // the key has no entry yet (same for every lane of the run)
+    const bool was_phantom = !has_state(s.exp);              // the key has no entry yet (same for every lane of the run)
 
     Decision fin;
     bool changed = false;
@@ -918,7 +918,7 @@ decide_runs_kernel(Table t, const u64 *__restrict__ sorted, const Req *__restric
         const u32 slot = (u32)(sorted[start] >> 32);
         RunState s0;
         load_state(t, slot, s0);
-        const bool was_phantom = s0.exp < 0;           // the key has no entry yet
+        const bool was_phantom = !has_state(s0.exp);           // the key has no entry yet
         Cands cd;
 #pragma unroll
         for (int c = 0; c < FSM_K; c++) { cd.tat[c] = s0.tat; cd.exp[c] = s0.exp; }
@@ -1027,7 +1027,7 @@ decide_runs_kernel(Table t, const u64 *__restrict__ sorted, const Req *__restric
                     out.template write<BY_ROW, R16>(idx, d, r);
                     n_allowed += d.allowed ? 1 : 0;
                     n_denied += d.allowed ? 0 : 1;
-                    if (d.allowed && !d.live && ce >= 0) exp_hits++;
+                    if (d.allowed && !d.live && has_state(ce)) exp_hits++;
                     pending = false;
                     if (((my_map >> (4 * in_idx)) & 0xF) == FSM_NEW) {
                         // this request created a state outside the candidate set: publish it
@@ -1128,7 +1128,7 @@ sweep_kernel(Table t, u64 total_slots, i64 now, int mode) {
         for (int u = 0; u < SWEEP_UNROLL; u++) {
             const u64 p = i + (u64)u * stride;
             const i64 ea = (i64)(a[u].x + a[u].y), eb = (i64)(b[u].x + b[u].y);
-            const bool xa = ea >= 0 && ea <= now, xb = eb >= 0 && eb <= now;   // entries Store::get no longer shows
+            const bool xa = has_state(ea) && !live_at(ea, now), xb = has_state(eb) && !live_at(eb, now);   // entries Store::get no longer shows
             if (xa | xb) {
                 longlong2 *dst = reinterpret_cast<longlong2 *>(&t.state[2 * p]);
                 const longlong2 va = xa ? make_longlong2(0, EXP_EMPTY) : make_longlong2((i64)a[u].x, (i64)a[u].y);
@@ -1157,7 +1157,7 @@ purge_kernel(Table t, u64 total_slots) {
     const u64 stride = (u64)gridDim.x * TILE_THREADS;
     for (u64 k = (u64)blockIdx.x * TILE_THREADS + threadIdx.x; k < total_slots; k += stride) {
         const ulonglong2 v = ld_stream(&t.state[k]);
-        if ((i64)(v.x + v.y) >= 0) continue;
+        if (has_state((i64)(v.x + v.y))) continue;
         if (t.keys[k] < 2) continue;
         const bool stash = k >= (u64)t.nb_main * 4;
         t.keys[k] = stash ? KEY_TOMB : KEY_EMPTY;
@@ -1191,7 +1191,7 @@ rehash_kernel(Table src, u64 src_slots, Table dst) {
         u64 k = src.keys[i];
         if (k < 2) continue;
         TatOff st = src.state[i];
-        if ((i64)((u64)st.tat + st.off) < 0) continue;   // keys without an entry are not carried over
+        if (!has_state((i64)((u64)st.tat + st.off))) continue;   // keys without an entry are not carried over
         bool fresh;
         u32 s = find_or_claim(dst, k, fresh);
         if (s == dst.null_slot) { atomicAdd(&dst.counters[C_INSERT_FAIL], 1ULL); continue; }
@@ -1209,10 +1209,6 @@ struct StoreOpResult { i64 value; int flag; int status; };
 
 // op: 0 get (adaptive_cleanup.rs:246-252), 1 cas (:221-244), 2 set_nx (:254-278),
 //     3 peek (entry as stored: res[0].value = tat, res[1].value = expiry)
-__device__ __forceinline__ i64 expiry_of(i64 now, u64 ttl) {
-    u64 e = (u64)now + ttl;
-    return (e < ttl || e > (u64)I64_MAX) ? I64_MAX : (i64)e;
-}
 
 __global__ void store_op_kernel(Table t, int op, u64 key, i64 a, i64 b, u64 ttl, i64 now,
                                 StoreOpResult *res) {
@@ -1226,14 +1222,14 @@ __global__ void store_op_kernel(Table t, int op, u64 key, i64 a, i64 b, u64 ttl,
             TatOff *l = t.state + s;
             if (fresh) atomicAdd(&t.counters[C_OCCUPIED], 1ULL);
             i64 ex = (i64)((u64)l->tat + l->off);   // EXP_EMPTY for a fresh or entry-less key
-            if (ex > now) {
+            if (live_at(ex, now)) {
                 r.flag = 0;                                  // live entry: :264-265
             } else {
                 l->tat = a;
-                l->off = (u64)expiry_of(now, ttl) - (u64)a;
+                l->off = (u64)expiry_code(now, ttl) - (u64)a;
                 r.flag = 1;
                 atomicAdd(&t.counters[C_ALLOWED], 1ULL);     // one mutating op
-                if (ex < 0) atomicAdd(&t.counters[C_REAL], 1ULL);
+                if (!has_state(ex)) atomicAdd(&t.counters[C_REAL], 1ULL);
                 else atomicAdd(&t.counters[C_EXPIRED_HITS], 1ULL);   // :267
             }
         }
@@ -1244,16 +1240,16 @@ __global__ void store_op_kernel(Table t, int op, u64 key, i64 a, i64 b, u64 ttl,
             i64 tat = l->tat;
             i64 ex = (i64)((u64)tat + l->off);
             if (op == 3) {
-                if (ex >= 0) { r.flag = 1; r.value = tat; res[1].value = ex; }
-            } else if (ex > now) {
+                if (has_state(ex)) { r.flag = 1; r.value = tat; res[1].value = expiry_value(ex); }
+            } else if (live_at(ex, now)) {
                 if (op == 0) { r.flag = 1; r.value = tat; }
                 else if (tat == a) {                         // :236-240
                     l->tat = b;
-                    l->off = (u64)expiry_of(now, ttl) - (u64)b;
+                    l->off = (u64)expiry_code(now, ttl) - (u64)b;
                     r.flag = 1;
                     atomicAdd(&t.counters[C_ALLOWED], 1ULL);
                 }
-            } else if (op == 1 && ex >= 0) {
+            } else if (op == 1 && has_state(ex)) {
                 atomicAdd(&t.counters[C_EXPIRED_HITS], 1ULL);        // :232-235
             }
         }
@@ -1359,7 +1355,7 @@ route_unpermute_kernel(const gcra_result *__restrict__ routed, const u32 *__rest
 // ---------------------------------------------------------------------------------------------
 // snapshot restore (gcra_snapshot_restore): one staged chunk of a snapshot file's key, state and ei sections
 // ---------------------------------------------------------------------------------------------
-// An entry is carried when its key word is >= 2 and its state is a real entry (expiry = tat + off >= 0, expired or
+// An entry is carried when its key word is >= 2 and its state is a real entry (has_state(tat + off), expired or
 // not, as rehash_kernel keeps them), and shard `rank` of `world` owns it: owner_of(unmix64(key word)).  The key hashes
 // whose mix64 is 0 or 1 share the key words 2 and 3 with those whose mix64 is 2 or 3 (stored_key); such a shared entry
 // goes to the owner of the unmixed key word, i.e. of the latter.
@@ -1376,7 +1372,7 @@ restore_kernel(Table t, const u64 *__restrict__ keys, const TatOff *__restrict__
     const u64 stride = (u64)gridDim.x * TILE_THREADS;
     for (u64 i = (u64)blockIdx.x * TILE_THREADS + threadIdx.x; i < n; i += stride) {
         const ulonglong2 v = ld_stream(&state[i]);
-        if ((i64)(v.x + v.y) < 0) continue;
+        if (!has_state((i64)(v.x + v.y))) continue;
         const u64 k = keys[i];
         if (k < 2 || owner_of(unmix64(k), world) != rank) continue;
         if (!INSERT) { owned++; continue; }
@@ -1385,7 +1381,7 @@ restore_kernel(Table t, const u64 *__restrict__ keys, const TatOff *__restrict__
         if (s == t.null_slot) { failed++; continue; }
         if (!fresh) {
             const TatOff cur = t.state[s];
-            if ((i64)((u64)cur.tat + cur.off) >= 0) { conflicts++; continue; }
+            if (has_state((i64)((u64)cur.tat + cur.off))) { conflicts++; continue; }
         }
         *reinterpret_cast<ulonglong2 *>(&t.state[s]) = v;
         t.ei[s] = ei[i];
