@@ -9,7 +9,13 @@ plain sequential application on random runs of requests on ONE key:
 
 This is a model of the ALGORITHM (the CUDA kernels are tested against the oracle on the GPU); it documents why
 the parallel evaluation reproduces the sequential semantics bit for bit, including keys that toggle between
-states (max_burst = 1 with zero-quantity requests)."""
+states (max_burst = 1 with zero-quantity requests).
+
+`fsm_rounds_kernel` follows the hot-run kernel itself (plain rounds first, its candidate bookkeeping, its strides) and
+reports which of its events a run reaches; tests/test_gpu_fsm_cycles.py uses it to prove that its key sequences
+reach the events they are meant to, then runs them on the GPU against the oracle."""
+import numpy as np
+import pytest
 from hypothesis import given, settings, strategies as st
 
 from test_oracle_vs_python_model import I64_MAX, U64, clamp, derive, wrap64, _tdiv
@@ -98,6 +104,173 @@ def fsm_rounds(run, s0, k=4, stride=16):
     return outs, cands[cur]
 
 
+# ---------------------------------------------------------------------------------------------------------
+# decide_runs_kernel (csrc/gcra_kernels.cuh) step by step: plain rounds until FSM_AFTER state changes, then
+# finite-state rounds over nibble maps; Cands::find (last match among the first nc), the round-robin victim,
+# one stride of the group (512 rows for a CTA, 4096 for a cluster) after another
+# ---------------------------------------------------------------------------------------------------------
+FSM_NEW = 0xF
+
+
+def fsm_ident(k):
+    return sum(c << (4 * c) for c in range(k))
+
+
+def fsm_compose(f, g, k):
+    """fsm_compose: first f, then g (nibble maps over k candidates; FSM_NEW stays FSM_NEW)"""
+    gg = g | (0xF << 60)
+    return sum(((gg >> (4 * ((f >> (4 * c)) & 0xF))) & 0xF) << (4 * c) for c in range(k))
+
+
+class Events:
+    """What a run made the kernel do: the largest nc, the evictions (of s0, of the candidate `cur` pointed at),
+    insertions of a state evicted earlier in the run, plain-round returns to a known candidate, changes back to the
+    candidate holding s0, the run position of every state change with its round kind and outcome, the run position of
+    the change that switches to finite-state rounds, and the number of finite-state rounds."""
+
+    def __init__(self):
+        self.max_nc, self.evictions, self.s0_evicted, self.cur_evicted = 1, 0, False, 0
+        self.evicted_returns, self.plain_returns, self.s0_returns, self.fsm_rounds = 0, 0, 0, 0
+        self.changes = []           # (run position, finite-state round?, "new" | "known")
+        self.switch_pos = None      # run position of the FSM_AFTER-th change
+        self.switch_mid_stride = False   # ... with rows of its stride still pending: a finite-state round follows
+
+    def new_at(self, stride):
+        """stride positions of the requests whose state joined the candidate set"""
+        return {p % stride for p, _, kind in self.changes if kind == "new"}
+
+
+def fsm_rounds_kernel(run, s0, stride, k=4, fsm_after=4):
+    """The hot-run kernel on one run: (outputs, final state, Events).  Each round evaluates the pending requests
+    of the stride in order until the first one that leaves the candidate set (plain rounds: the first one that
+    changes the state); the requests before it and itself are final, exactly what the kernel's min-reduction or
+    prefix scan of composed maps decides.  The requests behind it wait for the next round, whose maps the kernel
+    computes afresh, so evaluating them now would change nothing."""
+    cache = {}
+
+    def dec(s, r):
+        v = cache.get((s, r))
+        if v is None:
+            v = cache[(s, r)] = decide(s, r)
+        return v
+
+    outs = [None] * len(run)
+    cands = [s0] * k
+    nc, cur, victim, n_changes = 1, 0, 0, 0
+    ev, evicted = Events(), set()
+
+    def find(s):                                             # Cands::find: the LAST match among the first nc
+        j = FSM_NEW
+        for c in range(k):
+            if c < nc and cands[c] == s:
+                j = c
+        return j
+
+    ident = fsm_ident(k)
+    for base in range(0, len(run), stride):
+        pending = list(range(base, min(base + stride, len(run))))
+        while True:
+            fsm = n_changes >= fsm_after
+            ev.fsm_rounds += fsm
+            creator, done = None, 0
+            if not fsm:                                      # plain round: up to the first state change
+                s = cands[cur]
+                for i in pending:
+                    done += 1
+                    outs[i] = dec(s, run[i])[2]
+                    if dec(s, run[i])[1] != s:
+                        creator, cin = i, cur
+                        break
+            else:                                            # finite-state round: maps and their prefix
+                excl = ident
+                for i in pending:
+                    m = 0
+                    for c in range(k):
+                        o = FSM_NEW
+                        if c < nc:
+                            ns = dec(cands[c], run[i])[1]
+                            o = c if ns == cands[c] else find(ns)
+                        m |= o << (4 * c)
+                    cin = (excl >> (4 * cur)) & 0xF          # this request's true input candidate
+                    done += 1
+                    outs[i] = dec(cands[cin], run[i])[2]
+                    to = (m >> (4 * cin)) & 0xF
+                    ev.s0_returns += to not in (FSM_NEW, cin) and cands[to] == s0
+                    excl = fsm_compose(excl, m, k)
+                    if (excl >> (4 * cur)) & 0xF == FSM_NEW:
+                        creator = i
+                        break
+            pending = pending[done:]
+            if creator is None:
+                if fsm:
+                    cur = (excl >> (4 * cur)) & 0xF
+                break
+            ps = dec(cands[cin], run[creator])[1]
+            v = find(ps)
+            if v == FSM_NEW:
+                if nc < k:
+                    v, nc = nc, nc + 1
+                else:
+                    v, victim = victim, (victim + 1) % k
+                    ev.evictions += 1
+                    ev.s0_evicted |= cands[v] == s0
+                    ev.cur_evicted += v == cur
+                    evicted.add(cands[v])
+                ev.evicted_returns += ps in evicted
+                cands[v] = ps
+                ev.changes.append((creator, fsm, "new"))
+            else:
+                ev.plain_returns += 1
+                ev.s0_returns += cands[v] == s0
+                ev.changes.append((creator, fsm, "known"))
+            ev.max_nc = max(ev.max_nc, nc)
+            cur = v
+            n_changes += 1
+            if n_changes == fsm_after:
+                ev.switch_pos, ev.switch_mid_stride = creator, len(pending) > 0
+    return outs, cands[cur], ev
+
+
+def residue_view(run, s0):
+    """The run as the index-order pipeline's residue tail decides it: the rows behind the first state change, from
+    the state that change committed (pass C).  (None, None) when nothing changes: no residue."""
+    s = s0
+    for i, r in enumerate(run):
+        ns = decide(s, r)[1]
+        if ns != s:
+            return run[i + 1:], ns
+    return None, None
+
+
+# K-cycles (DESIGN.md section 5): policies with one rate (10 per 60 s) and max_burst 8, 7, ..., 3.  With a live entry
+# whose tat is at or above now, a q = 0 request with dvt = ei * (max_burst - 1) is allowed when tat <= now + dvt, leaves
+# tat and sets the expiry to tat + dvt: rotating through K of these policies at one clock walks the entry through
+# exactly K states.  A q = 1 request moves tat up by ei (a new family of states); q = DENY is never allowed.
+CYCLE_POLICIES = [(8 - c, 10, 60) for c in range(6)]
+DENY = 40
+
+
+def cycle_steps(n, k, start=0, rng=None, q1_at=(), deny_at=()):
+    """(policy index into CYCLE_POLICIES, quantity) of n rows rotating through the first k policies from `start`
+    (or, with `rng`, drawing each row's policy at random among them), with q = 1 rows and denied rows at the given
+    positions."""
+    pol = (start + np.arange(n)) % k if rng is None else rng.integers(0, k, n)
+    q = np.zeros(n, np.int64)
+    q[list(q1_at)] = 1
+    q[list(deny_at)] = DENY
+    return pol.astype(np.int64), q
+
+
+def model_run(pol, q, now, policies=CYCLE_POLICIES):
+    der = [derive(*p) for p in policies]
+    return [(int(t), der[p][1], der[p][2], int(x)) for p, x, t in zip(pol.tolist(), q.tolist(), np.broadcast_to(now, len(pol)).tolist())]
+
+
+def run_stride(n):
+    """the group a run of n rows gets: None (warp chunks), 512 (one CTA) or 4096 (an 8-CTA cluster)"""
+    return None if n < 256 else 512 if n < 4096 else 4096
+
+
 T0 = 1_700_000_000 * 10**9
 policies = st.sampled_from([(1, 1, 1), (1, 3, 3600), (2, 120, 60), (5, 10, 60), (100, 1000, 60), (3, 7, 60)])
 req = st.tuples(policies, st.sampled_from([0, 0, 1, 1, 1, 1, 2, 5]), st.sampled_from([0, 0, 0, 1000, 10**9, 7 * 10**9]))
@@ -115,7 +288,80 @@ def test_parallel_schemes_equal_sequential(reqs, start_with_entry):
     want = sequential(run, s0)
     assert speculate_commit(run, s0) == want
     assert fsm_rounds(run, s0) == want
+    for stride in (16, 512):
+        assert fsm_rounds_kernel(run, s0, stride)[:2] == want
 
+
+CYCLE_DER = [derive(*p) for p in CYCLE_POLICIES]
+
+
+def cycle_state(c, j, now=T0):
+    """the state of a live entry in family j (tat = now - ei + j * ei) after a q = 0 row of cycle policy c"""
+    _, ei, dvt = CYCLE_DER[c]
+    return (now - ei + j * ei, now - ei + j * ei + dvt)
+
+
+@settings(max_examples=60, deadline=None)
+@given(st.integers(1, 6), st.integers(1, 9000), st.sampled_from([512, 4096]), st.integers(0, 2**32 - 1), st.booleans(),
+       st.sampled_from(["fresh", "cycle", "family"]), st.integers(0, 4), st.sampled_from([0.0, 0.02, 0.3]),
+       st.sampled_from([0, 10**6, 6 * 10**9]))
+def test_kernel_rounds_on_k_cycles(k, n, stride, seed, periodic, start, n_q1, deny, step):
+    """K-cycle runs (K = 1..6, periodic or random order, with q = 1 and denied rows, clocks that stand still or move)
+    through the kernel-faithful model at both group strides, and their index-order residues."""
+    rng = np.random.default_rng(seed)
+    pol, q = cycle_steps(n, k, start=int(rng.integers(k)), rng=None if periodic else rng,
+                         q1_at=rng.choice(n, min(n_q1, n), replace=False), deny_at=np.nonzero(rng.random(n) < deny)[0])
+    now = T0 + np.cumsum(np.where(rng.random(n) < 0.01, step, 0))
+    run = model_run(pol, q, now)
+    s0 = {"fresh": None, "cycle": cycle_state(0, 0), "family": cycle_state(2, 2)}[start]
+    want = sequential(run, s0)
+    outs, fin, ev = fsm_rounds_kernel(run, s0, stride)
+    assert (outs, fin) == want
+    assert ev.max_nc <= 4 and ev.evictions <= len(ev.changes)
+    res, rs0 = residue_view(run, s0)
+    if res is not None:
+        outs, fin, _ = fsm_rounds_kernel(res, rs0, stride)
+        assert (outs, fin) == (want[0][len(run) - len(res):], want[1])
+
+
+@pytest.mark.parametrize("stride", [512, 4096])
+@pytest.mark.parametrize("k", range(1, 7))
+def test_k_cycle_events(k, stride):
+    """The events a plain rotation through K policies makes the kernel reach over 3 strides and one row.  K <= 3 from
+    no entry (s0 differs from every cycle state): K + 1 candidates, K = 3 fills the set; K >= 4 from the state of the
+    first cycle policy (s0 is a cycle state): K = 4 fills the set exactly and returns to s0, K = 5 and 6 evict s0
+    and then every state they come back to."""
+    n = 3 * stride + 1
+    pol, q = cycle_steps(n, k, start=1 if k >= 4 else 0)
+    run = model_run(pol, q, T0)
+    s0 = cycle_state(0, 0) if k >= 4 else None
+    want = sequential(run, s0)
+    outs, fin, ev = fsm_rounds_kernel(run, s0, stride)
+    assert (outs, fin) == want
+    assert ev.max_nc == min(k + (k <= 3), 4)
+    assert (ev.evictions > 0) == (k >= 5)
+    assert ev.fsm_rounds > 0 if k >= 2 else ev.fsm_rounds == 0
+    assert ev.switch_pos == (3 if k >= 2 else None) and ev.switch_mid_stride == (k >= 2)
+    if k >= 2:
+        assert [p for p, fsm, _ in ev.changes[:4]] == [0, 1, 2, 3] and not any(f for _, f, _ in ev.changes[:4])
+    if k == 4:
+        assert ev.s0_returns > 0
+    if k >= 5:
+        assert ev.s0_evicted and ev.evicted_returns == ev.evictions - (k - 4) > 0
+        assert ev.new_at(stride) >= {stride - 1, 0}         # new states at both edges of a stride
+
+
+
+@pytest.mark.parametrize("scenario", ["shape_trace-2", "shape_trace-3", "shape_trace-4", "shape_trace-5", "shape_trace-6",
+                                      "switch_trace", "many_runs_trace", "compact_trace", "pipelined_trace",
+                                      "small_trace"])
+def test_gpu_cycle_scenarios_reach_their_events(scenario):
+    """The key sequences of tests/test_gpu_fsm_cycles.py reach the kernel events each scenario names, in the sort
+    pipeline's view and in the index-order residue's view (each builder asserts its events)."""
+    import test_gpu_fsm_cycles as g
+    name, _, k = scenario.partition("-")
+    tr = getattr(g, name)(*([int(k)] if k else []))
+    assert tr.batches
 
 def test_toggling_key_needs_few_finite_state_rounds():
     """max_burst = 1 with zero-quantity requests: the entry flips between two states (SURVEY V8)."""
