@@ -16,6 +16,7 @@
 #include <memory>
 #include <string>
 #include <sys/stat.h>
+#include <type_traits>
 #include <unistd.h>
 #include <vector>
 
@@ -255,7 +256,7 @@ struct gcra_engine {
     uint32_t index_min = 0;          // batches of at least this many rows take the index-order pipeline (0: never)
     int prefetch_state = 0;
     uint32_t max_tiles = 0;
-    uint32_t grid_probe[3] = {}, grid_decide[3] = {};   // resident CTAs of the persistent kernels [RowFmt]
+    uint32_t grid_probe[FMT_COUNT] = {}, grid_decide[FMT_COUNT] = {};   // resident CTAs of the persistent kernels [RowFmt]
     uint32_t dbg = 0;                // timing experiments only (gcra_debug_set): skips parts of pass B
     uint32_t last_nres = 0, last_nres_rows = 0;   // newest residue size that has reached the host (and its batch's rows)
     bool adaptive = true;            // choose the pipeline from the residue feedback (off when a test / env forces one)
@@ -266,7 +267,7 @@ struct gcra_engine {
     // ring
     std::vector<RingSlot> ring;
     uint32_t ring_cap = 0;
-    int ring_mode = 0;               // gcra_ring_create: 0, 1 or 2 = the slots' RowFmt
+    int ring_fmt = FMT_48_32;        // the slots' RowFmt (gcra_ring_create)
     // denied requests per key (gcra_track_denied): device table, updated by a pass over every finished batch
     DeniedArrays denied_arrays;
     DeniedTable denied{};
@@ -595,6 +596,15 @@ static int enqueue_sort(gcra_engine *h, Scratch &sc, uint32_t n_max, const u32 *
     return GCRA_OK;
 }
 
+// The one place where a batch's run-time row format picks kernel instantiations: calls f(F) with F =
+// std::integral_constant<int, fmt>, so that `kernel<F>` and `Rows<F>` name the ones for `fmt`.
+template <typename Fn>
+static auto with_fmt(int fmt, Fn &&f) {
+    if (fmt == FMT_16_16) return f(std::integral_constant<int, FMT_16_16>{});
+    if (fmt == FMT_16_32) return f(std::integral_constant<int, FMT_16_32>{});
+    return f(std::integral_constant<int, FMT_48_32>{});
+}
+
 template <bool BY_ROW, bool R16>
 static int enqueue_decide_sorted_t(gcra_engine *h, Scratch &sc, uint32_t n_max, const u32 *n_dev, const u64 *src,
                                    const OutMap &om, cudaStream_t st) {
@@ -623,14 +633,13 @@ static int enqueue_decide_sorted_t(gcra_engine *h, Scratch &sc, uint32_t n_max, 
     return GCRA_OK;
 }
 
-// the warp-cooperative compare-and-update over sorted keys + the hot-run kernels; r16: 16-byte results (FMT_16_16)
+// the warp-cooperative compare-and-update over sorted keys + the hot-run kernels, writing result rows of format `fmt`
 static int enqueue_decide_sorted(gcra_engine *h, Scratch &sc, uint32_t n_max, const u32 *n_dev, const u64 *src,
-                                 const OutMap &om, bool r16, cudaStream_t st) {
-    if (r16)
-        return om.by_row ? enqueue_decide_sorted_t<true, true>(h, sc, n_max, n_dev, src, om, st)
-                         : enqueue_decide_sorted_t<false, true>(h, sc, n_max, n_dev, src, om, st);
-    return om.by_row ? enqueue_decide_sorted_t<true, false>(h, sc, n_max, n_dev, src, om, st)
-                     : enqueue_decide_sorted_t<false, false>(h, sc, n_max, n_dev, src, om, st);
+                                 const OutMap &om, int fmt, cudaStream_t st) {
+    return with_fmt(fmt, [&](auto F) {
+        return om.by_row ? enqueue_decide_sorted_t<true, Rows<F>::R16>(h, sc, n_max, n_dev, src, om, st)
+                         : enqueue_decide_sorted_t<false, Rows<F>::R16>(h, sc, n_max, n_dev, src, om, st);
+    });
 }
 
 // every set's per-row buffers of the index-order pipeline, for batches of up to `rows` row ids (never shrinking), made
@@ -659,9 +668,7 @@ static int alloc_index_scratch(gcra_engine *h, uint32_t rows) {
 static int enqueue_denied(gcra_engine *h, const BatchView &v, int fmt, cudaStream_t st) {
     if (!h->denied_max || v.nseg != 1 || v.n == 0) return GCRA_OK;
     const uint32_t tiles = (v.n + TILE_THREADS - 1) / TILE_THREADS;
-    if (fmt == FMT_16_16) denied_count_kernel<FMT_16_16><<<tiles, TILE_THREADS, 0, st>>>(v.req0, v.res0, v.n, h->denied);
-    else if (fmt == FMT_16_32) denied_count_kernel<FMT_16_32><<<tiles, TILE_THREADS, 0, st>>>(v.req0, v.res0, v.n, h->denied);
-    else denied_count_kernel<FMT_48_32><<<tiles, TILE_THREADS, 0, st>>>(v.req0, v.res0, v.n, h->denied);
+    with_fmt(fmt, [&](auto F) { denied_count_kernel<F><<<tiles, TILE_THREADS, 0, st>>>(v.req0, v.res0, v.n, h->denied); });
     h->launches++;
     CK(cudaGetLastError());
     return GCRA_OK;
@@ -689,15 +696,10 @@ static int enqueue_front(gcra_engine *h, Scratch &sc, const BatchView &v, bool i
         const uint32_t grid = std::min<uint32_t>(tiles, h->grid_probe[fmt]);    // persistent, software-pipelined CTAs
         CK(cudaMemsetAsync(sc.ctrl_block.get(), 0, ((size_t)h->max_tiles + 1) * sizeof(u64), st));
         if (timed) CK(cudaEventRecord(h->evd[0].get(), st));
-        if (fmt == FMT_16_16)
-            probe_kernel<FMT_16_16><<<grid, TILE_THREADS, 0, st>>>(h->tab, v, h->d_pol.get(), h->npol, now_batch, sc.slot_arr.get(),
-                                                                   sc.bitmap.get(), h->bm_mask, h->prefetch_state);
-        else if (fmt == FMT_16_32)
-            probe_kernel<FMT_16_32><<<grid, TILE_THREADS, 0, st>>>(h->tab, v, h->d_pol.get(), h->npol, now_batch, sc.slot_arr.get(),
-                                                                   sc.bitmap.get(), h->bm_mask, h->prefetch_state);
-        else
-            probe_kernel<FMT_48_32><<<grid, TILE_THREADS, 0, st>>>(h->tab, v, nullptr, 0, 0, sc.slot_arr.get(), sc.bitmap.get(), h->bm_mask,
-                                                               h->prefetch_state);
+        with_fmt(fmt, [&](auto F) {
+            probe_kernel<F><<<grid, TILE_THREADS, 0, st>>>(h->tab, v, h->d_pol.get(), h->npol, now_batch, sc.slot_arr.get(), sc.bitmap.get(),
+                                                           h->bm_mask, h->prefetch_state);
+        });
         if (timed) CK(cudaEventRecord(h->evd[1].get(), st));
         h->launches += 1;
         if (timed) { CK(cudaEventRecord(h->ev[1].get(), st)); CK(cudaEventRecord(h->evd[2].get(), st)); }
@@ -705,15 +707,10 @@ static int enqueue_front(gcra_engine *h, Scratch &sc, const BatchView &v, bool i
     }
     const uint32_t n = v.n;
     const uint32_t tiles = (n + TILE_THREADS - 1) / TILE_THREADS;
-    if (fmt == FMT_16_16)
-        ingest_kernel<FMT_16_16><<<tiles, TILE_THREADS, 0, st>>>(h->tab, v.req0, h->d_pol.get(), h->npol, now_batch, n,
-                                                                 sc.drec.get(), sc.keys_a.get(), v.res0);
-    else if (fmt == FMT_16_32)
-        ingest_kernel<FMT_16_32><<<tiles, TILE_THREADS, 0, st>>>(h->tab, v.req0, h->d_pol.get(), h->npol, now_batch, n,
-                                                                 sc.drec.get(), sc.keys_a.get(), v.res0);
-    else
-        ingest_kernel<FMT_48_32><<<tiles, TILE_THREADS, 0, st>>>(h->tab, v.req0, nullptr, 0, 0, n, sc.drec.get(),
-                                                             sc.keys_a.get(), v.res0);
+    with_fmt(fmt, [&](auto F) {
+        ingest_kernel<F><<<tiles, TILE_THREADS, 0, st>>>(h->tab, v.req0, h->d_pol.get(), h->npol, now_batch, n, sc.drec.get(),
+                                                         sc.keys_a.get(), v.res0);
+    });
     h->launches++;
     if (timed) CK(cudaEventRecord(h->ev[1].get(), st));
     RC(enqueue_sort(h, sc, n, nullptr, st, sorted_out));
@@ -738,30 +735,15 @@ static int enqueue_mid_index(gcra_engine *h, Scratch &sc, Scratch &next, const B
     const uint32_t rgrid = std::min<uint32_t>((rows + RES_TILE - 1) / RES_TILE + v.nseg, 6 * h->sms);
     u32 *ctrl = reinterpret_cast<u32 *>(sc.ctrl_block.get());
     u64 *status = sc.ctrl_block.get() + 1;
-    if (fmt == FMT_16_16) {
-        decide_index_kernel<FMT_16_16><<<grid, TILE_THREADS, 0, st>>>(h->tab, v, h->d_pol.get(), h->npol, now_batch, sc.slot_arr.get(),
-                                                                      sc.bitmap.get(), sc.pend.get(), h->bm_mask, sc.flags.get(), h->epoch, hp,
-                                                                      h->dbg);
+    RC(with_fmt(fmt, [&](auto F) {
+        decide_index_kernel<F><<<grid, TILE_THREADS, 0, st>>>(h->tab, v, h->d_pol.get(), h->npol, now_batch, sc.slot_arr.get(), sc.bitmap.get(),
+                                                              sc.pend.get(), h->bm_mask, sc.flags.get(), h->epoch, hp, h->dbg);
         if (timed) CK(cudaEventRecord(h->evd[3].get(), st));
-        resolve_kernel<FMT_16_16><<<rgrid, TILE_THREADS, 0, st>>>(h->tab, v, h->d_pol.get(), h->npol, now_batch, sc.slot_arr.get(),
-                                                                  h->bm_mask, sc.flags.get(), h->epoch, ctrl, status, sc.keys_a.get(),
-                                                                  next.pend.get(), sc.h_nres.get(), h->max_batch);
-    } else if (fmt == FMT_16_32) {
-        decide_index_kernel<FMT_16_32><<<grid, TILE_THREADS, 0, st>>>(h->tab, v, h->d_pol.get(), h->npol, now_batch, sc.slot_arr.get(),
-                                                                      sc.bitmap.get(), sc.pend.get(), h->bm_mask, sc.flags.get(), h->epoch, hp,
-                                                                      h->dbg);
-        if (timed) CK(cudaEventRecord(h->evd[3].get(), st));
-        resolve_kernel<FMT_16_32><<<rgrid, TILE_THREADS, 0, st>>>(h->tab, v, h->d_pol.get(), h->npol, now_batch, sc.slot_arr.get(),
-                                                                  h->bm_mask, sc.flags.get(), h->epoch, ctrl, status, sc.keys_a.get(),
-                                                                  next.pend.get(), sc.h_nres.get(), h->max_batch);
-    } else {
-        decide_index_kernel<FMT_48_32><<<grid, TILE_THREADS, 0, st>>>(h->tab, v, nullptr, 0, 0, sc.slot_arr.get(), sc.bitmap.get(), sc.pend.get(),
-                                                                  h->bm_mask, sc.flags.get(), h->epoch, hp, h->dbg);
-        if (timed) CK(cudaEventRecord(h->evd[3].get(), st));
-        resolve_kernel<FMT_48_32><<<rgrid, TILE_THREADS, 0, st>>>(h->tab, v, nullptr, 0, 0, sc.slot_arr.get(), h->bm_mask,
-                                                              sc.flags.get(), h->epoch, ctrl, status, sc.keys_a.get(),
-                                                              next.pend.get(), sc.h_nres.get(), h->max_batch);
-    }
+        resolve_kernel<F><<<rgrid, TILE_THREADS, 0, st>>>(h->tab, v, h->d_pol.get(), h->npol, now_batch, sc.slot_arr.get(), h->bm_mask,
+                                                          sc.flags.get(), h->epoch, ctrl, status, sc.keys_a.get(), next.pend.get(),
+                                                          sc.h_nres.get(), h->max_batch);
+        return GCRA_OK;
+    }));
     h->launches += 2;
     h->n_index_batches++;
     if (timed) CK(cudaEventRecord(h->evd[4].get(), st));
@@ -792,12 +774,12 @@ static int enqueue_tail_index(gcra_engine *h, Scratch &sc, const BatchView &v, i
     OutMap om{};
     om.out = nullptr;
     om.by_row = 1;
-    om.compact = fmt != FMT_48_32 ? 1 : 0;
+    om.compact = req_bytes(fmt) == sizeof(gcra_request16) ? 1 : 0;
     om.view = v;
     om.pol = h->d_pol.get();
     om.npol = h->npol;
     om.now_batch = now_batch;
-    RC(enqueue_decide_sorted(h, sc, n_max, n_res, rs, om, fmt == FMT_16_16, st));
+    RC(enqueue_decide_sorted(h, sc, n_max, n_res, rs, om, fmt, st));
     if (timed) { CK(cudaEventRecord(h->ev[3].get(), st)); h->ev_valid = true; CK(cudaEventRecord(h->evd[7].get(), st)); h->evd_valid = true; }
     CK(cudaGetLastError());
     return GCRA_OK;
@@ -809,7 +791,7 @@ static int enqueue_back_sorted(gcra_engine *h, Scratch &sc, const BatchView &v, 
     OutMap om{};
     om.out = v.res0;
     om.by_row = 0;
-    RC(enqueue_decide_sorted(h, sc, v.n, nullptr, sorted, om, fmt == FMT_16_16, st));
+    RC(enqueue_decide_sorted(h, sc, v.n, nullptr, sorted, om, fmt, st));
     if (timed) { CK(cudaEventRecord(h->ev[3].get(), st)); h->ev_valid = true; }
     CK(cudaGetLastError());
     return GCRA_OK;
@@ -817,7 +799,7 @@ static int enqueue_back_sorted(gcra_engine *h, Scratch &sc, const BatchView &v, 
 
 static int check_batch(gcra_engine *h, uint32_t n, int fmt) {
     if (n > h->max_batch) { h->err = "batch larger than max_batch"; return GCRA_INTERNAL; }
-    if (fmt != FMT_48_32 && h->npol == 0) { h->err = "no policy table registered"; return GCRA_INTERNAL; }
+    if (req_bytes(fmt) == sizeof(gcra_request16) && h->npol == 0) { h->err = "no policy table registered"; return GCRA_INTERNAL; }
     return ensure_room(h, n);
 }
 
@@ -826,7 +808,7 @@ static int launch_batch(gcra_engine *h, uint32_t n, const void *d_req, int fmt, 
                         void *d_res_rows, cudaStream_t st, bool timed) {
     if (n == 0) return GCRA_OK;
     RC(check_batch(h, n, fmt));
-    gcra_result *d_res = (gcra_result *)d_res_rows;     // (gcra_result16 rows for FMT_16_16: see BatchView::res16_at)
+    gcra_result *d_res = (gcra_result *)d_res_rows;     // (or gcra_result16 rows: see BatchView::res16_at)
     const uint32_t k = h->scr_next;
     Scratch &sc = h->scr[k];
     h->scr_next = (h->scr_next + 1) % gcra_engine::N_SCR;
@@ -839,12 +821,9 @@ static int launch_batch(gcra_engine *h, uint32_t n, const void *d_req, int fmt, 
         // small batch (a single rate_limit call, a lightly loaded actor): one CTA does ingest, ordering and
         // the compare-and-update in a single launch
         if (timed) { CK(cudaEventRecord(h->ev[0].get(), st)); CK(cudaEventRecord(h->ev[1].get(), st)); CK(cudaEventRecord(h->ev[2].get(), st)); }
-        if (fmt == FMT_16_16)
-            small_batch_kernel<FMT_16_16><<<1, TILE_THREADS, 0, st>>>(h->tab, d_req, h->d_pol.get(), h->npol, now_batch, n, sc.drec.get(), d_res);
-        else if (fmt == FMT_16_32)
-            small_batch_kernel<FMT_16_32><<<1, TILE_THREADS, 0, st>>>(h->tab, d_req, h->d_pol.get(), h->npol, now_batch, n, sc.drec.get(), d_res);
-        else
-            small_batch_kernel<FMT_48_32><<<1, TILE_THREADS, 0, st>>>(h->tab, d_req, nullptr, 0, 0, n, sc.drec.get(), d_res);
+        with_fmt(fmt, [&](auto F) {
+            small_batch_kernel<F><<<1, TILE_THREADS, 0, st>>>(h->tab, d_req, h->d_pol.get(), h->npol, now_batch, n, sc.drec.get(), d_res);
+        });
         h->launches++;
         if (timed) { CK(cudaEventRecord(h->ev[3].get(), st)); h->ev_valid = true; }
         CK(cudaGetLastError());
@@ -880,7 +859,7 @@ static int launch_batch(gcra_engine *h, uint32_t n, const void *d_req, int fmt, 
 static int launch_pipelined_view(gcra_engine *h, const BatchView &v, uint32_t n_rows, int fmt, int64_t now_batch,
                                  cudaEvent_t ready, cudaEvent_t *done) {
     // 16-byte results are a single-GPU format: the multi-GPU ticks return 32-byte rows into peers' outboxes
-    if (fmt == FMT_16_16 && v.nseg != 1) { h->err = "16-byte results need a single-segment batch"; return GCRA_INTERNAL; }
+    if (res_bytes(fmt) == sizeof(gcra_result16) && v.nseg != 1) { h->err = "16-byte results need a single-segment batch"; return GCRA_INTERNAL; }
     RC(check_batch(h, n_rows, fmt));
     const uint32_t k = h->scr_next;
     Scratch &sc = h->scr[k];
@@ -974,8 +953,11 @@ static void preload(K kernel) {
 }
 
 static void preload_kernels() {
-    preload(ingest_kernel<FMT_48_32>); preload(ingest_kernel<FMT_16_32>); preload(ingest_kernel<FMT_16_16>);
-    preload(small_batch_kernel<FMT_48_32>); preload(small_batch_kernel<FMT_16_32>); preload(small_batch_kernel<FMT_16_16>);
+    for (int fmt = 0; fmt < FMT_COUNT; fmt++)
+        with_fmt(fmt, [](auto F) {
+            preload(ingest_kernel<F>); preload(small_batch_kernel<F>); preload(denied_count_kernel<F>);
+            preload(probe_kernel<F>); preload(decide_index_kernel<F>); preload(resolve_kernel<F>);
+        });
     preload(sort_digits_kernel); preload(sort_sweep_kernel);
     preload(decide_kernel<false, false>); preload(decide_kernel<true, false>);
     preload(decide_kernel<false, true>); preload(decide_kernel<true, true>);
@@ -983,14 +965,10 @@ static void preload_kernels() {
     preload(decide_runs_kernel<1, true, false>); preload(decide_runs_kernel<CLUSTER_CTAS, true, false>);
     preload(decide_runs_kernel<1, false, true>); preload(decide_runs_kernel<CLUSTER_CTAS, false, true>);
     preload(decide_runs_kernel<1, true, true>); preload(decide_runs_kernel<CLUSTER_CTAS, true, true>);
-    preload(probe_kernel<FMT_48_32>); preload(probe_kernel<FMT_16_32>); preload(probe_kernel<FMT_16_16>);
-    preload(decide_index_kernel<FMT_48_32>); preload(decide_index_kernel<FMT_16_32>); preload(decide_index_kernel<FMT_16_16>);
-    preload(resolve_kernel<FMT_48_32>); preload(resolve_kernel<FMT_16_32>); preload(resolve_kernel<FMT_16_16>);
     preload(sweep_kernel); preload(purge_kernel); preload(clear_slots_kernel); preload(rehash_kernel); preload(store_op_kernel);
     preload(route_count_kernel); preload(route_scan_kernel); preload(route_scatter_kernel); preload(route_unpermute_kernel);
     preload(p2p_scan_kernel); preload(p2p_scatter_kernel); preload(p2p_signal_req_kernel); preload(p2p_signal_res_kernel);
     preload(p2p_wait_kernel); preload(p2p_unpermute_kernel);
-    preload(denied_count_kernel<FMT_48_32>); preload(denied_count_kernel<FMT_16_32>); preload(denied_count_kernel<FMT_16_16>);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -1052,15 +1030,15 @@ static int init_engine(gcra_engine *h, const gcra_config *cfg) {
         if (const char *g = getenv("GCRA_ADAPTIVE")) h->adaptive = atoi(g) != 0;
         h->prefetch_state = 0;
         if (const char *g = getenv("GCRA_PREFETCH")) h->prefetch_state = atoi(g);
-        int nb = 0;
-        h->grid_probe[0] = h->grid_probe[1] = h->grid_probe[2] = 4 * h->sms;      // used when the occupancy query fails
-        h->grid_decide[0] = h->grid_decide[1] = h->grid_decide[2] = 3 * h->sms;
-        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, probe_kernel<FMT_48_32>, TILE_THREADS, 0) == cudaSuccess && nb > 0) h->grid_probe[0] = (uint32_t)(nb * sms);
-        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, probe_kernel<FMT_16_32>, TILE_THREADS, 0) == cudaSuccess && nb > 0) h->grid_probe[1] = (uint32_t)(nb * sms);
-        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, probe_kernel<FMT_16_16>, TILE_THREADS, 0) == cudaSuccess && nb > 0) h->grid_probe[2] = (uint32_t)(nb * sms);
-        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, decide_index_kernel<FMT_48_32>, TILE_THREADS, 0) == cudaSuccess && nb > 0) h->grid_decide[0] = (uint32_t)(nb * sms);
-        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, decide_index_kernel<FMT_16_32>, TILE_THREADS, 0) == cudaSuccess && nb > 0) h->grid_decide[1] = (uint32_t)(nb * sms);
-        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, decide_index_kernel<FMT_16_16>, TILE_THREADS, 0) == cudaSuccess && nb > 0) h->grid_decide[2] = (uint32_t)(nb * sms);
+        for (int fmt = 0; fmt < FMT_COUNT; fmt++) {
+            h->grid_probe[fmt] = 4 * h->sms;      // used when the occupancy query fails
+            h->grid_decide[fmt] = 3 * h->sms;
+            with_fmt(fmt, [&](auto F) {
+                int nb = 0;
+                if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, probe_kernel<F>, TILE_THREADS, 0) == cudaSuccess && nb > 0) h->grid_probe[fmt] = (uint32_t)(nb * sms);
+                if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, decide_index_kernel<F>, TILE_THREADS, 0) == cudaSuccess && nb > 0) h->grid_decide[fmt] = (uint32_t)(nb * sms);
+            });
+        }
         // tuning: CTAs per SM of the persistent kernels (fewer leave room for the other stages' kernels)
         if (const char *g = getenv("GCRA_CTAS_PROBE")) { uint32_t c = (uint32_t)atoi(g) * sms; if (c) for (auto &x : h->grid_probe) x = std::min(x, c); }
         if (const char *g = getenv("GCRA_CTAS_DECIDE")) { uint32_t c = (uint32_t)atoi(g) * sms; if (c) for (auto &x : h->grid_decide) x = std::min(x, c); }
@@ -1304,16 +1282,14 @@ int32_t gcra_pipeline_join(gcra_engine *h, void *stream) {
 
 static int host_batch(gcra_engine *h, uint64_t n, const void *req, int fmt, int64_t now_batch, void *res) {
     CK(cudaSetDevice(h->device));
-    const bool compact = fmt != FMT_48_32;
-    const size_t rsz = compact ? sizeof(gcra_request16) : sizeof(gcra_request);
-    const size_t ressz = fmt == FMT_16_16 ? sizeof(gcra_result16) : sizeof(gcra_result);
+    const size_t rsz = req_bytes(fmt), ressz = res_bytes(fmt);
     uint64_t done = 0;
     while (done < n) {
         uint32_t m = (uint32_t)std::min<uint64_t>(n - done, h->max_batch);
         const unsigned char *src = (const unsigned char *)req + done * rsz;
         // like the reference's mutating ops, sweep (if the store's policy says so) BEFORE the work
         // (adaptive_cleanup.rs:229,261), with the clock of the first request of the chunk
-        int64_t now_hint = compact ? now_batch : ((const gcra_request *)req)[done].now_ns;
+        int64_t now_hint = rsz == sizeof(gcra_request) ? ((const gcra_request *)req)[done].now_ns : now_batch;
         int rc = apply_policy(h, now_hint);
         if (rc) return rc;
         CK(cudaMemcpyAsync(h->d_req.get(), src, (size_t)m * rsz, cudaMemcpyHostToDevice, h->stream.get()));
@@ -1416,8 +1392,7 @@ int32_t gcra_ring_create(gcra_engine *h, uint32_t slots, uint32_t slot_capacity,
     if (slot_capacity == 0 || slot_capacity > h->max_batch) { h->err = "slot_capacity must be in 1..max_batch"; return GCRA_INTERNAL; }
     // 0: 48-byte requests, 32-byte results; any other value but 2: 16-byte requests, 32-byte results; 2: 16 / 16
     const int fmt = mode == 0 ? FMT_48_32 : mode == 2 ? FMT_16_16 : FMT_16_32;
-    const size_t rsz = fmt != FMT_48_32 ? sizeof(gcra_request16) : sizeof(gcra_request);
-    const size_t ressz = fmt == FMT_16_16 ? sizeof(gcra_result16) : sizeof(gcra_result);
+    const size_t rsz = req_bytes(fmt), ressz = res_bytes(fmt);
     std::vector<RingSlot> ring(slots);    // (a failed call leaves no ring)
     for (auto &s : ring) {
         // request slots are only WRITTEN by the host: optionally write-combined pinned memory (GCRA_RING_WC=1)
@@ -1430,16 +1405,16 @@ int32_t gcra_ring_create(gcra_engine *h, uint32_t slots, uint32_t slot_capacity,
     }
     h->ring = std::move(ring);
     h->ring_cap = slot_capacity;
-    h->ring_mode = fmt;
+    h->ring_fmt = fmt;
     return GCRA_OK;
 }
 
 void *gcra_ring_requests(gcra_engine *h, uint32_t slot) { return slot < h->ring.size() ? h->ring[slot].h_req.get() : nullptr; }
 gcra_result *gcra_ring_results(gcra_engine *h, uint32_t slot) {
-    return slot < h->ring.size() && h->ring_mode != FMT_16_16 ? (gcra_result *)h->ring[slot].h_res.get() : nullptr;
+    return slot < h->ring.size() && res_bytes(h->ring_fmt) == sizeof(gcra_result) ? (gcra_result *)h->ring[slot].h_res.get() : nullptr;
 }
 gcra_result16 *gcra_ring_results16(gcra_engine *h, uint32_t slot) {
-    return slot < h->ring.size() && h->ring_mode == FMT_16_16 ? (gcra_result16 *)h->ring[slot].h_res.get() : nullptr;
+    return slot < h->ring.size() && res_bytes(h->ring_fmt) == sizeof(gcra_result16) ? (gcra_result16 *)h->ring[slot].h_res.get() : nullptr;
 }
 
 int32_t gcra_ring_submit(gcra_engine *h, uint32_t slot, uint32_t n, int64_t now_ns) {
@@ -1449,13 +1424,12 @@ int32_t gcra_ring_submit(gcra_engine *h, uint32_t slot, uint32_t n, int64_t now_
     if (s.in_flight) { h->err = "ring slot still in flight"; return GCRA_INTERNAL; }
     // sweep policy with the counters of the batches finished so far (no stall)
     if (cudaEventQuery(h->ev_counters.get()) == cudaSuccess) { int rc = apply_policy(h, now_ns); if (rc) return rc; }
-    const size_t rsz = h->ring_mode != FMT_48_32 ? sizeof(gcra_request16) : sizeof(gcra_request);
-    const size_t ressz = h->ring_mode == FMT_16_16 ? sizeof(gcra_result16) : sizeof(gcra_result);
+    const size_t rsz = req_bytes(h->ring_fmt), ressz = res_bytes(h->ring_fmt);
     CK(cudaMemcpyAsync(s.d_req.get(), s.h_req.get(), (size_t)n * rsz, cudaMemcpyHostToDevice, h->in_stream.get()));
     CK(cudaEventRecord(s.ev_in.get(), h->in_stream.get()));
     // front half (ingest + order) of this slot overlaps the back half (decide) of the previous one
     cudaEvent_t done = nullptr;
-    int rc = launch_pipelined(h, n, s.d_req.get(), h->ring_mode, now_ns, s.d_res.get(), s.ev_in.get(), &done);
+    int rc = launch_pipelined(h, n, s.d_req.get(), h->ring_fmt, now_ns, s.d_res.get(), s.ev_in.get(), &done);
     if (rc) return rc;
     if (done) CK(cudaStreamWaitEvent(h->out_stream.get(), done, 0));
     CK(cudaMemcpyAsync(h->h_counters.get(), h->tab.counters, C_COUNT * sizeof(u64), cudaMemcpyDeviceToHost, h->out_stream.get()));

@@ -150,9 +150,8 @@ template <int FMT>
 __global__ void __launch_bounds__(TILE_THREADS)
 probe_kernel(Table t, BatchView b, const PolicyDerived *__restrict__ pol, u32 npol, i64 now_batch,
              u32 *__restrict__ slot_arr, u32 *__restrict__ counters, u32 bm_mask, int prefetch_state) {
-    constexpr bool COMPACT = FMT != FMT_48_32;
-    constexpr u32 RSZ = COMPACT ? sizeof(gcra_request16) : sizeof(gcra_request);
-    __shared__ __align__(128) unsigned char stage[2][TILE_THREADS * RSZ];
+    using Row = Rows<FMT>;
+    __shared__ __align__(128) unsigned char stage[2][TILE_THREADS * Row::REQ_BYTES];
     __shared__ __align__(8) u64 bar[2];
     // the distinct slots of the current tile and how often each occurs (see "counters" above)
     __shared__ u32 hkey[NOTE_HASH];
@@ -167,32 +166,32 @@ probe_kernel(Table t, BatchView b, const PolicyDerived *__restrict__ pol, u32 np
     const u32 G = gridDim.x;
     u32 tile = blockIdx.x;
     TileRef cur, nxt;
-    if (!tile_lookup(b, tile, RSZ, cur)) return;
-    bool has_nxt = tile_lookup(b, tile + G, RSZ, nxt);
+    if (!tile_lookup(b, tile, Row::REQ_BYTES, cur)) return;
+    bool has_nxt = tile_lookup(b, tile + G, Row::REQ_BYTES, nxt);
     if (threadIdx.x == 0) {
-        issue_tile(stage[0], &bar[0], cur, RSZ);
-        if (has_nxt) issue_tile(stage[1], &bar[1], nxt, RSZ);
+        issue_tile(stage[0], &bar[0], cur, Row::REQ_BYTES);
+        if (has_nxt) issue_tile(stage[1], &bar[1], nxt, Row::REQ_BYTES);
     }
     u32 par = 0;                 // phase parity of the two barriers, one bit each
     u32 buf = 0;
     mbar_wait(&bar[0], 0);
     par ^= 1;
     KeyProbe kc;
-    probe_start(t, stage[0] + (size_t)threadIdx.x * RSZ, threadIdx.x < cur.cnt, kc);
+    probe_start(t, stage[0] + (size_t)threadIdx.x * Row::REQ_BYTES, threadIdx.x < cur.cnt, kc);
     u32 n_fresh = 0, n_err = 0;
     for (;;) {
         KeyProbe kn;
         if (has_nxt) {
             mbar_wait(&bar[buf ^ 1], (par >> (buf ^ 1)) & 1);
             par ^= 1u << (buf ^ 1);
-            probe_start(t, stage[buf ^ 1] + (size_t)threadIdx.x * RSZ, threadIdx.x < nxt.cnt, kn);
+            probe_start(t, stage[buf ^ 1] + (size_t)threadIdx.x * Row::REQ_BYTES, threadIdx.x < nxt.cnt, kn);
         }
         const bool in_range = threadIdx.x < cur.cnt;
         const u32 row = cur.row0 + threadIdx.x;
         if (in_range) {
             u64 key_hash = 0;
             Req r = {0, 0, 0, 0};
-            int status = parse_request<COMPACT>(stage[buf] + (size_t)threadIdx.x * RSZ, pol, npol, now_batch, key_hash, r);
+            int status = parse_request<Row::COMPACT>(stage[buf] + (size_t)threadIdx.x * Row::REQ_BYTES, pol, npol, now_batch, key_hash, r);
             u32 slot = t.null_slot;
             if (status == 0) {
                 bool fresh;
@@ -202,7 +201,7 @@ probe_kernel(Table t, BatchView b, const PolicyDerived *__restrict__ pol, u32 np
             }
             slot_arr[row] = slot;
             if (status != 0) {
-                if (FMT == FMT_16_16) write_result16(b.res16_at(row), 0, status, 0);
+                if (Row::R16) write_result16(b.res16_at(row), 0, status, 0);
                 else write_result(b.res_at(row), 0, 0, 0, status, 0);
                 n_err++;
             }
@@ -231,8 +230,8 @@ probe_kernel(Table t, BatchView b, const PolicyDerived *__restrict__ pol, u32 np
         tile += G;
         cur = nxt;
         kc = kn;
-        has_nxt = tile_lookup(b, tile + G, RSZ, nxt);
-        if (has_nxt && threadIdx.x == 0) issue_tile(stage[buf], &bar[buf], nxt, RSZ);
+        has_nxt = tile_lookup(b, tile + G, Row::REQ_BYTES, nxt);
+        if (has_nxt && threadIdx.x == 0) issue_tile(stage[buf], &bar[buf], nxt, Row::REQ_BYTES);
         buf ^= 1;
     }
     n_fresh = __reduce_add_sync(0xffffffffu, n_fresh);
@@ -286,10 +285,9 @@ __global__ void __launch_bounds__(TILE_THREADS, GCRA_B_MINBLOCKS)
 decide_index_kernel(Table t, BatchView b, const PolicyDerived *__restrict__ pol, u32 npol, i64 now_batch,
                     const u32 *__restrict__ slot_arr, const u32 *__restrict__ counters, const u32 *__restrict__ pend,
                     u32 bm_mask, unsigned char *__restrict__ flags, u32 epoch, u32 honour_pend, u32 dbg) {
-    constexpr bool COMPACT = FMT != FMT_48_32, R16 = FMT == FMT_16_16;
-    constexpr u32 RSZ = COMPACT ? sizeof(gcra_request16) : sizeof(gcra_request);
-    constexpr u32 PIECES = R16 ? 1 : 2;          // 16-byte pieces per result row
-    __shared__ __align__(128) unsigned char stage[2][TILE_THREADS * RSZ];
+    using Row = Rows<FMT>;
+    constexpr u32 PIECES = Row::RES_BYTES / 16;       // 16-byte pieces per result row
+    __shared__ __align__(128) unsigned char stage[2][TILE_THREADS * Row::REQ_BYTES];
     __shared__ __align__(8) u64 bar[2];
     // results leave through shared memory: a tile's 256 results are written out as 256 x PIECES consecutive 16-byte
     // pieces (a warp store covers 512 contiguous bytes: 16 rows of 32 bytes, 32 rows of 16).  A segment's result array
@@ -305,11 +303,11 @@ decide_index_kernel(Table t, BatchView b, const PolicyDerived *__restrict__ pol,
     const u32 G = gridDim.x;
     u32 tile = blockIdx.x;
     TileRef cur, nxt, nn;
-    if (!tile_lookup(b, tile, RSZ, cur)) return;
-    bool has_nxt = tile_lookup(b, tile + G, RSZ, nxt);
+    if (!tile_lookup(b, tile, Row::REQ_BYTES, cur)) return;
+    bool has_nxt = tile_lookup(b, tile + G, Row::REQ_BYTES, nxt);
     if (threadIdx.x == 0) {
-        issue_tile(stage[0], &bar[0], cur, RSZ);
-        if (has_nxt) issue_tile(stage[1], &bar[1], nxt, RSZ);
+        issue_tile(stage[0], &bar[0], cur, Row::REQ_BYTES);
+        if (has_nxt) issue_tile(stage[1], &bar[1], nxt, Row::REQ_BYTES);
     }
     u32 par = 0;                 // phase parity of the two barriers, one bit each
     u32 buf = 0;
@@ -334,7 +332,7 @@ decide_index_kernel(Table t, BatchView b, const PolicyDerived *__restrict__ pol,
                                       ((honour_pend && pend_of(pend, bm_mask, slot_n)) ? F_DEFER : 0);
         }
         // the tile after that: its slots
-        const bool has_nn = has_nxt && tile_lookup(b, tile + 2 * G, RSZ, nn);
+        const bool has_nn = has_nxt && tile_lookup(b, tile + 2 * G, Row::REQ_BYTES, nn);
         const u32 slot_nn = (has_nn && threadIdx.x < nn.cnt) ? slot_arr[nn.row0 + threadIdx.x] : t.null_slot;
 
         mbar_wait(&bar[buf], (par >> buf) & 1);
@@ -351,13 +349,13 @@ decide_index_kernel(Table t, BatchView b, const PolicyDerived *__restrict__ pol,
         } else if (slot != t.null_slot) {
             u64 key_hash;
             Req r;
-            parse_request<COMPACT>(stage[buf] + (size_t)threadIdx.x * RSZ, pol, npol, now_batch, key_hash, r);
+            parse_request<Row::COMPACT>(stage[buf] + (size_t)threadIdx.x * Row::REQ_BYTES, pol, npol, now_batch, key_hash, r);
             Decision d;
             Outputs o;
             if (dbg & 8) { d.allowed = (r.q & 1) != 0; d.live = true; d.new_tat = r.now; d.new_exp = r.now + r.dvt; d.tat = s.tat; d.allow_at = 0; o.remaining = r.q; o.reset_after = r.ei; o.retry_after = 0; }
-            else { d = decide(s.tat, s.exp, r); if (!R16) o = outputs_of(d, r); }
+            else { d = decide(s.tat, s.exp, r); if (!Row::R16) o = outputs_of(d, r); }
             if (!(dbg & 2)) {
-                if (R16) {
+                if (Row::R16) {
                     rstage[buf][threadIdx.x] = make_longlong2(d.allowed ? d.new_tat : d.tat, (i64)(u32)0 | ((i64)(d.allowed ? 1 : 0) << 32));
                 } else {
                     rstage[buf][threadIdx.x * 2] = make_longlong2(o.remaining, o.reset_after);
@@ -395,7 +393,7 @@ decide_index_kernel(Table t, BatchView b, const PolicyDerived *__restrict__ pol,
         {
             // rows that failed validation (pass A wrote their error) or were deferred (the tail will write them) keep
             // their place: only staged rows are stored
-            longlong2 *dst = R16 ? reinterpret_cast<longlong2 *>(b.res16_at(cur.row0)) : reinterpret_cast<longlong2 *>(b.res_at(cur.row0));
+            longlong2 *dst = Row::R16 ? reinterpret_cast<longlong2 *>(b.res16_at(cur.row0)) : reinterpret_cast<longlong2 *>(b.res_at(cur.row0));
 #pragma unroll
             for (int k = 0; k < (int)PIECES; k++) {
                 const u32 c = threadIdx.x + k * TILE_THREADS;
@@ -403,7 +401,7 @@ decide_index_kernel(Table t, BatchView b, const PolicyDerived *__restrict__ pol,
             }
         }
         if (!has_nxt) break;
-        if (has_nn && threadIdx.x == 0) issue_tile(stage[buf], &bar[buf], nn, RSZ);
+        if (has_nn && threadIdx.x == 0) issue_tile(stage[buf], &bar[buf], nn, Row::REQ_BYTES);
         tile += G;
         cur = nxt; nxt = nn;
         slot_c = slot_n; s_c = s_n; bits_c = bits_n;
@@ -465,8 +463,7 @@ resolve_kernel(Table t, BatchView b, const PolicyDerived *__restrict__ pol, u32 
                const unsigned char *__restrict__ flags, u32 epoch, u32 *__restrict__ ctrl,
                volatile u64 *__restrict__ tile_status, u64 *__restrict__ res_keys,
                u32 *__restrict__ next_pend, volatile u32 *__restrict__ host_nres, u32 res_cap) {
-    constexpr bool COMPACT = FMT != FMT_48_32;
-    constexpr u32 RSZ = COMPACT ? sizeof(gcra_request16) : sizeof(gcra_request);
+    using Row = Rows<FMT>;
     __shared__ u32 part[TILE_THREADS / 32];
     __shared__ u32 sm_tile, sm_base;
     const u32 lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
@@ -523,7 +520,7 @@ resolve_kernel(Table t, BatchView b, const PolicyDerived *__restrict__ pol, u32 
                         // the first state change of the key in this batch: redo its decision and commit
                         u64 key_hash;
                         Req r;
-                        parse_request<COMPACT>(b.req_at(row, RSZ), pol, npol, now_batch, key_hash, r);
+                        parse_request<Row::COMPACT>(b.req_at(row, Row::REQ_BYTES), pol, npol, now_batch, key_hash, r);
                         RunState s;
                         load_state(t, slot[k], s);
                         const Decision d = decide(s.tat, s.exp, r);
@@ -560,7 +557,7 @@ resolve_kernel(Table t, BatchView b, const PolicyDerived *__restrict__ pol, u32 
             if (p >= res_cap) {
                 // more residue than the engine's batch capacity (a multi-GPU tick far beyond max_batch): the row
                 // is answered with an internal error instead of overrunning the sort buffers
-                if (FMT == FMT_16_16) write_result16(b.res16_at(row), 0, GCRA_INTERNAL, 0);
+                if (Row::R16) write_result16(b.res16_at(row), 0, GCRA_INTERNAL, 0);
                 else write_result(b.res_at(row), 0, 0, 0, GCRA_INTERNAL, 0);
                 atomicAdd(&t.counters[C_ERRORS], 1ULL);
                 continue;

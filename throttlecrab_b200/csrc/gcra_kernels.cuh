@@ -79,12 +79,35 @@ __device__ __forceinline__ void write_result16(gcra_result16 *out, i64 cur, int 
 
 // Row format of a batch, request bytes / result bytes.  16-byte results exist for compact requests only (the host
 // re-derives the outputs from the policy table), and only for single-segment batches.
-enum RowFmt { FMT_48_32 = 0, FMT_16_32 = 1, FMT_16_16 = 2 };
+enum RowFmt { FMT_48_32 = 0, FMT_16_32 = 1, FMT_16_16 = 2, FMT_COUNT };
+
+// Everything a row format decides, defined once.  COMPACT: a request names a policy of the engine's table
+// (gcra_request16) instead of carrying its parameters (gcra_request).  R16: a result is `cur` (gcra_result16)
+// instead of the three outputs (gcra_result).
+template <int FMT>
+struct Rows {
+    static constexpr bool COMPACT = FMT != FMT_48_32;
+    static constexpr bool R16 = FMT == FMT_16_16;
+    static constexpr u32 REQ_BYTES = COMPACT ? 16 : 48;
+    static constexpr u32 RES_BYTES = R16 ? 16 : 32;
+};
+static_assert(Rows<FMT_48_32>::REQ_BYTES == sizeof(gcra_request) && Rows<FMT_16_32>::REQ_BYTES == sizeof(gcra_request16),
+              "request rows are the ABI's request structs");
+static_assert(Rows<FMT_48_32>::RES_BYTES == sizeof(gcra_result) && Rows<FMT_16_16>::RES_BYTES == sizeof(gcra_result16),
+              "result rows are the ABI's result structs");
+
+// the row sizes of a format known at run time only (the host's copies and buffers)
+__host__ __device__ constexpr u32 req_bytes(int fmt) {
+    return fmt == FMT_16_16 ? Rows<FMT_16_16>::REQ_BYTES : fmt == FMT_16_32 ? Rows<FMT_16_32>::REQ_BYTES : Rows<FMT_48_32>::REQ_BYTES;
+}
+__host__ __device__ constexpr u32 res_bytes(int fmt) {
+    return fmt == FMT_16_16 ? Rows<FMT_16_16>::RES_BYTES : fmt == FMT_16_32 ? Rows<FMT_16_32>::RES_BYTES : Rows<FMT_48_32>::RES_BYTES;
+}
 
 // an error row (validation failed, table full, refused residue) in the batch's result format
 template <int FMT>
 __device__ __forceinline__ void write_error(gcra_result *out, u32 i, int status) {
-    if (FMT == FMT_16_16) write_result16(reinterpret_cast<gcra_result16 *>(out) + i, 0, status, 0);
+    if (Rows<FMT>::R16) write_result16(reinterpret_cast<gcra_result16 *>(out) + i, 0, status, 0);
     else write_result(out + i, 0, 0, 0, status, 0);
 }
 
@@ -137,11 +160,10 @@ template <int FMT>
 __device__ __forceinline__ u64 ingest_one(const Table &t, const unsigned char *rec, bool in_range,
                                           const PolicyDerived *__restrict__ pol, u32 npol, i64 now_batch, u32 i,
                                           Req *__restrict__ drec, gcra_result *__restrict__ out) {
-    constexpr bool COMPACT = FMT != FMT_48_32;
     int status = 0;
     u64 key_hash = 0;
     Req r = {0, 0, 0, 0};
-    if (in_range) status = parse_request<COMPACT>(rec, pol, npol, now_batch, key_hash, r);
+    if (in_range) status = parse_request<Rows<FMT>::COMPACT>(rec, pol, npol, now_batch, key_hash, r);
     u32 slot = t.null_slot;
     bool fresh = false;
     if (in_range && status == 0) {
@@ -168,8 +190,8 @@ __global__ void __launch_bounds__(TILE_THREADS)
 ingest_kernel(Table t, const void *__restrict__ req_base, const PolicyDerived *__restrict__ pol,
               u32 npol, i64 now_batch, u32 n, Req *__restrict__ drec, u64 *__restrict__ sortkeys,
               gcra_result *__restrict__ out) {
-    constexpr u32 RSZ = FMT != FMT_48_32 ? sizeof(gcra_request16) : sizeof(gcra_request);
-    __shared__ __align__(128) unsigned char stage[TILE_THREADS * RSZ];
+    using Row = Rows<FMT>;
+    __shared__ __align__(128) unsigned char stage[TILE_THREADS * Row::REQ_BYTES];
     __shared__ __align__(8) u64 bar;
 
     const u32 base = blockIdx.x * TILE_THREADS;
@@ -180,14 +202,14 @@ ingest_kernel(Table t, const void *__restrict__ req_base, const PolicyDerived *_
     }
     __syncthreads();
     if (threadIdx.x == 0) {
-        mbar_expect_tx(&bar, cnt * RSZ);
-        bulk_g2s(stage, (const unsigned char *)req_base + (size_t)base * RSZ, cnt * RSZ, &bar);
+        mbar_expect_tx(&bar, cnt * Row::REQ_BYTES);
+        bulk_g2s(stage, (const unsigned char *)req_base + (size_t)base * Row::REQ_BYTES, cnt * Row::REQ_BYTES, &bar);
     }
     mbar_wait(&bar, 0);
 
     const u32 i = base + threadIdx.x;
     const bool in_range = threadIdx.x < cnt;
-    const u64 key = ingest_one<FMT>(t, stage + (size_t)threadIdx.x * RSZ, in_range, pol, npol, now_batch, i, drec, out);
+    const u64 key = ingest_one<FMT>(t, stage + (size_t)threadIdx.x * Row::REQ_BYTES, in_range, pol, npol, now_batch, i, drec, out);
     if (in_range) sortkeys[i] = key;
 }
 
@@ -460,7 +482,7 @@ struct BatchView {
         if (nseg == 1) return res0 + i;
         return (gcra_result *)__ldg((const u64 *)&segs[i >> cap_shift].res) + (i & ((1u << cap_shift) - 1));
     }
-    // FMT_16_16 batches (always one segment): res0 holds gcra_result16 rows
+    // batches with 16-byte results (always one segment): res0 holds gcra_result16 rows
     __device__ __forceinline__ gcra_result16 *res16_at(u32 i) const { return reinterpret_cast<gcra_result16 *>(res0) + i; }
     __device__ __forceinline__ const unsigned char *req_at(u32 i, u32 rsz) const {
         if (nseg == 1) return req0 + (size_t)i * rsz;
@@ -486,7 +508,7 @@ struct OutMap {
         return BY_ROW ? view.res16_at(i) : reinterpret_cast<gcra_result16 *>(out) + i;
     }
 
-    // the result row of a finished decision: R16 (FMT_16_16 batches) stores `cur` alone, else the 32-byte result
+    // the result row of a finished decision: R16 (16-byte results) stores `cur` alone, else the 32-byte result
     template <bool BY_ROW, bool R16>
     __device__ __forceinline__ void write(u32 i, const Decision &d, const Req &r) const {
         if (R16) {
@@ -807,12 +829,11 @@ template <int FMT>
 __global__ void __launch_bounds__(TILE_THREADS)
 small_batch_kernel(Table t, const void *__restrict__ req_base, const PolicyDerived *__restrict__ pol, u32 npol,
                    i64 now_batch, u32 n, Req *__restrict__ drec, gcra_result *__restrict__ out) {
-    constexpr u32 RSZ = FMT != FMT_48_32 ? sizeof(gcra_request16) : sizeof(gcra_request);
     __shared__ u64 keys[TILE_THREADS];
     const u32 tid = threadIdx.x;
     const bool in_range = tid < n;
-    const u64 key = ingest_one<FMT>(t, (const unsigned char *)req_base + (size_t)(in_range ? tid : 0) * RSZ, in_range,
-                                        pol, npol, now_batch, tid, drec, out);
+    const u64 key = ingest_one<FMT>(t, (const unsigned char *)req_base + (size_t)(in_range ? tid : 0) * Rows<FMT>::REQ_BYTES,
+                                    in_range, pol, npol, now_batch, tid, drec, out);
     keys[tid] = in_range ? key : ~0ULL;
     __syncthreads();
     // bitonic sort of 256 keys; (slot << 32 | index) is a total order, so equal slots stay in index order
@@ -831,7 +852,7 @@ small_batch_kernel(Table t, const void *__restrict__ req_base, const PolicyDeriv
     OutMap om;
     om.out = out;
     om.by_row = 0;
-    decide_chunk<false, FMT == FMT_16_16>(t, keys, drec, n, om, nullptr, nullptr, nullptr, tid >> 5, tid & 31);
+    decide_chunk<false, Rows<FMT>::R16>(t, keys, drec, n, om, nullptr, nullptr, nullptr, tid >> 5, tid & 31);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -1425,7 +1446,6 @@ constexpr u32 DENIED_HASH = 512;
 template <int FMT>
 __global__ void __launch_bounds__(TILE_THREADS)
 denied_count_kernel(const unsigned char *__restrict__ req, const gcra_result *__restrict__ res, u32 n, DeniedTable t) {
-    constexpr u32 RSZ = FMT != FMT_48_32 ? sizeof(gcra_request16) : sizeof(gcra_request);
     __shared__ u64 hkey[DENIED_HASH];
     __shared__ u32 hcnt[DENIED_HASH];
     for (u32 i = threadIdx.x; i < DENIED_HASH; i += TILE_THREADS) { hkey[i] = 0; hcnt[i] = 0; }
@@ -1433,11 +1453,11 @@ denied_count_kernel(const unsigned char *__restrict__ req, const gcra_result *__
     const u32 i = blockIdx.x * TILE_THREADS + threadIdx.x;
     if (i < n) {
         // (retry_after | cur_tat_ns), status | allowed << 32: the second half of a 32-byte row, a whole 16-byte row
-        const longlong2 tail = FMT == FMT_16_16 ? reinterpret_cast<const longlong2 *>(res)[i]
-                                                : reinterpret_cast<const longlong2 *>(res + i)[1];
+        const longlong2 tail = Rows<FMT>::R16 ? reinterpret_cast<const longlong2 *>(res)[i]
+                                              : reinterpret_cast<const longlong2 *>(res + i)[1];
         const bool denied = (u32)tail.y == GCRA_OK && ((tail.y >> 32) & 0xff) == 0;
         if (denied) {
-            u64 k = *reinterpret_cast<const u64 *>(req + (size_t)i * RSZ);
+            u64 k = *reinterpret_cast<const u64 *>(req + (size_t)i * Rows<FMT>::REQ_BYTES);
             if (k == 0) k = 1;                                                          // 0 marks an empty entry
             u32 h = (u32)(mix64(k) >> 55);                                              // 9 bits
             for (;;) {
