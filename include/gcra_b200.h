@@ -245,7 +245,9 @@ int32_t gcra_top_denied(gcra_engine *h, uint32_t k, uint64_t *key_hashes, uint64
 /* table entry of a key after the fact: returns found, tat and expiry (saturated to INT64_MAX) */
 int32_t gcra_peek(gcra_engine *h, uint64_t key_hash, int64_t *tat, int64_t *expiry_ns, uint8_t *found);
 /* dump the table to a file / load it back (the reference keeps its state in memory only and loses it on
- * restart); decisions after a load are identical to those of the engine that saved */
+ * restart); decisions after a load are identical to those of the engine that saved.  gcra_snapshot_save writes a
+ * version 2 file (every slot); gcra_snapshot_load also reads version 3 files (gcra_snapshot_begin), inserting their
+ * entries into a cleared table of the file's geometry that replaces the engine's table once all are in. */
 int32_t gcra_snapshot_save(gcra_engine *h, const char *path);
 int32_t gcra_snapshot_load(gcra_engine *h, const char *path);
 /* Insert the entries of a snapshot file (gcra_snapshot_save, any geometry, any source engine) that shard `rank`
@@ -253,8 +255,9 @@ int32_t gcra_snapshot_load(gcra_engine *h, const char *path);
  * how a deployment changes its GPU count: every new rank restores every old rank's file (world = 1, rank = 0 takes
  * every entry).
  *   - Checked before any change (else GCRA_INTERNAL, engine untouched): the path opens; world > 0 and rank < world;
- *     the header (magic, version 2, nb_main x 4 + stash_slots <= total_lines x 4); the file length is the header +
- *     total_lines x 4 x (8 + 16 + 8) bytes.  The file's geometry need not be one this build would choose: entries are
+ *     the header (magic, version 2 or 3, nb_main x 4 + stash_slots <= total_lines x 4); the file length is the header
+ *     + total_lines x 4 x (8 + 16 + 8) bytes (version 2), or the header + 8 + n x 32 bytes (version 3, n entries:
+ *     gcra_snapshot_begin).  The file's geometry need not be one this build would choose: entries are
  *     re-inserted, not copied.
  *   - Carried: every slot whose key word is >= 2 and whose state is an entry (expiry = tat + off >= 0), expired but
  *     not swept ones included; tat, off and ei verbatim.  Keys that hold no entry (swept, only ever denied) are not.
@@ -273,6 +276,24 @@ int32_t gcra_snapshot_load(gcra_engine *h, const char *path);
  * gcra_shard_join) on every rank. */
 int32_t gcra_snapshot_restore(gcra_engine *h, const char *path, uint32_t rank, uint32_t world, uint64_t *restored,
                               uint64_t *conflicts);
+/* Background snapshot.  The cut is the call's position in submission order: the file holds the table as every batch
+ * (ring slot, device / pipelined / sharded / peer-memory submission, Store-trait call) submitted to this engine before
+ * the call left it, and no later one.  Returns without waiting for the device.  The capture runs on the GPU after
+ * those batches; later batches wait for the capture only (one streaming pass over the table); an engine thread then
+ * copies the captured entries to the host and writes them to `path` (written to a temporary file in the same
+ * directory, flushed, renamed into place: `path` is either the old file or the complete new one).
+ * One background save per engine at a time (a second begin returns GCRA_INTERNAL and leaves the first running).
+ *   - The file is version 3: the version 2 header (geometry, capacity, the counters at the cut, the hash seed), a
+ *     uint64 entry count n, then keys[n], (tat, off)[n] and ei[n] -- the slots gcra_snapshot_restore carries, in slot
+ *     order.  gcra_snapshot_load and gcra_snapshot_restore read it as well as version 2.
+ *   - begin fails (GCRA_INTERNAL, engine untouched, nothing written) when it cannot create the temporary file or the
+ *     staging buffers, which it makes or reuses before it enqueues anything.
+ *   - An error of the writer is reported by poll and wait (gcra_last_error gives its text), on the caller's thread.
+ *     A finished save's status and count stay until the next begin.
+ *   - gcra_destroy during a save waits for the file first. */
+int32_t gcra_snapshot_begin(gcra_engine *h, const char *path);
+int32_t gcra_snapshot_poll(gcra_engine *h, int32_t *done);        /* done = 1: no save in flight (finished or none) */
+int32_t gcra_snapshot_wait(gcra_engine *h, uint64_t *entries);     /* blocks; the save's status, entries written */
 /* block until all device work of this handle has finished */
 int32_t gcra_sync(gcra_engine *h);
 /* device time (ms) of the kernels of the most recent batch call, measured with CUDA events on

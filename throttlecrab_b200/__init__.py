@@ -279,6 +279,23 @@ class _GpuStore:
     def load(self, path):
         self._check(self._L.gcra_snapshot_load(self._h, os.fsencode(path)))
 
+    def save_begin(self, path):
+        """Begin a background save (gcra_snapshot_begin): the file will hold the table as every batch submitted before
+        this call left it.  Returns at once; traffic continues while the file is written."""
+        self._check(self._L.gcra_snapshot_begin(self._h, os.fsencode(path)))
+
+    def save_poll(self):
+        """True when no background save is in flight (the last one's file is complete); raises if it failed."""
+        d = C.c_int32()
+        self._check(self._L.gcra_snapshot_poll(self._h, C.byref(d)))
+        return bool(d.value)
+
+    def save_wait(self):
+        """Wait for the background save; returns the number of entries written."""
+        n = C.c_uint64()
+        self._check(self._L.gcra_snapshot_wait(self._h, C.byref(n)))
+        return n.value
+
     def restore(self, path, rank=0, world=1):
         """Insert the entries of a snapshot file that shard `rank` of `world` owns next to what this store holds
         (gcra_snapshot_restore); returns (restored, conflicts)."""

@@ -111,6 +111,9 @@ SYMBOLS = {
     "gcra_snapshot_save": (_i32, [_vp, C.c_char_p]),
     "gcra_snapshot_load": (_i32, [_vp, C.c_char_p]),
     "gcra_snapshot_restore": (_i32, [_vp, C.c_char_p, _u32, _u32, _pu64, _pu64]),
+    "gcra_snapshot_begin": (_i32, [_vp, C.c_char_p]),
+    "gcra_snapshot_poll": (_i32, [_vp, C.POINTER(_i32)]),
+    "gcra_snapshot_wait": (_i32, [_vp, _pu64]),
     "gcra_sync": (_i32, [_vp]),
     "gcra_last_kernel_ms": (_i32, [_vp, C.POINTER(C.c_float * 4)]),
     "gcra_last_kernel_ms_detail": (_i32, [_vp, C.POINTER(C.c_float * 7)]),

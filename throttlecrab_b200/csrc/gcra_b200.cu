@@ -8,6 +8,7 @@
 #include <cuda_runtime.h>
 
 #include <algorithm>
+#include <atomic>
 #include <cstdio>
 #include <cstdlib>
 #include <dlfcn.h>
@@ -16,6 +17,7 @@
 #include <memory>
 #include <string>
 #include <sys/stat.h>
+#include <thread>
 #include <type_traits>
 #include <unistd.h>
 #include <vector>
@@ -187,6 +189,33 @@ struct Scratch {
 struct TableArrays { DevBuf<u64> keys, mark; DevBuf<TatOff> state; DevBuf<i64> ei; };
 struct DeniedArrays { DevBuf<u64> keys, counts, dropped; };
 
+// What background saves (gcra_snapshot_begin) keep on the engine and reuse: made by the first save, grown by a later
+// one that needs more room, released by gcra_destroy.
+struct SnapshotStaging {
+    Stream stream;                   // the capture, then the writer thread's copies (one thread at a time uses it)
+    Event ev_store, ev_capture, ev_chunk[2];
+    StreamBuf<unsigned char> dev;    // ctrl words | keys | (tat, off) pairs | ei
+    size_t dev_bytes = 0;
+    PinnedBuf<char> chunk[2];        // double-buffered copies on their way to the file
+    PinnedBuf<u64> meta;             // [C_COUNT] the counters at the cut, then the entry count
+    uint32_t grid = 0;               // persistent CTAs of snapshot_capture_kernel
+};
+
+// one background save: what its writer thread needs, and what it reports (read once `finished` is set)
+struct SnapshotJob {
+    std::thread writer;
+    std::atomic<bool> finished{false};
+    int rc = 0;
+    std::string err;
+    uint64_t entries = 0;
+    int fd = -1;
+    std::string tmp, path;
+    uint32_t total_lines = 0, nb_main = 0, stash_slots = 0;    // the table at the cut
+    uint64_t capacity = 0, hash_seed[2] = {0, 0};
+    uint64_t cap = 0;                                          // entries the staging sections hold
+    size_t keys_off = 0, state_off = 0, ei_off = 0;            // the sections in the staging
+};
+
 // Members are released in reverse declaration order, after gcra_destroy has synchronized the device: no release waits.
 struct gcra_engine {
     int device = 0;
@@ -274,8 +303,21 @@ struct gcra_engine {
     uint32_t denied_max = 0;
     uint64_t denied_cap = 0;
     uint64_t hash_seed[2] = {0, 0};  // SipHash key of the string-keyed entry points ((0,0): the unkeyed gcra_hash_key)
+    // background saves (gcra_snapshot_begin); gcra_destroy joins the writer thread before anything is released
+    std::unique_ptr<SnapshotStaging> snap;
+    std::unique_ptr<SnapshotJob> job;
+    bool capture_pending = false;    // launches that touch the table wait for snap->ev_capture
     std::string err;
 };
+
+// Until the capture of a background save has completed, work that may touch the table waits for it on `st`; once
+// it has completed, this is one flag test.
+static int after_capture(gcra_engine *h, cudaStream_t st) {
+    if (!h->capture_pending) return GCRA_OK;
+    if (cudaEventQuery(h->snap->ev_capture.get()) == cudaSuccess) { h->capture_pending = false; return GCRA_OK; }
+    CK(cudaStreamWaitEvent(st, h->snap->ev_capture.get(), 0));
+    return GCRA_OK;
+}
 
 static uint32_t ceil_log2(uint64_t x) {
     uint32_t b = 0;
@@ -419,10 +461,9 @@ static int grow(gcra_engine *h, uint64_t need) {
     return GCRA_OK;
 }
 
-static int ensure_room(gcra_engine *h, uint64_t n) {
-    if (h->occupied_ub + n <= load_limit(h)) { h->occupied_ub += n; return GCRA_OK; }
-    // the bound is stale (it assumes every request claimed a slot): tighten it from the newest
-    // counter snapshot that has already arrived, without stalling the stream
+// The bound is stale (it assumes every request claimed a slot): tighten it from the newest counter snapshot that has
+// already arrived, without stalling the stream.
+static void tighten_occupied_ub(gcra_engine *h) {
     for (int back = 1; back <= gcra_engine::N_SNAP; back++) {
         int k = (int)((h->snap_next + gcra_engine::N_SNAP - back) % gcra_engine::N_SNAP);
         if (!h->snap_used[k]) break;
@@ -431,6 +472,11 @@ static int ensure_room(gcra_engine *h, uint64_t n) {
         if (ub < h->occupied_ub) h->occupied_ub = ub;
         break;
     }
+}
+
+static int ensure_room(gcra_engine *h, uint64_t n) {
+    if (h->occupied_ub + n <= load_limit(h)) { h->occupied_ub += n; return GCRA_OK; }
+    tighten_occupied_ub(h);
     if (h->occupied_ub + n <= load_limit(h)) { h->occupied_ub += n; return GCRA_OK; }
     int rc = refresh_counters(h, true);
     if (rc) return rc;
@@ -816,6 +862,7 @@ static int launch_batch(gcra_engine *h, uint32_t n, const void *d_req, int fmt, 
     // order after every earlier batch (they may have been submitted pipelined on the engine's streams),
     // which also frees this scratch set
     for (auto &o : h->scr) if (o.back_recorded) CK(cudaStreamWaitEvent(st, o.ev_back.get(), 0));
+    RC(after_capture(h, st));
     static const bool no_small = getenv("GCRA_NO_SMALL") && atoi(getenv("GCRA_NO_SMALL"));   // A/B switch for tools/latency_probe.py
     if (n <= SMALL_MAX && !no_small) {
         // small batch (a single rate_limit call, a lightly loaded actor): one CTA does ingest, ordering and
@@ -868,6 +915,7 @@ static int launch_pipelined_view(gcra_engine *h, const BatchView &v, uint32_t n_
     cudaStream_t fs = h->front_stream.get();                  // (all sets share one front stream, see gcra_create)
     if (ready) CK(cudaStreamWaitEvent(fs, ready, 0));
     if (sc.back_recorded) CK(cudaStreamWaitEvent(fs, sc.ev_back.get(), 0));   // scratch set free again
+    RC(after_capture(h, fs));                                 // (the later stages follow this batch's front)
     u64 *sorted = nullptr;
     // residue feedback: the newest pass-C count that has reached the host
     bool residue_large = false;
@@ -969,6 +1017,7 @@ static void preload_kernels() {
     preload(route_count_kernel); preload(route_scan_kernel); preload(route_scatter_kernel); preload(route_unpermute_kernel);
     preload(p2p_scan_kernel); preload(p2p_scatter_kernel); preload(p2p_signal_req_kernel); preload(p2p_signal_res_kernel);
     preload(p2p_wait_kernel); preload(p2p_unpermute_kernel);
+    preload(snapshot_capture_kernel);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -1105,6 +1154,7 @@ int32_t gcra_create(const gcra_config *cfg, gcra_engine **out) {
 // the synchronize comes first: no member is released under work still running
 void gcra_destroy(gcra_engine *h) {
     if (!h) return;
+    if (h->job && h->job->writer.joinable()) h->job->writer.join();    // a background save finishes its file first
     cudaSetDevice(h->device);
     cudaDeviceSynchronize();
     delete h;
@@ -1197,6 +1247,7 @@ static int store_op(gcra_engine *h, int op, uint64_t key_hash, int64_t a, int64_
     // a Store-trait call reads / writes a slot's state: after every batch still in flight on the engine's or a
     // caller's stream (launch_batch orders itself the same way)
     for (auto &o : h->scr) if (o.back_recorded) CK(cudaStreamWaitEvent(h->stream.get(), o.ev_back.get(), 0));
+    RC(after_capture(h, h->stream.get()));
     store_op_kernel<<<1, 1, 0, h->stream.get()>>>(h->tab, op, stored_key(key_hash), a, b, ttl, now, h->d_op.get());
     h->launches++;
     CK(cudaMemcpyAsync(h->h_op.get(), h->d_op.get(), 2 * sizeof(StoreOpResult), cudaMemcpyDeviceToHost, h->stream.get()));
@@ -1669,14 +1720,216 @@ int32_t gcra_snapshot_save(gcra_engine *h, const char *path) {
     return rc;
 }
 
+// Streams the file through the GPU twice, in chunks of RESTORE_CHUNK slots (one staging set = SNAP_CHUNK bytes over
+// the three sections; two sets, so that reading chunk i + 1 overlaps the kernel over chunk i): a COUNT pass sizes the
+// table for the entries this shard takes, an INSERT pass inserts them.
+namespace {
+const size_t RESTORE_CHUNK = SNAP_CHUNK / (sizeof(u64) + sizeof(TatOff) + sizeof(i64));
+
+struct RestoreBuffers {
+    PinnedBuf<char> host[2];           // keys | state | ei of one chunk
+    DevBuf<char> dev[2];
+    DevBuf<u64> counts;                // [RESTORE_COUNTS]
+    Event done[2];                     // the set's copy + kernel finished: its host buffer may be refilled
+    int fd = -1;
+};
+}  // namespace
+
+static bool pread_all(int fd, void *buf, size_t bytes, uint64_t off) {
+    for (size_t got = 0; got < bytes;) {
+        const ssize_t r = pread(fd, (char *)buf + got, bytes - got, (off_t)(off + got));
+        if (r <= 0) return false;
+        got += (size_t)r;
+    }
+    return true;
+}
+
+// The sections of a snapshot file, checked against the file's length.  Version 2: every slot of the table (header,
+// keys, (tat, off) pairs, ei).  Version 3 (gcra_snapshot_begin): the header, the entry count n, then the same three
+// sections restricted to the n carried entries.
+struct SnapSections { uint64_t rows, keys_off, state_off, ei_off; };
+
+static const char *snapshot_sections(int fd, const SnapshotHeader &hd, SnapSections &sec) {
+    struct stat sb;
+    if (fstat(fd, &sb) != 0) return "cannot stat the file";
+    const uint64_t size = (uint64_t)sb.st_size, row = sizeof(u64) + sizeof(TatOff) + sizeof(i64);
+    const uint64_t slots = (uint64_t)hd.total_lines * 4;
+    if ((uint64_t)hd.nb_main * 4 + hd.stash_slots > slots) return "bad geometry";
+    if (hd.version == 2) {
+        sec.rows = slots;
+        sec.keys_off = sizeof(hd);
+    } else {
+        uint64_t n = 0;
+        if (size < sizeof(hd) + sizeof(n) || !pread_all(fd, &n, sizeof(n), sizeof(hd))) return "file length does not match its header";
+        if (n > (size - sizeof(hd) - sizeof(n)) / row) return "file length does not match its header";
+        sec.rows = n;
+        sec.keys_off = sizeof(hd) + sizeof(n);
+    }
+    if (size != sec.keys_off + sec.rows * row) return "file length does not match its header";
+    sec.state_off = sec.keys_off + sec.rows * sizeof(u64);
+    sec.ei_off = sec.state_off + sec.rows * sizeof(TatOff);
+    return nullptr;
+}
+
+static int make_restore_buffers(gcra_engine *h, RestoreBuffers &b) {
+    for (int s = 0; s < 2; s++) {
+        CK(b.host[s].make(SNAP_CHUNK));
+        CK(b.dev[s].make(SNAP_CHUNK));
+        CK(b.done[s].make(cudaEventDisableTiming));
+    }
+    CK(b.counts.make(RESTORE_COUNTS));
+    CK(cudaMemsetAsync(b.counts.get(), 0, RESTORE_COUNTS * sizeof(u64), h->stream.get()));
+    return GCRA_OK;
+}
+
+// one pass of restore_kernel over the `sec.rows` rows of a file's sections into table `t`
+static int restore_pass(gcra_engine *h, RestoreBuffers &b, const Table &t, const SnapSections &sec, uint32_t rank,
+                        uint32_t world, bool insert) {
+    for (uint64_t first = 0, c = 0; first < sec.rows; first += RESTORE_CHUNK, c++) {
+        const int s = (int)(c & 1);
+        const uint64_t n = std::min<uint64_t>(RESTORE_CHUNK, sec.rows - first);
+        char *hk = b.host[s].get(), *hs = hk + RESTORE_CHUNK * sizeof(u64), *he = hs + RESTORE_CHUNK * sizeof(TatOff);
+        char *dk = b.dev[s].get(), *ds = dk + RESTORE_CHUNK * sizeof(u64), *de = ds + RESTORE_CHUNK * sizeof(TatOff);
+        CK(cudaEventSynchronize(b.done[s].get()));
+        if (!pread_all(b.fd, hk, n * sizeof(u64), sec.keys_off + first * sizeof(u64)) ||
+            !pread_all(b.fd, hs, n * sizeof(TatOff), sec.state_off + first * sizeof(TatOff)) ||
+            (insert && !pread_all(b.fd, he, n * sizeof(i64), sec.ei_off + first * sizeof(i64)))) {
+            h->err = "snapshot restore: short read";
+            return GCRA_INTERNAL;
+        }
+        CK(cudaMemcpyAsync(dk, hk, n * sizeof(u64), cudaMemcpyHostToDevice, h->stream.get()));
+        CK(cudaMemcpyAsync(ds, hs, n * sizeof(TatOff), cudaMemcpyHostToDevice, h->stream.get()));
+        if (insert) CK(cudaMemcpyAsync(de, he, n * sizeof(i64), cudaMemcpyHostToDevice, h->stream.get()));
+        const uint32_t grid = (uint32_t)std::min<uint64_t>((n + TILE_THREADS - 1) / TILE_THREADS, 8 * h->sms);
+        (insert ? restore_kernel<true> : restore_kernel<false>)<<<grid, TILE_THREADS, 0, h->stream.get()>>>(
+            t, (const u64 *)dk, (const TatOff *)ds, (const i64 *)de, n, rank, world, b.counts.get());
+        h->launches++;
+        CK(cudaGetLastError());
+        CK(cudaEventRecord(b.done[s].get(), h->stream.get()));
+    }
+    CK(cudaStreamSynchronize(h->stream.get()));
+    return GCRA_OK;
+}
+
+static int restore_file(gcra_engine *h, RestoreBuffers &b, uint32_t rank, uint32_t world, uint64_t *restored,
+                        uint64_t *conflicts) {
+    SnapshotHeader hd{};
+    if (!pread_all(b.fd, &hd, sizeof(hd), 0) || memcmp(hd.magic, SNAP_MAGIC, 8) != 0 || (hd.version != 2 && hd.version != 3)) {
+        h->err = "snapshot restore: bad header";
+        return GCRA_INTERNAL;
+    }
+    SnapSections sec;
+    if (const char *why = snapshot_sections(b.fd, hd, sec)) { h->err = std::string("snapshot restore: ") + why; return GCRA_INTERNAL; }
+    CK(cudaDeviceSynchronize());
+    RC(refresh_counters(h, true));
+    const bool adopt_seed = h->h_counters.get()[C_REAL] == 0;
+    if (!adopt_seed && (hd.hash_seed[0] != h->hash_seed[0] || hd.hash_seed[1] != h->hash_seed[1])) {
+        h->err = "snapshot restore: the file's key-hash seed differs from that of the entries held";
+        return GCRA_INTERNAL;
+    }
+    RC(make_restore_buffers(h, b));
+    RC(restore_pass(h, b, h->tab, sec, rank, world, false));
+    u64 counts[RESTORE_COUNTS];
+    CK(cudaMemcpy(counts, b.counts.get(), sizeof(counts), cudaMemcpyDeviceToHost));
+    RC(ensure_room(h, counts[RESTORE_OWNED]));     // may purge or grow: h->tab is read after it
+    RC(restore_pass(h, b, h->tab, sec, rank, world, true));
+    CK(cudaMemcpy(counts, b.counts.get(), sizeof(counts), cudaMemcpyDeviceToHost));
+    RC(refresh_counters(h, true));
+    h->occupied_ub = h->h_counters.get()[C_OCCUPIED];
+    for (int i = 0; i < gcra_engine::N_SNAP; i++) h->snap_used[i] = false;
+    if (counts[RESTORE_FAILED]) {
+        h->err = "snapshot restore: table full (" + std::to_string(counts[RESTORE_FAILED]) + " entries not inserted)";
+        return GCRA_INTERNAL;
+    }
+    if (adopt_seed) { h->hash_seed[0] = hd.hash_seed[0]; h->hash_seed[1] = hd.hash_seed[1]; }
+    if (restored) *restored = counts[RESTORE_INSERTED];
+    if (conflicts) *conflicts = counts[RESTORE_CONFLICTS];
+    return GCRA_OK;
+}
+
+// the staging buffers of `b` may still be read by queued copies: wait for them before `b` releases them
+static void close_restore(RestoreBuffers &b) {
+    for (Event &e : b.done) if (e.get()) cudaEventSynchronize(e.get());
+    close(b.fd);
+}
+
+int32_t gcra_snapshot_restore(gcra_engine *h, const char *path, uint32_t rank, uint32_t world, uint64_t *restored,
+                              uint64_t *conflicts) {
+    if (restored) *restored = 0;
+    if (conflicts) *conflicts = 0;
+    CK(cudaSetDevice(h->device));
+    if (world == 0 || rank >= world) { h->err = "snapshot restore: needs rank < world"; return GCRA_INTERNAL; }
+    RestoreBuffers b;
+    b.fd = open(path, O_RDONLY);
+    if (b.fd < 0) { h->err = std::string("snapshot restore: cannot open ") + path; return GCRA_INTERNAL; }
+    const int rc = restore_file(h, b, rank, world, restored, conflicts);
+    close_restore(b);
+    return rc;
+}
+
+// gcra_snapshot_load of a version 3 file: its entries inserted into a cleared table of the file's geometry, which
+// replaces the engine's table only once every entry is in.  The traffic totals are the file's; len, occupied slots
+// and stash follow the insertion (occupied = len: keys without an entry are not in the file).
+static int load_compact(gcra_engine *h, RestoreBuffers &b, const SnapshotHeader &hd) {
+    SnapSections sec;
+    if (const char *why = snapshot_sections(b.fd, hd, sec)) { h->err = std::string("snapshot: ") + why; return GCRA_INTERNAL; }
+    uint32_t tl, nb, ss;
+    table_geometry(hd.capacity, h->tight, tl, nb, ss);
+    if (tl != hd.total_lines || nb != hd.nb_main || ss != hd.stash_slots) {
+        h->err = "snapshot: geometry not reproducible with this build/flags";
+        return GCRA_INTERNAL;
+    }
+    RC(make_restore_buffers(h, b));
+    DevBuf<u64> nc;                    // the new table's counters while it is filled
+    CK(nc.make(C_COUNT));
+    CK(cudaMemsetAsync(nc.get(), 0, C_COUNT * sizeof(u64), h->stream.get()));
+    TableArrays na;
+    Table nt{};
+    uint32_t nl = 0;
+    RC(alloc_table(h, hd.capacity, na, nt, nl, nc.get()));
+    RC(restore_pass(h, b, nt, sec, 0, 1, true));
+    u64 counts[RESTORE_COUNTS], fresh[C_COUNT];
+    CK(cudaMemcpy(counts, b.counts.get(), sizeof(counts), cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(fresh, nc.get(), sizeof(fresh), cudaMemcpyDeviceToHost));
+    if (counts[RESTORE_FAILED] || counts[RESTORE_CONFLICTS]) {
+        h->err = "snapshot: the file's entries do not fit its own geometry (a key twice, or a full table)";
+        return GCRA_INTERNAL;
+    }
+    u64 c[C_COUNT];
+    memcpy(c, hd.counters, sizeof(c));
+    c[C_OCCUPIED] = fresh[C_OCCUPIED];
+    c[C_REAL] = fresh[C_REAL];
+    c[C_STASH] = fresh[C_STASH];
+    CK(cudaMemcpy(h->tab.counters, c, sizeof(c), cudaMemcpyHostToDevice));
+    nt.counters = h->tab.counters;
+    h->tab_arrays = std::move(na);
+    h->tab = nt; h->total_lines = nl; h->capacity = hd.capacity;
+    h->hash_seed[0] = hd.hash_seed[0];
+    h->hash_seed[1] = hd.hash_seed[1];
+    h->occupied_ub = c[C_OCCUPIED];
+    h->seen_allowed = c[C_ALLOWED];
+    h->seen_expired_hits = c[C_EXPIRED_HITS];
+    for (int i = 0; i < gcra_engine::N_SNAP; i++) h->snap_used[i] = false;
+    return GCRA_OK;
+}
+
 int32_t gcra_snapshot_load(gcra_engine *h, const char *path) {
     CK(cudaSetDevice(h->device));
     CK(cudaDeviceSynchronize());
     FILE *f = fopen(path, "rb");
     if (!f) { h->err = std::string("snapshot: cannot open ") + path; return GCRA_INTERNAL; }
     SnapshotHeader hd{};
-    if (fread(&hd, sizeof(hd), 1, f) != 1 || memcmp(hd.magic, SNAP_MAGIC, 8) != 0 || hd.version != 2) {
+    if (fread(&hd, sizeof(hd), 1, f) != 1 || memcmp(hd.magic, SNAP_MAGIC, 8) != 0 || (hd.version != 2 && hd.version != 3)) {
         fclose(f); h->err = "snapshot: bad header"; return GCRA_INTERNAL;
+    }
+    if (hd.version == 3) {
+        fclose(f);
+        RestoreBuffers b;
+        b.fd = open(path, O_RDONLY);
+        if (b.fd < 0) { h->err = std::string("snapshot: cannot open ") + path; return GCRA_INTERNAL; }
+        const int rc = load_compact(h, b, hd);
+        close_restore(b);
+        return rc;
     }
     int rc = GCRA_OK;
     if (hd.total_lines != h->total_lines || hd.nb_main != h->tab.nb_main || hd.stash_slots != h->tab.stash_slots) {
@@ -1712,121 +1965,187 @@ int32_t gcra_snapshot_load(gcra_engine *h, const char *path) {
     return GCRA_OK;
 }
 
-// Streams the file through the GPU twice, in chunks of RESTORE_CHUNK slots (one staging set = SNAP_CHUNK bytes over
-// the three sections; two sets, so that reading chunk i + 1 overlaps the kernel over chunk i): a COUNT pass sizes the
-// table for the entries this shard takes, an INSERT pass inserts them.
-namespace {
-const size_t RESTORE_CHUNK = SNAP_CHUNK / (sizeof(u64) + sizeof(TatOff) + sizeof(i64));
-
-struct RestoreBuffers {
-    PinnedBuf<char> host[2];           // keys | state | ei of one chunk
-    DevBuf<char> dev[2];
-    DevBuf<u64> counts;                // [RESTORE_COUNTS]
-    Event done[2];                     // the set's copy + kernel finished: its host buffer may be refilled
-    int fd = -1;
-};
-}  // namespace
-
-static bool pread_all(int fd, void *buf, size_t bytes, uint64_t off) {
-    for (size_t got = 0; got < bytes;) {
-        const ssize_t r = pread(fd, (char *)buf + got, bytes - got, (off_t)(off + got));
+// ---- background snapshot: capture on the GPU at the call's place in submission order, write on a thread ----------
+static bool pwrite_all(int fd, const void *buf, size_t bytes, uint64_t off) {
+    for (size_t put = 0; put < bytes;) {
+        const ssize_t r = pwrite(fd, (const char *)buf + put, bytes - put, (off_t)(off + put));
         if (r <= 0) return false;
-        got += (size_t)r;
+        put += (size_t)r;
     }
     return true;
 }
 
-static int restore_pass(gcra_engine *h, RestoreBuffers &b, uint64_t slots, uint32_t rank, uint32_t world, bool insert) {
-    const uint64_t keys_off = sizeof(SnapshotHeader), state_off = keys_off + slots * sizeof(u64),
-                   ei_off = state_off + slots * sizeof(TatOff);
-    for (uint64_t first = 0, c = 0; first < slots; first += RESTORE_CHUNK, c++) {
-        const int s = (int)(c & 1);
-        const uint64_t n = std::min<uint64_t>(RESTORE_CHUNK, slots - first);
-        char *hk = b.host[s].get(), *hs = hk + RESTORE_CHUNK * sizeof(u64), *he = hs + RESTORE_CHUNK * sizeof(TatOff);
-        char *dk = b.dev[s].get(), *ds = dk + RESTORE_CHUNK * sizeof(u64), *de = ds + RESTORE_CHUNK * sizeof(TatOff);
-        CK(cudaEventSynchronize(b.done[s].get()));
-        if (!pread_all(b.fd, hk, n * sizeof(u64), keys_off + first * sizeof(u64)) ||
-            !pread_all(b.fd, hs, n * sizeof(TatOff), state_off + first * sizeof(TatOff)) ||
-            (insert && !pread_all(b.fd, he, n * sizeof(i64), ei_off + first * sizeof(i64)))) {
-            h->err = "snapshot restore: short read";
-            return GCRA_INTERNAL;
-        }
-        CK(cudaMemcpyAsync(dk, hk, n * sizeof(u64), cudaMemcpyHostToDevice, h->stream.get()));
-        CK(cudaMemcpyAsync(ds, hs, n * sizeof(TatOff), cudaMemcpyHostToDevice, h->stream.get()));
-        if (insert) CK(cudaMemcpyAsync(de, he, n * sizeof(i64), cudaMemcpyHostToDevice, h->stream.get()));
-        const uint32_t grid = (uint32_t)std::min<uint64_t>((n + TILE_THREADS - 1) / TILE_THREADS, 8 * h->sms);
-        (insert ? restore_kernel<true> : restore_kernel<false>)<<<grid, TILE_THREADS, 0, h->stream.get()>>>(
-            h->tab, (const u64 *)dk, (const TatOff *)ds, (const i64 *)de, n, rank, world, b.counts.get());
-        h->launches++;
-        CK(cudaGetLastError());
-        CK(cudaEventRecord(b.done[s].get(), h->stream.get()));
-    }
-    CK(cudaStreamSynchronize(h->stream.get()));
-    return GCRA_OK;
-}
-
-static int restore_file(gcra_engine *h, RestoreBuffers &b, uint32_t rank, uint32_t world, uint64_t *restored,
-                        uint64_t *conflicts) {
+// The writer thread's whole job.  It waits only for the staging's own events and stream, so it never holds up the
+// engine's traffic or another engine's; the file appears at `path` (rename) only when it is complete and on disk.
+static int write_snapshot_file(SnapshotJob *j, SnapshotStaging *sg, int device) {
+    cudaError_t e = cudaSuccess;
+    auto fail = [&](const std::string &what) {
+        j->err = "snapshot: " + what + (e != cudaSuccess ? std::string(": ") + cudaGetErrorString(e) : std::string());
+        return GCRA_INTERNAL;
+    };
+    if ((e = cudaSetDevice(device)) || (e = cudaEventSynchronize(sg->ev_capture.get()))) return fail("capture");
+    const u64 n = sg->meta.get()[C_COUNT];
+    if (n > j->cap) return fail("more entries than the staging holds");
     SnapshotHeader hd{};
-    struct stat sb;
-    if (fstat(b.fd, &sb) != 0 || !pread_all(b.fd, &hd, sizeof(hd), 0) || memcmp(hd.magic, SNAP_MAGIC, 8) != 0 ||
-        hd.version != 2) {
-        h->err = "snapshot restore: bad header";
-        return GCRA_INTERNAL;
+    memcpy(hd.magic, SNAP_MAGIC, 8);
+    hd.version = 3;
+    hd.total_lines = j->total_lines; hd.nb_main = j->nb_main; hd.stash_slots = j->stash_slots;
+    hd.capacity = j->capacity;
+    memcpy(hd.counters, sg->meta.get(), sizeof(hd.counters));
+    hd.hash_seed[0] = j->hash_seed[0]; hd.hash_seed[1] = j->hash_seed[1];
+    if (!pwrite_all(j->fd, &hd, sizeof(hd), 0) || !pwrite_all(j->fd, &n, sizeof(n), sizeof(hd))) return fail("short write");
+    struct Piece { const unsigned char *src; size_t bytes; uint64_t off; };
+    std::vector<Piece> pieces;
+    const unsigned char *dev = sg->dev.get();
+    const Piece sections[3] = {{dev + j->keys_off, n * sizeof(u64), sizeof(hd) + sizeof(n)},
+                               {dev + j->state_off, n * sizeof(TatOff), sizeof(hd) + sizeof(n) + n * sizeof(u64)},
+                               {dev + j->ei_off, n * sizeof(i64), sizeof(hd) + sizeof(n) + n * (sizeof(u64) + sizeof(TatOff))}};
+    for (const Piece &p : sections)
+        for (size_t o = 0; o < p.bytes; o += SNAP_CHUNK) pieces.push_back({p.src + o, std::min(SNAP_CHUNK, p.bytes - o), p.off + o});
+    // piece i + 1 is copied while piece i is written; its pinned chunk last held piece i - 1, written already
+    auto issue = [&](size_t i) {
+        const int c = (int)(i & 1);
+        if ((e = cudaMemcpyAsync(sg->chunk[c].get(), pieces[i].src, pieces[i].bytes, cudaMemcpyDeviceToHost, sg->stream.get()))) return false;
+        return (e = cudaEventRecord(sg->ev_chunk[c].get(), sg->stream.get())) == cudaSuccess;
+    };
+    if (!pieces.empty() && !issue(0)) return fail("copy");
+    for (size_t i = 0; i < pieces.size(); i++) {
+        if (i + 1 < pieces.size() && !issue(i + 1)) return fail("copy");
+        if ((e = cudaEventSynchronize(sg->ev_chunk[i & 1].get()))) return fail("copy");
+        if (!pwrite_all(j->fd, sg->chunk[i & 1].get(), pieces[i].bytes, pieces[i].off)) return fail("short write");
     }
-    const uint64_t slots = (uint64_t)hd.total_lines * 4;
-    if ((uint64_t)hd.nb_main * 4 + hd.stash_slots > slots) { h->err = "snapshot restore: bad geometry"; return GCRA_INTERNAL; }
-    if ((uint64_t)sb.st_size != sizeof(hd) + slots * (sizeof(u64) + sizeof(TatOff) + sizeof(i64))) {
-        h->err = "snapshot restore: file length does not match its header";
-        return GCRA_INTERNAL;
-    }
-    CK(cudaDeviceSynchronize());
-    RC(refresh_counters(h, true));
-    const bool adopt_seed = h->h_counters.get()[C_REAL] == 0;
-    if (!adopt_seed && (hd.hash_seed[0] != h->hash_seed[0] || hd.hash_seed[1] != h->hash_seed[1])) {
-        h->err = "snapshot restore: the file's key-hash seed differs from that of the entries held";
-        return GCRA_INTERNAL;
-    }
-    for (int s = 0; s < 2; s++) {
-        CK(b.host[s].make(SNAP_CHUNK));
-        CK(b.dev[s].make(SNAP_CHUNK));
-        CK(b.done[s].make(cudaEventDisableTiming));
-    }
-    CK(b.counts.make(RESTORE_COUNTS));
-    CK(cudaMemsetAsync(b.counts.get(), 0, RESTORE_COUNTS * sizeof(u64), h->stream.get()));
-    RC(restore_pass(h, b, slots, rank, world, false));
-    u64 counts[RESTORE_COUNTS];
-    CK(cudaMemcpy(counts, b.counts.get(), sizeof(counts), cudaMemcpyDeviceToHost));
-    RC(ensure_room(h, counts[RESTORE_OWNED]));     // may purge or grow: h->tab is read after it
-    RC(restore_pass(h, b, slots, rank, world, true));
-    CK(cudaMemcpy(counts, b.counts.get(), sizeof(counts), cudaMemcpyDeviceToHost));
-    RC(refresh_counters(h, true));
-    h->occupied_ub = h->h_counters.get()[C_OCCUPIED];
-    for (int i = 0; i < gcra_engine::N_SNAP; i++) h->snap_used[i] = false;
-    if (counts[RESTORE_FAILED]) {
-        h->err = "snapshot restore: table full (" + std::to_string(counts[RESTORE_FAILED]) + " entries not inserted)";
-        return GCRA_INTERNAL;
-    }
-    if (adopt_seed) { h->hash_seed[0] = hd.hash_seed[0]; h->hash_seed[1] = hd.hash_seed[1]; }
-    if (restored) *restored = counts[RESTORE_INSERTED];
-    if (conflicts) *conflicts = counts[RESTORE_CONFLICTS];
+    if (fsync(j->fd) != 0) return fail("fsync");
+    const int fd = j->fd;
+    j->fd = -1;
+    if (close(fd) != 0) return fail("close");
+    if (rename(j->tmp.c_str(), j->path.c_str()) != 0) return fail("rename");
+    j->entries = n;
     return GCRA_OK;
 }
 
-int32_t gcra_snapshot_restore(gcra_engine *h, const char *path, uint32_t rank, uint32_t world, uint64_t *restored,
-                              uint64_t *conflicts) {
-    if (restored) *restored = 0;
-    if (conflicts) *conflicts = 0;
+static void snapshot_writer(SnapshotJob *j, SnapshotStaging *sg, int device) {
+    j->rc = write_snapshot_file(j, sg, device);
+    if (j->rc != GCRA_OK) {
+        // the copies may still be reading into the pinned chunks: done before the next save reuses them
+        cudaStreamSynchronize(sg->stream.get());
+        if (j->fd >= 0) close(j->fd);
+        unlink(j->tmp.c_str());
+    }
+    j->finished.store(true);
+}
+
+static int make_snapshot_staging(gcra_engine *h) {
+    if (h->snap) return GCRA_OK;
+    std::unique_ptr<SnapshotStaging> sg(new SnapshotStaging());
+    CK(sg->stream.make());
+    for (Event *e : {&sg->ev_store, &sg->ev_capture, &sg->ev_chunk[0], &sg->ev_chunk[1]}) CK(e->make(cudaEventDisableTiming));
+    for (auto &c : sg->chunk) CK(c.make(SNAP_CHUNK));
+    CK(sg->meta.make(C_COUNT + 1));
+    int nb = 0;
+    sg->grid = 2 * h->sms;
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, snapshot_capture_kernel, TILE_THREADS, 0) == cudaSuccess && nb > 0)
+        sg->grid = (uint32_t)nb * h->sms;
+    h->snap = std::move(sg);
+    return GCRA_OK;
+}
+
+// Everything that can fail is done before the capture is enqueued: the temporary file, the staging.
+static int snapshot_begin(gcra_engine *h, SnapshotJob &j) {
     CK(cudaSetDevice(h->device));
-    if (world == 0 || rank >= world) { h->err = "snapshot restore: needs rank < world"; return GCRA_INTERNAL; }
-    RestoreBuffers b;
-    b.fd = open(path, O_RDONLY);
-    if (b.fd < 0) { h->err = std::string("snapshot restore: cannot open ") + path; return GCRA_INTERNAL; }
-    const int rc = restore_file(h, b, rank, world, restored, conflicts);
-    // copies still in flight read the pinned staging buffers: wait for them before `b` releases them
-    for (Event &e : b.done) if (e.get()) cudaEventSynchronize(e.get());
-    close(b.fd);
-    return rc;
+    RC(make_snapshot_staging(h));
+    SnapshotStaging &sg = *h->snap;
+    // an upper bound of the entries at the cut, known without waiting for the device
+    tighten_occupied_ub(h);
+    const uint64_t slots = (uint64_t)h->total_lines * 4, tiles = (slots + SNAP_TILE - 1) / SNAP_TILE;
+    j.cap = std::min<uint64_t>(h->occupied_ub, slots);
+    auto up = [](size_t x) { return (x + 255) / 256 * 256; };
+    const size_t ctrl_bytes = (SC_STATUS + tiles) * sizeof(u64);
+    j.keys_off = up(ctrl_bytes);
+    j.state_off = j.keys_off + up(j.cap * sizeof(u64));
+    j.ei_off = j.state_off + up(j.cap * sizeof(TatOff));
+    const size_t need = j.ei_off + up(j.cap * sizeof(i64));
+    if (need > sg.dev_bytes) {
+        // Twice the need, so that the bound's drift between saves does not make each save allocate (a large allocation
+        // takes tens of ms), but never more than the whole table needs.  The smaller buffer is released in stream
+        // order, after the last save's copies.
+        const size_t full = j.keys_off + up(slots * sizeof(u64)) + up(slots * sizeof(TatOff)) + up(slots * sizeof(i64));
+        const size_t bytes = std::min(up(2 * need), full);
+        StreamBuf<unsigned char> fresh;
+        CK(fresh.make(bytes, sg.stream.get()));
+        sg.dev = std::move(fresh);
+        sg.dev_bytes = bytes;
+    }
+    j.total_lines = h->total_lines; j.nb_main = h->tab.nb_main; j.stash_slots = h->tab.stash_slots;
+    j.capacity = h->capacity;
+    j.hash_seed[0] = h->hash_seed[0]; j.hash_seed[1] = h->hash_seed[1];
+    // the cut: after every batch submitted so far (their last stage records ev_back) and every Store-trait op
+    cudaStream_t st = sg.stream.get();
+    for (auto &o : h->scr) if (o.back_recorded) CK(cudaStreamWaitEvent(st, o.ev_back.get(), 0));
+    CK(cudaEventRecord(sg.ev_store.get(), h->stream.get()));
+    CK(cudaStreamWaitEvent(st, sg.ev_store.get(), 0));
+    u64 *ctrl = (u64 *)sg.dev.get();
+    CK(cudaMemsetAsync(ctrl, 0, ctrl_bytes, st));
+    const uint32_t grid = (uint32_t)std::min<uint64_t>(tiles, sg.grid);
+    snapshot_capture_kernel<<<grid, TILE_THREADS, 0, st>>>(h->tab, slots, ctrl, (u64 *)(sg.dev.get() + j.keys_off),
+                                                         (TatOff *)(sg.dev.get() + j.state_off), (i64 *)(sg.dev.get() + j.ei_off), j.cap);
+    h->launches++;
+    CK(cudaGetLastError());
+    CK(cudaMemcpyAsync(sg.meta.get(), h->tab.counters, C_COUNT * sizeof(u64), cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(sg.meta.get() + C_COUNT, ctrl + SC_ENTRIES, sizeof(u64), cudaMemcpyDeviceToHost, st));
+    CK(cudaEventRecord(sg.ev_capture.get(), st));
+    h->capture_pending = true;
+    h->pend_set = -1;          // the next batch's stage 2 waits for every tail: no overlap reaches across the capture
+    return GCRA_OK;
+}
+
+int32_t gcra_snapshot_begin(gcra_engine *h, const char *path) {
+    if (h->job && !h->job->finished.load()) { h->err = "snapshot: a background save is already in flight"; return GCRA_INTERNAL; }
+    if (h->job) {                  // a finished save (wait may have joined its writer already)
+        if (h->job->writer.joinable()) h->job->writer.join();
+        h->job.reset();
+    }
+    std::unique_ptr<SnapshotJob> j(new SnapshotJob());
+    j->path = path;
+    std::vector<char> tmpl(j->path.begin(), j->path.end());
+    const char suffix[] = ".tmp.XXXXXX";
+    tmpl.insert(tmpl.end(), suffix, suffix + sizeof(suffix));
+    j->fd = mkstemp(tmpl.data());
+    if (j->fd < 0) { h->err = std::string("snapshot: cannot create a file next to ") + path; return GCRA_INTERNAL; }
+    j->tmp = tmpl.data();
+    fchmod(j->fd, 0644);
+    int rc = snapshot_begin(h, *j);
+    if (rc == GCRA_OK) {
+        try {
+            j->writer = std::thread(snapshot_writer, j.get(), h->snap.get(), h->device);
+        } catch (const std::exception &) {
+            h->err = "snapshot: cannot start the writer thread";
+            rc = GCRA_INTERNAL;
+        }
+    }
+    if (rc != GCRA_OK) {
+        close(j->fd);
+        unlink(j->tmp.c_str());
+        return rc;
+    }
+    h->job = std::move(j);
+    return GCRA_OK;
+}
+
+int32_t gcra_snapshot_poll(gcra_engine *h, int32_t *done) {
+    *done = 1;
+    if (!h->job) return GCRA_OK;
+    if (!h->job->finished.load()) { *done = 0; return GCRA_OK; }
+    if (h->job->rc != GCRA_OK) { h->err = h->job->err; return GCRA_INTERNAL; }
+    return GCRA_OK;
+}
+
+int32_t gcra_snapshot_wait(gcra_engine *h, uint64_t *entries) {
+    if (entries) *entries = 0;
+    if (!h->job) return GCRA_OK;
+    if (h->job->writer.joinable()) h->job->writer.join();
+    if (h->job->rc != GCRA_OK) { h->err = h->job->err; return GCRA_INTERNAL; }
+    if (entries) *entries = h->job->entries;
+    return GCRA_OK;
 }
 
 

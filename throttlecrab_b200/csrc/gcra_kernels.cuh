@@ -1426,6 +1426,130 @@ restore_kernel(Table t, const u64 *__restrict__ keys, const TatOff *__restrict__
     }
 }
 
+// ---------------------------------------------------------------------------------------------
+// background snapshot (gcra_snapshot_begin): the carried entries of the table, compacted in slot order
+// ---------------------------------------------------------------------------------------------
+// Carries exactly what restore_kernel and rehash_kernel carry: key word >= 2 and has_state(tat + off), expired but
+// unswept entries included.  Persistent CTAs take tiles of SNAP_TILE slots by ticket; a tile's entries go to
+// [exclusive prefix, + count) of the three output sections (keys | (tat, off) pairs | ei), the prefix found by a
+// decoupled look-back over the tiles' status words.  Every earlier tile was handed to a CTA that runs already, so each
+// wait ends.  Positions at or past `cap` are not written; ctrl[SC_ENTRIES] receives the whole count, so a count above
+// `cap` tells the host that the output was cut short.  ctrl is zeroed before the launch.
+constexpr u32 SNAP_ROWS = 4;                               // rows of 2 x TILE_THREADS slots per tile
+constexpr u32 SNAP_TILE = SNAP_ROWS * 2 * TILE_THREADS;
+enum { SC_TICKET = 0, SC_ENTRIES, SC_STATUS };             // ctrl words; tile t's status word is ctrl[SC_STATUS + t]
+constexpr u64 SC_AGG = 1ULL << 62, SC_INC = 1ULL << 63, SC_COUNT = SC_AGG - 1;
+
+__device__ __forceinline__ u64 ld_volatile_u64(const u64 *p) {
+    u64 v;
+    asm volatile("ld.volatile.u64 %0, [%1];" : "=l"(v) : "l"(p) : "memory");
+    return v;
+}
+__device__ __forceinline__ void st_volatile_u64(u64 *p, u64 v) {
+    asm volatile("st.volatile.u64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
+}
+
+__global__ void __launch_bounds__(TILE_THREADS)
+snapshot_capture_kernel(Table t, u64 total_slots, u64 *__restrict__ ctrl, u64 *__restrict__ out_keys,
+                        TatOff *__restrict__ out_state, i64 *__restrict__ out_ei, u64 cap) {
+    constexpr u32 NW = TILE_THREADS / 32;
+    static_assert(SNAP_ROWS * NW == 32, "one warp scans the tile's (row, warp) counts");
+    __shared__ u32 wofs[SNAP_ROWS * NW];     // entries of each (row, warp), then their offset in the tile
+    __shared__ u64 s_base;
+    __shared__ u32 s_tile;
+    const u32 w = threadIdx.x >> 5, lane = threadIdx.x & 31, lt = (1u << lane) - 1;
+    const u64 num_tiles = (total_slots + SNAP_TILE - 1) / SNAP_TILE;
+    for (;;) {
+        if (threadIdx.x == 0) s_tile = (u32)atomicAdd(&ctrl[SC_TICKET], 1ULL);
+        __syncthreads();
+        const u32 tile = s_tile;
+        if (tile >= num_tiles) break;                      // uniform over the CTA
+        // row r, thread i: slots s and s + 1 (the slot count is a power of two >= 64: both exist or neither)
+        const u64 first = (u64)tile * SNAP_TILE + 2 * threadIdx.x;
+        ulonglong2 key[SNAP_ROWS], sa[SNAP_ROWS], sb[SNAP_ROWS], ei[SNAP_ROWS];
+#pragma unroll
+        for (u32 r = 0; r < SNAP_ROWS; r++) {
+            const u64 s = first + (u64)r * 2 * TILE_THREADS;
+            key[r] = make_ulonglong2(0, 0);
+            sa[r] = sb[r] = make_ulonglong2(0, (u64)EXP_EMPTY);
+            ei[r] = make_ulonglong2(0, 0);
+            if (s < total_slots) {
+                key[r] = ld_stream(&t.keys[s]);
+                sa[r] = ld_stream(&t.state[s]);
+                sb[r] = ld_stream(&t.state[s + 1]);
+                ei[r] = ld_stream(&t.ei[s]);
+            }
+        }
+        bool k0[SNAP_ROWS], k1[SNAP_ROWS];
+        u32 rank[SNAP_ROWS];
+#pragma unroll
+        for (u32 r = 0; r < SNAP_ROWS; r++) {
+            k0[r] = key[r].x >= 2 && has_state((i64)(sa[r].x + sa[r].y));
+            k1[r] = key[r].y >= 2 && has_state((i64)(sb[r].x + sb[r].y));
+            const u32 b0 = __ballot_sync(0xffffffffu, k0[r]), b1 = __ballot_sync(0xffffffffu, k1[r]);
+            if (lane == 0) wofs[r * NW + w] = __popc(b0) + __popc(b1);
+            rank[r] = __popc(b0 & lt) + __popc(b1 & lt);
+        }
+        __syncthreads();
+        if (w == 0) {
+            // (row, warp) counts in slot order -> exclusive offsets and the tile's count
+            const u32 v = wofs[lane];
+            u32 inc = v;
+#pragma unroll
+            for (u32 o = 1; o < 32; o <<= 1) {
+                const u32 y = __shfl_up_sync(0xffffffffu, inc, o);
+                if (lane >= o) inc += y;
+            }
+            wofs[lane] = inc - v;
+            const u64 total = __shfl_sync(0xffffffffu, inc, 31);
+            u64 excl = 0;
+            if (tile > 0) {
+                if (lane == 0) st_volatile_u64(&ctrl[SC_STATUS + tile], SC_AGG | total);
+                // lane l reads tile j - l; the walk ends at the nearest inclusive prefix (tile 0 publishes one at once)
+                for (long long j = (long long)tile - 1;; j -= 32) {
+                    const long long idx = j - (long long)lane;
+                    u64 st = SC_INC;
+                    if (idx >= 0) {
+                        do st = ld_volatile_u64(&ctrl[SC_STATUS + idx]); while (st == 0);
+                    }
+                    const u32 incs = __ballot_sync(0xffffffffu, (st & SC_INC) != 0);
+                    const u32 stop = incs ? __ffs(incs) - 1 : 31;
+                    u64 part = lane <= stop ? (st & SC_COUNT) : 0;
+#pragma unroll
+                    for (u32 o = 16; o; o >>= 1) part += __shfl_xor_sync(0xffffffffu, part, o);
+                    excl += part;
+                    if (incs) break;
+                }
+            }
+            if (lane == 0) {
+                st_volatile_u64(&ctrl[SC_STATUS + tile], SC_INC | (excl + total));
+                if (tile == num_tiles - 1) ctrl[SC_ENTRIES] = excl + total;
+                s_base = excl;
+            }
+        }
+        __syncthreads();
+        const u64 base = s_base;
+#pragma unroll
+        for (u32 r = 0; r < SNAP_ROWS; r++) {
+            u64 pos = base + wofs[r * NW + w] + rank[r];
+            if (k0[r]) {
+                if (pos < cap) {
+                    out_keys[pos] = key[r].x;
+                    *reinterpret_cast<ulonglong2 *>(&out_state[pos]) = sa[r];
+                    out_ei[pos] = (i64)ei[r].x;
+                }
+                pos++;
+            }
+            if (k1[r] && pos < cap) {
+                out_keys[pos] = key[r].y;
+                *reinterpret_cast<ulonglong2 *>(&out_state[pos]) = sb[r];
+                out_ei[pos] = (i64)ei[r].y;
+            }
+        }
+        __syncthreads();                                   // (s_tile, wofs and s_base are reused by the next tile)
+    }
+}
+
 
 // ---------------------------------------------------------------------------------------------
 // metrics bridge: denied requests per key, from the kernels' own outputs

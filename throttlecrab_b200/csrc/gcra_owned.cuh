@@ -28,6 +28,29 @@ struct DevBuf : Owned<void *, cudaFree> {
     T *get() const { return static_cast<T *>(h_); }
 };
 
+// device memory for n elements from the stream-ordered allocator: allocated and released in the order of `stream`'s
+// work (cudaMallocAsync / cudaFreeAsync), so neither waits for the device.  The stream must outlive the buffer.
+template <typename T>
+class StreamBuf {
+  public:
+    StreamBuf() = default;
+    StreamBuf(StreamBuf &&o) noexcept : p_(std::exchange(o.p_, nullptr)), s_(o.s_) {}
+    StreamBuf &operator=(StreamBuf &&o) noexcept { std::swap(p_, o.p_); std::swap(s_, o.s_); return *this; }
+    ~StreamBuf() { reset(); }
+    void reset() { if (p_) cudaFreeAsync(std::exchange(p_, nullptr), s_); }
+    cudaError_t make(size_t n, cudaStream_t stream) {
+        reset();
+        s_ = stream;
+        const cudaError_t e = cudaMallocAsync(&p_, n * sizeof(T), stream);
+        if (e) p_ = nullptr;
+        return e;
+    }
+    T *get() const { return static_cast<T *>(p_); }
+  private:
+    void *p_ = nullptr;
+    cudaStream_t s_ = nullptr;
+};
+
 template <typename T>   // pinned host memory for n elements (cudaHostAllocDefault: what cudaMallocHost allocates)
 struct PinnedBuf : Owned<void *, cudaFreeHost> {
     cudaError_t make(size_t n, unsigned flags = cudaHostAllocDefault) { reset(); return took(cudaHostAlloc(&h_, n * sizeof(T), flags)); }

@@ -40,6 +40,18 @@ class _Snapshots:
         self.lim.store.save(path)          # gcra_snapshot_save waits for the device
         return path
 
+    def save_begin(self, directory):
+        """Begin a background save of this rank's table to <directory>/rank<r>.gcra without joining any tick: the cut
+        is this call's place among the ticks submitted here.  Ranks that each call it after submitting the same tick
+        take one consistent cut, and ticks continue meanwhile.  save_wait() waits for the file."""
+        path = os.path.join(directory, "rank%d.gcra" % self.rank)
+        self.lim.store.save_begin(path)
+        return path
+
+    def save_wait(self):
+        """Wait for this rank's background save; returns the number of entries written."""
+        return self.lim.store.save_wait()
+
     def restore(self, paths):
         """Insert this rank's share of every snapshot file in `paths` (all files of a save(), any world size), next to
         what the engine holds.  Call it between ticks, on every rank.  Returns (restored, conflicts) over the files."""
