@@ -171,7 +171,7 @@ struct Scratch {
     DevBuf<u32> sort_ws;                // enqueue_sort: tickets, digit counts, status words (sort_ws_words)
     DevBuf<LongRun> long_runs, giant_runs;
     DevBuf<u32> long_count;
-    Event ev_front, ev_mid, ev_back, ev_fork, ev_join;
+    Event ev_front, ev_mid, ev_back, ev_fork, ev_join, ev_join_giant;
     bool back_recorded = false;
     // index-order pipeline (gcra_index_path.cuh)
     DevBuf<u32> slot_arr;               // [rows] slot of every row (null slot: the row failed validation)
@@ -220,7 +220,8 @@ struct SnapshotJob {
 struct gcra_engine {
     int device = 0;
     uint32_t sms = 0;                // streaming multiprocessors of the device: sizes the grids of the streaming kernels
-    Stream stream, in_stream, out_stream, aux_stream, aux2_stream;
+    Stream stream, in_stream, out_stream;
+    Stream aux_stream, aux2_stream;  // hot runs beside the decide kernel: one CTA per run, one cluster per run
     DevBuf<u64> counters;            // the table's counters: replaced by grow, kept by gcra_snapshot_load
     TableArrays tab_arrays;
     Table tab{};
@@ -580,9 +581,11 @@ static int apply_policy(gcra_engine *h, int64_t now_ns) {
 
 // the cluster kernel: cluster dimension given at launch (cudaLaunchKernelEx)
 template <bool BY_ROW, bool R16>
-static int launch_giant(gcra_engine *h, Scratch &sc, const u64 *src, const OutMap &om, cudaStream_t st) {
+static int launch_giant(gcra_engine *h, Scratch &sc, const u64 *src, const OutMap &om, uint32_t n_max, cudaStream_t st) {
     cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3((128 / CLUSTER_CTAS) * CLUSTER_CTAS);
+    // 16 clusters, or fewer when the batch cannot hold that many giant runs
+    const uint32_t clusters = std::max<uint32_t>(std::min<uint32_t>(16, n_max / GIANT_RUN_MIN), 1);
+    cfg.gridDim = dim3(clusters * CLUSTER_CTAS);
     cfg.blockDim = dim3(LONG_THREADS);
     cfg.stream = st;
     cudaLaunchAttribute attr[1];
@@ -659,23 +662,36 @@ static int enqueue_decide_sorted_t(gcra_engine *h, Scratch &sc, uint32_t n_max, 
     const uint32_t warps = (n_max + 31) / 32;
     uint32_t grid = (warps + DECIDE_THREADS / 32 - 1) / (DECIDE_THREADS / 32);
     if (n_dev) grid = std::min<uint32_t>(grid, 4 * h->sms);
-    decide_kernel<BY_ROW, R16><<<grid, DECIDE_THREADS, 0, st>>>(h->tab, src, sc.drec.get(), n_max, n_dev, om, sc.long_runs.get(), sc.giant_runs.get(),
-                                                           sc.long_count.get(), 0);
+    auto decide = [&]() {   // everything but the hot runs
+        decide_kernel<BY_ROW, R16><<<grid, DECIDE_THREADS, 0, st>>>(h->tab, src, sc.drec.get(), n_max, n_dev, om);
+        h->launches++;
+    };
+    if (n_max < LONG_RUN_MIN) {   // no run can be hot
+        decide();
+        return GCRA_OK;
+    }
+    // The hot runs are listed first, so that their kernels run beside the decide of everything else instead of
+    // after it.  Each goes to a side stream of the highest priority (fork/join with events): the cluster kernel
+    // first, it holds the longest chains.  The three kernels touch disjoint slots and result rows.
+    list_runs_kernel<<<grid, DECIDE_THREADS, 0, st>>>(h->tab, src, n_max, n_dev, sc.long_runs.get(), sc.giant_runs.get(), sc.long_count.get());
     h->launches++;
+    CK(cudaEventRecord(sc.ev_fork.get(), st));
     if (n_max >= GIANT_RUN_MIN) {
-        // the two hot-run kernels work on disjoint runs: the one-CTA-per-run kernel goes to a side
-        // stream and overlaps the cluster kernel (fork/join with events)
-        CK(cudaEventRecord(sc.ev_fork.get(), st));
-        CK(cudaStreamWaitEvent(h->aux_stream.get(), sc.ev_fork.get(), 0));
-        decide_runs_kernel<1, BY_ROW, R16><<<h->sms, LONG_THREADS, 0, h->aux_stream.get()>>>(h->tab, src, sc.drec.get(), om, sc.long_runs.get(), sc.long_count.get());
-        CK(cudaEventRecord(sc.ev_join.get(), h->aux_stream.get()));
-        RC((launch_giant<BY_ROW, R16>(h, sc, src, om, st)));   // hottest keys: one cluster per run
-        CK(cudaStreamWaitEvent(st, sc.ev_join.get(), 0));
-        h->launches += 2;
-    } else if (n_max >= LONG_RUN_MIN) {
-        decide_runs_kernel<1, BY_ROW, R16><<<h->sms, LONG_THREADS, 0, st>>>(h->tab, src, sc.drec.get(), om, sc.long_runs.get(), sc.long_count.get());
+        CK(cudaStreamWaitEvent(h->aux2_stream.get(), sc.ev_fork.get(), 0));
+        RC((launch_giant<BY_ROW, R16>(h, sc, src, om, n_max, h->aux2_stream.get())));   // hottest keys: one cluster per run
+        CK(cudaEventRecord(sc.ev_join_giant.get(), h->aux2_stream.get()));
         h->launches++;
     }
+    // (at most n_max / LONG_RUN_MIN runs: no more CTAs than that)
+    const uint32_t long_grid = std::min<uint32_t>(h->sms, n_max / LONG_RUN_MIN);
+    CK(cudaStreamWaitEvent(h->aux_stream.get(), sc.ev_fork.get(), 0));
+    decide_runs_kernel<1, BY_ROW, R16><<<long_grid, LONG_THREADS, 0, h->aux_stream.get()>>>(h->tab, src, sc.drec.get(), om, sc.long_runs.get(),
+                                                                                          sc.long_count.get());
+    CK(cudaEventRecord(sc.ev_join.get(), h->aux_stream.get()));
+    h->launches++;
+    decide();
+    CK(cudaStreamWaitEvent(st, sc.ev_join.get(), 0));
+    if (n_max >= GIANT_RUN_MIN) CK(cudaStreamWaitEvent(st, sc.ev_join_giant.get(), 0));
     return GCRA_OK;
 }
 
@@ -1008,7 +1024,7 @@ static void preload_kernels() {
         });
     preload(sort_digits_kernel); preload(sort_sweep_kernel);
     preload(decide_kernel<false, false>); preload(decide_kernel<true, false>);
-    preload(decide_kernel<false, true>); preload(decide_kernel<true, true>);
+    preload(decide_kernel<false, true>); preload(decide_kernel<true, true>); preload(list_runs_kernel);
     preload(decide_runs_kernel<1, false, false>); preload(decide_runs_kernel<CLUSTER_CTAS, false, false>);
     preload(decide_runs_kernel<1, true, false>); preload(decide_runs_kernel<CLUSTER_CTAS, true, false>);
     preload(decide_runs_kernel<1, false, true>); preload(decide_runs_kernel<CLUSTER_CTAS, false, true>);
@@ -1037,9 +1053,13 @@ static int init_engine(gcra_engine *h, const gcra_config *cfg) {
     if (sms <= 0) { h->err = "no streaming multiprocessors"; return GCRA_INTERNAL; }
     h->sms = (uint32_t)sms;
     if (const char *g = getenv("GCRA_L2_FETCH")) cudaDeviceSetLimit(cudaLimitMaxL2FetchGranularity, (size_t)atoi(g));
-    for (Stream *s : {&h->stream, &h->in_stream, &h->out_stream, &h->aux_stream, &h->aux2_stream, &h->front_stream,
-                      &h->back_stream, &h->tail_stream})
+    for (Stream *s : {&h->stream, &h->in_stream, &h->out_stream, &h->front_stream, &h->back_stream, &h->tail_stream})
         CK(s->make());
+    // the hot-run kernels' streams: highest priority, so that their few CTAs are dispatched ahead of the decide
+    // kernel's thousands that are launched after them
+    int least_prio = 0, greatest_prio = 0;
+    CK(cudaDeviceGetStreamPriorityRange(&least_prio, &greatest_prio));
+    for (Stream *s : {&h->aux_stream, &h->aux2_stream}) CK(s->make(greatest_prio));
     for (Event *e : {&h->ev_ready, &h->ev_counters}) CK(e->make(cudaEventDisableTiming));
     for (Event &e : h->ev_snap) CK(e.make(cudaEventDisableTiming));
     for (Event &e : h->ev) CK(e.make(cudaEventDefault));         // (timed)
@@ -1108,7 +1128,7 @@ static int init_engine(gcra_engine *h, const gcra_config *cfg) {
         CK(sc.long_runs.make(mb / LONG_RUN_MIN + 1));
         CK(sc.giant_runs.make(mb / GIANT_RUN_MIN + 1));
         CK(sc.long_count.make(2));
-        for (Event *e : {&sc.ev_front, &sc.ev_back, &sc.ev_mid, &sc.ev_fork, &sc.ev_join})
+        for (Event *e : {&sc.ev_front, &sc.ev_back, &sc.ev_mid, &sc.ev_fork, &sc.ev_join, &sc.ev_join_giant})
             CK(e->make(cudaEventDisableTiming));
         CK(sc.h_nres.make(1));
         *sc.h_nres.get() = 0;

@@ -586,7 +586,9 @@ __device__ __forceinline__ void run_chunk(u32 lane, bool mine, u32 gmask, const 
 #endif
 constexpr u32 LONG_RUN_MIN = GCRA_LONG_MIN;     // >= this: one CTA per run (decide_runs_kernel<1>)
 constexpr u32 GIANT_RUN_MIN = GCRA_GIANT_MIN;   // >= this: one cluster per run (decide_runs_kernel<CLUSTER_CTAS>)
-constexpr int LONG_THREADS = 512;
+// 256 threads of ~110 registers: a hot-run CTA leaves room on its SM for a decide_kernel or a sort_sweep_kernel CTA,
+// so that the hot runs are decided beside those kernels (DESIGN §4.2)
+constexpr int LONG_THREADS = 256;
 constexpr int CLUSTER_CTAS = GCRA_CLUSTER;
 struct LongRun { u32 start, len; };
 
@@ -645,9 +647,10 @@ template <bool BY_ROW, bool R16>
 __device__ __forceinline__ void decide_chunk(const Table &t, const u64 *sorted, const Req *__restrict__ drec, u32 n,
                                              const OutMap &out, LongRun *__restrict__ long_runs,
                                              LongRun *__restrict__ giant_runs, u32 *__restrict__ long_count,
-                                             u32 warp_global, u32 lane, int mode = 0) {
-    // mode 0: find the hot runs (work lists) and decide everything else; 1: only find the hot runs; 2: only
-    // decide (the lists were written by a mode-1 launch, the hot-run kernels already work on them)
+                                             u32 warp_global, u32 lane, bool list_runs = false) {
+    // list_runs: only find the hot runs and append them to the work lists; else decide everything but the hot runs
+    // (a list_runs launch before wrote the lists, the hot-run kernels work on them).  Both walk the same run
+    // boundaries below, so the runs that are listed and the runs that are skipped are the same.
     const u32 base = warp_global * 32;
     if (base >= n) return;   // whole warp
 
@@ -687,21 +690,26 @@ __device__ __forceinline__ void decide_chunk(const Table &t, const u64 *sorted, 
     const u32 gmask31 = __shfl_sync(0xffffffffu, gmask, 31);
     if (cont) {
         const u32 run_start = base + (u32)(__ffs(gmask31) - 1);
-        const u32 end = run_end(sorted, n, base + 32, slot31, lane);
-        if (end - run_start >= LONG_RUN_MIN) {
-            // hot key: hand the whole run (including its lanes here) to decide_long_kernel
-            if (lane == 0 && mode != 2) {
-                const bool giant = end - run_start >= GIANT_RUN_MIN;
-                u32 w = atomicAdd(long_count + (giant ? 1 : 0), 1u);
-                LongRun *dst = giant ? giant_runs : long_runs;
-                dst[w].start = run_start;
-                dst[w].len = end - run_start;
+        // sorted, so a run is contiguous: it is hot iff its LONG_RUN_MIN-th request is on the same key.  Only the
+        // listing searches a hot run's end (from there).
+        const u32 hot_at = run_start + LONG_RUN_MIN - 1;   // > base + 32
+        if (hot_at < n && (u32)(sorted[hot_at] >> 32) == slot31) {
+            // hot key: hand the whole run (including its lanes here) to the hot-run kernels
+            if (list_runs) {
+                const u32 end = run_end(sorted, n, hot_at, slot31, lane);
+                if (lane == 0) {
+                    const bool giant = end - run_start >= GIANT_RUN_MIN;
+                    u32 w = atomicAdd(long_count + (giant ? 1 : 0), 1u);
+                    LongRun *dst = giant ? giant_runs : long_runs;
+                    dst[w].start = run_start;
+                    dst[w].len = end - run_start;
+                }
             }
             if ((gmask31 >> lane) & 1) mine = false;
             cont = false;
         }
     }
-    if (mode == 1) return;
+    if (list_runs) return;
 
     Req r = {0, 0, 0, 0};
     const u32 idx = (u32)e;
@@ -811,12 +819,22 @@ __device__ __forceinline__ void decide_chunk(const Table &t, const u64 *sorted, 
 template <bool BY_ROW, bool R16>
 __global__ void __launch_bounds__(DECIDE_THREADS, GCRA_DECIDE_MINBLOCKS)
 decide_kernel(Table t, const u64 *__restrict__ sorted, const Req *__restrict__ drec, u32 n_host,
-              const u32 *__restrict__ n_dev, OutMap out, LongRun *__restrict__ long_runs,
-              LongRun *__restrict__ giant_runs, u32 *__restrict__ long_count, int mode) {
+              const u32 *__restrict__ n_dev, OutMap out) {
     const u32 n = sort_count(n_host, n_dev);
     const u32 warps_total = gridDim.x * (DECIDE_THREADS / 32);
     for (u32 wg = (blockIdx.x * DECIDE_THREADS + threadIdx.x) >> 5; wg * 32 < n; wg += warps_total)
-        decide_chunk<BY_ROW, R16>(t, sorted, drec, n, out, long_runs, giant_runs, long_count, wg, threadIdx.x & 31, mode);
+        decide_chunk<BY_ROW, R16>(t, sorted, drec, n, out, nullptr, nullptr, nullptr, wg, threadIdx.x & 31);
+}
+
+// The hot runs of a sorted batch, into the work lists of the hot-run kernels: decide_chunk's run boundaries without
+// its decisions (which it leaves to decide_kernel), in a kernel of few registers that fills the SMs.
+__global__ void __launch_bounds__(DECIDE_THREADS)
+list_runs_kernel(Table t, const u64 *__restrict__ sorted, u32 n_host, const u32 *__restrict__ n_dev,
+                 LongRun *__restrict__ long_runs, LongRun *__restrict__ giant_runs, u32 *__restrict__ long_count) {
+    const u32 n = sort_count(n_host, n_dev);
+    const u32 warps_total = gridDim.x * (DECIDE_THREADS / 32);
+    for (u32 wg = (blockIdx.x * DECIDE_THREADS + threadIdx.x) >> 5; wg * 32 < n; wg += warps_total)
+        decide_chunk<false, false>(t, sorted, nullptr, n, OutMap{}, long_runs, giant_runs, long_count, wg, threadIdx.x & 31, true);
 }
 
 // Small batches (n < LONG_RUN_MIN, e.g. one RateLimiter::rate_limit call or a lightly loaded actor): ONE CTA
@@ -910,7 +928,7 @@ struct Cands {
 struct PubState { i64 tat, exp; };
 
 template <int CTAS, bool BY_ROW, bool R16>
-__global__ void __launch_bounds__(LONG_THREADS, 1)
+__global__ void __launch_bounds__(LONG_THREADS, 2)
 decide_runs_kernel(Table t, const u64 *__restrict__ sorted, const Req *__restrict__ drec,
                    OutMap out, const LongRun *__restrict__ runs,
                    const u32 *__restrict__ count_ptr) {

@@ -59,6 +59,8 @@ struct PinnedBuf : Owned<void *, cudaFreeHost> {
 
 struct Stream : Owned<cudaStream_t, cudaStreamDestroy> {
     cudaError_t make() { reset(); return took(cudaStreamCreateWithFlags(&h_, cudaStreamNonBlocking)); }
+    // priority: as cudaDeviceGetStreamPriorityRange reports it (lower numbers are higher priorities)
+    cudaError_t make(int priority) { reset(); return took(cudaStreamCreateWithPriority(&h_, cudaStreamNonBlocking, priority)); }
     cudaStream_t get() const { return h_; }
 };
 
