@@ -18,6 +18,7 @@ import numpy as np
 import pytest
 from hypothesis import given, settings, strategies as st
 
+import kernel_geometry as kg
 from test_oracle_vs_python_model import I64_MAX, U64, clamp, derive, wrap64, _tdiv
 
 NEW = "new"
@@ -107,7 +108,7 @@ def fsm_rounds(run, s0, k=4, stride=16):
 # ---------------------------------------------------------------------------------------------------------
 # decide_runs_kernel (csrc/gcra_kernels.cuh) step by step: plain rounds until FSM_AFTER state changes, then
 # finite-state rounds over nibble maps; Cands::find (last match among the first nc), the round-robin victim,
-# one stride of the group (512 rows for a CTA, 4096 for a cluster) after another
+# one stride of the group (kernel_geometry: CTA_STRIDE rows for a CTA, CLUSTER_STRIDE for a cluster) after another
 # ---------------------------------------------------------------------------------------------------------
 FSM_NEW = 0xF
 
@@ -267,8 +268,39 @@ def model_run(pol, q, now, policies=CYCLE_POLICIES):
 
 
 def run_stride(n):
-    """the group a run of n rows gets: None (warp chunks), 512 (one CTA) or 4096 (an 8-CTA cluster)"""
-    return None if n < 256 else 512 if n < 4096 else 4096
+    """the stride of the group a run of n rows gets: None (warp chunks), CTA_STRIDE (one CTA) or CLUSTER_STRIDE (one
+    cluster)"""
+    return None if n < kg.LONG_RUN_MIN else kg.CTA_STRIDE if n < kg.GIANT_RUN_MIN else kg.CLUSTER_STRIDE
+
+
+# The hot-run geometry this model, its event proofs and the GPU scenarios built on them (test_gpu_fsm_cycles.py,
+# test_gpu_hot_run_listing.py) were written for.  A change of the kernels' geometry fails the test below: the
+# positions those scenarios call stride edges, and the events they are proved to reach, have to be looked at again.
+MODEL_GEOMETRY = {"LONG_THREADS": 256, "CLUSTER_CTAS": 8, "LONG_RUN_MIN": 256, "GIANT_RUN_MIN": 4096, "SMALL_MAX": 255}
+
+
+def test_model_geometry_is_the_kernels():
+    """The model's strides and thresholds are the ones gcra_kernels.cuh compiles with, and the hot-run kernel and its
+    launches step through a run by those strides."""
+    assert kg.GEOMETRY == MODEL_GEOMETRY
+    assert (kg.CTA_STRIDE, kg.CLUSTER_STRIDE) == (256, 2048)
+    lo, hi = kg.LONG_RUN_MIN, kg.GIANT_RUN_MIN
+    assert [run_stride(n) for n in (kg.SMALL_MAX, lo - 1, lo, hi - 1, hi, 1 << 20)] == \
+        [None, None, kg.CTA_STRIDE, kg.CTA_STRIDE, kg.CLUSTER_STRIDE, kg.CLUSTER_STRIDE]
+    assert kg.SMALL_MAX < lo < hi and kg.CLUSTER_STRIDE == kg.CLUSTER_CTAS * kg.LONG_THREADS
+    with open(kg.HEADER) as f:
+        src = f.read()
+    for line in ("constexpr u32 STRIDE = CTAS * LONG_THREADS;", "const u32 gpos = rank * LONG_THREADS + tid;",
+                 "const u32 hot_at = run_start + LONG_RUN_MIN - 1;",
+                 "const bool giant = end - run_start >= GIANT_RUN_MIN;"):
+        assert line in src, line
+    # the model's rounds at the parsed strides: a run one row past two strides ends in a one-row stride
+    for stride in (kg.CTA_STRIDE, kg.CLUSTER_STRIDE):
+        pol, q = cycle_steps(2 * stride + 1, 5)
+        run = model_run(pol, q, T0)
+        outs, fin, ev = fsm_rounds_kernel(run, None, stride)
+        assert (outs, fin) == sequential(run, None)
+        assert ev.new_at(stride) >= {stride - 1, 0}
 
 
 T0 = 1_700_000_000 * 10**9
@@ -288,7 +320,7 @@ def test_parallel_schemes_equal_sequential(reqs, start_with_entry):
     want = sequential(run, s0)
     assert speculate_commit(run, s0) == want
     assert fsm_rounds(run, s0) == want
-    for stride in (16, 512):
+    for stride in (16, kg.CTA_STRIDE):
         assert fsm_rounds_kernel(run, s0, stride)[:2] == want
 
 
@@ -302,8 +334,8 @@ def cycle_state(c, j, now=T0):
 
 
 @settings(max_examples=60, deadline=None)
-@given(st.integers(1, 6), st.integers(1, 9000), st.sampled_from([512, 4096]), st.integers(0, 2**32 - 1), st.booleans(),
-       st.sampled_from(["fresh", "cycle", "family"]), st.integers(0, 4), st.sampled_from([0.0, 0.02, 0.3]),
+@given(st.integers(1, 6), st.integers(1, 9000), st.sampled_from([kg.CTA_STRIDE, kg.CLUSTER_STRIDE]),
+       st.integers(0, 2**32 - 1), st.booleans(), st.sampled_from(["fresh", "cycle", "family"]), st.integers(0, 4), st.sampled_from([0.0, 0.02, 0.3]),
        st.sampled_from([0, 10**6, 6 * 10**9]))
 def test_kernel_rounds_on_k_cycles(k, n, stride, seed, periodic, start, n_q1, deny, step):
     """K-cycle runs (K = 1..6, periodic or random order, with q = 1 and denied rows, clocks that stand still or move)
@@ -324,7 +356,7 @@ def test_kernel_rounds_on_k_cycles(k, n, stride, seed, periodic, start, n_q1, de
         assert (outs, fin) == (want[0][len(run) - len(res):], want[1])
 
 
-@pytest.mark.parametrize("stride", [512, 4096])
+@pytest.mark.parametrize("stride", [kg.CTA_STRIDE, kg.CLUSTER_STRIDE])
 @pytest.mark.parametrize("k", range(1, 7))
 def test_k_cycle_events(k, stride):
     """The events a plain rotation through K policies makes the kernel reach over 3 strides and one row.  K <= 3 from

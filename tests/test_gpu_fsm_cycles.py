@@ -1,7 +1,8 @@
 """Hot keys whose entries cycle through 2 to 6 states, against the oracle.
 
-A run of 256 to 4095 rows on one key gets one CTA of `decide_runs_kernel`, a run of 4096 or more an 8-CTA cluster
-(csrc/gcra_kernels.cuh).  After FSM_AFTER (4) state changes in a run the group switches to finite-state rounds: up to
+A run of LONG_RUN_MIN (256) to GIANT_RUN_MIN - 1 (4095) rows on one key gets one CTA of `decide_runs_kernel`, which
+steps through it CTA_STRIDE (256) rows at a time; a longer run gets an 8-CTA cluster, CLUSTER_STRIDE (2048) rows at a
+time (csrc/gcra_kernels.cuh, read by kernel_geometry.py).  After FSM_AFTER (4) state changes in a run the group switches to finite-state rounds: up to
 FSM_K (4) candidate states, one nibble map per request, maps composed over warps, CTAs and the cluster's distributed
 shared memory, a state outside the set published through `sm_pub` into a free candidate or over the round-robin
 `victim`.  Before the switch, plain rounds go back to a known candidate with `Cands::find`.
@@ -25,6 +26,7 @@ import oracle_cur
 import throttlecrab_b200 as tc
 import traces
 from gpu_util import engine_requests, first_mismatch
+from kernel_geometry import CLUSTER_STRIDE as CLUSTER, CTA_STRIDE as CTA, GIANT_RUN_MIN, LONG_RUN_MIN
 from test_algorithm_model import CYCLE_POLICIES, cycle_state, cycle_steps, fsm_rounds_kernel, model_run, residue_view, \
     run_stride, sequential
 from test_gpu_compact_results import assert_pair
@@ -41,7 +43,6 @@ P_INVALID = P_BG + len(traces.POLICIES)          # max_burst = 0 (compact reques
 POLICIES = np.array(CYCLE_POLICIES + [(1, 3, 3600)] + [tuple(p) for p in traces.POLICIES.tolist()] + [(0, 10, 60)],
                     np.int64)
 TOGGLER, BG_KEYS = 999, 500
-CTA, CLUSTER = 512, 4096                         # rows per stride of one CTA and of one cluster (LONG_THREADS = 512)
 
 
 def interleave(rng, runs):
@@ -80,7 +81,7 @@ class Trace:
             self.cycling.add(int(k))
             run, s0 = model_run(p, x, now, CYCLE_POLICIES), self.state.get(int(k))
             for view, (r, rs0) in (("sort", (run, s0)), ("residue", residue_view(run, s0))):
-                if len(key) >= 256 and r is not None and run_stride(len(r)):
+                if len(key) >= LONG_RUN_MIN and r is not None and run_stride(len(r)):
                     self.events[view].append((int(k), len(r), rs0, fsm_rounds_kernel(r, rs0, run_stride(len(r)))[2]))
             self.state[int(k)] = sequential(run, s0)[1]
         self.batches.append((key, pol, q, int(now)))
@@ -150,7 +151,12 @@ def stride_edges(events, stride):
 # ---------------------------------------------------------------------------------------------------------------
 # cycle length x run shape
 # ---------------------------------------------------------------------------------------------------------------
-LENGTHS = [255, 256, 511, 512, 513, 4095, 4096, 4097, 3 * 4096 + 1]
+# around 1, 2 and 3 strides of a CTA (LONG_RUN_MIN - 1 .. + 1: warp chunks, the first CTA run, its first stride edge)
+# and of a cluster (one CTA run of 8 CTA strides; GIANT_RUN_MIN - 1 .. + 1: the CTA / cluster boundary and the second
+# cluster stride edge; GIANT_RUN_MIN + CLUSTER_STRIDE - 1 .. + 1: the third)
+LENGTHS = sorted(n for n in {m * s + d for s in (CTA, CLUSTER) for m in (1, 2, 3) for d in (-1, 0, 1)}
+                 | {LONG_RUN_MIN + d for d in (-1, 0, 1)} | {GIANT_RUN_MIN + d for d in (-1, 0, 1)}
+                 | {GIANT_RUN_MIN + CLUSTER + d for d in (-1, 0, 1)} if n >= LONG_RUN_MIN - 1)
 LEAD = 5                  # cycle policy of the first row of a K <= 3 key: a state outside its cycle
 
 
@@ -171,7 +177,7 @@ def shape_trace(k):
             pol[0] = LEAD
         runs.append((base + j, pol, q))
     if k >= 5:
-        for j, n in enumerate([700, 2500, 4095, 4100, 3 * 4096 + 1]):
+        for j, n in enumerate([700, 2500, GIANT_RUN_MIN - 1, GIANT_RUN_MIN + 4, 3 * CLUSTER + 1]):
             runs.append((base + 100 + j, *cycle_steps(n, k, rng=tr.rng)))
     if k >= 4:
         pre = [(key, np.zeros(1, np.int64), np.zeros(1, np.int64)) for key, _, _ in runs]
@@ -206,9 +212,9 @@ def shape_trace(k):
 
 @pytest.mark.parametrize("k", [2, 3, 4, 5, 6])
 def test_cycle_length_by_run_shape(k):
-    """K-cycles at run lengths 255 (warp chunks), 256 and 511-513 (one CTA, around one stride), 4095 and 4096 (the
-    CTA / cluster boundary), 4097 and 3 * 4096 + 1 (cluster, stride crossings), among 3000 background rows and a
-    toggling key.  K = 4 fills the candidate set exactly and keeps coming back to s0; K = 5 and 6 evict s0, then evict
+    """K-cycles at run lengths 255 (warp chunks), 256-257 and 511-513, 767-769 (one CTA, around one to three strides),
+    2047-2049 (one CTA, eight strides), 4095-4097 (the CTA / cluster boundary, two cluster strides) and 6143-6145 (three
+    cluster strides), among 3000 background rows and a toggling key.  K = 4 fills the candidate set exactly and keeps coming back to s0; K = 5 and 6 evict s0, then evict
     every state they come back to, evict the candidate `cur` points at (random order) and create new states at both
     edges of a stride."""
     tr = shape_trace(k)
@@ -234,19 +240,20 @@ def schedule(n, k, changes, seq, q1_at=()):
 def switch_trace():
     """Keys whose first changes go back and forth between two states (plain rounds back to a known candidate, s0 among
     them for the keys with an entry), whose 4th change falls inside a stride or on either side of its edge, and whose
-    q = 1 rows create new states at stride positions 510-513 and 4094-4097, then again a stride later.  The first row
+    q = 1 rows create new states at the two rows either side of the first stride edge (254-257 in a CTA, 2046-2049 in
+    a cluster), then again a stride later.  The first row
     of every key changes its state, so the residue tail sees the same positions one row earlier."""
     tr = Trace(7)
     now = T0 + 2 * S
     runs = []
     for j, (n, chg, k) in enumerate([
-            (1500, [0, 37, 90, 200, 300], 4),            # the 4th change in the middle of the first stride
-            (1500, [0, 1, 2, 511, 600], 3),              # ... on its last row
-            (1500, [0, 1, 2, 512, 600], 4),              # ... on the first row of the second stride
+            (1500, [0, 37, 90, 200, 230], 4),            # the 4th change in the middle of the first stride
+            (1500, [0, 1, 2, CTA - 1, CTA + 88], 3),       # ... on its last row
+            (1500, [0, 1, 2, CTA, CTA + 88], 4),           # ... on the first row of the second stride
             (1200, [0, 5, 9, 14, 20], 2),
-            (9000, [0, 1000, 2000, 3000, 3500], 4),      # cluster: the 4th change in the middle of the first stride
-            (9000, [0, 1, 2, 4095, 4200], 3),
-            (9000, [0, 1, 2, 4096, 4200], 2)]):
+            (9000, [0, 500, 1000, 1500, 1750], 4),       # cluster: the 4th change in the middle of the first stride
+            (9000, [0, 1, 2, CLUSTER - 1, CLUSTER + 104], 3),
+            (9000, [0, 1, 2, CLUSTER, CLUSTER + 104], 2)]):
         stride = run_stride(n)
         edges = [e + d for e in (stride, 2 * stride) for d in (-2, -1, 0, 1)]
         for entry in (False, True):
@@ -267,7 +274,7 @@ def switch_trace():
 def test_switch_at_the_fourth_change_and_stride_edges():
     """Plain rounds back to known states (s0 included) up to the 4th change; the switch to finite-state rounds in the
     middle of a stride, on its last row and on the first row of the next; new states created by the last thread of a
-    stride and by the first thread of the next, in one CTA (511 / 512) and in a cluster (4095 / 4096)."""
+    stride and by the first thread of the next, in one CTA (255 / 256) and in a cluster (2047 / 2048)."""
     tr = switch_trace()
     req, want, ora = tr.oracle()
     run_blocking(tr, want, ora)
