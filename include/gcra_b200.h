@@ -246,8 +246,9 @@ int32_t gcra_top_denied(gcra_engine *h, uint32_t k, uint64_t *key_hashes, uint64
 int32_t gcra_peek(gcra_engine *h, uint64_t key_hash, int64_t *tat, int64_t *expiry_ns, uint8_t *found);
 /* dump the table to a file / load it back (the reference keeps its state in memory only and loses it on
  * restart); decisions after a load are identical to those of the engine that saved.  gcra_snapshot_save writes a
- * version 2 file (every slot); gcra_snapshot_load also reads version 3 files (gcra_snapshot_begin), inserting their
- * entries into a cleared table of the file's geometry that replaces the engine's table once all are in. */
+ * version 2 file (every slot); gcra_snapshot_load also reads version 3 files (gcra_snapshot_begin).  A load fills a
+ * new table of the file's geometry -- a version 2 file slot for slot, a version 3 file's entries inserted -- that
+ * replaces the engine's table only once every entry is in: a failed load leaves the engine as it was. */
 int32_t gcra_snapshot_save(gcra_engine *h, const char *path);
 int32_t gcra_snapshot_load(gcra_engine *h, const char *path);
 /* Insert the entries of a snapshot file (gcra_snapshot_save, any geometry, any source engine) that shard `rank`

@@ -264,6 +264,53 @@ def test_load_and_restore_v3_and_refuse_malformed_files(tmp_path, k1_path):
         assert bad is None, bad
 
 
+def _shifted(req, by):
+    req = req.copy()
+    req["key"] += np.uint64(by)
+    return req
+
+
+@pytest.mark.parametrize("k1_path", ["auto"], indirect=True)
+def test_load_refuses_malformed_v2_files_and_round_trips_good_ones(tmp_path, k1_path):
+    """A version 2 file of engine A, malformed four ways, loaded into an engine of A's geometry that holds other
+    entries and into one of another geometry: each load is refused and leaves the engine's stats and its next
+    decisions as they were.  The good file, loaded into either engine and saved again, comes back byte for byte."""
+    n_keys, cap, tick = 3000, 1 << 16, 1 << 12        # (cap: room for every row of a batch, so that no batch grows it)
+    a = _engine(cap)
+    _run(a, np.concatenate([traces.warm_pass(n_keys), traces.config4(n_keys=n_keys, n_ticks=1, tick_size=1 << 15, hot=20)]))
+    path = str(tmp_path / "a.v2")
+    a.store.save(path)
+    raw = open(path, "rb").read()
+    slots = a.store.stats()["table_slots"]
+    assert len(raw) == HDR.itemsize + 32 * slots
+    bad_files = {"truncated in ei": raw[:-4096], "truncated in keys": raw[:HDR.itemsize + 8 * (slots // 2)],
+                 "magic": b"X" + raw[1:], "trailing byte": raw + b"\0"}
+    for i, (name, data) in enumerate(bad_files.items()):
+        (tmp_path / ("bad%d" % i)).write_bytes(data)
+    # (engine, its oracle, its key universe: the keys of the trace shifted by `shift`)
+    engines = [(_engine(cap), _oracle(n_keys), n_keys, n_keys),        # A's geometry, other entries
+               (_engine(100), _oracle(50), 50, 10 * n_keys)]           # another geometry
+    for e, ora, n, shift in engines:
+        t = _shifted(np.concatenate([traces.warm_pass(n), traces.config4(n_keys=n, n_ticks=1, tick_size=tick, hot=20)]), shift)
+        assert first_mismatch(ora.replay(t), _run(e, t), t) is None
+    assert engines[0][0].store.stats()["table_slots"] == slots != engines[1][0].store.stats()["table_slots"]
+    keys = ("len", "table_slots", "occupied_slots", "stash_entries")
+    for k, (e, ora, n, shift) in enumerate(engines):
+        for i, name in enumerate(bad_files):
+            before = e.store.stats()
+            with pytest.raises(tc.Internal):
+                e.store.load(str(tmp_path / ("bad%d" % i)))
+            s = e.store.stats()
+            assert [s[f] for f in keys] == [before[f] for f in keys], (k, name)
+            more = _shifted(traces.config4(n_keys=n, n_ticks=1, tick_size=tick, start_tick=1 + i, hot=20), shift)
+            bad = first_mismatch(ora.replay(more), _run(e, more), more)
+            assert bad is None, (k, name, bad)
+        e.store.load(path)
+        again = str(tmp_path / ("again%d" % k))
+        e.store.save(again)
+        assert open(again, "rb").read() == raw, k
+
+
 @pytest.mark.parametrize("k1_path", ["auto"], indirect=True)
 def test_errors_and_lifecycle(tmp_path, k1_path):
     n_keys, tick = 20_000, 1 << 15

@@ -185,9 +185,35 @@ struct Scratch {
     uint32_t nres_rows = 0;             // rows of that batch
 };
 
-// the arrays of the table and of the denied-key table: gcra_engine::tab and ::denied are the views the kernels take
-struct TableArrays { DevBuf<u64> keys, mark; DevBuf<TatOff> state; DevBuf<i64> ei; };
+// One hash table: its arrays, its counters, the view of both that the kernels take, and the capacity it was made for
+// (make_table).  The engine's table is replaced only whole (install_table).
+struct HostTable {
+    DevBuf<u64> keys, mark;
+    DevBuf<TatOff> state;
+    DevBuf<i64> ei;
+    DevBuf<u64> counters;            // [C_COUNT]
+    Table view{};
+    uint64_t capacity = 0;
+    uint64_t load_limit = 0;         // claimed slots past which the table grows (table_geometry)
+    uint64_t slots() const { return (uint64_t)view.null_slot + 1; }
+    uint32_t lines() const { return view.null_slot / 4 + 1; }
+};
+
+// the arrays of the denied-key table: gcra_engine::denied is the view the kernels take
 struct DeniedArrays { DevBuf<u64> keys, counts, dropped; };
+
+// the header of a snapshot file (gcra_snapshot_save, gcra_snapshot_begin)
+namespace {
+struct SnapshotHeader {
+    char magic[8];
+    uint32_t version, total_lines, nb_main, stash_slots;
+    uint64_t capacity;
+    uint64_t counters[C_COUNT];
+    uint64_t hash_seed[2];           // (version 2) the identities in the table were made with this seed
+};
+const char SNAP_MAGIC[8] = {'G', 'C', 'R', 'A', 'B', '2', '0', '0'};
+const size_t SNAP_CHUNK = 32u << 20;
+}  // namespace
 
 // What background saves (gcra_snapshot_begin) keep on the engine and reuse: made by the first save, grown by a later
 // one that needs more room, released by gcra_destroy.
@@ -210,8 +236,7 @@ struct SnapshotJob {
     uint64_t entries = 0;
     int fd = -1;
     std::string tmp, path;
-    uint32_t total_lines = 0, nb_main = 0, stash_slots = 0;    // the table at the cut
-    uint64_t capacity = 0, hash_seed[2] = {0, 0};
+    SnapshotHeader hd{};                                       // the table at the cut; the writer adds the counters
     uint64_t cap = 0;                                          // entries the staging sections hold
     size_t keys_off = 0, state_off = 0, ei_off = 0;            // the sections in the staging
 };
@@ -222,11 +247,7 @@ struct gcra_engine {
     uint32_t sms = 0;                // streaming multiprocessors of the device: sizes the grids of the streaming kernels
     Stream stream, in_stream, out_stream;
     Stream aux_stream, aux2_stream;  // hot runs beside the decide kernel: one CTA per run, one cluster per run
-    DevBuf<u64> counters;            // the table's counters: replaced by grow, kept by gcra_snapshot_load
-    TableArrays tab_arrays;
-    Table tab{};
-    uint32_t total_lines = 0;
-    uint64_t capacity = 0;
+    HostTable tab;                   // replaced whole by grow and gcra_snapshot_load
     bool tight = false;              // GCRA_FLAG_TIGHT_TABLE: tests only, exercises stash + growth
     // scratch for one batch
     uint32_t max_batch = 0;
@@ -326,52 +347,77 @@ static uint32_t ceil_log2(uint64_t x) {
     return b;
 }
 
-static void table_geometry(uint64_t capacity, bool tight, uint32_t &total_lines, uint32_t &nb_main, uint32_t &stash_slots) {
+// The shape of a table for `capacity` entries: its lines of 4 slots, the buckets the two hash choices address, the
+// stash, and the claimed slots past which the table grows.
+struct Geometry { uint32_t total_lines, nb_main, stash_slots; uint64_t load_limit; };
+
+static Geometry table_geometry(uint64_t capacity, bool tight) {
     // first-fit two-choice buckets of 4 stay below ~0.4 % stash traffic up to load 0.5
     uint64_t slots = 1ULL << ceil_log2(std::max<uint64_t>(tight ? capacity : capacity * 2, tight ? 64 : 256));
-    total_lines = (uint32_t)(slots / 4);
-    uint32_t ns = std::max<uint32_t>(tight ? total_lines / 4 : total_lines / 64, 8);
-    nb_main = total_lines - ns;
-    stash_slots = (ns - 1) * 4;   // the last line is reserved (null slot)
+    Geometry g;
+    g.total_lines = (uint32_t)(slots / 4);
+    uint32_t ns = std::max<uint32_t>(tight ? g.total_lines / 4 : g.total_lines / 64, 8);
+    g.nb_main = g.total_lines - ns;
+    g.stash_slots = (ns - 1) * 4;   // the last line is reserved (null slot)
+    const uint64_t main_slots = (uint64_t)g.nb_main * 4;
+    g.load_limit = tight ? main_slots * 13 / 16 : main_slots / 2;
+    return g;
 }
 
-// a new table in `a`, `t` its view
-static int alloc_table(gcra_engine *h, uint64_t capacity, TableArrays &a, Table &t, uint32_t &total_lines, u64 *counters) {
-    uint32_t nb, ss;
-    table_geometry(capacity, h->tight, total_lines, nb, ss);
-    const size_t slots = (size_t)total_lines * 4;
-    CK(a.keys.make(slots));
-    CK(a.state.make(slots));
-    CK(a.ei.make(slots));
-    CK(a.mark.make(slots));
-    t.keys = a.keys.get(); t.state = a.state.get(); t.ei = a.ei.get(); t.mark = a.mark.get();
-    CK(cudaMemsetAsync(t.mark, 0xff, slots * sizeof(u64), h->stream.get()));   // no batch epoch matches
-    t.nb_main = nb;
-    t.stash_slots = ss;
-    t.null_slot = total_lines * 4 - 1;
-    t.slot_bits = ceil_log2((uint64_t)total_lines * 4);
-    t.counters = counters;
+// an empty table for `capacity` entries in `t`, zeroed counters included (enqueued on h->stream)
+static int make_table(gcra_engine *h, uint64_t capacity, HostTable &t) {
+    const Geometry g = table_geometry(capacity, h->tight);
+    const size_t slots = (size_t)g.total_lines * 4;
+    CK(t.counters.make(C_COUNT));
+    CK(cudaMemsetAsync(t.counters.get(), 0, C_COUNT * sizeof(u64), h->stream.get()));
+    CK(t.keys.make(slots));
+    CK(t.state.make(slots));
+    CK(t.ei.make(slots));
+    CK(t.mark.make(slots));
+    Table &v = t.view;
+    v.keys = t.keys.get(); v.state = t.state.get(); v.ei = t.ei.get(); v.mark = t.mark.get();
+    CK(cudaMemsetAsync(v.mark, 0xff, slots * sizeof(u64), h->stream.get()));   // no batch epoch matches
+    v.nb_main = g.nb_main;
+    v.stash_slots = g.stash_slots;
+    v.null_slot = g.total_lines * 4 - 1;
+    v.slot_bits = ceil_log2((uint64_t)g.total_lines * 4);
+    v.counters = t.counters.get();
+    t.capacity = capacity;
+    t.load_limit = g.load_limit;
     uint32_t grid = (uint32_t)std::min<size_t>((slots + TILE_THREADS - 1) / TILE_THREADS, 16 * h->sms);
-    clear_slots_kernel<<<grid, TILE_THREADS, 0, h->stream.get()>>>(t, 0, slots);
+    clear_slots_kernel<<<grid, TILE_THREADS, 0, h->stream.get()>>>(v, 0, slots);
     h->launches++;
     CK(cudaGetLastError());
     return GCRA_OK;
 }
 
-static uint64_t load_limit(const gcra_engine *h) {
-    uint64_t main_slots = (uint64_t)h->tab.nb_main * 4;
-    return h->tight ? main_slots * 13 / 16 : main_slots / 2;
+// `occupied` claimed slots were just read from the device: the host's bound restarts from it, and the occupancy
+// snapshots taken before it are stale
+static void reset_occupancy(gcra_engine *h, uint64_t occupied) {
+    h->occupied_ub = occupied;
+    for (bool &used : h->snap_used) used = false;
 }
 
-static uint64_t load_limit_for(uint64_t capacity, bool tight) {
-    uint32_t tl, nb, ss;
-    table_geometry(capacity, tight, tl, nb, ss);
-    uint64_t main_slots = (uint64_t)nb * 4;
-    return tight ? main_slots * 13 / 16 : main_slots / 2;
+// The counters of a table filled from another one (growth, a version 3 load): the traffic totals `c` carries over,
+// with the occupancy that the new table counted while it was filled (`fresh`).
+static void take_occupancy(u64 c[C_COUNT], const u64 fresh[C_COUNT]) {
+    c[C_OCCUPIED] = fresh[C_OCCUPIED];
+    c[C_REAL] = fresh[C_REAL];
+    c[C_STASH] = fresh[C_STASH];
+}
+
+// `t` (filled, nothing in flight on it) replaces the engine's table, with `counters` as its counter words.  The sweep
+// policy's view of the counters (seen_allowed, seen_expired_hits) is the caller's to set.
+static int install_table(gcra_engine *h, HostTable &&t, const u64 counters[C_COUNT]) {
+    CK(cudaMemcpyAsync(t.counters.get(), counters, C_COUNT * sizeof(u64), cudaMemcpyHostToDevice, h->stream.get()));
+    CK(cudaStreamSynchronize(h->stream.get()));
+    h->tab = std::move(t);
+    reset_occupancy(h, counters[C_OCCUPIED]);
+    return GCRA_OK;
 }
 
 static int refresh_counters(gcra_engine *h, bool wait) {
-    CK(cudaMemcpyAsync(h->h_counters.get(), h->tab.counters, C_COUNT * sizeof(u64), cudaMemcpyDeviceToHost, h->stream.get()));
+    CK(cudaMemcpyAsync(h->h_counters.get(), h->tab.view.counters, C_COUNT * sizeof(u64), cudaMemcpyDeviceToHost, h->stream.get()));
     CK(cudaEventRecord(h->ev_counters.get(), h->stream.get()));
     if (wait) CK(cudaEventSynchronize(h->ev_counters.get()));
     return GCRA_OK;
@@ -382,17 +428,16 @@ static int do_sweep(gcra_engine *h, int64_t now_ns, uint64_t *removed) {
     CK(cudaDeviceSynchronize());   // the sweep is exclusive: batches may be in flight on caller streams
     RC(refresh_counters(h, true));
     uint64_t before = h->h_counters.get()[C_SWEPT];
-    uint32_t grid = (uint32_t)std::min<uint64_t>(((uint64_t)h->total_lines * 2 + TILE_THREADS * SWEEP_UNROLL - 1) / (TILE_THREADS * SWEEP_UNROLL), 16 * h->sms);
+    uint32_t grid = (uint32_t)std::min<uint64_t>((h->tab.slots() / 2 + TILE_THREADS * SWEEP_UNROLL - 1) / (TILE_THREADS * SWEEP_UNROLL), 16 * h->sms);
     CK(cudaEventRecord(h->ev_sweep[0].get(), h->stream.get()));
     static const int sweep_mode = getenv("GCRA_SWEEP_MODE") ? atoi(getenv("GCRA_SWEEP_MODE")) : 0;
-    sweep_kernel<<<grid, TILE_THREADS, 0, h->stream.get()>>>(h->tab, (u64)h->total_lines * 4, now_ns, sweep_mode);
+    sweep_kernel<<<grid, TILE_THREADS, 0, h->stream.get()>>>(h->tab.view, h->tab.slots(), now_ns, sweep_mode);
     CK(cudaEventRecord(h->ev_sweep[1].get(), h->stream.get()));
     h->sweep_timed = true;
     h->launches++;
     CK(cudaGetLastError());
     RC(refresh_counters(h, true));
-    h->occupied_ub = h->h_counters.get()[C_OCCUPIED];
-    for (int i = 0; i < gcra_engine::N_SNAP; i++) h->snap_used[i] = false;
+    reset_occupancy(h, h->h_counters.get()[C_OCCUPIED]);
     h->n_sweeps++;
     if (removed) *removed = h->h_counters.get()[C_SWEPT] - before;
     return GCRA_OK;
@@ -401,22 +446,21 @@ static int do_sweep(gcra_engine *h, int64_t now_ns, uint64_t *removed) {
 // reclaim the slots of keys without an entry (exclusive); returns with fresh counters
 static int purge(gcra_engine *h) {
     CK(cudaDeviceSynchronize());
-    const uint64_t slots = (uint64_t)h->total_lines * 4;
+    const uint64_t slots = h->tab.slots();
     uint32_t grid = (uint32_t)std::min<uint64_t>((slots + TILE_THREADS - 1) / TILE_THREADS, 16 * h->sms);
-    purge_kernel<<<grid, TILE_THREADS, 0, h->stream.get()>>>(h->tab, slots);
+    purge_kernel<<<grid, TILE_THREADS, 0, h->stream.get()>>>(h->tab.view, slots);
     h->launches++;
     CK(cudaGetLastError());
     RC(refresh_counters(h, true));
     if (h->h_counters.get()[C_STASH] == 0) {
         // no key lives in the stash any more: drop its tombstones
-        uint64_t first = (uint64_t)h->tab.nb_main * 4, cnt = slots - first;
+        uint64_t first = (uint64_t)h->tab.view.nb_main * 4, cnt = slots - first;
         clear_slots_kernel<<<(uint32_t)((cnt + TILE_THREADS - 1) / TILE_THREADS), TILE_THREADS, 0, h->stream.get()>>>(
-            h->tab, first, cnt);
+            h->tab.view, first, cnt);
         h->launches++;
         CK(cudaGetLastError());
     }
-    h->occupied_ub = h->h_counters.get()[C_OCCUPIED];
-    for (int i = 0; i < gcra_engine::N_SNAP; i++) h->snap_used[i] = false;
+    reset_occupancy(h, h->h_counters.get()[C_OCCUPIED]);
     h->n_purges++;
     return GCRA_OK;
 }
@@ -424,18 +468,12 @@ static int purge(gcra_engine *h) {
 // HashMap growth: rebuild into a table twice the size
 static int grow(gcra_engine *h, uint64_t need) {
     CK(cudaStreamSynchronize(h->stream.get()));
-    uint64_t newcap = std::max<uint64_t>(h->capacity * 2, 256);
-    while (load_limit_for(newcap, h->tight) < need) newcap *= 2;
-    TableArrays na;
-    Table nt{};
-    uint32_t nl = 0;
-    DevBuf<u64> nc;
-    CK(nc.make(C_COUNT));
-    u64 *ncounters = nc.get();
-    CK(cudaMemsetAsync(ncounters, 0, C_COUNT * sizeof(u64), h->stream.get()));
-    RC(alloc_table(h, newcap, na, nt, nl, ncounters));
-    uint32_t grid = std::min<uint32_t>((h->total_lines + TILE_THREADS - 1) / TILE_THREADS, 8 * h->sms);
-    rehash_kernel<<<grid, TILE_THREADS, 0, h->stream.get()>>>(h->tab, (u64)h->total_lines * 4, nt);
+    uint64_t newcap = std::max<uint64_t>(h->tab.capacity * 2, 256);
+    while (table_geometry(newcap, h->tight).load_limit < need) newcap *= 2;
+    HostTable nt;
+    RC(make_table(h, newcap, nt));
+    uint32_t grid = std::min<uint32_t>((h->tab.lines() + TILE_THREADS - 1) / TILE_THREADS, 8 * h->sms);
+    rehash_kernel<<<grid, TILE_THREADS, 0, h->stream.get()>>>(h->tab.view, h->tab.slots(), nt.view);
     h->launches++;
     CK(cudaGetLastError());
     // carry the running totals over
@@ -443,21 +481,11 @@ static int grow(gcra_engine *h, uint64_t need) {
     u64 keep[C_COUNT];
     memcpy(keep, h->h_counters.get(), sizeof(keep));
     u64 fresh[C_COUNT];
-    CK(cudaMemcpyAsync(fresh, ncounters, sizeof(fresh), cudaMemcpyDeviceToHost, h->stream.get()));
+    CK(cudaMemcpyAsync(fresh, nt.counters.get(), sizeof(fresh), cudaMemcpyDeviceToHost, h->stream.get()));
     CK(cudaStreamSynchronize(h->stream.get()));
     if (fresh[C_INSERT_FAIL]) { h->err = "table growth lost entries"; return GCRA_INTERNAL; }
-    keep[C_OCCUPIED] = fresh[C_OCCUPIED];
-    keep[C_REAL] = fresh[C_REAL];
-    keep[C_STASH] = fresh[C_STASH];
-    CK(cudaMemcpyAsync(ncounters, keep, sizeof(keep), cudaMemcpyHostToDevice, h->stream.get()));
-    CK(cudaStreamSynchronize(h->stream.get()));
-    h->tab_arrays = std::move(na);
-    h->counters = std::move(nc);
-    h->tab = nt;
-    h->total_lines = nl;
-    h->capacity = newcap;
-    h->occupied_ub = keep[C_OCCUPIED];
-    for (int i = 0; i < gcra_engine::N_SNAP; i++) h->snap_used[i] = false;
+    take_occupancy(keep, fresh);
+    RC(install_table(h, std::move(nt), keep));
     h->n_grows++;
     return GCRA_OK;
 }
@@ -476,21 +504,21 @@ static void tighten_occupied_ub(gcra_engine *h) {
 }
 
 static int ensure_room(gcra_engine *h, uint64_t n) {
-    if (h->occupied_ub + n <= load_limit(h)) { h->occupied_ub += n; return GCRA_OK; }
+    if (h->occupied_ub + n <= h->tab.load_limit) { h->occupied_ub += n; return GCRA_OK; }
     tighten_occupied_ub(h);
-    if (h->occupied_ub + n <= load_limit(h)) { h->occupied_ub += n; return GCRA_OK; }
+    if (h->occupied_ub + n <= h->tab.load_limit) { h->occupied_ub += n; return GCRA_OK; }
     int rc = refresh_counters(h, true);
     if (rc) return rc;
     CK(cudaDeviceSynchronize());   // batches may be in flight on caller streams
     rc = refresh_counters(h, true);
     if (rc) return rc;
     h->occupied_ub = h->h_counters.get()[C_OCCUPIED];
-    if (h->occupied_ub + n > load_limit(h) && h->h_counters.get()[C_OCCUPIED] > h->h_counters.get()[C_REAL]) {
+    if (h->occupied_ub + n > h->tab.load_limit && h->h_counters.get()[C_OCCUPIED] > h->h_counters.get()[C_REAL]) {
         // crowded: first give back the slots of keys that hold no entry (swept or only ever denied)
         rc = purge(h);
         if (rc) return rc;
     }
-    if (h->occupied_ub + n > load_limit(h)) {
+    if (h->occupied_ub + n > h->tab.load_limit) {
         rc = grow(h, (h->occupied_ub + n));
         if (rc) return rc;
     }
@@ -502,7 +530,7 @@ static int snapshot_async(gcra_engine *h, uint64_t n, cudaStream_t st) {
     h->rows_launched += n;
     int k = (int)h->snap_next;
     h->snap_next = (h->snap_next + 1) % gcra_engine::N_SNAP;
-    CK(cudaMemcpyAsync(h->h_snap.get() + (size_t)k * C_COUNT, h->tab.counters, C_COUNT * sizeof(u64), cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(h->h_snap.get() + (size_t)k * C_COUNT, h->tab.view.counters, C_COUNT * sizeof(u64), cudaMemcpyDeviceToHost, st));
     CK(cudaEventRecord(h->ev_snap[k].get(), st));
     h->snap_rows_after[k] = h->rows_launched;
     h->snap_used[k] = true;
@@ -518,7 +546,7 @@ static bool adaptive_should_clean(const gcra_engine *h, __int128 now, uint64_t l
         double threshold = (h->last_removed > h->last_total / 4) ? 0.2 / 2.0 : 0.2 * 1.25;
         if (ratio > threshold) return true;
     }
-    if (len > load_limit(h) * 3 / 4) return true;
+    if (len > h->tab.load_limit * 3 / 4) return true;
     return false;
 }
 
@@ -599,7 +627,7 @@ static int launch_giant(gcra_engine *h, Scratch &sc, const u64 *src, const OutMa
         static bool once = false;
         if (!once) { cudaFuncSetAttribute(decide_runs_kernel<CLUSTER_CTAS, BY_ROW, R16>, cudaFuncAttributeNonPortableClusterSizeAllowed, 1); once = true; }
     }
-    CK(cudaLaunchKernelEx(&cfg, decide_runs_kernel<CLUSTER_CTAS, BY_ROW, R16>, h->tab, (const u64 *)src, (const Req *)sc.drec.get(), om,
+    CK(cudaLaunchKernelEx(&cfg, decide_runs_kernel<CLUSTER_CTAS, BY_ROW, R16>, h->tab.view, (const u64 *)src, (const Req *)sc.drec.get(), om,
                           (const LongRun *)sc.giant_runs.get(), (const u32 *)(sc.long_count.get() + 1)));
     return GCRA_OK;
 }
@@ -617,7 +645,7 @@ static BatchView single_view(const void *d_req, gcra_result *d_res, uint32_t n) 
 // stable LSD radix sort of `n` (host count) or `*n_dev` (device count) keys on the slot bits; returns the buffer
 // that holds the sorted keys.  One digit-count launch, then one sweep launch per pass.
 static int enqueue_sort(gcra_engine *h, Scratch &sc, uint32_t n_max, const u32 *n_dev, cudaStream_t st, u64 **sorted_out) {
-    const uint32_t bits = h->tab.slot_bits;
+    const uint32_t bits = h->tab.view.slot_bits;
     const uint32_t passes = (bits + SORT_MAX_BITS - 1) / SORT_MAX_BITS;
     const uint32_t tiles = (n_max + SORT_TILE - 1) / SORT_TILE;
     // With a device count (the residue of the index-order pipeline, usually a small part of n_max) both grids are
@@ -663,7 +691,7 @@ static int enqueue_decide_sorted_t(gcra_engine *h, Scratch &sc, uint32_t n_max, 
     uint32_t grid = (warps + DECIDE_THREADS / 32 - 1) / (DECIDE_THREADS / 32);
     if (n_dev) grid = std::min<uint32_t>(grid, 4 * h->sms);
     auto decide = [&]() {   // everything but the hot runs
-        decide_kernel<BY_ROW, R16><<<grid, DECIDE_THREADS, 0, st>>>(h->tab, src, sc.drec.get(), n_max, n_dev, om);
+        decide_kernel<BY_ROW, R16><<<grid, DECIDE_THREADS, 0, st>>>(h->tab.view, src, sc.drec.get(), n_max, n_dev, om);
         h->launches++;
     };
     if (n_max < LONG_RUN_MIN) {   // no run can be hot
@@ -673,7 +701,7 @@ static int enqueue_decide_sorted_t(gcra_engine *h, Scratch &sc, uint32_t n_max, 
     // The hot runs are listed first, so that their kernels run beside the decide of everything else instead of
     // after it.  Each goes to a side stream of the highest priority (fork/join with events): the cluster kernel
     // first, it holds the longest chains.  The three kernels touch disjoint slots and result rows.
-    list_runs_kernel<<<grid, DECIDE_THREADS, 0, st>>>(h->tab, src, n_max, n_dev, sc.long_runs.get(), sc.giant_runs.get(), sc.long_count.get());
+    list_runs_kernel<<<grid, DECIDE_THREADS, 0, st>>>(h->tab.view, src, n_max, n_dev, sc.long_runs.get(), sc.giant_runs.get(), sc.long_count.get());
     h->launches++;
     CK(cudaEventRecord(sc.ev_fork.get(), st));
     if (n_max >= GIANT_RUN_MIN) {
@@ -685,7 +713,7 @@ static int enqueue_decide_sorted_t(gcra_engine *h, Scratch &sc, uint32_t n_max, 
     // (at most n_max / LONG_RUN_MIN runs: no more CTAs than that)
     const uint32_t long_grid = std::min<uint32_t>(h->sms, n_max / LONG_RUN_MIN);
     CK(cudaStreamWaitEvent(h->aux_stream.get(), sc.ev_fork.get(), 0));
-    decide_runs_kernel<1, BY_ROW, R16><<<long_grid, LONG_THREADS, 0, h->aux_stream.get()>>>(h->tab, src, sc.drec.get(), om, sc.long_runs.get(),
+    decide_runs_kernel<1, BY_ROW, R16><<<long_grid, LONG_THREADS, 0, h->aux_stream.get()>>>(h->tab.view, src, sc.drec.get(), om, sc.long_runs.get(),
                                                                                           sc.long_count.get());
     CK(cudaEventRecord(sc.ev_join.get(), h->aux_stream.get()));
     h->launches++;
@@ -759,7 +787,7 @@ static int enqueue_front(gcra_engine *h, Scratch &sc, const BatchView &v, bool i
         CK(cudaMemsetAsync(sc.ctrl_block.get(), 0, ((size_t)h->max_tiles + 1) * sizeof(u64), st));
         if (timed) CK(cudaEventRecord(h->evd[0].get(), st));
         with_fmt(fmt, [&](auto F) {
-            probe_kernel<F><<<grid, TILE_THREADS, 0, st>>>(h->tab, v, h->d_pol.get(), h->npol, now_batch, sc.slot_arr.get(), sc.bitmap.get(),
+            probe_kernel<F><<<grid, TILE_THREADS, 0, st>>>(h->tab.view, v, h->d_pol.get(), h->npol, now_batch, sc.slot_arr.get(), sc.bitmap.get(),
                                                            h->bm_mask, h->prefetch_state);
         });
         if (timed) CK(cudaEventRecord(h->evd[1].get(), st));
@@ -770,7 +798,7 @@ static int enqueue_front(gcra_engine *h, Scratch &sc, const BatchView &v, bool i
     const uint32_t n = v.n;
     const uint32_t tiles = (n + TILE_THREADS - 1) / TILE_THREADS;
     with_fmt(fmt, [&](auto F) {
-        ingest_kernel<F><<<tiles, TILE_THREADS, 0, st>>>(h->tab, v.req0, h->d_pol.get(), h->npol, now_batch, n, sc.drec.get(),
+        ingest_kernel<F><<<tiles, TILE_THREADS, 0, st>>>(h->tab.view, v.req0, h->d_pol.get(), h->npol, now_batch, n, sc.drec.get(),
                                                          sc.keys_a.get(), v.res0);
     });
     h->launches++;
@@ -789,7 +817,7 @@ static int enqueue_mid_index(gcra_engine *h, Scratch &sc, Scratch &next, const B
     const u32 hp = honour_pend ? 1u : 0u;
     if (++h->epoch == 0) {
         // the 32-bit batch epoch wrapped: forget every mark (once per 4 G batches)
-        CK(cudaMemsetAsync(h->tab.mark, 0xff, (size_t)h->total_lines * 4 * sizeof(u64), st));
+        CK(cudaMemsetAsync(h->tab.view.mark, 0xff, h->tab.slots() * sizeof(u64), st));
         h->epoch = 1;
     }
     const uint32_t rows = view_max_rows(v);
@@ -798,10 +826,10 @@ static int enqueue_mid_index(gcra_engine *h, Scratch &sc, Scratch &next, const B
     u32 *ctrl = reinterpret_cast<u32 *>(sc.ctrl_block.get());
     u64 *status = sc.ctrl_block.get() + 1;
     RC(with_fmt(fmt, [&](auto F) {
-        decide_index_kernel<F><<<grid, TILE_THREADS, 0, st>>>(h->tab, v, h->d_pol.get(), h->npol, now_batch, sc.slot_arr.get(), sc.bitmap.get(),
+        decide_index_kernel<F><<<grid, TILE_THREADS, 0, st>>>(h->tab.view, v, h->d_pol.get(), h->npol, now_batch, sc.slot_arr.get(), sc.bitmap.get(),
                                                               sc.pend.get(), h->bm_mask, sc.flags.get(), h->epoch, hp, h->dbg);
         if (timed) CK(cudaEventRecord(h->evd[3].get(), st));
-        resolve_kernel<F><<<rgrid, TILE_THREADS, 0, st>>>(h->tab, v, h->d_pol.get(), h->npol, now_batch, sc.slot_arr.get(), h->bm_mask,
+        resolve_kernel<F><<<rgrid, TILE_THREADS, 0, st>>>(h->tab.view, v, h->d_pol.get(), h->npol, now_batch, sc.slot_arr.get(), h->bm_mask,
                                                           sc.flags.get(), h->epoch, ctrl, status, sc.keys_a.get(), next.pend.get(),
                                                           sc.h_nres.get(), h->max_batch);
         return GCRA_OK;
@@ -885,7 +913,7 @@ static int launch_batch(gcra_engine *h, uint32_t n, const void *d_req, int fmt, 
         // the compare-and-update in a single launch
         if (timed) { CK(cudaEventRecord(h->ev[0].get(), st)); CK(cudaEventRecord(h->ev[1].get(), st)); CK(cudaEventRecord(h->ev[2].get(), st)); }
         with_fmt(fmt, [&](auto F) {
-            small_batch_kernel<F><<<1, TILE_THREADS, 0, st>>>(h->tab, d_req, h->d_pol.get(), h->npol, now_batch, n, sc.drec.get(), d_res);
+            small_batch_kernel<F><<<1, TILE_THREADS, 0, st>>>(h->tab.view, d_req, h->d_pol.get(), h->npol, now_batch, n, sc.drec.get(), d_res);
         });
         h->launches++;
         if (timed) { CK(cudaEventRecord(h->ev[3].get(), st)); h->ev_valid = true; }
@@ -1065,7 +1093,6 @@ static int init_engine(gcra_engine *h, const gcra_config *cfg) {
     for (Event &e : h->ev) CK(e.make(cudaEventDefault));         // (timed)
     for (Event &e : h->evd) CK(e.make(cudaEventDefault));
     for (Event &e : h->ev_sweep) CK(e.make(cudaEventDefault));
-    h->capacity = cfg->capacity ? cfg->capacity : 1000;      // DEFAULT_CAPACITY adaptive_cleanup.rs:10
     h->max_batch = cfg->max_batch ? cfg->max_batch : (1u << 20);
     h->tight = (cfg->flags & GCRA_FLAG_TIGHT_TABLE) != 0;
     h->hash_seed[0] = cfg->hash_seed[0];
@@ -1077,9 +1104,7 @@ static int init_engine(gcra_engine *h, const gcra_config *cfg) {
         if (!got) { h->err = "cannot read /dev/urandom for the hash seed"; return GCRA_INTERNAL; }
         h->hash_seed[0] |= 1;      // never (0, 0)
     }
-    CK(h->counters.make(C_COUNT));
-    CK(cudaMemsetAsync(h->counters.get(), 0, C_COUNT * sizeof(u64), h->stream.get()));
-    RC(alloc_table(h, h->capacity, h->tab_arrays, h->tab, h->total_lines, h->counters.get()));
+    RC(make_table(h, cfg->capacity ? cfg->capacity : 1000, h->tab));   // DEFAULT_CAPACITY adaptive_cleanup.rs:10
     const size_t mb = h->max_batch;
     {
         // index-order pipeline: hashed batch counters (32 bits) and pend bits, 8 entries per row of the largest
@@ -1268,7 +1293,7 @@ static int store_op(gcra_engine *h, int op, uint64_t key_hash, int64_t a, int64_
     // caller's stream (launch_batch orders itself the same way)
     for (auto &o : h->scr) if (o.back_recorded) CK(cudaStreamWaitEvent(h->stream.get(), o.ev_back.get(), 0));
     RC(after_capture(h, h->stream.get()));
-    store_op_kernel<<<1, 1, 0, h->stream.get()>>>(h->tab, op, stored_key(key_hash), a, b, ttl, now, h->d_op.get());
+    store_op_kernel<<<1, 1, 0, h->stream.get()>>>(h->tab.view, op, stored_key(key_hash), a, b, ttl, now, h->d_op.get());
     h->launches++;
     CK(cudaMemcpyAsync(h->h_op.get(), h->d_op.get(), 2 * sizeof(StoreOpResult), cudaMemcpyDeviceToHost, h->stream.get()));
     CK(cudaStreamSynchronize(h->stream.get()));
@@ -1503,7 +1528,7 @@ int32_t gcra_ring_submit(gcra_engine *h, uint32_t slot, uint32_t n, int64_t now_
     int rc = launch_pipelined(h, n, s.d_req.get(), h->ring_fmt, now_ns, s.d_res.get(), s.ev_in.get(), &done);
     if (rc) return rc;
     if (done) CK(cudaStreamWaitEvent(h->out_stream.get(), done, 0));
-    CK(cudaMemcpyAsync(h->h_counters.get(), h->tab.counters, C_COUNT * sizeof(u64), cudaMemcpyDeviceToHost, h->out_stream.get()));
+    CK(cudaMemcpyAsync(h->h_counters.get(), h->tab.view.counters, C_COUNT * sizeof(u64), cudaMemcpyDeviceToHost, h->out_stream.get()));
     CK(cudaEventRecord(h->ev_counters.get(), h->out_stream.get()));
     CK(cudaMemcpyAsync(s.h_res.get(), s.d_res.get(), (size_t)n * ressz, cudaMemcpyDeviceToHost, h->out_stream.get()));
     CK(cudaEventRecord(s.ev_done.get(), h->out_stream.get()));
@@ -1563,7 +1588,7 @@ int32_t gcra_get_stats(gcra_engine *h, gcra_stats *out) {
     const u64 *c = h->h_counters.get();
     out->len = c[C_REAL];
     out->occupied_slots = c[C_OCCUPIED];
-    out->table_slots = (uint64_t)h->total_lines * 4;
+    out->table_slots = h->tab.slots();
     out->stash_entries = c[C_STASH];
     out->allowed = c[C_ALLOWED];
     out->denied = c[C_DENIED];
@@ -1689,17 +1714,16 @@ int32_t gcra_last_sweep_ms(gcra_engine *h, float *ms) {
 uint64_t gcra_launch_count(gcra_engine *h) { return h->launches; }
 
 // ---- snapshot / restore (absent in the reference: its state is lost on restart; SURVEY 8f #4) -----------
-namespace {
-struct SnapshotHeader {
-    char magic[8];
-    uint32_t version, total_lines, nb_main, stash_slots;
-    uint64_t capacity;
-    uint64_t counters[C_COUNT];
-    uint64_t hash_seed[2];           // (version 2) the identities in the table were made with this seed
-};
-const char SNAP_MAGIC[8] = {'G', 'C', 'R', 'A', 'B', '2', '0', '0'};
-const size_t SNAP_CHUNK = 32u << 20;
-}  // namespace
+// the header of a file of the engine's table; the caller fills in the counters
+static SnapshotHeader header_of(const gcra_engine *h, uint32_t version) {
+    SnapshotHeader hd{};
+    memcpy(hd.magic, SNAP_MAGIC, 8);
+    hd.version = version;
+    hd.total_lines = h->tab.lines(); hd.nb_main = h->tab.view.nb_main; hd.stash_slots = h->tab.view.stash_slots;
+    hd.capacity = h->tab.capacity;
+    hd.hash_seed[0] = h->hash_seed[0]; hd.hash_seed[1] = h->hash_seed[1];
+    return hd;
+}
 
 static int copy_to_file(gcra_engine *h, FILE *f, const void *dptr, size_t bytes, std::vector<char> &buf) {
     for (size_t off = 0; off < bytes; off += SNAP_CHUNK) {
@@ -1710,39 +1734,26 @@ static int copy_to_file(gcra_engine *h, FILE *f, const void *dptr, size_t bytes,
     return GCRA_OK;
 }
 
-static int copy_from_file(gcra_engine *h, FILE *f, void *dptr, size_t bytes, std::vector<char> &buf) {
-    for (size_t off = 0; off < bytes; off += SNAP_CHUNK) {
-        size_t m = std::min(SNAP_CHUNK, bytes - off);
-        if (fread(buf.data(), 1, m, f) != m) { h->err = "snapshot: short read"; return GCRA_INTERNAL; }
-        CK(cudaMemcpy((char *)dptr + off, buf.data(), m, cudaMemcpyHostToDevice));
-    }
-    return GCRA_OK;
-}
-
 int32_t gcra_snapshot_save(gcra_engine *h, const char *path) {
     CK(cudaSetDevice(h->device));
     CK(cudaDeviceSynchronize());
     FILE *f = fopen(path, "wb");
     if (!f) { h->err = std::string("snapshot: cannot open ") + path; return GCRA_INTERNAL; }
-    SnapshotHeader hd{};
-    memcpy(hd.magic, SNAP_MAGIC, 8);
-    hd.version = 2; hd.hash_seed[0] = h->hash_seed[0]; hd.hash_seed[1] = h->hash_seed[1]; hd.total_lines = h->total_lines; hd.nb_main = h->tab.nb_main; hd.stash_slots = h->tab.stash_slots;
-    hd.capacity = h->capacity;
+    SnapshotHeader hd = header_of(h, 2);
     int rc = GCRA_OK;
-    if (cudaMemcpy(hd.counters, h->tab.counters, sizeof(hd.counters), cudaMemcpyDeviceToHost) != cudaSuccess ||
+    if (cudaMemcpy(hd.counters, h->tab.view.counters, sizeof(hd.counters), cudaMemcpyDeviceToHost) != cudaSuccess ||
         fwrite(&hd, sizeof(hd), 1, f) != 1) { h->err = "snapshot: header"; rc = GCRA_INTERNAL; }
     std::vector<char> buf(SNAP_CHUNK);
-    const size_t slots = (size_t)h->total_lines * 4;
-    if (!rc) rc = copy_to_file(h, f, h->tab.keys, slots * sizeof(u64), buf);
-    if (!rc) rc = copy_to_file(h, f, h->tab.state, slots * sizeof(TatOff), buf);
-    if (!rc) rc = copy_to_file(h, f, h->tab.ei, slots * sizeof(i64), buf);
+    const size_t slots = h->tab.slots();
+    if (!rc) rc = copy_to_file(h, f, h->tab.view.keys, slots * sizeof(u64), buf);
+    if (!rc) rc = copy_to_file(h, f, h->tab.view.state, slots * sizeof(TatOff), buf);
+    if (!rc) rc = copy_to_file(h, f, h->tab.view.ei, slots * sizeof(i64), buf);
     if (fclose(f) != 0 && !rc) { h->err = "snapshot: close"; rc = GCRA_INTERNAL; }
     return rc;
 }
 
-// Streams the file through the GPU twice, in chunks of RESTORE_CHUNK slots (one staging set = SNAP_CHUNK bytes over
-// the three sections; two sets, so that reading chunk i + 1 overlaps the kernel over chunk i): a COUNT pass sizes the
-// table for the entries this shard takes, an INSERT pass inserts them.
+// Streams a file through the GPU in chunks of RESTORE_CHUNK slots (one staging set = SNAP_CHUNK bytes over the three
+// sections; two sets, so that reading chunk i + 1 overlaps the copy and kernel of chunk i).
 namespace {
 const size_t RESTORE_CHUNK = SNAP_CHUNK / (sizeof(u64) + sizeof(TatOff) + sizeof(i64));
 
@@ -1753,6 +1764,10 @@ struct RestoreBuffers {
     Event done[2];                     // the set's copy + kernel finished: its host buffer may be refilled
     int fd = -1;
 };
+
+// What restore_pass does with each chunk: restore_kernel counts the entries this shard takes (COUNT) or inserts them
+// (INSERT); COPY writes the sections to the same slots of the table (a version 2 load: they are its arrays).
+enum RestorePass { PASS_COUNT, PASS_INSERT, PASS_COPY };
 }  // namespace
 
 static bool pread_all(int fd, void *buf, size_t bytes, uint64_t off) {
@@ -1769,7 +1784,10 @@ static bool pread_all(int fd, void *buf, size_t bytes, uint64_t off) {
 // sections restricted to the n carried entries.
 struct SnapSections { uint64_t rows, keys_off, state_off, ei_off; };
 
-static const char *snapshot_sections(int fd, const SnapshotHeader &hd, SnapSections &sec) {
+// the header of the file open at `fd` and where its sections lie; null, or why the file is refused
+static const char *read_header(int fd, SnapshotHeader &hd, SnapSections &sec) {
+    if (!pread_all(fd, &hd, sizeof(hd), 0) || memcmp(hd.magic, SNAP_MAGIC, 8) != 0 || (hd.version != 2 && hd.version != 3))
+        return "bad header";
     struct stat sb;
     if (fstat(fd, &sb) != 0) return "cannot stat the file";
     const uint64_t size = (uint64_t)sb.st_size, row = sizeof(u64) + sizeof(TatOff) + sizeof(i64);
@@ -1802,29 +1820,32 @@ static int make_restore_buffers(gcra_engine *h, RestoreBuffers &b) {
     return GCRA_OK;
 }
 
-// one pass of restore_kernel over the `sec.rows` rows of a file's sections into table `t`
+// one pass over the `sec.rows` rows of a file's sections into table `t`
 static int restore_pass(gcra_engine *h, RestoreBuffers &b, const Table &t, const SnapSections &sec, uint32_t rank,
-                        uint32_t world, bool insert) {
+                        uint32_t world, RestorePass pass) {
     for (uint64_t first = 0, c = 0; first < sec.rows; first += RESTORE_CHUNK, c++) {
         const int s = (int)(c & 1);
         const uint64_t n = std::min<uint64_t>(RESTORE_CHUNK, sec.rows - first);
         char *hk = b.host[s].get(), *hs = hk + RESTORE_CHUNK * sizeof(u64), *he = hs + RESTORE_CHUNK * sizeof(TatOff);
         char *dk = b.dev[s].get(), *ds = dk + RESTORE_CHUNK * sizeof(u64), *de = ds + RESTORE_CHUNK * sizeof(TatOff);
+        if (pass == PASS_COPY) { dk = (char *)(t.keys + first); ds = (char *)(t.state + first); de = (char *)(t.ei + first); }
         CK(cudaEventSynchronize(b.done[s].get()));
         if (!pread_all(b.fd, hk, n * sizeof(u64), sec.keys_off + first * sizeof(u64)) ||
             !pread_all(b.fd, hs, n * sizeof(TatOff), sec.state_off + first * sizeof(TatOff)) ||
-            (insert && !pread_all(b.fd, he, n * sizeof(i64), sec.ei_off + first * sizeof(i64)))) {
-            h->err = "snapshot restore: short read";
+            (pass != PASS_COUNT && !pread_all(b.fd, he, n * sizeof(i64), sec.ei_off + first * sizeof(i64)))) {
+            h->err = "snapshot: short read";
             return GCRA_INTERNAL;
         }
         CK(cudaMemcpyAsync(dk, hk, n * sizeof(u64), cudaMemcpyHostToDevice, h->stream.get()));
         CK(cudaMemcpyAsync(ds, hs, n * sizeof(TatOff), cudaMemcpyHostToDevice, h->stream.get()));
-        if (insert) CK(cudaMemcpyAsync(de, he, n * sizeof(i64), cudaMemcpyHostToDevice, h->stream.get()));
-        const uint32_t grid = (uint32_t)std::min<uint64_t>((n + TILE_THREADS - 1) / TILE_THREADS, 8 * h->sms);
-        (insert ? restore_kernel<true> : restore_kernel<false>)<<<grid, TILE_THREADS, 0, h->stream.get()>>>(
-            t, (const u64 *)dk, (const TatOff *)ds, (const i64 *)de, n, rank, world, b.counts.get());
-        h->launches++;
-        CK(cudaGetLastError());
+        if (pass != PASS_COUNT) CK(cudaMemcpyAsync(de, he, n * sizeof(i64), cudaMemcpyHostToDevice, h->stream.get()));
+        if (pass != PASS_COPY) {
+            const uint32_t grid = (uint32_t)std::min<uint64_t>((n + TILE_THREADS - 1) / TILE_THREADS, 8 * h->sms);
+            (pass == PASS_INSERT ? restore_kernel<true> : restore_kernel<false>)<<<grid, TILE_THREADS, 0, h->stream.get()>>>(
+                t, (const u64 *)dk, (const TatOff *)ds, (const i64 *)de, n, rank, world, b.counts.get());
+            h->launches++;
+            CK(cudaGetLastError());
+        }
         CK(cudaEventRecord(b.done[s].get(), h->stream.get()));
     }
     CK(cudaStreamSynchronize(h->stream.get()));
@@ -1834,12 +1855,8 @@ static int restore_pass(gcra_engine *h, RestoreBuffers &b, const Table &t, const
 static int restore_file(gcra_engine *h, RestoreBuffers &b, uint32_t rank, uint32_t world, uint64_t *restored,
                         uint64_t *conflicts) {
     SnapshotHeader hd{};
-    if (!pread_all(b.fd, &hd, sizeof(hd), 0) || memcmp(hd.magic, SNAP_MAGIC, 8) != 0 || (hd.version != 2 && hd.version != 3)) {
-        h->err = "snapshot restore: bad header";
-        return GCRA_INTERNAL;
-    }
     SnapSections sec;
-    if (const char *why = snapshot_sections(b.fd, hd, sec)) { h->err = std::string("snapshot restore: ") + why; return GCRA_INTERNAL; }
+    if (const char *why = read_header(b.fd, hd, sec)) { h->err = std::string("snapshot restore: ") + why; return GCRA_INTERNAL; }
     CK(cudaDeviceSynchronize());
     RC(refresh_counters(h, true));
     const bool adopt_seed = h->h_counters.get()[C_REAL] == 0;
@@ -1848,15 +1865,14 @@ static int restore_file(gcra_engine *h, RestoreBuffers &b, uint32_t rank, uint32
         return GCRA_INTERNAL;
     }
     RC(make_restore_buffers(h, b));
-    RC(restore_pass(h, b, h->tab, sec, rank, world, false));
+    RC(restore_pass(h, b, h->tab.view, sec, rank, world, PASS_COUNT));
     u64 counts[RESTORE_COUNTS];
     CK(cudaMemcpy(counts, b.counts.get(), sizeof(counts), cudaMemcpyDeviceToHost));
     RC(ensure_room(h, counts[RESTORE_OWNED]));     // may purge or grow: h->tab is read after it
-    RC(restore_pass(h, b, h->tab, sec, rank, world, true));
+    RC(restore_pass(h, b, h->tab.view, sec, rank, world, PASS_INSERT));
     CK(cudaMemcpy(counts, b.counts.get(), sizeof(counts), cudaMemcpyDeviceToHost));
     RC(refresh_counters(h, true));
-    h->occupied_ub = h->h_counters.get()[C_OCCUPIED];
-    for (int i = 0; i < gcra_engine::N_SNAP; i++) h->snap_used[i] = false;
+    reset_occupancy(h, h->h_counters.get()[C_OCCUPIED]);
     if (counts[RESTORE_FAILED]) {
         h->err = "snapshot restore: table full (" + std::to_string(counts[RESTORE_FAILED]) + " entries not inserted)";
         return GCRA_INTERNAL;
@@ -1887,102 +1903,54 @@ int32_t gcra_snapshot_restore(gcra_engine *h, const char *path, uint32_t rank, u
     return rc;
 }
 
-// gcra_snapshot_load of a version 3 file: its entries inserted into a cleared table of the file's geometry, which
-// replaces the engine's table only once every entry is in.  The traffic totals are the file's; len, occupied slots
-// and stash follow the insertion (occupied = len: keys without an entry are not in the file).
-static int load_compact(gcra_engine *h, RestoreBuffers &b, const SnapshotHeader &hd) {
+// gcra_snapshot_load: a new table of the file's geometry is filled -- a version 2 file's sections copied slot for slot,
+// a version 3 file's entries inserted -- and replaces the engine's table only once every entry is in.  The counters
+// are the file's; after a version 3 file len, occupied slots and stash follow the insertion (occupied = len: keys
+// without an entry are not in the file).
+static int load_file(gcra_engine *h, RestoreBuffers &b) {
+    SnapshotHeader hd{};
     SnapSections sec;
-    if (const char *why = snapshot_sections(b.fd, hd, sec)) { h->err = std::string("snapshot: ") + why; return GCRA_INTERNAL; }
-    uint32_t tl, nb, ss;
-    table_geometry(hd.capacity, h->tight, tl, nb, ss);
-    if (tl != hd.total_lines || nb != hd.nb_main || ss != hd.stash_slots) {
+    if (const char *why = read_header(b.fd, hd, sec)) { h->err = std::string("snapshot: ") + why; return GCRA_INTERNAL; }
+    const Geometry g = table_geometry(hd.capacity, h->tight);
+    if (g.total_lines != hd.total_lines || g.nb_main != hd.nb_main || g.stash_slots != hd.stash_slots) {
         h->err = "snapshot: geometry not reproducible with this build/flags";
         return GCRA_INTERNAL;
     }
     RC(make_restore_buffers(h, b));
-    DevBuf<u64> nc;                    // the new table's counters while it is filled
-    CK(nc.make(C_COUNT));
-    CK(cudaMemsetAsync(nc.get(), 0, C_COUNT * sizeof(u64), h->stream.get()));
-    TableArrays na;
-    Table nt{};
-    uint32_t nl = 0;
-    RC(alloc_table(h, hd.capacity, na, nt, nl, nc.get()));
-    RC(restore_pass(h, b, nt, sec, 0, 1, true));
-    u64 counts[RESTORE_COUNTS], fresh[C_COUNT];
-    CK(cudaMemcpy(counts, b.counts.get(), sizeof(counts), cudaMemcpyDeviceToHost));
-    CK(cudaMemcpy(fresh, nc.get(), sizeof(fresh), cudaMemcpyDeviceToHost));
-    if (counts[RESTORE_FAILED] || counts[RESTORE_CONFLICTS]) {
-        h->err = "snapshot: the file's entries do not fit its own geometry (a key twice, or a full table)";
-        return GCRA_INTERNAL;
-    }
+    HostTable t;
+    RC(make_table(h, hd.capacity, t));
     u64 c[C_COUNT];
     memcpy(c, hd.counters, sizeof(c));
-    c[C_OCCUPIED] = fresh[C_OCCUPIED];
-    c[C_REAL] = fresh[C_REAL];
-    c[C_STASH] = fresh[C_STASH];
-    CK(cudaMemcpy(h->tab.counters, c, sizeof(c), cudaMemcpyHostToDevice));
-    nt.counters = h->tab.counters;
-    h->tab_arrays = std::move(na);
-    h->tab = nt; h->total_lines = nl; h->capacity = hd.capacity;
+    if (hd.version == 2) {
+        RC(restore_pass(h, b, t.view, sec, 0, 1, PASS_COPY));
+    } else {
+        RC(restore_pass(h, b, t.view, sec, 0, 1, PASS_INSERT));
+        u64 counts[RESTORE_COUNTS], fresh[C_COUNT];
+        CK(cudaMemcpy(counts, b.counts.get(), sizeof(counts), cudaMemcpyDeviceToHost));
+        CK(cudaMemcpy(fresh, t.counters.get(), sizeof(fresh), cudaMemcpyDeviceToHost));
+        if (counts[RESTORE_FAILED] || counts[RESTORE_CONFLICTS]) {
+            h->err = "snapshot: the file's entries do not fit its own geometry (a key twice, or a full table)";
+            return GCRA_INTERNAL;
+        }
+        take_occupancy(c, fresh);
+    }
+    RC(install_table(h, std::move(t), c));
     h->hash_seed[0] = hd.hash_seed[0];
     h->hash_seed[1] = hd.hash_seed[1];
-    h->occupied_ub = c[C_OCCUPIED];
     h->seen_allowed = c[C_ALLOWED];
     h->seen_expired_hits = c[C_EXPIRED_HITS];
-    for (int i = 0; i < gcra_engine::N_SNAP; i++) h->snap_used[i] = false;
     return GCRA_OK;
 }
 
 int32_t gcra_snapshot_load(gcra_engine *h, const char *path) {
     CK(cudaSetDevice(h->device));
     CK(cudaDeviceSynchronize());
-    FILE *f = fopen(path, "rb");
-    if (!f) { h->err = std::string("snapshot: cannot open ") + path; return GCRA_INTERNAL; }
-    SnapshotHeader hd{};
-    if (fread(&hd, sizeof(hd), 1, f) != 1 || memcmp(hd.magic, SNAP_MAGIC, 8) != 0 || (hd.version != 2 && hd.version != 3)) {
-        fclose(f); h->err = "snapshot: bad header"; return GCRA_INTERNAL;
-    }
-    if (hd.version == 3) {
-        fclose(f);
-        RestoreBuffers b;
-        b.fd = open(path, O_RDONLY);
-        if (b.fd < 0) { h->err = std::string("snapshot: cannot open ") + path; return GCRA_INTERNAL; }
-        const int rc = load_compact(h, b, hd);
-        close_restore(b);
-        return rc;
-    }
-    int rc = GCRA_OK;
-    if (hd.total_lines != h->total_lines || hd.nb_main != h->tab.nb_main || hd.stash_slots != h->tab.stash_slots) {
-        // other geometry: replace the table by one of the snapshot's shape
-        uint32_t tl, nb, ss;
-        table_geometry(hd.capacity, h->tight, tl, nb, ss);
-        if (tl != hd.total_lines || nb != hd.nb_main || ss != hd.stash_slots) {
-            fclose(f); h->err = "snapshot: geometry not reproducible with this build/flags"; return GCRA_INTERNAL;
-        }
-        TableArrays na;
-        Table nt{};
-        uint32_t nl = 0;
-        rc = alloc_table(h, hd.capacity, na, nt, nl, h->tab.counters);
-        if (rc) { fclose(f); return rc; }
-        CK(cudaStreamSynchronize(h->stream.get()));
-        h->tab_arrays = std::move(na);
-        h->tab = nt; h->total_lines = nl; h->capacity = hd.capacity;
-    }
-    std::vector<char> buf(SNAP_CHUNK);
-    const size_t slots = (size_t)h->total_lines * 4;
-    if (!rc) rc = copy_from_file(h, f, h->tab.keys, slots * sizeof(u64), buf);
-    if (!rc) rc = copy_from_file(h, f, h->tab.state, slots * sizeof(TatOff), buf);
-    if (!rc) rc = copy_from_file(h, f, h->tab.ei, slots * sizeof(i64), buf);
-    fclose(f);
-    if (rc) return rc;
-    CK(cudaMemcpy(h->tab.counters, hd.counters, sizeof(hd.counters), cudaMemcpyHostToDevice));
-    h->hash_seed[0] = hd.hash_seed[0];
-    h->hash_seed[1] = hd.hash_seed[1];
-    h->occupied_ub = hd.counters[C_OCCUPIED];
-    h->seen_allowed = hd.counters[C_ALLOWED];
-    h->seen_expired_hits = hd.counters[C_EXPIRED_HITS];
-    for (int i = 0; i < gcra_engine::N_SNAP; i++) h->snap_used[i] = false;
-    return GCRA_OK;
+    RestoreBuffers b;
+    b.fd = open(path, O_RDONLY);
+    if (b.fd < 0) { h->err = std::string("snapshot: cannot open ") + path; return GCRA_INTERNAL; }
+    const int rc = load_file(h, b);
+    close_restore(b);
+    return rc;
 }
 
 // ---- background snapshot: capture on the GPU at the call's place in submission order, write on a thread ----------
@@ -2006,13 +1974,8 @@ static int write_snapshot_file(SnapshotJob *j, SnapshotStaging *sg, int device) 
     if ((e = cudaSetDevice(device)) || (e = cudaEventSynchronize(sg->ev_capture.get()))) return fail("capture");
     const u64 n = sg->meta.get()[C_COUNT];
     if (n > j->cap) return fail("more entries than the staging holds");
-    SnapshotHeader hd{};
-    memcpy(hd.magic, SNAP_MAGIC, 8);
-    hd.version = 3;
-    hd.total_lines = j->total_lines; hd.nb_main = j->nb_main; hd.stash_slots = j->stash_slots;
-    hd.capacity = j->capacity;
+    SnapshotHeader &hd = j->hd;
     memcpy(hd.counters, sg->meta.get(), sizeof(hd.counters));
-    hd.hash_seed[0] = j->hash_seed[0]; hd.hash_seed[1] = j->hash_seed[1];
     if (!pwrite_all(j->fd, &hd, sizeof(hd), 0) || !pwrite_all(j->fd, &n, sizeof(n), sizeof(hd))) return fail("short write");
     struct Piece { const unsigned char *src; size_t bytes; uint64_t off; };
     std::vector<Piece> pieces;
@@ -2076,7 +2039,7 @@ static int snapshot_begin(gcra_engine *h, SnapshotJob &j) {
     SnapshotStaging &sg = *h->snap;
     // an upper bound of the entries at the cut, known without waiting for the device
     tighten_occupied_ub(h);
-    const uint64_t slots = (uint64_t)h->total_lines * 4, tiles = (slots + SNAP_TILE - 1) / SNAP_TILE;
+    const uint64_t slots = h->tab.slots(), tiles = (slots + SNAP_TILE - 1) / SNAP_TILE;
     j.cap = std::min<uint64_t>(h->occupied_ub, slots);
     auto up = [](size_t x) { return (x + 255) / 256 * 256; };
     const size_t ctrl_bytes = (SC_STATUS + tiles) * sizeof(u64);
@@ -2095,9 +2058,7 @@ static int snapshot_begin(gcra_engine *h, SnapshotJob &j) {
         sg.dev = std::move(fresh);
         sg.dev_bytes = bytes;
     }
-    j.total_lines = h->total_lines; j.nb_main = h->tab.nb_main; j.stash_slots = h->tab.stash_slots;
-    j.capacity = h->capacity;
-    j.hash_seed[0] = h->hash_seed[0]; j.hash_seed[1] = h->hash_seed[1];
+    j.hd = header_of(h, 3);
     // the cut: after every batch submitted so far (their last stage records ev_back) and every Store-trait op
     cudaStream_t st = sg.stream.get();
     for (auto &o : h->scr) if (o.back_recorded) CK(cudaStreamWaitEvent(st, o.ev_back.get(), 0));
@@ -2106,11 +2067,11 @@ static int snapshot_begin(gcra_engine *h, SnapshotJob &j) {
     u64 *ctrl = (u64 *)sg.dev.get();
     CK(cudaMemsetAsync(ctrl, 0, ctrl_bytes, st));
     const uint32_t grid = (uint32_t)std::min<uint64_t>(tiles, sg.grid);
-    snapshot_capture_kernel<<<grid, TILE_THREADS, 0, st>>>(h->tab, slots, ctrl, (u64 *)(sg.dev.get() + j.keys_off),
+    snapshot_capture_kernel<<<grid, TILE_THREADS, 0, st>>>(h->tab.view, slots, ctrl, (u64 *)(sg.dev.get() + j.keys_off),
                                                          (TatOff *)(sg.dev.get() + j.state_off), (i64 *)(sg.dev.get() + j.ei_off), j.cap);
     h->launches++;
     CK(cudaGetLastError());
-    CK(cudaMemcpyAsync(sg.meta.get(), h->tab.counters, C_COUNT * sizeof(u64), cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(sg.meta.get(), h->tab.view.counters, C_COUNT * sizeof(u64), cudaMemcpyDeviceToHost, st));
     CK(cudaMemcpyAsync(sg.meta.get() + C_COUNT, ctrl + SC_ENTRIES, sizeof(u64), cudaMemcpyDeviceToHost, st));
     CK(cudaEventRecord(sg.ev_capture.get(), st));
     h->capture_pending = true;
