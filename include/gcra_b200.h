@@ -233,12 +233,23 @@ int32_t gcra_policy_tick(gcra_engine *h, int64_t now_ns, uint64_t *swept);
 uint64_t gcra_len(gcra_engine *h);
 int32_t gcra_get_stats(gcra_engine *h, gcra_stats *out);
 /* metrics bridge (throttlecrab-server/src/metrics.rs:24-64,162-173: top denied keys).  After gcra_track_denied(h,
- * max_keys > 0) a pass over every finished single-GPU batch counts its denied requests per key hash in a device
- * table; gcra_top_denied returns the k most denied (hash, count) pairs, most denied first, and prunes the table to
- * its max_keys top entries once more than 3 x max_keys keys have accumulated (the reference's cleanup rule).  Keys
- * are hashes here -- the caller of the batch entry points owns the strings.  max_keys = 0 switches tracking off.
- * max_keys is at most 2^27 (the table holds 16 entries per key, at most 2^31); a larger value, or a failed
- * allocation, returns GCRA_INTERNAL and leaves the previous setting and its counts as they were. */
+ * max_keys > 0) a pass over every batch the engine finishes counts its denied requests (status GCRA_OK, allowed 0)
+ * per key hash in a device table; gcra_top_denied returns the k most denied (hash, count) pairs, most denied first
+ * (ties: smaller hash first), and prunes the table to its max_keys top entries once more than 3 x max_keys keys have
+ * accumulated (the reference's cleanup rule).  Keys are hashes here -- the caller of the batch entry points owns the
+ * strings.  max_keys = 0 switches tracking off.  max_keys is at most 2^27 (the table holds 16 entries per key, at
+ * most 2^31); a larger value, or a failed allocation, returns GCRA_INTERNAL and leaves the previous setting and its
+ * counts as they were.
+ *   - Multi-GPU: every pipeline counts a denied request on the engine that owns its key (gcra_owner_of): the owner's
+ *     batches of gcra_shard_*, of gcra_p2p_* and of gcra_route_* with the caller's own all-to-all, as well as
+ *     single-GPU batches.  The ranks' lists therefore hold disjoint keys, and the global top k is the top k of the
+ *     ranks' concatenated top-k lists (no count is summed across ranks).  max_keys, the pruning rule and *dropped
+ *     are per rank.
+ *   - While tracking is on, a peer-memory tick counts its rows before it publishes its results, so the count is on
+ *     the tick's path; with tracking off no kernel is launched.
+ *   - gcra_top_denied waits for the engine's submitted batches.  On engines of a multi-GPU pipeline call it between
+ *     ticks, after gcra_p2p_join (or gcra_shard_join) on every rank, like gcra_snapshot_restore: the engine's
+ *     kernels of a tick wait for its peers' rows. */
 int32_t gcra_track_denied(gcra_engine *h, uint32_t max_keys);
 int32_t gcra_top_denied(gcra_engine *h, uint32_t k, uint64_t *key_hashes, uint64_t *counts, uint32_t *n_out,
                         uint64_t *dropped);

@@ -308,6 +308,7 @@ struct gcra_engine {
     int prefetch_state = 0;
     uint32_t max_tiles = 0;
     uint32_t grid_probe[FMT_COUNT] = {}, grid_decide[FMT_COUNT] = {};   // resident CTAs of the persistent kernels [RowFmt]
+    uint32_t grid_denied_seg = 0;    // resident CTAs of denied_count_seg_kernel
     uint32_t dbg = 0;                // timing experiments only (gcra_debug_set): skips parts of pass B
     uint32_t last_nres = 0, last_nres_rows = 0;   // newest residue size that has reached the host (and its batch's rows)
     bool adaptive = true;            // choose the pipeline from the residue feedback (off when a test / env forces one)
@@ -754,11 +755,20 @@ static int alloc_index_scratch(gcra_engine *h, uint32_t rows) {
     return GCRA_OK;
 }
 
-// metrics bridge: count this batch's denied rows per key (single-segment batches: request and result rows local)
+// metrics bridge: count this batch's denied rows per key.  A single-segment batch has its request and result rows
+// here and a host-known row count; a segmented one (the peer-memory tick, 48-byte requests and 32-byte results only)
+// has its results in the senders' outboxes and its row counts on the device: a persistent grid over the real tiles.
 static int enqueue_denied(gcra_engine *h, const BatchView &v, int fmt, cudaStream_t st) {
-    if (!h->denied_max || v.nseg != 1 || v.n == 0) return GCRA_OK;
-    const uint32_t tiles = (v.n + TILE_THREADS - 1) / TILE_THREADS;
-    with_fmt(fmt, [&](auto F) { denied_count_kernel<F><<<tiles, TILE_THREADS, 0, st>>>(v.req0, v.res0, v.n, h->denied); });
+    if (!h->denied_max) return GCRA_OK;
+    if (v.nseg != 1) {
+        if (fmt != FMT_48_32) { h->err = "a segmented batch counts denied rows of 48-byte requests only"; return GCRA_INTERNAL; }
+        const uint32_t tiles = (uint32_t)((((uint64_t)v.nseg << v.cap_shift) + TILE_THREADS - 1) / TILE_THREADS);
+        denied_count_seg_kernel<<<std::min(tiles, h->grid_denied_seg), TILE_THREADS, 0, st>>>(v, h->denied);
+    } else {
+        if (v.n == 0) return GCRA_OK;
+        const uint32_t tiles = (v.n + TILE_THREADS - 1) / TILE_THREADS;
+        with_fmt(fmt, [&](auto F) { denied_count_kernel<F><<<tiles, TILE_THREADS, 0, st>>>(v.req0, v.res0, v.n, h->denied); });
+    }
     h->launches++;
     CK(cudaGetLastError());
     return GCRA_OK;
@@ -1012,6 +1022,8 @@ static int launch_pipelined_view(gcra_engine *h, const BatchView &v, uint32_t n_
         cudaStream_t ts = h->tail_stream.get();
         CK(cudaStreamWaitEvent(ts, sc.ev_mid.get(), 0));
         RC(enqueue_tail_index(h, sc, v, fmt, now_batch, ts, false));
+        // before ev_back: a peer-memory tick publishes its results after ev_back (gcra_p2p_submit_finish), and from
+        // then on a sender may reuse the inbox and outbox rows this count reads
         RC(enqueue_denied(h, v, fmt, ts));
         CK(cudaEventRecord(sc.ev_back.get(), ts));
         sc.back_recorded = true;
@@ -1061,7 +1073,7 @@ static void preload_kernels() {
     preload(route_count_kernel); preload(route_scan_kernel); preload(route_scatter_kernel); preload(route_unpermute_kernel);
     preload(p2p_scan_kernel); preload(p2p_scatter_kernel); preload(p2p_signal_req_kernel); preload(p2p_signal_res_kernel);
     preload(p2p_wait_kernel); preload(p2p_unpermute_kernel);
-    preload(snapshot_capture_kernel);
+    preload(snapshot_capture_kernel); preload(denied_count_seg_kernel);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -1132,6 +1144,11 @@ static int init_engine(gcra_engine *h, const gcra_config *cfg) {
                 if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, probe_kernel<F>, TILE_THREADS, 0) == cudaSuccess && nb > 0) h->grid_probe[fmt] = (uint32_t)(nb * sms);
                 if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, decide_index_kernel<F>, TILE_THREADS, 0) == cudaSuccess && nb > 0) h->grid_decide[fmt] = (uint32_t)(nb * sms);
             });
+        }
+        h->grid_denied_seg = 4 * h->sms;
+        {
+            int nb = 0;
+            if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&nb, denied_count_seg_kernel, TILE_THREADS, 0) == cudaSuccess && nb > 0) h->grid_denied_seg = (uint32_t)(nb * sms);
         }
         // tuning: CTAs per SM of the persistent kernels (fewer leave room for the other stages' kernels)
         if (const char *g = getenv("GCRA_CTAS_PROBE")) { uint32_t c = (uint32_t)atoi(g) * sms; if (c) for (auto &x : h->grid_probe) x = std::min(x, c); }
@@ -1639,7 +1656,8 @@ int32_t gcra_track_denied(gcra_engine *h, uint32_t max_keys) {
 
 // the k most denied keys (hash, count), most denied first; *dropped = denials of keys that found the table full.
 // Like the reference's cleanup (metrics.rs:52-64) the table is pruned to its `max_keys` top entries when more than
-// three times as many have accumulated.
+// three times as many have accumulated.  Waits for every scratch set's ev_back, which a peer-memory tick records
+// after its count and before it publishes its results: multi-GPU callers query between ticks, after joining them.
 int32_t gcra_top_denied(gcra_engine *h, uint32_t k, uint64_t *key_hashes, uint64_t *counts, uint32_t *n_out, uint64_t *dropped) {
     CK(cudaSetDevice(h->device));
     if (n_out) *n_out = 0;

@@ -1585,6 +1585,35 @@ struct DeniedTable {
 };
 constexpr u32 DENIED_HASH = 512;
 
+// one denied row of key `k` into the tile's shared-memory hash set
+__device__ __forceinline__ void denied_tile_add(u64 *hkey, u32 *hcnt, u64 k) {
+    if (k == 0) k = 1;                                                              // 0 marks an empty entry
+    u32 h = (u32)(mix64(k) >> 55);                                                  // 9 bits
+    for (;;) {
+        const u64 old = atomicCAS(&hkey[h], 0ULL, k);
+        if (old == 0 || old == k) { atomicAdd(&hcnt[h], 1u); break; }
+        h = (h + 1) & (DENIED_HASH - 1);
+    }
+}
+
+// the tile's distinct keys into the table (after a __syncthreads that follows the tile's adds)
+__device__ __forceinline__ void denied_tile_flush(const u64 *hkey, const u32 *hcnt, const DeniedTable &t) {
+    for (u32 e = threadIdx.x; e < DENIED_HASH; e += TILE_THREADS) {
+        const u64 k = hkey[e];
+        if (k == 0) continue;
+        u32 h = (u32)(mix64(k ^ 0x9E3779B97F4A7C15ULL)) & t.mask;
+        bool done = false;
+        for (u32 probe = 0; probe < 64 && !done; probe++) {
+            u64 cur = t.keys[h];                                    // (a stale L1 line shows "empty": then the CAS decides)
+            if (cur == 0) { const u64 old = atomicCAS(&t.keys[h], 0ULL, k); cur = old == 0 ? k : old; }
+            if (cur == k) { atomicAdd(&t.counts[h], (u64)hcnt[e]); done = true; }
+            else h = (h + 1) & t.mask;
+        }
+        if (!done) atomicAdd(t.dropped, (u64)hcnt[e]);
+    }
+}
+
+// single-segment batch: one CTA per 256-row tile
 template <int FMT>
 __global__ void __launch_bounds__(TILE_THREADS)
 denied_count_kernel(const unsigned char *__restrict__ req, const gcra_result *__restrict__ res, u32 n, DeniedTable t) {
@@ -1598,30 +1627,45 @@ denied_count_kernel(const unsigned char *__restrict__ req, const gcra_result *__
         const longlong2 tail = Rows<FMT>::R16 ? reinterpret_cast<const longlong2 *>(res)[i]
                                               : reinterpret_cast<const longlong2 *>(res + i)[1];
         const bool denied = (u32)tail.y == GCRA_OK && ((tail.y >> 32) & 0xff) == 0;
-        if (denied) {
-            u64 k = *reinterpret_cast<const u64 *>(req + (size_t)i * Rows<FMT>::REQ_BYTES);
-            if (k == 0) k = 1;                                                          // 0 marks an empty entry
-            u32 h = (u32)(mix64(k) >> 55);                                              // 9 bits
-            for (;;) {
-                const u64 old = atomicCAS(&hkey[h], 0ULL, k);
-                if (old == 0 || old == k) { atomicAdd(&hcnt[h], 1u); break; }
-                h = (h + 1) & (DENIED_HASH - 1);
-            }
-        }
+        if (denied) denied_tile_add(hkey, hcnt, *reinterpret_cast<const u64 *>(req + (size_t)i * Rows<FMT>::REQ_BYTES));
     }
     __syncthreads();
-    for (u32 e = threadIdx.x; e < DENIED_HASH; e += TILE_THREADS) {
-        const u64 k = hkey[e];
-        if (k == 0) continue;
-        u32 h = (u32)(mix64(k ^ 0x9E3779B97F4A7C15ULL)) & t.mask;
-        bool done = false;
-        for (u32 probe = 0; probe < 64 && !done; probe++) {
-            u64 cur = t.keys[h];                                    // (a stale L1 line shows "empty": then the CAS decides)
-            if (cur == 0) { const u64 old = atomicCAS(&t.keys[h], 0ULL, k); cur = old == 0 ? k : old; }
-            if (cur == k) { atomicAdd(&t.counts[h], (u64)hcnt[e]); done = true; }
-            else h = (h + 1) & t.mask;
+    denied_tile_flush(hkey, hcnt, t);
+}
+
+// Segmented batch (the peer-memory tick: 48-byte requests in this GPU's inbox, 32-byte results in the senders'
+// outboxes, one segment per sender).  The segments' row counts exist only on the device, and the row-id space
+// (nseg << cap_shift) is mostly empty, so a persistent grid turns a dense tile index into (segment, tile) with a
+// prefix over the counts and takes tiles until the real rows run out.  Per tile: as denied_count_kernel.
+__global__ void __launch_bounds__(TILE_THREADS)
+denied_count_seg_kernel(BatchView v, DeniedTable t) {
+    __shared__ u64 hkey[DENIED_HASH];
+    __shared__ u32 hcnt[DENIED_HASH];
+    __shared__ u32 s_cnt[MAX_SEGS], s_tile0[MAX_SEGS + 1];     // rows of segment s, its first dense tile
+    if (threadIdx.x < MAX_SEGS) s_cnt[threadIdx.x] = threadIdx.x < v.nseg ? min(v.dev_counts[threadIdx.x], 1u << v.cap_shift) : 0;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        u32 acc = 0;
+        for (u32 s = 0; s < MAX_SEGS; s++) { s_tile0[s] = acc; acc += (s_cnt[s] + TILE_THREADS - 1) / TILE_THREADS; }
+        s_tile0[MAX_SEGS] = acc;
+    }
+    __syncthreads();
+    const u32 n_tiles = s_tile0[MAX_SEGS];
+    for (u32 tile = blockIdx.x; tile < n_tiles; tile += gridDim.x) {
+        for (u32 i = threadIdx.x; i < DENIED_HASH; i += TILE_THREADS) { hkey[i] = 0; hcnt[i] = 0; }
+        u32 s = 0;
+        while (tile >= s_tile0[s + 1]) s++;                     // (uniform over the CTA: s < nseg)
+        const u32 j = (tile - s_tile0[s]) * TILE_THREADS + threadIdx.x;
+        __syncthreads();
+        if (j < s_cnt[s]) {
+            const u32 row = (s << v.cap_shift) | j;
+            const longlong2 tail = reinterpret_cast<const longlong2 *>(v.res_at(row))[1];      // as above, 32-byte rows
+            const bool denied = (u32)tail.y == GCRA_OK && ((tail.y >> 32) & 0xff) == 0;
+            if (denied) denied_tile_add(hkey, hcnt, *reinterpret_cast<const u64 *>(v.req_at(row, sizeof(gcra_request))));
         }
-        if (!done) atomicAdd(t.dropped, (u64)hcnt[e]);
+        __syncthreads();
+        denied_tile_flush(hkey, hcnt, t);
+        __syncthreads();                                        // (the hash set is cleared for the next tile)
     }
 }
 

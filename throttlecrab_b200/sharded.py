@@ -22,6 +22,7 @@ torch is plumbing only: device buffers, the NCCL process group and stream/event 
 """
 import os
 
+import numpy as np
 import torch
 
 REQ_B, RES_B = 48, 32
@@ -63,6 +64,50 @@ class _Snapshots:
         return restored, conflicts
 
 
+def merge_top_denied(lists, k):
+    """The global top k of the ranks' top-denied lists ([(key_hash, count)] each, as RateLimiter.store.top_denied
+    returns them).  Every pipeline counts a denied request on the engine that owns its key, so the lists hold
+    disjoint keys and the global top k is the top k of their concatenation; the order is gcra_top_denied's: count
+    descending, then hash ascending.  A key in more than one list means the lists are not of one sharded key space."""
+    merged = [(int(h), int(c)) for lst in lists for h, c in lst]
+    if len({h for h, _ in merged}) != len(merged):
+        raise ValueError("merge_top_denied: a key appears in more than one list")
+    merged.sort(key=lambda hc: (-hc[1], hc[0]))
+    return merged[:k]
+
+
+class _DeniedKeys:
+    """Top denied keys of a sharded key space (gcra_track_denied / gcra_top_denied on every rank's engine)."""
+
+    def track_denied(self, max_keys):
+        """Count denied requests per key on this rank's engine (0 = off); max_keys is per rank.  Call it between
+        ticks: only later ticks are counted."""
+        self.finish()
+        self.lim.store.track_denied(max_keys)
+
+    def top_denied(self, k):
+        """Collective: every rank calls it between ticks, after the same tick.  Waits for every tick submitted here,
+        all-gathers each rank's top k and its dropped count, and returns on every rank the global top k
+        (merge_top_denied) and the sum of the ranks' dropped counts.  Each rank's own query prunes its table by the
+        per-rank rule of gcra_top_denied."""
+        self.finish()
+        mine, dropped = self.lim.store.top_denied(k)
+        buf = np.zeros((k + 1, 2), np.uint64)
+        buf[0] = (len(mine), dropped)
+        if mine:
+            buf[1:len(mine) + 1] = np.array(mine, np.uint64)
+        t = torch.from_numpy(buf.view(np.int64)).to(self.dev)
+        every = [torch.empty_like(t) for _ in range(self.world)]
+        self.dist.all_gather(every, t)
+        lists, total = [], 0
+        for e in every:
+            a = e.cpu().numpy().view(np.uint64)
+            n = int(a[0, 0])
+            total += int(a[0, 1])
+            lists.append([(int(h), int(c)) for h, c in a[1:n + 1]])
+        return merge_top_denied(lists, k), total
+
+
 class CudaOps:
     """The three device steps, all through the C ABI."""
 
@@ -102,7 +147,7 @@ class _Slot:
         self.done_ev = None        # results un-permuted into the caller's buffer
 
 
-class ShardedLimiter(_Snapshots):
+class ShardedLimiter(_Snapshots, _DeniedKeys):
     def __init__(self, limiter, dist, device, ops=None, max_rows=None):
         self.lim, self.dist, self.dev = limiter, dist, device
         self.world, self.rank = dist.get_world_size(), dist.get_rank()
@@ -231,7 +276,7 @@ class ShardedLimiter(_Snapshots):
         return n_recv
 
 
-class NativeShardedLimiter(_Snapshots):
+class NativeShardedLimiter(_Snapshots, _DeniedKeys):
     """The same pipeline driven by ONE C call per tick (gcra_shard_submit): partition, NCCL count exchange and
     all-to-alls (libnccl resolved with dlopen inside the library), the engine's pipelined kernels and the way
     back all live in libgcra_b200.so.  torch.distributed is used once, to hand the three ncclUniqueIds that
@@ -276,7 +321,7 @@ class NativeShardedLimiter(_Snapshots):
         return "native NCCL pipeline (gcra_shard_submit: partition, count exchange, all-to-all, decide, all-to-all)"
 
 
-class PeerShardedLimiter(_Snapshots):
+class PeerShardedLimiter(_Snapshots, _DeniedKeys):
     """The sharded tick over NVLink peer memory (gcra_p2p_*, csrc/gcra_p2p.cuh): the partition kernel stores every
     request row straight into its owner's inbox, the owner's engine runs over the inbox as one batch of `world`
     segments and stores every result straight into the sender's outbox; ranks synchronise with tick numbers in peer
