@@ -342,6 +342,17 @@ static int after_capture(gcra_engine *h, cudaStream_t st) {
     return GCRA_OK;
 }
 
+// Whatever touches the table outside a batch comes after every batch in flight, whichever streams it was submitted
+// on (the last stage of each records its scratch set's ev_back, finish_batch): on `st`, or on the host.
+static int order_after_batches(gcra_engine *h, cudaStream_t st) {
+    for (auto &o : h->scr) if (o.back_recorded) CK(cudaStreamWaitEvent(st, o.ev_back.get(), 0));
+    return GCRA_OK;
+}
+static int wait_for_batches(gcra_engine *h) {
+    for (auto &o : h->scr) if (o.back_recorded) CK(cudaEventSynchronize(o.ev_back.get()));
+    return GCRA_OK;
+}
+
 static uint32_t ceil_log2(uint64_t x) {
     uint32_t b = 0;
     while ((1ULL << b) < x) b++;
@@ -885,16 +896,51 @@ static int enqueue_tail_index(gcra_engine *h, Scratch &sc, const BatchView &v, i
     return GCRA_OK;
 }
 
-// Stage 2 of a sort-pipeline batch: the compare-and-update kernels over the sorted keys
-static int enqueue_back_sorted(gcra_engine *h, Scratch &sc, const BatchView &v, int fmt, const u64 *sorted, cudaStream_t st,
-                               bool timed) {
-    OutMap om{};
-    om.out = v.res0;
-    om.by_row = 0;
-    RC(enqueue_decide_sorted(h, sc, v.n, nullptr, sorted, om, fmt, st));
-    if (timed) { CK(cudaEventRecord(h->ev[3].get(), st)); h->ev_valid = true; }
-    CK(cudaGetLastError());
-    return GCRA_OK;
+struct Lanes { cudaStream_t front, mid, tail; };   // a batch's stages run on the engine's three streams (pipelined) or all on the caller's (serial)
+struct BatchPlan { bool index_path, overlap; };    // which pipeline; may stage 2 (index-order) overlap the previous batch's tail
+
+// The end of every batch, on the stream of its last stage, in this order.  The denied count comes before ev_back: a
+// peer-memory tick publishes its results after ev_back (gcra_p2p_submit_finish), and from then on a sender may reuse
+// the inbox and outbox rows the count reads.  Everything that follows the batch waits for ev_back (`*done`, the
+// set's next use, order_after_batches), so only the copy of the occupancy counters is enqueued behind it.
+static int finish_batch(gcra_engine *h, Scratch &sc, const BatchView &v, uint32_t n_rows, int fmt, cudaStream_t st, cudaEvent_t *done) {
+    RC(enqueue_denied(h, v, fmt, st));
+    CK(cudaEventRecord(sc.ev_back.get(), st));
+    sc.back_recorded = true;
+    if (done) *done = sc.ev_back.get();
+    return snapshot_async(h, n_rows, st);
+}
+
+// The stages of one batch (any but a small serial batch) in scratch set `k`, each on its lane, then the end of the
+// batch on the last one.  Two lanes that are the same stream hand over without an event.  Knows nothing of earlier
+// batches: the caller has already enqueued, on the lanes, what this one has to wait for.
+static int enqueue_stages(gcra_engine *h, uint32_t k, const BatchView &v, uint32_t n_rows, int fmt, int64_t now_batch,
+                          BatchPlan plan, Lanes on, bool timed, cudaEvent_t *done) {
+    Scratch &sc = h->scr[k];
+    const uint32_t kn = (k + 1) % gcra_engine::N_SCR;         // the set the next batch takes
+    u64 *sorted = nullptr;
+    RC(enqueue_front(h, sc, v, plan.index_path, fmt, now_batch, on.front, timed, &sorted));
+    if (on.mid != on.front) {
+        CK(cudaEventRecord(sc.ev_front.get(), on.front));
+        CK(cudaStreamWaitEvent(on.mid, sc.ev_front.get(), 0));
+    }
+    if (plan.index_path) {
+        RC(enqueue_mid_index(h, sc, h->scr[kn], v, fmt, now_batch, plan.overlap, on.mid, timed));
+        CK(cudaEventRecord(sc.ev_mid.get(), on.mid));         // on one lane as well: the residue feedback reads it
+        sc.mid_recorded = true;
+        if (on.tail != on.mid) CK(cudaStreamWaitEvent(on.tail, sc.ev_mid.get(), 0));
+        RC(enqueue_tail_index(h, sc, v, fmt, now_batch, on.tail, timed));
+    } else {
+        // stage 2 of a sort-pipeline batch: the compare-and-update kernels over the sorted keys
+        OutMap om{};                                          // (by_row = 0: a sorted key's payload is its batch index)
+        om.out = v.res0;
+        RC(enqueue_decide_sorted(h, sc, v.n, nullptr, sorted, om, fmt, on.mid));
+        if (timed) { CK(cudaEventRecord(h->ev[3].get(), on.mid)); h->ev_valid = true; }
+        CK(cudaGetLastError());
+        sc.mid_recorded = false;                              // (no residue count from this batch)
+    }
+    h->pend_set = plan.index_path ? (int)kn : -1;             // pass C left this batch's PEND bits in the next set
+    return finish_batch(h, sc, v, n_rows, fmt, plan.index_path ? on.tail : on.mid, done);
 }
 
 static int check_batch(gcra_engine *h, uint32_t n, int fmt) {
@@ -910,17 +956,16 @@ static int launch_batch(gcra_engine *h, uint32_t n, const void *d_req, int fmt, 
     RC(check_batch(h, n, fmt));
     gcra_result *d_res = (gcra_result *)d_res_rows;     // (or gcra_result16 rows: see BatchView::res16_at)
     const uint32_t k = h->scr_next;
-    Scratch &sc = h->scr[k];
     h->scr_next = (h->scr_next + 1) % gcra_engine::N_SCR;
-    Scratch &next = h->scr[h->scr_next];
-    // order after every earlier batch (they may have been submitted pipelined on the engine's streams),
-    // which also frees this scratch set
-    for (auto &o : h->scr) if (o.back_recorded) CK(cudaStreamWaitEvent(st, o.ev_back.get(), 0));
+    const BatchView v = single_view(d_req, d_res, n);
+    // after every earlier batch (some may be in flight on the engine's streams), which also frees this scratch set
+    RC(order_after_batches(h, st));
     RC(after_capture(h, st));
     static const bool no_small = getenv("GCRA_NO_SMALL") && atoi(getenv("GCRA_NO_SMALL"));   // A/B switch for tools/latency_probe.py
     if (n <= SMALL_MAX && !no_small) {
         // small batch (a single rate_limit call, a lightly loaded actor): one CTA does ingest, ordering and
         // the compare-and-update in a single launch
+        Scratch &sc = h->scr[k];
         if (timed) { CK(cudaEventRecord(h->ev[0].get(), st)); CK(cudaEventRecord(h->ev[1].get(), st)); CK(cudaEventRecord(h->ev[2].get(), st)); }
         with_fmt(fmt, [&](auto F) {
             small_batch_kernel<F><<<1, TILE_THREADS, 0, st>>>(h->tab.view, d_req, h->d_pol.get(), h->npol, now_batch, n, sc.drec.get(), d_res);
@@ -928,49 +973,16 @@ static int launch_batch(gcra_engine *h, uint32_t n, const void *d_req, int fmt, 
         h->launches++;
         if (timed) { CK(cudaEventRecord(h->ev[3].get(), st)); h->ev_valid = true; }
         CK(cudaGetLastError());
-    } else {
-        u64 *sorted = nullptr;
-        const BatchView v = single_view(d_req, d_res, n);
-        const bool ip = use_index_path(h, n);
-        RC(enqueue_front(h, sc, v, ip, fmt, now_batch, st, timed, &sorted));
-        if (ip) {
-            RC(enqueue_mid_index(h, sc, next, v, fmt, now_batch, false, st, timed));
-            CK(cudaEventRecord(sc.ev_mid.get(), st));
-            sc.mid_recorded = true;
-            RC(enqueue_tail_index(h, sc, v, fmt, now_batch, st, timed));
-        } else {
-            RC(enqueue_back_sorted(h, sc, v, fmt, sorted, st, timed));
-            sc.mid_recorded = false;
-        }
-    }
-    RC(enqueue_denied(h, single_view(d_req, d_res, n), fmt, st));
-    CK(cudaEventRecord(sc.ev_back.get(), st));
-    sc.back_recorded = true;
+        RC(finish_batch(h, sc, v, n, fmt, st, nullptr));
+    } else RC(enqueue_stages(h, k, v, n, fmt, now_batch, {use_index_path(h, n), false}, {st, st, st}, timed, nullptr));
     h->pend_set = -1;          // everything of this batch is ordered on `st`: the next batch waits for all of it
-    return snapshot_async(h, n, st);
+    return GCRA_OK;
 }
 
 // ---- one batch, pipelined over the engine's streams --------------------------------------------------
-// index-order pipeline: stage 1 (probe) of batch j+1 overlaps stage 2 (decide, resolve) of batch j and stage 3
-// (the sorted residue) of batch j-1.  Stage 2 of batch j may run while the tail of batch j-1 is still at work
-// because pass C of batch j-1 left PEND bits for exactly the keys that tail owns.  Sort pipeline: stage 1 =
-// ingest + sort, stage 2 = decide, after every earlier batch has completely finished.
-// `ready` (may be null) is an event after which the requests may be read; `*done` is set to an event after which
-// the results are complete.
-static int launch_pipelined_view(gcra_engine *h, const BatchView &v, uint32_t n_rows, int fmt, int64_t now_batch,
-                                 cudaEvent_t ready, cudaEvent_t *done) {
-    // 16-byte results are a single-GPU format: the multi-GPU ticks return 32-byte rows into peers' outboxes
-    if (res_bytes(fmt) == sizeof(gcra_result16) && v.nseg != 1) { h->err = "16-byte results need a single-segment batch"; return GCRA_INTERNAL; }
-    RC(check_batch(h, n_rows, fmt));
-    const uint32_t k = h->scr_next;
-    Scratch &sc = h->scr[k];
-    h->scr_next = (h->scr_next + 1) % gcra_engine::N_SCR;
-    const uint32_t kn = h->scr_next;
-    cudaStream_t fs = h->front_stream.get();                  // (all sets share one front stream, see gcra_create)
-    if (ready) CK(cudaStreamWaitEvent(fs, ready, 0));
-    if (sc.back_recorded) CK(cudaStreamWaitEvent(fs, sc.ev_back.get(), 0));   // scratch set free again
-    RC(after_capture(h, fs));                                 // (the later stages follow this batch's front)
-    u64 *sorted = nullptr;
+// How the next pipelined batch, in scratch set `k`, runs.  A host state machine over the residue counts that earlier
+// batches' pass C reported: it queries events and enqueues nothing.
+static BatchPlan plan_pipelined(gcra_engine *h, uint32_t k, const BatchView &v, uint32_t n_rows) {
     // residue feedback: the newest pass-C count that has reached the host
     bool residue_large = false;
     for (int back = 1; back < gcra_engine::N_SCR; back++) {
@@ -993,10 +1005,6 @@ static int launch_pipelined_view(gcra_engine *h, const BatchView &v, uint32_t n_
             h->sort_hold = 31; h->last_nres = 0; h->last_nres_rows = 0; ip = false; h->n_path_switches++;
         }
     }
-    RC(enqueue_front(h, sc, v, ip, fmt, now_batch, fs, false, &sorted));
-    CK(cudaEventRecord(sc.ev_front.get(), fs));
-    cudaStream_t ms = h->back_stream.get();
-    CK(cudaStreamWaitEvent(ms, sc.ev_front.get(), 0));
     // May stage 2 of this batch overlap the tail of the batch submitted just before?  Only if that batch left its
     // PEND bits in this set's pend bitmap.  Keys the tail owns stay deferred for as long as they keep appearing
     // (their requests go from tail to tail), so the overlap is given up -- stage 2 waits for every tail and ignores
@@ -1008,37 +1016,34 @@ static int launch_pipelined_view(gcra_engine *h, const BatchView &v, uint32_t n_
         if (h->since_drain >= 64) overlap = false;
         if (!overlap) { if (h->pend_set == (int)k) h->n_drains++; h->since_drain = 0; } else h->since_drain++;
     }
-    for (int o = 0; o < gcra_engine::N_SCR; o++) {
-        Scratch &os = h->scr[o];
-        if (o == (int)k || !os.back_recorded) continue;
-        const bool is_prev = o == (int)((k + gcra_engine::N_SCR - 1) % gcra_engine::N_SCR);
-        if (overlap && is_prev) continue;
-        CK(cudaStreamWaitEvent(ms, os.ev_back.get(), 0));
+    return {ip, overlap};
+}
+
+// index-order pipeline: stage 1 (probe) of batch j+1 overlaps stage 2 (decide, resolve) of batch j and stage 3
+// (the sorted residue) of batch j-1.  Stage 2 of batch j may run while the tail of batch j-1 is still at work
+// because pass C of batch j-1 left PEND bits for exactly the keys that tail owns.  Sort pipeline: stage 1 =
+// ingest + sort, stage 2 = decide, after every earlier batch has completely finished.
+// `ready` (may be null) is an event after which the requests may be read; `*done` is set to an event after which
+// the results are complete.
+static int launch_pipelined_view(gcra_engine *h, const BatchView &v, uint32_t n_rows, int fmt, int64_t now_batch,
+                                 cudaEvent_t ready, cudaEvent_t *done) {
+    // 16-byte results are a single-GPU format: the multi-GPU ticks return 32-byte rows into peers' outboxes
+    if (res_bytes(fmt) == sizeof(gcra_result16) && v.nseg != 1) { h->err = "16-byte results need a single-segment batch"; return GCRA_INTERNAL; }
+    RC(check_batch(h, n_rows, fmt));
+    const uint32_t k = h->scr_next;
+    h->scr_next = (h->scr_next + 1) % gcra_engine::N_SCR;
+    const Lanes on = {h->front_stream.get(), h->back_stream.get(), h->tail_stream.get()};   // (all sets share one front stream, see gcra_create)
+    if (ready) CK(cudaStreamWaitEvent(on.front, ready, 0));
+    if (h->scr[k].back_recorded) CK(cudaStreamWaitEvent(on.front, h->scr[k].ev_back.get(), 0));   // scratch set free again
+    RC(after_capture(h, on.front));                           // (the later stages follow this batch's front)
+    const BatchPlan plan = plan_pipelined(h, k, v, n_rows);
+    // stage 2 follows every earlier batch whole, but for the tail of the batch just before when it may overlap it
+    const uint32_t prev = (k + gcra_engine::N_SCR - 1) % gcra_engine::N_SCR;
+    for (uint32_t o = 0; o < gcra_engine::N_SCR; o++) {
+        if (o == k || (o == prev && plan.overlap) || !h->scr[o].back_recorded) continue;
+        CK(cudaStreamWaitEvent(on.mid, h->scr[o].ev_back.get(), 0));
     }
-    if (ip) {
-        RC(enqueue_mid_index(h, sc, h->scr[kn], v, fmt, now_batch, overlap, ms, false));
-        CK(cudaEventRecord(sc.ev_mid.get(), ms));
-        sc.mid_recorded = true;
-        cudaStream_t ts = h->tail_stream.get();
-        CK(cudaStreamWaitEvent(ts, sc.ev_mid.get(), 0));
-        RC(enqueue_tail_index(h, sc, v, fmt, now_batch, ts, false));
-        // before ev_back: a peer-memory tick publishes its results after ev_back (gcra_p2p_submit_finish), and from
-        // then on a sender may reuse the inbox and outbox rows this count reads
-        RC(enqueue_denied(h, v, fmt, ts));
-        CK(cudaEventRecord(sc.ev_back.get(), ts));
-        sc.back_recorded = true;
-        h->pend_set = (int)kn;
-        if (done) *done = sc.ev_back.get();
-        return snapshot_async(h, n_rows, ts);
-    }
-    RC(enqueue_back_sorted(h, sc, v, fmt, sorted, ms, false));
-    RC(enqueue_denied(h, v, fmt, ms));
-    sc.mid_recorded = false;   // (no residue count from this batch)
-    CK(cudaEventRecord(sc.ev_back.get(), ms));
-    sc.back_recorded = true;
-    h->pend_set = -1;
-    if (done) *done = sc.ev_back.get();
-    return snapshot_async(h, n_rows, ms);
+    return enqueue_stages(h, k, v, n_rows, fmt, now_batch, plan, on, false, done);
 }
 
 static int launch_pipelined(gcra_engine *h, uint32_t n, const void *d_req, int fmt, int64_t now_batch,
@@ -1306,9 +1311,8 @@ static int store_op(gcra_engine *h, int op, uint64_t key_hash, int64_t a, int64_
     // the table encodes 'no state' as a negative expiry (has_state): times before the epoch are outside its domain
     if (op != 3 && now < 0) { h->err = "pre-epoch time is not supported"; return GCRA_INTERNAL; }
     if (op == 2) { int rc = ensure_room(h, 1); if (rc) return rc; }
-    // a Store-trait call reads / writes a slot's state: after every batch still in flight on the engine's or a
-    // caller's stream (launch_batch orders itself the same way)
-    for (auto &o : h->scr) if (o.back_recorded) CK(cudaStreamWaitEvent(h->stream.get(), o.ev_back.get(), 0));
+    // a Store-trait call reads / writes a slot's state
+    RC(order_after_batches(h, h->stream.get()));
     RC(after_capture(h, h->stream.get()));
     store_op_kernel<<<1, 1, 0, h->stream.get()>>>(h->tab.view, op, stored_key(key_hash), a, b, ttl, now, h->d_op.get());
     h->launches++;
@@ -1385,12 +1389,7 @@ int32_t gcra_rate_limit_batch_device_pipelined(gcra_engine *h, uint64_t n, const
 
 int32_t gcra_pipeline_join(gcra_engine *h, void *stream) {
     CK(cudaSetDevice(h->device));
-    for (auto &o : h->scr) {
-        if (!o.back_recorded) continue;
-        if (stream) CK(cudaStreamWaitEvent((cudaStream_t)stream, o.ev_back.get(), 0));
-        else CK(cudaEventSynchronize(o.ev_back.get()));
-    }
-    return GCRA_OK;
+    return stream ? order_after_batches(h, (cudaStream_t)stream) : wait_for_batches(h);
 }
 
 static int host_batch(gcra_engine *h, uint64_t n, const void *req, int fmt, int64_t now_batch, void *res) {
@@ -1584,7 +1583,7 @@ int32_t gcra_policy_tick(gcra_engine *h, int64_t now_ns, uint64_t *swept) {
     CK(cudaSetDevice(h->device));
     if (swept) *swept = 0;
     if (h->kind == GCRA_STORE_MANUAL) return GCRA_OK;
-    for (auto &o : h->scr) if (o.back_recorded) CK(cudaEventSynchronize(o.ev_back.get()));
+    RC(wait_for_batches(h));
     RC(refresh_counters(h, true));
     const uint64_t before = h->h_counters.get()[C_SWEPT];
     RC(apply_policy(h, now_ns));
@@ -1662,7 +1661,7 @@ int32_t gcra_top_denied(gcra_engine *h, uint32_t k, uint64_t *key_hashes, uint64
     CK(cudaSetDevice(h->device));
     if (n_out) *n_out = 0;
     if (!h->denied_max) { h->err = "gcra_track_denied first"; return GCRA_INTERNAL; }
-    for (auto &o : h->scr) if (o.back_recorded) CK(cudaEventSynchronize(o.ev_back.get()));
+    RC(wait_for_batches(h));
     std::vector<u64> keys(h->denied_cap), cnts(h->denied_cap);
     CK(cudaMemcpy(keys.data(), h->denied.keys, keys.size() * sizeof(u64), cudaMemcpyDeviceToHost));
     CK(cudaMemcpy(cnts.data(), h->denied.counts, cnts.size() * sizeof(u64), cudaMemcpyDeviceToHost));
@@ -2079,7 +2078,7 @@ static int snapshot_begin(gcra_engine *h, SnapshotJob &j) {
     j.hd = header_of(h, 3);
     // the cut: after every batch submitted so far (their last stage records ev_back) and every Store-trait op
     cudaStream_t st = sg.stream.get();
-    for (auto &o : h->scr) if (o.back_recorded) CK(cudaStreamWaitEvent(st, o.ev_back.get(), 0));
+    RC(order_after_batches(h, st));
     CK(cudaEventRecord(sg.ev_store.get(), h->stream.get()));
     CK(cudaStreamWaitEvent(st, sg.ev_store.get(), 0));
     u64 *ctrl = (u64 *)sg.dev.get();
