@@ -95,6 +95,15 @@ typedef struct {
     int64_t max_burst, count_per_period, period;
 } gcra_policy;
 
+/* Key reference: the key is the bytes [off, off + len) of a byte arena.  It travels in a request row's key_hash field
+ * (offset 0 of gcra_request and gcra_request16) until the hash pass (gcra_hash_keys_device) replaces it with the
+ * engine's hash of those bytes; rows keep their size.  GCRA_KEY_REF(off, len) is the same 64-bit value. */
+typedef struct {
+    uint32_t off;
+    uint32_t len;
+} gcra_key_ref;
+#define GCRA_KEY_REF(off, len) (((uint64_t)(uint32_t)(len) << 32) | (uint64_t)(uint32_t)(off))
+
 /* 16-byte result of a compact request: what rate_limiter.rs:208 calls `cur`, plus status and allowed.
  * gcra_expand_results16 turns it into the gcra_result the 32-byte path returns, bit for bit. */
 typedef struct {
@@ -137,7 +146,10 @@ const char *gcra_last_error(gcra_engine *h);
  * the string-keyed entry points (gcra_rate_limit, gcra_store_*, gcra_actor_throttle) then hash with SipHash-2-4
  * under that seed, and callers of the batch entry points fill gcra_request.key_hash with gcra_engine_hash_key (or
  * gcra_hash_key_seeded and the seed, which gcra_get_hash_seed returns; a snapshot carries it; engines that shard one
- * key space must share it).  gcra_hash_key stays for trusted / synthetic key universes (tests, benches). */
+ * key space must share it).  gcra_hash_key stays for trusted / synthetic key universes (tests, benches).
+ * Callers that hold key STRINGS need not hash on the host: they put the key bytes in an arena and a key reference
+ * (gcra_key_ref) in each row, and the hash pass on the GPU (gcra_hash_keys_device, gcra_rate_limit_batch_keys, the
+ * keyed ring, gcra_resp_parse_throttle_keyed) writes exactly gcra_engine_hash_key of those bytes into the row. */
 uint64_t gcra_hash_key(const void *key, uint64_t len);
 uint64_t gcra_hash_key_seeded(const void *key, uint64_t len, uint64_t seed0, uint64_t seed1);
 uint64_t gcra_engine_hash_key(gcra_engine *h, const void *key, uint64_t len);
@@ -174,6 +186,19 @@ int32_t gcra_rate_limit_batch(gcra_engine *h, uint64_t n, const gcra_request *re
 /* same with device-resident buffers, asynchronous on `stream` (n <= max_batch) */
 int32_t gcra_rate_limit_batch_device(gcra_engine *h, uint64_t n, const gcra_request *d_req,
                                      gcra_result *d_res, void *stream);
+/* The hash pass: in n device-resident rows of row_bytes = 48 (gcra_request) or 16 (gcra_request16) bytes, replace
+ * every key reference with gcra_engine_hash_key(h, d_keys + off, len), in place, asynchronously on `stream` (NULL =
+ * the engine's stream).  Enqueue it in front of any batch call that takes device rows (gcra_rate_limit_batch*_device,
+ * the pipelined and the multi-GPU submissions).  Reads nothing outside [d_keys, d_keys + keys_len).  A row whose
+ * reference leaves the arena (off + len > keys_len) gets key_hash 0 and now_ns = -1 (48 bytes) or policy =
+ * UINT32_MAX (16 bytes): the batch answers it GCRA_INTERNAL, counts it in `errors` and touches no entry. */
+int32_t gcra_hash_keys_device(gcra_engine *h, uint64_t n, void *d_rows, uint32_t row_bytes, const void *d_keys,
+                              uint64_t keys_len, void *stream);
+/* gcra_rate_limit_batch with key references in req[i].key_hash into the host arena `keys` (keys_len bytes): the
+ * arena goes to the device once, and the hash pass runs before every chunk.  Same chunking by max_batch and the same
+ * sweep policy before every chunk; `req` is not modified. */
+int32_t gcra_rate_limit_batch_keys(gcra_engine *h, uint64_t n, const gcra_request *req, const void *keys,
+                                   uint64_t keys_len, gcra_result *res);
 
 /* pipelined submission: the batch's ingest + ordering run on an engine stream as soon as `ready_stream`
  * (a cudaStream_t, may be NULL = inputs are ready now) reaches this point, overlapping the decide kernels
@@ -221,6 +246,15 @@ gcra_result16 *gcra_ring_results16(gcra_engine *h, uint32_t slot);  /* pinned, v
 int32_t gcra_ring_submit(gcra_engine *h, uint32_t slot, uint32_t n, int64_t now_ns);
 int32_t gcra_ring_wait(gcra_engine *h, uint32_t slot);
 int32_t gcra_ring_poll(gcra_engine *h, uint32_t slot, int32_t *done);
+/* keyed ring: the same ring (any mode) plus a pinned and a device key arena of key_capacity bytes (1 .. 2^32) per
+ * slot.  The caller writes key bytes into gcra_ring_keys(h, slot) and key references into the rows; submit_keyed
+ * copies the rows and the first keys_len arena bytes to the device and runs the hash pass before the batch.  Submit
+ * (rows that already hold hashes), wait and poll work on a keyed ring as on any other.  keys_len > key_capacity, or a
+ * ring without arenas, returns GCRA_INTERNAL and enqueues nothing. */
+int32_t gcra_ring_create_keyed(gcra_engine *h, uint32_t slots, uint32_t slot_capacity, int32_t mode,
+                               uint64_t key_capacity);
+void *gcra_ring_keys(gcra_engine *h, uint32_t slot);             /* pinned, caller fills; NULL unless keyed */
+int32_t gcra_ring_submit_keyed(gcra_engine *h, uint32_t slot, uint32_t n, uint64_t keys_len, int64_t now_ns);
 
 /* ---- sweep and introspection ------------------------------------------------------------ */
 /* HashMap::retain(expiry > now) (adaptive_cleanup.rs:176-182), unconditionally */
@@ -404,6 +438,16 @@ void gcra_actor_destroy(gcra_actor *a);
  * again), 3 max_frames reached.  h (may be NULL) supplies the engine's key-hash seed. */
 int32_t gcra_resp_parse_throttle(gcra_engine *h, const void *buf, uint64_t len, int64_t now_ns, uint32_t max_frames,
                                  gcra_request *req_out, uint64_t *consumed, uint32_t *n_frames, int32_t *stop);
+/* the same walk (same frames, same UTF-8 rule, same stop codes), but no hashing on the host: each key is copied to
+ * keys_out at offset *keys_used (in: bytes already used, out: after this call's keys) and the row gets its key
+ * reference; the hash pass hashes them on the GPU (e.g. keys_out = the ring slot's arena, then
+ * gcra_ring_submit_keyed).  A frame whose key does not fit in keys_cap stops the walk unconsumed with *stop = 3,
+ * like max_frames ("slot full").  A key longer than the whole arena never fits: when the walk stops there with
+ * *keys_used = 0 and no frame taken, hash that one frame on the host (gcra_resp_parse_throttle, max_frames = 1) and
+ * submit it as an unkeyed batch, as resp.process_pipeline_native does. */
+int32_t gcra_resp_parse_throttle_keyed(gcra_engine *h, const void *buf, uint64_t len, int64_t now_ns,
+                                       uint32_t max_frames, gcra_request *req_out, void *keys_out, uint64_t keys_cap,
+                                       uint64_t *keys_used, uint64_t *consumed, uint32_t *n_frames, int32_t *stop);
 /* replies of n decided THROTTLE commands, in order (mod.rs:274-285, seconds as types.rs:87-97); needs cap >= 160 n */
 uint64_t gcra_resp_format_replies(const gcra_request *req, const gcra_result *res, uint32_t n, void *out,
                                   uint64_t cap);

@@ -25,8 +25,8 @@ from ._native import (REQ_DTYPE, RES_DTYPE, REQ16_DTYPE, RES16_DTYPE, POLICY_DTY
 
 __all__ = ["RateLimiter", "RateLimitResult", "Rate", "CellError", "NegativeQuantity", "InvalidRateLimit",
            "Internal", "AdaptiveStore", "PeriodicStore", "ProbabilisticStore", "ManualStore",
-           "hash_key", "derive_params", "expand_results16", "REQ_DTYPE", "RES_DTYPE", "REQ16_DTYPE", "RES16_DTYPE",
-           "POLICY_DTYPE"]
+           "hash_key", "key_ref", "pack_keys", "derive_params", "expand_results16", "REQ_DTYPE", "RES_DTYPE",
+           "REQ16_DTYPE", "RES16_DTYPE", "POLICY_DTYPE"]
 
 NS = 1_000_000_000
 
@@ -83,6 +83,24 @@ def _ns(t):
 def hash_key(key):
     k = _kb(key)
     return int(_native.lib().gcra_hash_key(k, len(k)))
+
+
+def key_ref(off, length):
+    """include/gcra_b200.h: the key reference of the bytes [off, off + length) of a key arena"""
+    return (int(length) << 32) | int(off)
+
+
+def pack_keys(keys):
+    """(refs, arena) for a sequence of keys (str or bytes): arena = the keys' bytes back to back (uint8), refs[i] =
+    GCRA_KEY_REF(off, len) of keys[i] in it (uint64) -- what the keyed calls take in a row's key_hash field."""
+    kb = [_kb(k) for k in keys]
+    lens = np.fromiter(map(len, kb), np.uint64, len(kb))
+    offs = np.zeros(len(kb), np.uint64)
+    if len(kb) > 1:
+        np.cumsum(lens[:-1], out=offs[1:])
+    if len(kb) and int(offs[-1]) > 0xFFFFFFFF:
+        raise ValueError("key references hold 32-bit offsets: the keys exceed 4 GiB")
+    return (lens << np.uint64(32)) | offs, np.frombuffer(b"".join(kb), np.uint8)
 
 
 def hash_key_ids(ids, prefix="k:"):
@@ -432,6 +450,26 @@ class RateLimiter:
         self.store._check(self._L.gcra_rate_limit_batch(self._h, len(req), req.ctypes.data, res.ctypes.data))
         return res
 
+    def rate_limit_batch_keys(self, keys, rows, out=None):
+        """rate_limit_batch with string keys: rows[i] (REQ_DTYPE, key_hash ignored) is decided for keys[i] (str or
+        bytes), which the GPU hashes as store.hash_key would (gcra_rate_limit_batch_keys)."""
+        refs, arena = pack_keys(keys)
+        req = np.array(rows, REQ_DTYPE, copy=True)
+        if len(req) != len(refs):
+            raise ValueError("keys and rows differ in length")
+        req["key_hash"] = refs
+        res = np.empty(len(req), RES_DTYPE) if out is None else out
+        self.store._check(self._L.gcra_rate_limit_batch_keys(self._h, len(req), req.ctypes.data, arena.ctypes.data,
+                                                             len(arena), res.ctypes.data))
+        return res
+
+    def hash_keys_device(self, n, d_rows_ptr, row_bytes, d_keys_ptr, keys_len, stream=None):
+        """The hash pass (gcra_hash_keys_device): n device rows of row_bytes (48 or 16) whose key_hash holds a key
+        reference into the device arena d_keys_ptr (keys_len bytes) get the engine's hash of those bytes, in place,
+        asynchronously on `stream`.  Enqueue it before a device batch call on the same stream."""
+        self.store._check(self._L.gcra_hash_keys_device(self._h, n, d_rows_ptr, row_bytes, d_keys_ptr, keys_len,
+                                                        stream))
+
     def set_policies(self, policies):
         pol = np.ascontiguousarray(policies, POLICY_DTYPE)
         self.store._check(self._L.gcra_set_policies(self._h, len(pol), pol.ctypes.data))
@@ -469,14 +507,19 @@ class RateLimiter:
 
 class Ring:
     """Pinned host ring (gcra_ring_*): fill a slot in place, submit, wait, read results in place.
-    compact: False = REQ_DTYPE / RES_DTYPE slots, True = REQ16_DTYPE / RES_DTYPE, 2 = REQ16_DTYPE / RES16_DTYPE."""
+    compact: False = REQ_DTYPE / RES_DTYPE slots, True = REQ16_DTYPE / RES_DTYPE, 2 = REQ16_DTYPE / RES16_DTYPE.
+    key_capacity > 0: every slot also has a pinned key arena `keys[slot]` (uint8, key_capacity bytes); rows then
+    hold key references (pack_keys) and submit(..., keys_len=...) hashes them on the GPU before the batch."""
 
-    def __init__(self, limiter, slots, slot_capacity, compact=False):
+    def __init__(self, limiter, slots, slot_capacity, compact=False, key_capacity=0):
         self.lim, self.store = limiter, limiter.store
         self._L, self._h = limiter._L, limiter._h
-        self.slots, self.cap, self.compact = slots, slot_capacity, compact
+        self.slots, self.cap, self.compact, self.key_capacity = slots, slot_capacity, compact, key_capacity
         mode = 2 if (compact == 2 and compact is not True) else (1 if compact else 0)
-        self.store._check(self._L.gcra_ring_create(self._h, slots, slot_capacity, mode))
+        if key_capacity:
+            self.store._check(self._L.gcra_ring_create_keyed(self._h, slots, slot_capacity, mode, key_capacity))
+        else:
+            self.store._check(self._L.gcra_ring_create(self._h, slots, slot_capacity, mode))
         dt = REQ16_DTYPE if mode else REQ_DTYPE
         rdt = RES16_DTYPE if mode == 2 else RES_DTYPE
         results = self._L.gcra_ring_results16 if mode == 2 else self._L.gcra_ring_results
@@ -488,9 +531,15 @@ class Ring:
             sb = (C.c_char * (slot_capacity * rdt.itemsize)).from_address(sp)
             self.req.append(np.frombuffer(rb, dtype=dt))
             self.res.append(np.frombuffer(sb, dtype=rdt))
+        self.keys = [np.frombuffer((C.c_char * key_capacity).from_address(self._L.gcra_ring_keys(self._h, s)),
+                                   dtype=np.uint8) for s in range(slots)] if key_capacity else None
 
-    def submit(self, slot, n, now=0):
-        self.store._check(self._L.gcra_ring_submit(self._h, slot, n, _ns(now)))
+    def submit(self, slot, n, now=0, keys_len=None):
+        """keys_len (keyed ring): the rows hold key references into the first keys_len bytes of keys[slot]."""
+        if keys_len is None:
+            self.store._check(self._L.gcra_ring_submit(self._h, slot, n, _ns(now)))
+        else:
+            self.store._check(self._L.gcra_ring_submit_keyed(self._h, slot, n, keys_len, _ns(now)))
 
     def wait(self, slot):
         self.store._check(self._L.gcra_ring_wait(self._h, slot))

@@ -86,6 +86,8 @@ SYMBOLS = {
     "gcra_rate_limit": (_i32, [_vp, C.c_char_p, _u64, _i64, _i64, _i64, _i64, _i64, _vp]),
     "gcra_rate_limit_batch": (_i32, [_vp, _u64, _vp, _vp]),
     "gcra_rate_limit_batch_device": (_i32, [_vp, _u64, _vp, _vp, _vp]),
+    "gcra_hash_keys_device": (_i32, [_vp, _u64, _vp, _u32, _vp, _u64, _vp]),
+    "gcra_rate_limit_batch_keys": (_i32, [_vp, _u64, _vp, _vp, _u64, _vp]),
     "gcra_rate_limit_batch_device_pipelined": (_i32, [_vp, _u64, _vp, _vp, _vp]),
     "gcra_pipeline_join": (_i32, [_vp, _vp]),
     "gcra_set_policies": (_i32, [_vp, _u32, _vp]),
@@ -101,6 +103,9 @@ SYMBOLS = {
     "gcra_ring_submit": (_i32, [_vp, _u32, _u32, _i64]),
     "gcra_ring_wait": (_i32, [_vp, _u32]),
     "gcra_ring_poll": (_i32, [_vp, _u32, C.POINTER(_i32)]),
+    "gcra_ring_create_keyed": (_i32, [_vp, _u32, _u32, _i32, _u64]),
+    "gcra_ring_keys": (_vp, [_vp, _u32]),
+    "gcra_ring_submit_keyed": (_i32, [_vp, _u32, _u32, _u64, _i64]),
     "gcra_sweep": (_i32, [_vp, _i64, _pu64]),
     "gcra_policy_tick": (_i32, [_vp, _i64, _pu64]),
     "gcra_len": (_u64, [_vp]),
@@ -140,6 +145,8 @@ SYMBOLS = {
     "gcra_actor_stats": (_i32, [_vp, C.POINTER(_u64 * 3)]),
     "gcra_actor_destroy": (None, [_vp]),
     "gcra_resp_parse_throttle": (_i32, [_vp, C.c_char_p, _u64, _i64, _u32, _vp, _pu64, C.POINTER(_u32), C.POINTER(_i32)]),
+    "gcra_resp_parse_throttle_keyed": (_i32, [_vp, C.c_char_p, _u64, _i64, _u32, _vp, _vp, _u64, _pu64, _pu64,
+                                              C.POINTER(_u32), C.POINTER(_i32)]),
     "gcra_resp_format_replies": (_u64, [_vp, _vp, _u32, _vp, _u64]),
     "gcra_owner_of": (_u32, [_u64, _u32]),
     "gcra_route_partition": (_i32, [_vp, _u64, _vp, _u32, _vp, _vp, _vp, _vp]),

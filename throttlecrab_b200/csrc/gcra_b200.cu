@@ -53,6 +53,8 @@ struct RingSlot {
     PinnedBuf<unsigned char> h_req;
     PinnedBuf<unsigned char> h_res;  // gcra_result, or gcra_result16 rows in ring mode 2
     DevBuf<unsigned char> d_req, d_res;
+    PinnedBuf<unsigned char> h_keys; // keyed ring: the key arena the rows' key references point into
+    DevBuf<unsigned char> d_keys;
     Event ev_in, ev_done;
     bool in_flight = false;
 };
@@ -320,6 +322,9 @@ struct gcra_engine {
     std::vector<RingSlot> ring;
     uint32_t ring_cap = 0;
     int ring_fmt = FMT_48_32;        // the slots' RowFmt (gcra_ring_create)
+    uint64_t ring_key_cap = 0;       // bytes of every slot's key arena (0: the ring is not keyed)
+    DevBuf<unsigned char> d_keys;    // gcra_rate_limit_batch_keys: the caller's key arena on the device
+    uint64_t d_keys_cap = 0;
     // denied requests per key (gcra_track_denied): device table, updated by a pass over every finished batch
     DeniedArrays denied_arrays;
     DeniedTable denied{};
@@ -1052,6 +1057,22 @@ static int launch_pipelined(gcra_engine *h, uint32_t n, const void *d_req, int f
     return launch_pipelined_view(h, single_view(d_req, (gcra_result *)d_res, n), n, fmt, now_batch, ready, done);
 }
 
+// ---- the hash pass: key references -> the engine's key hashes, in place, on `st` --------------------------------
+static int enqueue_hash_keys(gcra_engine *h, uint64_t n, void *d_rows, uint32_t row_bytes, const void *d_keys,
+                             uint64_t keys_len, cudaStream_t st) {
+    if (row_bytes != sizeof(gcra_request) && row_bytes != sizeof(gcra_request16)) {
+        h->err = "row_bytes must be 48 or 16"; return GCRA_INTERNAL;
+    }
+    if (n > 0xffffffffULL) { h->err = "more than 2^32 - 1 rows"; return GCRA_INTERNAL; }
+    if (n == 0) return GCRA_OK;
+    hash_keys_kernel<<<(uint32_t)((n + TILE_THREADS - 1) / TILE_THREADS), TILE_THREADS, 0, st>>>(
+        (unsigned char *)d_rows, (uint32_t)n, row_bytes, (const unsigned char *)d_keys, keys_len, h->hash_seed[0],
+        h->hash_seed[1]);
+    h->launches++;
+    CK(cudaGetLastError());
+    return GCRA_OK;
+}
+
 // CUDA loads a kernel's code lazily, at its FIRST launch, and that load may wait for running kernels.  The
 // multi-GPU pipelines keep kernels running that wait for work other launches deliver (flags in peer memory), so a
 // first launch behind such a kernel would stall until the wait gives up: load everything when the engine is made.
@@ -1078,7 +1099,7 @@ static void preload_kernels() {
     preload(route_count_kernel); preload(route_scan_kernel); preload(route_scatter_kernel); preload(route_unpermute_kernel);
     preload(p2p_scan_kernel); preload(p2p_scatter_kernel); preload(p2p_signal_req_kernel); preload(p2p_signal_res_kernel);
     preload(p2p_wait_kernel); preload(p2p_unpermute_kernel);
-    preload(snapshot_capture_kernel); preload(denied_count_seg_kernel);
+    preload(snapshot_capture_kernel); preload(denied_count_seg_kernel); preload(hash_keys_kernel);
 }
 
 // ---------------------------------------------------------------------------------------------
@@ -1229,55 +1250,18 @@ void gcra_destroy(gcra_engine *h) {
 
 const char *gcra_last_error(gcra_engine *h) { return h ? h->err.c_str() : "null handle"; }
 
+// (both hashes are defined once, for the host and the hash pass, in gcra_device.cuh)
 uint64_t gcra_hash_key(const void *key, uint64_t len) {
-    const unsigned char *p = (const unsigned char *)key;
-    uint64_t hsh = 0x2545F4914F6CDD1DULL ^ (len * 0x9E3779B97F4A7C15ULL);
-    while (len >= 8) {
-        uint64_t w;
-        memcpy(&w, p, 8);
-        hsh = mix64(hsh ^ w) + 0xD1B54A32D192ED03ULL;
-        p += 8; len -= 8;
-    }
-    if (len) {
-        uint64_t w = 0;
-        memcpy(&w, p, len);
-        hsh = mix64(hsh ^ w ^ (len << 56));
-    }
-    return mix64(hsh);
+    return hash_key_unkeyed(KeyBytes{(const unsigned char *)key}, len);
 }
 
-// SipHash-2-4 (Aumasson & Bernstein), 64-bit output: the keyed hash for keys an adversary may choose
-static inline uint64_t rotl64(uint64_t x, int b) { return (x << b) | (x >> (64 - b)); }
 uint64_t gcra_hash_key_seeded(const void *key, uint64_t len, uint64_t k0, uint64_t k1) {
-    uint64_t v0 = 0x736f6d6570736575ULL ^ k0, v1 = 0x646f72616e646f6dULL ^ k1;
-    uint64_t v2 = 0x6c7967656e657261ULL ^ k0, v3 = 0x7465646279746573ULL ^ k1;
-    const unsigned char *p = (const unsigned char *)key;
-    const unsigned char *end = p + (len & ~7ULL);
-#define GCRA_SIPROUND                                                                 \
-    do {                                                                              \
-        v0 += v1; v1 = rotl64(v1, 13); v1 ^= v0; v0 = rotl64(v0, 32);                \
-        v2 += v3; v3 = rotl64(v3, 16); v3 ^= v2;                                      \
-        v0 += v3; v3 = rotl64(v3, 21); v3 ^= v0;                                      \
-        v2 += v1; v1 = rotl64(v1, 17); v1 ^= v2; v2 = rotl64(v2, 32);                \
-    } while (0)
-    for (; p != end; p += 8) {
-        uint64_t m;
-        memcpy(&m, p, 8);
-        v3 ^= m; GCRA_SIPROUND; GCRA_SIPROUND; v0 ^= m;
-    }
-    uint64_t b = len << 56;
-    for (uint64_t i = 0; i < (len & 7); i++) b |= (uint64_t)p[i] << (8 * i);
-    v3 ^= b; GCRA_SIPROUND; GCRA_SIPROUND; v0 ^= b;
-    v2 ^= 0xff;
-    GCRA_SIPROUND; GCRA_SIPROUND; GCRA_SIPROUND; GCRA_SIPROUND;
-#undef GCRA_SIPROUND
-    return v0 ^ v1 ^ v2 ^ v3;
+    return hash_key_siphash(KeyBytes{(const unsigned char *)key}, len, k0, k1);
 }
 
 // the identity the engine's own string-keyed entry points give a key: keyed when the engine has a seed
 static uint64_t engine_hash(const gcra_engine *h, const void *key, uint64_t len) {
-    return (h->hash_seed[0] | h->hash_seed[1]) ? gcra_hash_key_seeded(key, len, h->hash_seed[0], h->hash_seed[1])
-                                               : gcra_hash_key(key, len);
+    return hash_key_engine(KeyBytes{(const unsigned char *)key}, len, h->hash_seed[0], h->hash_seed[1]);
 }
 
 uint64_t gcra_engine_hash_key(gcra_engine *h, const void *key, uint64_t len) { return engine_hash(h, key, len); }
@@ -1392,9 +1376,23 @@ int32_t gcra_pipeline_join(gcra_engine *h, void *stream) {
     return stream ? order_after_batches(h, (cudaStream_t)stream) : wait_for_batches(h);
 }
 
-static int host_batch(gcra_engine *h, uint64_t n, const void *req, int fmt, int64_t now_batch, void *res) {
+struct KeyArena { const void *keys; uint64_t len; };
+
+// arena != null: the rows hold key references into the host arena, which goes to the device first; the hash pass
+// runs on every chunk before its batch
+static int host_batch(gcra_engine *h, uint64_t n, const void *req, int fmt, int64_t now_batch, void *res,
+                      const KeyArena *arena = nullptr) {
     CK(cudaSetDevice(h->device));
     const size_t rsz = req_bytes(fmt), ressz = res_bytes(fmt);
+    const uint64_t keys_len = arena ? arena->len : 0;
+    if (keys_len > h->d_keys_cap) {
+        DevBuf<unsigned char> grown;              // (a failed call keeps the old arena)
+        CK(cudaStreamSynchronize(h->stream.get()));
+        CK(grown.make(keys_len));
+        h->d_keys = std::move(grown);
+        h->d_keys_cap = keys_len;
+    }
+    if (keys_len) CK(cudaMemcpyAsync(h->d_keys.get(), arena->keys, keys_len, cudaMemcpyHostToDevice, h->stream.get()));
     uint64_t done = 0;
     while (done < n) {
         uint32_t m = (uint32_t)std::min<uint64_t>(n - done, h->max_batch);
@@ -1405,6 +1403,7 @@ static int host_batch(gcra_engine *h, uint64_t n, const void *req, int fmt, int6
         int rc = apply_policy(h, now_hint);
         if (rc) return rc;
         CK(cudaMemcpyAsync(h->d_req.get(), src, (size_t)m * rsz, cudaMemcpyHostToDevice, h->stream.get()));
+        if (arena) RC(enqueue_hash_keys(h, m, h->d_req.get(), (uint32_t)rsz, h->d_keys.get(), keys_len, h->stream.get()));
         rc = launch_batch(h, m, h->d_req.get(), fmt, now_batch, h->d_res.get(), h->stream.get(), true);
         if (rc) return rc;
         CK(cudaMemcpyAsync((unsigned char *)res + done * ressz, h->d_res.get(), (size_t)m * ressz, cudaMemcpyDeviceToHost, h->stream.get()));
@@ -1417,6 +1416,19 @@ static int host_batch(gcra_engine *h, uint64_t n, const void *req, int fmt, int6
 
 int32_t gcra_rate_limit_batch(gcra_engine *h, uint64_t n, const gcra_request *req, gcra_result *res) {
     return host_batch(h, n, req, FMT_48_32, 0, res);
+}
+
+int32_t gcra_rate_limit_batch_keys(gcra_engine *h, uint64_t n, const gcra_request *req, const void *keys,
+                                   uint64_t keys_len, gcra_result *res) {
+    if (!keys && keys_len) { h->err = "null key arena"; return GCRA_INTERNAL; }
+    const KeyArena arena = {keys, keys_len};
+    return host_batch(h, n, req, FMT_48_32, 0, res, &arena);
+}
+
+int32_t gcra_hash_keys_device(gcra_engine *h, uint64_t n, void *d_rows, uint32_t row_bytes, const void *d_keys,
+                              uint64_t keys_len, void *stream) {
+    CK(cudaSetDevice(h->device));
+    return enqueue_hash_keys(h, n, d_rows, row_bytes, d_keys, keys_len, stream ? (cudaStream_t)stream : h->stream.get());
 }
 
 int32_t gcra_rate_limit_batch16(gcra_engine *h, uint64_t n, const gcra_request16 *req, int64_t now_ns,
@@ -1498,10 +1510,12 @@ int32_t gcra_expand_results16(uint64_t n, const gcra_request16 *req, int64_t now
 }
 
 // ---- ring --------------------------------------------------------------------------------------
-int32_t gcra_ring_create(gcra_engine *h, uint32_t slots, uint32_t slot_capacity, int32_t mode) {
+// key_capacity > 0: every slot also gets a pinned and a device key arena of that many bytes (gcra_ring_create_keyed)
+static int ring_create(gcra_engine *h, uint32_t slots, uint32_t slot_capacity, int32_t mode, uint64_t key_capacity) {
     CK(cudaSetDevice(h->device));
     if (!h->ring.empty()) { h->err = "ring already created"; return GCRA_INTERNAL; }
     if (slot_capacity == 0 || slot_capacity > h->max_batch) { h->err = "slot_capacity must be in 1..max_batch"; return GCRA_INTERNAL; }
+    if (key_capacity > (1ULL << 32)) { h->err = "key_capacity must be at most 2^32 (32-bit key offsets)"; return GCRA_INTERNAL; }
     // 0: 48-byte requests, 32-byte results; any other value but 2: 16-byte requests, 32-byte results; 2: 16 / 16
     const int fmt = mode == 0 ? FMT_48_32 : mode == 2 ? FMT_16_16 : FMT_16_32;
     const size_t rsz = req_bytes(fmt), ressz = res_bytes(fmt);
@@ -1513,13 +1527,27 @@ int32_t gcra_ring_create(gcra_engine *h, uint32_t slots, uint32_t slot_capacity,
         CK(s.h_res.make(slot_capacity * ressz));
         CK(s.d_req.make(slot_capacity * rsz));
         CK(s.d_res.make(slot_capacity * ressz));
+        if (key_capacity) { CK(s.h_keys.make(key_capacity)); CK(s.d_keys.make(key_capacity)); }
         for (Event *e : {&s.ev_in, &s.ev_done}) CK(e->make(cudaEventDisableTiming));
     }
     h->ring = std::move(ring);
     h->ring_cap = slot_capacity;
     h->ring_fmt = fmt;
+    h->ring_key_cap = key_capacity;
     return GCRA_OK;
 }
+
+int32_t gcra_ring_create(gcra_engine *h, uint32_t slots, uint32_t slot_capacity, int32_t mode) {
+    return ring_create(h, slots, slot_capacity, mode, 0);
+}
+
+int32_t gcra_ring_create_keyed(gcra_engine *h, uint32_t slots, uint32_t slot_capacity, int32_t mode,
+                               uint64_t key_capacity) {
+    if (key_capacity == 0) { h->err = "key_capacity must be at least 1"; return GCRA_INTERNAL; }
+    return ring_create(h, slots, slot_capacity, mode, key_capacity);
+}
+
+void *gcra_ring_keys(gcra_engine *h, uint32_t slot) { return slot < h->ring.size() ? h->ring[slot].h_keys.get() : nullptr; }
 
 void *gcra_ring_requests(gcra_engine *h, uint32_t slot) { return slot < h->ring.size() ? h->ring[slot].h_req.get() : nullptr; }
 gcra_result *gcra_ring_results(gcra_engine *h, uint32_t slot) {
@@ -1529,15 +1557,22 @@ gcra_result16 *gcra_ring_results16(gcra_engine *h, uint32_t slot) {
     return slot < h->ring.size() && res_bytes(h->ring_fmt) == sizeof(gcra_result16) ? (gcra_result16 *)h->ring[slot].h_res.get() : nullptr;
 }
 
-int32_t gcra_ring_submit(gcra_engine *h, uint32_t slot, uint32_t n, int64_t now_ns) {
+// keys_len != null: the rows hold key references into the slot's arena, whose first *keys_len bytes go to the device
+// with the rows; the hash pass runs on in_stream before ev_in, so everything after it is the unkeyed path
+static int ring_submit(gcra_engine *h, uint32_t slot, uint32_t n, int64_t now_ns, const uint64_t *keys_len) {
     CK(cudaSetDevice(h->device));
     if (slot >= h->ring.size() || n > h->ring_cap) { h->err = "bad ring slot / size"; return GCRA_INTERNAL; }
+    if (keys_len && *keys_len > h->ring_key_cap) { h->err = "keys_len larger than the ring's key_capacity"; return GCRA_INTERNAL; }
     RingSlot &s = h->ring[slot];
     if (s.in_flight) { h->err = "ring slot still in flight"; return GCRA_INTERNAL; }
     // sweep policy with the counters of the batches finished so far (no stall)
     if (cudaEventQuery(h->ev_counters.get()) == cudaSuccess) { int rc = apply_policy(h, now_ns); if (rc) return rc; }
     const size_t rsz = req_bytes(h->ring_fmt), ressz = res_bytes(h->ring_fmt);
     CK(cudaMemcpyAsync(s.d_req.get(), s.h_req.get(), (size_t)n * rsz, cudaMemcpyHostToDevice, h->in_stream.get()));
+    if (keys_len) {
+        if (*keys_len) CK(cudaMemcpyAsync(s.d_keys.get(), s.h_keys.get(), *keys_len, cudaMemcpyHostToDevice, h->in_stream.get()));
+        RC(enqueue_hash_keys(h, n, s.d_req.get(), (uint32_t)rsz, s.d_keys.get(), *keys_len, h->in_stream.get()));
+    }
     CK(cudaEventRecord(s.ev_in.get(), h->in_stream.get()));
     // front half (ingest + order) of this slot overlaps the back half (decide) of the previous one
     cudaEvent_t done = nullptr;
@@ -1550,6 +1585,15 @@ int32_t gcra_ring_submit(gcra_engine *h, uint32_t slot, uint32_t n, int64_t now_
     CK(cudaEventRecord(s.ev_done.get(), h->out_stream.get()));
     s.in_flight = true;
     return GCRA_OK;
+}
+
+int32_t gcra_ring_submit(gcra_engine *h, uint32_t slot, uint32_t n, int64_t now_ns) {
+    return ring_submit(h, slot, n, now_ns, nullptr);
+}
+
+int32_t gcra_ring_submit_keyed(gcra_engine *h, uint32_t slot, uint32_t n, uint64_t keys_len, int64_t now_ns) {
+    if (h->ring_key_cap == 0) { h->err = "the ring has no key arenas (gcra_ring_create_keyed)"; return GCRA_INTERNAL; }
+    return ring_submit(h, slot, n, now_ns, &keys_len);
 }
 
 int32_t gcra_ring_wait(gcra_engine *h, uint32_t slot) {

@@ -4,6 +4,7 @@
 // (emission interval) and core/store/adaptive_cleanup.rs:221-278 (entry liveness / TTL).
 #pragma once
 #include <cstdint>
+#include <cstring>
 #include <cuda_runtime.h>
 
 namespace gcra {
@@ -107,6 +108,90 @@ __host__ __device__ __forceinline__ u64 unmix64(u64 x) {
 __host__ __device__ __forceinline__ u64 stored_key(u64 key_hash) {
     u64 k = mix64(key_hash);
     return k < 2 ? k + 2 : k;   // 0 / 1 are the empty / tombstone marks
+}
+
+// ------------------------------------------------------------------ key bytes -> key hash
+// The two key hashes of the string-keyed entry points, ONE definition for the host (gcra_hash_key,
+// gcra_hash_key_seeded) and the hash pass (hash_keys_kernel).  Both read a key as little-endian 64-bit words and a
+// tail of 0..7 bytes through a byte source: word(i) = the 8 bytes at i, tail(i, r) = the r < 8 bytes at i,
+// zero-extended.  A source never reads outside the key.
+struct KeyBytes {
+    const unsigned char *p;
+    __host__ __device__ __forceinline__ u64 word(u64 i) const { u64 w; memcpy(&w, p + i, 8); return w; }
+    __host__ __device__ __forceinline__ u64 tail(u64 i, u32 r) const {
+        u64 w = 0;
+        for (u32 j = 0; j < r; j++) w |= (u64)p[i + j] << (8 * j);
+        return w;
+    }
+};
+
+// unkeyed: for trusted / synthetic key universes (see "KEY IDENTITY" in gcra_b200.h)
+template <class Src>
+__host__ __device__ __forceinline__ u64 hash_key_unkeyed(const Src &src, u64 len) {
+    u64 h = 0x2545F4914F6CDD1DULL ^ (len * 0x9E3779B97F4A7C15ULL);
+    u64 i = 0;
+    for (; len - i >= 8; i += 8) h = mix64(h ^ src.word(i)) + 0xD1B54A32D192ED03ULL;
+    const u32 r = (u32)(len & 7);
+    if (r) h = mix64(h ^ src.tail(i, r) ^ ((u64)r << 56));
+    return mix64(h);
+}
+
+__host__ __device__ __forceinline__ u64 rotl64(u64 x, int b) { return (x << b) | (x >> (64 - b)); }
+
+// SipHash-2-4 (Aumasson & Bernstein), 64-bit output: the keyed hash for keys an adversary may choose
+template <class Src>
+__host__ __device__ __forceinline__ u64 hash_key_siphash(const Src &src, u64 len, u64 k0, u64 k1) {
+    u64 v0 = 0x736f6d6570736575ULL ^ k0, v1 = 0x646f72616e646f6dULL ^ k1;
+    u64 v2 = 0x6c7967656e657261ULL ^ k0, v3 = 0x7465646279746573ULL ^ k1;
+#define GCRA_SIPROUND                                                                 \
+    do {                                                                              \
+        v0 += v1; v1 = rotl64(v1, 13); v1 ^= v0; v0 = rotl64(v0, 32);                \
+        v2 += v3; v3 = rotl64(v3, 16); v3 ^= v2;                                      \
+        v0 += v3; v3 = rotl64(v3, 21); v3 ^= v0;                                      \
+        v2 += v1; v1 = rotl64(v1, 17); v1 ^= v2; v2 = rotl64(v2, 32);                \
+    } while (0)
+    u64 i = 0;
+    for (; len - i >= 8; i += 8) {
+        const u64 m = src.word(i);
+        v3 ^= m; GCRA_SIPROUND; GCRA_SIPROUND; v0 ^= m;
+    }
+    const u64 b = (len << 56) | src.tail(i, (u32)(len & 7));
+    v3 ^= b; GCRA_SIPROUND; GCRA_SIPROUND; v0 ^= b;
+    v2 ^= 0xff;
+    GCRA_SIPROUND; GCRA_SIPROUND; GCRA_SIPROUND; GCRA_SIPROUND;
+#undef GCRA_SIPROUND
+    return v0 ^ v1 ^ v2 ^ v3;
+}
+
+// The hash pass's copy of the arena bytes [keys + lo, keys + lo + ext) into a warp's staging (hash_keys_kernel):
+// 16-byte chunks from the first byte rounded down to 16 up to the last rounded up (the staging holds chunk_end(...) -
+// chunk_begin(...) bytes); one lane takes chunks first, first + step, ...  A chunk wholly inside the arena
+// [keys, keys + keys_len) is one 16-byte load, wide(address, staging offset); of any other chunk only the bytes inside
+// [keys + lo, keys + lo + ext) are copied, one at a time, narrow(address, staging offset) -- so nothing outside the
+// arena is read, not even up to a 16-byte boundary.  (A CPU test runs this with recording callbacks.)
+__host__ __device__ __forceinline__ uintptr_t chunk_begin(uintptr_t keys, u32 lo) { return (keys + lo) & ~(uintptr_t)15; }
+__host__ __device__ __forceinline__ uintptr_t chunk_end(uintptr_t keys, u32 lo, u32 ext) {
+    return (keys + lo + ext + 15) & ~(uintptr_t)15;
+}
+template <class Wide, class Narrow>
+__host__ __device__ __forceinline__ void stage_key_span(uintptr_t keys, u64 keys_len, u32 lo, u32 ext, u32 first,
+                                                        u32 step, Wide &&wide, Narrow &&narrow) {
+    const uintptr_t g0 = chunk_begin(keys, lo), g1 = chunk_end(keys, lo, ext);
+    const uintptr_t a_hi = keys + keys_len, k_lo = keys + lo, k_hi = k_lo + ext;
+    for (uintptr_t c = g0 + 16 * (uintptr_t)first; c < g1; c += 16 * (uintptr_t)step) {
+        if (c >= keys && c + 16 <= a_hi) {
+            wide(c, (u32)(c - g0));
+        } else {
+            const uintptr_t b1 = c + 16 < k_hi ? c + 16 : k_hi;
+            for (uintptr_t b = c > k_lo ? c : k_lo; b < b1; b++) narrow(b, (u32)(b - g0));
+        }
+    }
+}
+
+// the identity an engine gives a key: SipHash-2-4 under its seed, the unkeyed hash when the seed is (0,0)
+template <class Src>
+__host__ __device__ __forceinline__ u64 hash_key_engine(const Src &src, u64 len, u64 k0, u64 k1) {
+    return (k0 | k1) ? hash_key_siphash(src, len, k0, k1) : hash_key_unkeyed(src, len);
 }
 
 // ------------------------------------------------------------------ parameter derivation

@@ -1669,4 +1669,69 @@ denied_count_seg_kernel(BatchView v, DeniedTable t) {
     }
 }
 
+// ---------------------------------------------------------------------------------------------
+// K0 hash pass: key references -> key hashes, in place
+// ---------------------------------------------------------------------------------------------
+// A row's key_hash field (offset 0 in both request formats) holds GCRA_KEY_REF(off, len): the key is the bytes
+// [off, off + len) of the caller's arena.  One lane per row.  A warp stages the span its 32 keys cover into shared
+// memory with aligned 16-byte loads when the span fits HASH_STAGE (consecutive rows' keys lie close together, as a
+// ring slot or the RESP parser lays them out); otherwise every lane reads its own key from global memory.  Both
+// paths feed the same hash (gcra_device.cuh), so a key's hash does not depend on the layout.  Nothing outside
+// [keys, keys + keys_len) is read: a 16-byte chunk of the staging that is not wholly inside the arena is copied
+// byte by byte.
+constexpr u32 HASH_STAGE = 2048;                   // bytes a warp stages: 32 keys of up to ~60 bytes
+constexpr u32 HASH_WARPS = TILE_THREADS / 32;
+
+// a key in a warp's staging: 64-bit words from aligned 32-bit shared loads and funnel shifts (the staging is padded
+// by 16 bytes, so a word read for the last bytes of a key stays inside it)
+struct StagedBytes {
+    const u32 *base;                               // the warp's staging
+    u32 pos;                                       // the key's first byte in it
+    __device__ __forceinline__ u64 word(u64 i) const {
+        const u32 a = pos + (u32)i, sh = (a & 3) * 8;
+        const u32 *w = base + (a >> 2);
+        const u32 w0 = w[0], w1 = w[1], w2 = w[2];
+        return (u64)__funnelshift_r(w0, w1, sh) | ((u64)__funnelshift_r(w1, w2, sh) << 32);
+    }
+    __device__ __forceinline__ u64 tail(u64 i, u32 r) const { return r ? word(i) & ((1ULL << (8 * r)) - 1) : 0; }
+};
+
+__global__ void __launch_bounds__(TILE_THREADS)
+hash_keys_kernel(unsigned char *rows, u32 n, u32 row_bytes, const unsigned char *keys, u64 keys_len, u64 k0, u64 k1) {
+    __shared__ __align__(16) u32 stage[HASH_WARPS][(HASH_STAGE + 16) / 4];
+    const u32 lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+    const u64 i = (u64)blockIdx.x * TILE_THREADS + threadIdx.x;
+    const bool active = i < n;
+    u64 *row = reinterpret_cast<u64 *>(rows + i * row_bytes);
+    const u64 ref = active ? row[0] : 0;
+    const u32 off = (u32)ref, len = (u32)(ref >> 32);
+    const bool ok = active && (u64)off + len <= keys_len;
+    // the warp's span [lo, lo + ext) over its in-arena keys with at least one byte
+    const bool used = ok && len > 0;
+    const u32 lo = __reduce_min_sync(0xffffffffu, used ? off : 0xffffffffu);
+    const u32 ext = __reduce_max_sync(0xffffffffu, used ? (u32)min((u64)off + len - lo, 0xffffffffULL) : 0u);
+    const uintptr_t g0 = chunk_begin((uintptr_t)keys, lo);
+    const bool staged = ext > 0 && chunk_end((uintptr_t)keys, lo, ext) - g0 <= HASH_STAGE;   // (uniform over the warp)
+    if (staged) {
+        unsigned char *sb = reinterpret_cast<unsigned char *>(stage[wid]);
+        stage_key_span((uintptr_t)keys, keys_len, lo, ext, lane, 32,
+                       [&](uintptr_t src, u32 dst) {
+                           *reinterpret_cast<uint4 *>(sb + dst) = __ldg(reinterpret_cast<const uint4 *>(src));
+                       },
+                       [&](uintptr_t src, u32 dst) { sb[dst] = *reinterpret_cast<const unsigned char *>(src); });
+        __syncwarp();
+    }
+    if (!active) return;
+    if (!ok) {
+        // a reference that leaves the arena: a row the decide kernels answer GCRA_INTERNAL without touching an entry
+        row[0] = 0;
+        if (row_bytes == sizeof(gcra_request)) row[5] = ~0ULL;                           // now_ns = -1 (pre-epoch)
+        else reinterpret_cast<u32 *>(row)[3] = 0xffffffffu;                              // policy >= any npol
+        return;
+    }
+    row[0] = staged && len > 0
+        ? hash_key_engine(StagedBytes{stage[wid], (u32)((uintptr_t)keys + off - g0)}, len, k0, k1)
+        : hash_key_engine(KeyBytes{keys + off}, len, k0, k1);
+}
+
 }  // namespace gcra

@@ -276,26 +276,45 @@ def process_pipeline_native(buffer, limiter, now_ns, ring=None, slot=0):
     writes the replies; only frames that are not plain THROTTLE commands (PING, QUIT, RESP-integer arguments, ...)
     go through the general parser above.  All THROTTLE commands of the buffer are ONE engine batch (the ring's
     submit / wait when a ring is given, else rate_limit_batch); replies come back in command order.
+    A keyed ring (Ring(..., key_capacity=...)) takes gcra_resp_parse_throttle_keyed instead: keys are copied into
+    the slot's key arena and hashed on the GPU, not on this thread; a key that no longer fits ends the batch there,
+    unconsumed, like a full slot.  A key longer than the whole arena can never fit: when it comes first, its frame
+    is hashed on this thread and decided alone, as a batch of host-hashed rows, so every frame is answered.
     Returns (reply_bytes, bytes_consumed, n_throttle, close)."""
     import ctypes as C
-    from . import RES_DTYPE
+    from . import RES_DTYPE, _kb, key_ref
     L, h = limiter._L, limiter._h
     data = bytes(buffer)
     cap = ring.cap if ring is not None else max(len(data) // 32 + 1, 16)
     req = ring.req[slot] if ring is not None else np.empty(cap, REQ_DTYPE)
+    arena = ring.keys[slot] if ring is not None and ring.keys is not None else None
+    kused = C.c_uint64(0)
+    host_hashed = arena is None                           # (the batch's rows hold key hashes, not key references)
     parser = RespParser()
     segs, n, consumed, close = [], 0, 0, None            # segs: ("rows", first, count) | ("reply", value) | ("row", index, limit, qty)
     now = int(now_ns() if callable(now_ns) else now_ns)
     while consumed < len(data) and n < cap:
         used, cnt, stop = C.c_uint64(), C.c_uint32(), C.c_int32()
         view = data[consumed:]
-        limiter.store._check(L.gcra_resp_parse_throttle(h, view, len(view), now, cap - n,
-                                                        req.ctypes.data + n * REQ_DTYPE.itemsize,
-                                                        C.byref(used), C.byref(cnt), C.byref(stop)))
+        rows = req.ctypes.data + n * REQ_DTYPE.itemsize
+        if arena is None:
+            limiter.store._check(L.gcra_resp_parse_throttle(h, view, len(view), now, cap - n, rows,
+                                                            C.byref(used), C.byref(cnt), C.byref(stop)))
+        else:
+            limiter.store._check(L.gcra_resp_parse_throttle_keyed(h, view, len(view), now, cap - n, rows,
+                                                                  arena.ctypes.data, len(arena), C.byref(kused),
+                                                                  C.byref(used), C.byref(cnt), C.byref(stop)))
+        if arena is not None and stop.value == 3 and n == 0 and cnt.value == 0:
+            # the first frame's key is longer than the arena: this one frame, hashed here, is the batch
+            limiter.store._check(L.gcra_resp_parse_throttle(h, view, len(view), now, 1, rows, C.byref(used),
+                                                            C.byref(cnt), C.byref(stop)))
+            host_hashed = True
         if cnt.value:
             segs.append(("rows", n, cnt.value))
             n += cnt.value
             consumed += used.value
+        if host_hashed and arena is not None:
+            break
         if stop.value != 2:
             break                                         # end of buffer, incomplete frame, or the slot is full
         try:                                              # one frame for the general parser
@@ -311,10 +330,24 @@ def process_pipeline_native(buffer, limiter, now_ns, ring=None, slot=0):
             if n >= cap:
                 consumed -= r[1]
                 break
-            req[n] = (hash_key(plan[1]) if not any(limiter.store.hash_seed()) else limiter.store.hash_key(plan[1]),
-                      plan[2], plan[3], plan[4], plan[5], now)
+            kb = _kb(plan[1])
+            if arena is not None and len(kb) > len(arena) - kused.value:
+                if n:
+                    consumed -= r[1]
+                    break
+                host_hashed = True                        # longer than the whole arena: decided alone (see above)
+            if host_hashed:
+                kh = hash_key(kb) if not any(limiter.store.hash_seed()) else limiter.store.hash_key(kb)
+            else:
+                at = kused.value
+                arena[at:at + len(kb)] = np.frombuffer(kb, np.uint8)
+                kused.value = at + len(kb)
+                kh = key_ref(at, len(kb))
+            req[n] = (kh, plan[2], plan[3], plan[4], plan[5], now)
             segs.append(("row", n, plan[2], plan[5]))
             n += 1
+            if host_hashed and arena is not None:
+                break
         else:
             segs.append(("reply", plan[1]))
         if _is_quit(r[0]):
@@ -323,7 +356,7 @@ def process_pipeline_native(buffer, limiter, now_ns, ring=None, slot=0):
     res = None
     if n:
         if ring is not None:
-            ring.submit(slot, n, now)
+            ring.submit(slot, n, now, keys_len=None if host_hashed else kused.value)
             ring.wait(slot)
             res = ring.res[slot]
         else:
