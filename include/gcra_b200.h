@@ -452,6 +452,55 @@ int32_t gcra_resp_parse_throttle_keyed(gcra_engine *h, const void *buf, uint64_t
 uint64_t gcra_resp_format_replies(const gcra_request *req, const gcra_result *res, uint32_t n, void *out,
                                   uint64_t cap);
 
+/* ---- RESP ring: connections' read buffers in, reply bytes out -------------------------------------------------
+ * The engine's ring (one per engine: it takes the place of gcra_ring_create), whose slots carry bytes instead of
+ * rows.  The caller reads its sockets into gcra_resp_ring_input(h, slot) and describes each connection's bytes in
+ * gcra_resp_ring_conns(h, slot)[c] = {off, len}, len <= GCRA_RESP_MAX_CONN_BYTES (the reference's MAX_BUFFER_SIZE,
+ * redis/mod.rs:83).  Submit parses every connection on the GPU, decides the rows as one batch and writes the replies;
+ * gcra_ring_wait / gcra_ring_poll complete the slot as for any ring.
+ *
+ * Contract: for connection c, in table order, the GPU takes exactly what
+ *     gcra_resp_parse_throttle(h, input + off_c, len_c, now_ns, row_capacity - base_c, rows + base_c, ...)
+ * takes -- the same rows (key hashes under the engine's seed), consumed, n_frames and stop -- where base_c is the
+ * number of rows of the connections before c.  The rows of all connections form one batch in that order.  After
+ * wait, gcra_resp_ring_outcome(h, slot)[c] gives consumed, n_frames, stop, and where the connection's replies lie in
+ * gcra_resp_ring_replies(h, slot): reply_len bytes at reply_off, one reply per frame, in frame order, each the bytes
+ * gcra_resp_format_replies writes for it.  What the caller does at each stop:
+ *   0  every byte was a plain THROTTLE frame: send the replies;
+ *   1  an incomplete frame follows at `consumed`: keep its bytes and read more;
+ *   2  a frame that is not a plain THROTTLE follows at `consumed`: hand that ONE frame to a general RESP parser
+ *      (PING, QUIT, RESP-integer arguments, malformed input), then submit the rest again;
+ *   3  the slot's row_capacity is used up: submit the rest again (every connection after c also stops with 3 unless it
+ *      is empty).
+ * Submit validates everything before it enqueues anything: n_conns > max_conns, a connection past in_capacity or
+ * longer than GCRA_RESP_MAX_CONN_BYTES, or a slot in flight returns GCRA_INTERNAL and leaves the engine usable.  Like
+ * gcra_ring_submit it applies the store's sweep policy first.  The replies travel to the host as they are written
+ * (pinned memory written by the kernel): exactly the reply bytes and 32 bytes of outcome per connection cross the
+ * link, not a bound. */
+#define GCRA_RESP_MAX_CONN_BYTES 65536u
+#define GCRA_RESP_REPLY_MAX 160u       /* bytes of reply per row that gcra_resp_ring_replies has room for */
+typedef struct {
+    uint32_t off, len;                 /* bytes [off, off + len) of the slot's input */
+} gcra_resp_conn;
+typedef struct {
+    uint32_t consumed, n_frames;
+    int32_t stop;                      /* 0 .. 3, as gcra_resp_parse_throttle */
+    uint32_t reserved;
+    uint64_t reply_off, reply_len;     /* the connection's replies in gcra_resp_ring_replies */
+} gcra_resp_outcome;
+/* slots x (in_capacity bytes of input (1 .. 2^32), max_conns connections (1 .. 65536), row_capacity rows
+ * (1 .. max_batch) and row_capacity x GCRA_RESP_REPLY_MAX bytes of replies) */
+int32_t gcra_resp_ring_create(gcra_engine *h, uint32_t slots, uint32_t max_conns, uint64_t in_capacity,
+                              uint32_t row_capacity);
+void *gcra_resp_ring_input(gcra_engine *h, uint32_t slot);                 /* pinned, caller fills */
+gcra_resp_conn *gcra_resp_ring_conns(gcra_engine *h, uint32_t slot);       /* pinned [max_conns], caller fills */
+int32_t gcra_resp_ring_submit(gcra_engine *h, uint32_t slot, uint32_t n_conns, int64_t now_ns);
+void *gcra_resp_ring_replies(gcra_engine *h, uint32_t slot);               /* pinned, valid after wait */
+gcra_resp_outcome *gcra_resp_ring_outcome(gcra_engine *h, uint32_t slot);  /* pinned [max_conns], valid after wait */
+/* cold path, after wait: the slot's parsed rows and their results (*n rows; GCRA_INTERNAL if cap < *n) */
+int32_t gcra_resp_ring_rows(gcra_engine *h, uint32_t slot, gcra_request *req_out, gcra_result *res_out, uint32_t cap,
+                            uint32_t *n);
+
 #ifdef __cplusplus
 }
 #endif

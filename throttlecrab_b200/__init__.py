@@ -21,11 +21,12 @@ import numpy as np
 
 from . import _native
 from ._native import (REQ_DTYPE, RES_DTYPE, REQ16_DTYPE, RES16_DTYPE, POLICY_DTYPE, OK, NEGATIVE_QUANTITY,
-                      INVALID_RATE_LIMIT, INTERNAL)
+                      INVALID_RATE_LIMIT, INTERNAL, RESP_CONN_DTYPE, RESP_OUTCOME_DTYPE, RESP_MAX_CONN_BYTES,
+                      RESP_REPLY_MAX)
 
 __all__ = ["RateLimiter", "RateLimitResult", "Rate", "CellError", "NegativeQuantity", "InvalidRateLimit",
            "Internal", "AdaptiveStore", "PeriodicStore", "ProbabilisticStore", "ManualStore",
-           "hash_key", "key_ref", "pack_keys", "derive_params", "expand_results16", "REQ_DTYPE", "RES_DTYPE",
+           "hash_key", "key_ref", "pack_keys", "RespRing", "derive_params", "expand_results16", "REQ_DTYPE", "RES_DTYPE",
            "REQ16_DTYPE", "RES16_DTYPE", "POLICY_DTYPE"]
 
 NS = 1_000_000_000
@@ -543,3 +544,41 @@ class Ring:
 
     def wait(self, slot):
         self.store._check(self._L.gcra_ring_wait(self._h, slot))
+
+
+class RespRing:
+    """The engine's ring as a RESP ring (gcra_resp_ring_*): connections' read buffers in, reply bytes out.
+    Fill input[slot] (uint8, in_capacity bytes) and conns[slot][:n] (RESP_CONN_DTYPE: off, len <= 65536), submit,
+    wait; outcome[slot][:n] (RESP_OUTCOME_DTYPE) then says what each connection consumed, how many frames it had
+    decided, where it stopped, and where its replies lie in replies[slot].  Contract and stop codes: gcra_b200.h.
+    An engine has one ring: this takes the place of Ring."""
+
+    def __init__(self, limiter, slots, max_conns, in_capacity, row_capacity):
+        self.lim, self.store = limiter, limiter.store
+        self._L, self._h = limiter._L, limiter._h
+        self.slots, self.max_conns, self.in_capacity, self.row_capacity = slots, max_conns, in_capacity, row_capacity
+        self.store._check(self._L.gcra_resp_ring_create(self._h, slots, max_conns, in_capacity, row_capacity))
+
+        def view(ptr, n, dt):
+            return np.frombuffer((C.c_char * (n * np.dtype(dt).itemsize)).from_address(ptr), dtype=dt)
+        L, h = self._L, self._h
+        self.input = [view(L.gcra_resp_ring_input(h, s), in_capacity, np.uint8) for s in range(slots)]
+        self.conns = [view(L.gcra_resp_ring_conns(h, s), max_conns, RESP_CONN_DTYPE) for s in range(slots)]
+        self.replies = [view(L.gcra_resp_ring_replies(h, s), row_capacity * RESP_REPLY_MAX, np.uint8)
+                        for s in range(slots)]
+        self.outcome = [view(L.gcra_resp_ring_outcome(h, s), max_conns, RESP_OUTCOME_DTYPE) for s in range(slots)]
+
+    def submit(self, slot, n_conns, now=0):
+        self.store._check(self._L.gcra_resp_ring_submit(self._h, slot, n_conns, _ns(now)))
+
+    def wait(self, slot):
+        self.store._check(self._L.gcra_ring_wait(self._h, slot))
+
+    def rows(self, slot):
+        """after wait: the slot's parsed rows and their results (REQ_DTYPE, RES_DTYPE), in batch order"""
+        req = np.empty(self.row_capacity, REQ_DTYPE)
+        res = np.empty(self.row_capacity, RES_DTYPE)
+        n = C.c_uint32()
+        self.store._check(self._L.gcra_resp_ring_rows(self._h, slot, req.ctypes.data, res.ctypes.data,
+                                                      self.row_capacity, C.byref(n)))
+        return req[:n.value], res[:n.value]

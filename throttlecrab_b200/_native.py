@@ -25,6 +25,10 @@ RES_DTYPE = np.dtype([("remaining", "<i8"), ("reset_after_ns", "<i8"), ("retry_a
 REQ16_DTYPE = np.dtype([("key_hash", "<u8"), ("quantity", "<i4"), ("policy", "<u4")])
 RES16_DTYPE = np.dtype([("cur_tat_ns", "<i8"), ("status", "<i4"), ("allowed", "u1"), ("pad", "u1", (3,))])
 POLICY_DTYPE = np.dtype([("max_burst", "<i8"), ("count_per_period", "<i8"), ("period", "<i8")])
+RESP_CONN_DTYPE = np.dtype([("off", "<u4"), ("len", "<u4")])                       # gcra_resp_conn
+RESP_OUTCOME_DTYPE = np.dtype([("consumed", "<u4"), ("n_frames", "<u4"), ("stop", "<i4"), ("reserved", "<u4"),
+                               ("reply_off", "<u8"), ("reply_len", "<u8")])         # gcra_resp_outcome
+RESP_MAX_CONN_BYTES, RESP_REPLY_MAX = 65536, 160
 assert REQ_DTYPE.itemsize == 48 and RES_DTYPE.itemsize == 32 and REQ16_DTYPE.itemsize == 16
 assert RES16_DTYPE.itemsize == 16
 
@@ -60,7 +64,8 @@ def build(force=False, verbose=False):
     if not force and os.path.exists(SO_PATH) and all(
             os.path.getmtime(s) <= os.path.getmtime(SO_PATH) for s in srcs):
         return SO_PATH
-    cmd = ["nvcc"] + NVCC_FLAGS + ["-o", SO_PATH, os.path.join(_SRC, "gcra_b200.cu")]
+    # (two translation units: gcra_resp_ring.cu keeps its dynamic shared memory out of gcra_b200.cu's kernels)
+    cmd = ["nvcc"] + NVCC_FLAGS + ["-o", SO_PATH] + [os.path.join(_SRC, f) for f in ("gcra_b200.cu", "gcra_resp_ring.cu")]
     if verbose:
         cmd.insert(1, "-Xptxas=-v")
     subprocess.check_call(cmd)
@@ -148,6 +153,13 @@ SYMBOLS = {
     "gcra_resp_parse_throttle_keyed": (_i32, [_vp, C.c_char_p, _u64, _i64, _u32, _vp, _vp, _u64, _pu64, _pu64,
                                               C.POINTER(_u32), C.POINTER(_i32)]),
     "gcra_resp_format_replies": (_u64, [_vp, _vp, _u32, _vp, _u64]),
+    "gcra_resp_ring_create": (_i32, [_vp, _u32, _u32, _u64, _u32]),
+    "gcra_resp_ring_input": (_vp, [_vp, _u32]),
+    "gcra_resp_ring_conns": (_vp, [_vp, _u32]),
+    "gcra_resp_ring_submit": (_i32, [_vp, _u32, _u32, _i64]),
+    "gcra_resp_ring_replies": (_vp, [_vp, _u32]),
+    "gcra_resp_ring_outcome": (_vp, [_vp, _u32]),
+    "gcra_resp_ring_rows": (_i32, [_vp, _u32, _vp, _vp, _u32, C.POINTER(_u32)]),
     "gcra_owner_of": (_u32, [_u64, _u32]),
     "gcra_route_partition": (_i32, [_vp, _u64, _vp, _u32, _vp, _vp, _vp, _vp]),
     "gcra_route_unpermute": (_i32, [_vp, _u64, _vp, _vp, _vp, _vp]),

@@ -1,0 +1,271 @@
+// gcra_resp_ring.cu -- the RESP ring's kernels (gcra_resp_ring_*): connections' read buffers -> request rows, and
+// results -> reply bytes.  The frame grammar and the reply text are gcra_resp.cuh, the host parser's own.  A
+// translation unit of its own: the parse kernel's dynamic shared memory would pad every kernel's static shared memory
+// in gcra_b200.cu to 16 bytes.  gcra_b200.cu launches these kernels through the functions at the end.
+//
+//   resp_parse_kernel    one CTA per connection: rows of the connection's plain-THROTTLE prefix, exactly what
+//                        gcra_resp_parse_throttle writes for it at the row cap that connections before it leave
+//   resp_reply_kernel    one thread per row: the reply bytes, packed in row order
+//   resp_outcome_kernel  one thread per connection: where its replies lie
+#include "gcra_resp_ring.cuh"
+#include "gcra_resp.cuh"
+
+namespace gcra {
+
+constexpr u32 RESP_KIND_SHIFT = 17;            // a candidate's word: frame end (0 .. 65536) | kind << 17
+constexpr u64 RESP_AGG = 1ULL << 62, RESP_INC = 1ULL << 63, RESP_VAL = RESP_AGG - 1;   // look-back status words
+
+__device__ __forceinline__ u64 ld_volatile_u64(const u64 *p) {
+    u64 v;
+    asm volatile("ld.volatile.u64 %0, [%1];" : "=l"(v) : "l"(p) : "memory");
+    return v;
+}
+__device__ __forceinline__ void st_volatile_u64(u64 *p, u64 v) {
+    asm volatile("st.volatile.u64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
+}
+
+// exclusive scan of one value per thread over the CTA; *sum receives the total
+__device__ __forceinline__ u64 resp_block_scan(u64 v, u64 *warp_sums, u64 *sum) {
+    const u32 lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+    u64 inc = v;
+#pragma unroll
+    for (u32 o = 1; o < 32; o <<= 1) {
+        const u64 y = __shfl_up_sync(0xffffffffu, inc, o);
+        if (lane >= o) inc += y;
+    }
+    if (lane == 31) warp_sums[w] = inc;
+    __syncthreads();
+    u64 before = 0, all = 0;
+    for (u32 i = 0; i < RESP_THREADS / 32; i++) {
+        if (i < w) before += warp_sums[i];
+        all += warp_sums[i];
+    }
+    *sum = all;
+    __syncthreads();                               // warp_sums may be reused
+    return before + inc - v;
+}
+
+// Decoupled look-back: publish this item's `value`, then add those of the items before it, taken by ticket, until
+// one that has published its inclusive prefix; publish this item's.  Returns the exclusive prefix.  Every earlier
+// item was handed to a CTA that runs already, so the wait ends.  (One thread.)
+__device__ __forceinline__ u64 resp_look_back(u64 *status, u32 item, u64 value) {
+    if (item == 0) { st_volatile_u64(&status[0], RESP_INC | value); return 0; }
+    st_volatile_u64(&status[item], RESP_AGG | value);
+    u64 excl = 0;
+    for (u32 j = item - 1;; j--) {
+        u64 st;
+        do { st = ld_volatile_u64(&status[j]); } while (!(st & (RESP_AGG | RESP_INC)));
+        excl += st & RESP_VAL;
+        if (st & RESP_INC) break;
+    }
+    st_volatile_u64(&status[item], RESP_INC | (excl + value));
+    return excl;
+}
+
+__device__ __forceinline__ u32 resp_rank(const u32 *bits, const u32 *before, u32 p) {
+    return before[p >> 5] + __popc(bits[p >> 5] & ((1u << (p & 31)) - 1));
+}
+
+// Connection c (taken by ticket, so in table order) = in[conns[c].off, + conns[c].len), len <= 65536.  Its rows go
+// to rows[base_c ...], base_c = the rows of the connections before it; at most row_cap rows in all, cut exactly where
+// gcra_resp_parse_throttle with max_frames = row_cap - base_c stops (stop 3).  Writes the connection's consumed,
+// n_frames and stop to outcome[c] (pinned host memory), {base_c, n_frames} to conn_rows[c]; the CTA of the last
+// connection writes the row count to *total and the segments' row counts of the batch view (segment s holds rows
+// [s << cap_shift, (s + 1) << cap_shift)).  status[0 .. n_conns) and *ticket are zero at launch.
+__global__ void __launch_bounds__(RESP_THREADS, 1)
+resp_parse_kernel(const unsigned char *__restrict__ in, const gcra_resp_conn *__restrict__ conns, u32 n_conns,
+                  u32 max_len, i64 now_ns, u32 row_cap, u64 k0, u64 k1, gcra_request *__restrict__ rows,
+                  u64 *status, u32 *ticket, uint2 *__restrict__ conn_rows, gcra_resp_outcome *outcome,
+                  u32 *__restrict__ total, u32 *__restrict__ seg_counts, u32 nseg, u32 cap_shift) {
+    // (no alignment is declared for the dynamic shared memory: that would pad every kernel's; RespSmem leaves room to
+    // round its start up to 16 bytes)
+    extern __shared__ unsigned char resp_dyn[];
+    unsigned char *smem = reinterpret_cast<unsigned char *>((reinterpret_cast<uintptr_t>(resp_dyn) + 15) & ~(uintptr_t)15);
+    __shared__ u64 warp_sums[RESP_THREADS / 32];
+    __shared__ u32 s_conn, s_base, s_n;
+    const RespSmem L(max_len);
+    u32 *bits = reinterpret_cast<u32 *>(smem + L.bits_off);
+    u32 *before = reinterpret_cast<u32 *>(smem + L.before_off);
+    u32 *cand = reinterpret_cast<u32 *>(smem + L.cand_off);
+
+    if (threadIdx.x == 0) s_conn = atomicAdd(ticket, 1u);
+    __syncthreads();
+    const u32 c = s_conn;
+    const gcra_resp_conn cn = conns[c];
+    const u32 len = cn.len;
+
+    // stage the segment: 16-byte loads of the chunks wholly inside it, single bytes at its ends (nothing outside it)
+    const uintptr_t seg = reinterpret_cast<uintptr_t>(in) + cn.off;
+    const unsigned char *sb = smem + (seg & 15);
+    stage_key_span(seg, len, 0, len, threadIdx.x, RESP_THREADS,
+                   [&](uintptr_t g, u32 o) { *reinterpret_cast<uint4 *>(smem + o) = __ldg(reinterpret_cast<const uint4 *>(g)); },
+                   [&](uintptr_t g, u32 o) { smem[o] = *reinterpret_cast<const unsigned char *>(g); });
+    __syncthreads();
+
+    // candidate frame starts: one bit per byte; each thread takes a run of 32-byte words
+    const u32 words = (len + 31) / 32, per = (words + RESP_THREADS - 1) / RESP_THREADS;
+    const u32 w0 = min(words, threadIdx.x * per), w1 = min(words, w0 + per);
+    u32 mine = 0;
+    for (u32 w = w0; w < w1; w++) {
+        u32 b = 0;
+        for (u32 j = 0; j < 32; j++) {
+            const u32 p = w * 32 + j;
+            if (p < len && sb[p] == '*' && (p == 0 || sb[p - 1] == '\n')) b |= 1u << j;
+        }
+        bits[w] = b;
+        mine += __popc(b);
+    }
+    u64 ncand;
+    u32 idx = (u32)resp_block_scan(mine, warp_sums, &ncand);
+    for (u32 w = w0; w < w1; w++) {
+        before[w] = idx;
+        for (u32 b = bits[w]; b; b &= b - 1) cand[idx++] = w * 32 + __ffs(b) - 1;
+    }
+    __syncthreads();
+
+    // every candidate parsed speculatively: its end, or why it is not a plain THROTTLE frame
+    for (u32 i = threadIdx.x; i < (u32)ncand; i += RESP_THREADS) {
+        gcra_resp::Cursor cu = {sb + cand[i], sb + len};
+        gcra_resp::Frame fr;
+        const int rc = gcra_resp::parse_frame(cu, fr);
+        cand[i] = rc ? (u32)rc << RESP_KIND_SHIFT : (u32)(cu.p - sb);
+    }
+    __syncthreads();
+
+    if (threadIdx.x == 0) {
+        // The true frames: the chain from the segment start.  A frame ends with "\r\n", so the next one starts at a
+        // candidate exactly when its first byte is '*'.  cand[k] becomes the start of the k-th frame (k <= the index
+        // read, so nothing still to be read is overwritten).
+        u32 n = 0, p = 0, why = 0;
+        while (p < len) {
+            if (sb[p] != '*') { why = 2; break; }
+            const u32 e = cand[resp_rank(bits, before, p)];
+            if (e >> RESP_KIND_SHIFT) { why = e >> RESP_KIND_SHIFT; break; }
+            cand[n++] = p;
+            p = e;
+        }
+        // rows of the connections before this one; the cap cuts this one as max_frames = row_cap - base would
+        const u64 excl = resp_look_back(status, c, n);
+        const u32 base = excl < row_cap ? (u32)excl : row_cap, room = row_cap - base;
+        u32 take = n, stop_at = p;
+        if (n > room || (n == room && p < len)) { take = room; why = 3; stop_at = take < n ? cand[take] : p; }
+        s_base = base; s_n = take;
+        gcra_resp_outcome o;
+        o.consumed = stop_at;
+        o.n_frames = take;
+        o.stop = (int32_t)why;
+        o.reserved = 0;
+        o.reply_off = 0;
+        o.reply_len = 0;
+        outcome[c] = o;
+        conn_rows[c] = make_uint2(base, take);
+        if (c == n_conns - 1) {
+            const u32 t = base + take;
+            *total = t;
+            for (u32 s = 0; s < nseg; s++) {
+                const u32 first = s << cap_shift;
+                seg_counts[s] = t <= first ? 0 : min(t - first, 1u << cap_shift);
+            }
+        }
+    }
+    __syncthreads();
+
+    // the rows: each frame parsed again, its key hashed from shared memory with the engine's hash
+    const u32 base = s_base, take = s_n;
+    for (u32 k = threadIdx.x; k < take; k += RESP_THREADS) {
+        gcra_resp::Cursor cu = {sb + cand[k], sb + len};
+        gcra_resp::Frame fr;
+        gcra_resp::parse_frame(cu, fr);
+        gcra_request r;
+        r.key_hash = hash_key_engine(KeyBytes{fr.key}, fr.klen, k0, k1);
+        r.max_burst = fr.a[0];
+        r.count_per_period = fr.a[1];
+        r.period = fr.a[2];
+        r.quantity = fr.a[3];
+        r.now_ns = now_ns;
+        rows[base + k] = r;
+    }
+}
+
+// The replies of rows [0, *total) in row order, straight into `out` (pinned host memory): each CTA takes a tile of
+// rows by ticket, measures its replies, finds the tile's offset by a look-back over the tiles before it, writes the
+// replies into shared memory and copies the tile's bytes out in one coalesced sweep.  row_off[i] = the offset of row
+// i's reply, row_off[*total] = all the bytes.  status[] and *ticket are zero at launch.
+__global__ void __launch_bounds__(RESP_THREADS)
+resp_reply_kernel(const gcra_request *__restrict__ rows, const gcra_result *__restrict__ res, const u32 *total_p,
+                  u64 *status, u32 *ticket, u64 *__restrict__ row_off, unsigned char *out) {
+    __shared__ __align__(16) char stage[RESP_THREADS * gcra_resp::REPLY_MAX];
+    __shared__ u64 warp_sums[RESP_THREADS / 32];
+    __shared__ u64 s_base;
+    __shared__ u32 s_tile;
+    if (threadIdx.x == 0) s_tile = atomicAdd(ticket, 1u);
+    __syncthreads();
+    const u32 tile = s_tile, total = *total_p;
+    if ((u64)tile * RESP_THREADS >= total) return;             // uniform over the CTA
+    const u32 row = tile * RESP_THREADS + threadIdx.x;
+    gcra_request q{};
+    gcra_result r{};
+    gcra_resp::Count cnt;
+    if (row < total) {
+        q = rows[row];
+        r = res[row];
+        gcra_resp::put_reply(cnt, q, r);
+    }
+    u64 tile_bytes;
+    const u64 at = resp_block_scan(cnt.n, warp_sums, &tile_bytes);
+    if (threadIdx.x == 0) s_base = resp_look_back(status, tile, tile_bytes);
+    if (row < total) {
+        gcra_resp::Write o{stage + at};
+        gcra_resp::put_reply(o, q, r);
+    }
+    __syncthreads();
+    const u64 base = s_base;
+    if (row < total) row_off[row] = base + at;
+    if (row + 1 == total) row_off[total] = base + at + cnt.n;
+    for (u32 i = threadIdx.x; i < (u32)tile_bytes; i += RESP_THREADS) out[base + i] = stage[i];
+}
+
+// connection c's replies: rows [base_c, base_c + n_c) -> outcome[c].reply_off, reply_len
+__global__ void resp_outcome_kernel(const uint2 *__restrict__ conn_rows, u32 n_conns, const u32 *total_p,
+                                    const u64 *__restrict__ row_off, gcra_resp_outcome *outcome) {
+    const u32 c = blockIdx.x * blockDim.x + threadIdx.x;
+    if (c >= n_conns) return;
+    const u32 total = *total_p;
+    const uint2 br = conn_rows[c];
+    const u64 a = total ? row_off[min(br.x, total)] : 0, b = total ? row_off[min(br.x + br.y, total)] : 0;
+    outcome[c].reply_off = a;
+    outcome[c].reply_len = b - a;
+}
+
+// ---- launches (gcra_resp.inc) ----
+cudaError_t resp_ring_setup() {
+    cudaFuncAttributes a;
+    for (const void *k : {(const void *)resp_parse_kernel, (const void *)resp_reply_kernel, (const void *)resp_outcome_kernel}) {
+        const cudaError_t e = cudaFuncGetAttributes(&a, k);    // (loads the code now: see preload in gcra_b200.cu)
+        if (e) return e;
+    }
+    return cudaFuncSetAttribute(resp_parse_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                (int)RespSmem(RESP_MAX_CONN_BYTES).total);
+}
+
+cudaError_t launch_resp_parse(const RespParse &a, cudaStream_t st) {
+    resp_parse_kernel<<<a.n_conns, RESP_THREADS, RespSmem(a.max_len).total, st>>>(
+        a.in, a.conns, a.n_conns, a.max_len, a.now_ns, a.row_cap, a.k0, a.k1, a.rows, a.status, a.ticket, a.conn_rows,
+        a.outcome, a.total, a.seg_counts, a.nseg, a.cap_shift);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_resp_reply(u32 tiles, const gcra_request *rows, const gcra_result *res, const u32 *total, u64 *ctrl,
+                              u64 *row_off, unsigned char *out, cudaStream_t st) {
+    resp_reply_kernel<<<tiles, RESP_THREADS, 0, st>>>(rows, res, total, ctrl + 1, reinterpret_cast<u32 *>(ctrl), row_off, out);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_resp_outcome(u32 n_conns, const uint2 *conn_rows, const u32 *total, const u64 *row_off,
+                                gcra_resp_outcome *outcome, cudaStream_t st) {
+    resp_outcome_kernel<<<(n_conns + RESP_THREADS - 1) / RESP_THREADS, RESP_THREADS, 0, st>>>(conn_rows, n_conns, total,
+                                                                                            row_off, outcome);
+    return cudaGetLastError();
+}
+
+}  // namespace gcra

@@ -1,0 +1,54 @@
+// gcra_resp_ring.cuh -- what gcra_b200.cu needs of the RESP ring's kernels (gcra_resp_ring.cu, a translation unit
+// of its own): their shared-memory layout and their launches.
+#pragma once
+#include <cuda_runtime.h>
+
+#include "gcra_device.cuh"
+#include "../../include/gcra_b200.h"
+
+namespace gcra {
+
+constexpr u32 RESP_THREADS = 256;
+constexpr u32 RESP_MAX_CONN_BYTES = 65536;     // MAX_BUFFER_SIZE of the reference's Redis transport (redis/mod.rs:83)
+
+// The dynamic shared memory of resp_parse_kernel for connections of up to `max_len` bytes: the staged bytes (16
+// more for the segment's misalignment), one candidate bit per byte, the candidates before each 32-byte word, and one
+// word per candidate -- a candidate is a '*' that starts the segment or follows a '\n', so at most every other byte.
+struct RespSmem {
+    u32 words, bytes_off, bits_off, before_off, cand_off, total;
+    __host__ __device__ explicit RespSmem(u32 max_len) {
+        words = (max_len + 31) / 32;
+        bytes_off = 0;
+        bits_off = (words * 32 + 16 + 15) & ~15u;
+        before_off = bits_off + 4 * words;
+        cand_off = before_off + 4 * words;
+        total = cand_off + 4 * (words * 16) + 16;   // (+16: the start rounded up to 16 bytes)
+    }
+};
+
+// resp_parse_kernel's arguments: connection c is in[conns[c].off, + conns[c].len)
+struct RespParse {
+    const unsigned char *in;
+    const gcra_resp_conn *conns;
+    u32 n_conns, max_len;
+    i64 now_ns;
+    u32 row_cap;
+    u64 k0, k1;                  // the engine's hash seed
+    gcra_request *rows;          // the slot's flat row array
+    u64 *status;                 // [n_conns] look-back status words, zero
+    u32 *ticket;                 // zero
+    uint2 *conn_rows;            // [n_conns] out: first row, rows
+    gcra_resp_outcome *outcome;  // [n_conns] out (pinned host memory)
+    u32 *total, *seg_counts;     // out: rows of the batch, rows of each segment
+    u32 nseg, cap_shift;
+};
+
+cudaError_t resp_ring_setup();   // once, before the first launch
+cudaError_t launch_resp_parse(const RespParse &a, cudaStream_t st);
+// ctrl: word 0 the ticket, then one status word per tile; all zero
+cudaError_t launch_resp_reply(u32 tiles, const gcra_request *rows, const gcra_result *res, const u32 *total, u64 *ctrl,
+                              u64 *row_off, unsigned char *out, cudaStream_t st);
+cudaError_t launch_resp_outcome(u32 n_conns, const uint2 *conn_rows, const u32 *total, const u64 *row_off,
+                                gcra_resp_outcome *outcome, cudaStream_t st);
+
+}  // namespace gcra

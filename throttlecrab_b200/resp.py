@@ -374,3 +374,84 @@ def process_pipeline_native(buffer, limiter, now_ns, ring=None, slot=0):
                                            res.ctypes.data + first * RES_DTYPE.itemsize, cnt, scratch, len(scratch))
             out.append(scratch.raw[:w])
     return b"".join(out), consumed, n, close
+
+
+def process_connections(buffers, limiter, now_ns, ring, slot=0):
+    """process_pipeline for many connections at once, with the parsing and the reply formatting of plain THROTTLE
+    frames on the GPU: `ring` is a RespRing of `limiter`'s engine.  Returns one (reply_bytes, bytes_consumed,
+    n_throttle, close) per buffer, with process_pipeline's meaning; an error or a QUIT closes only its own connection.
+    Each buffer holds at most 65,536 bytes (the reference's MAX_BUFFER_SIZE) and fits in the ring's input.
+
+    Rounds run until every connection has ended at the end of its bytes, at an incomplete frame, or closed.  In a
+    round, the GPU takes every open connection's plain-THROTTLE prefix: one batch per submit, rows in list order of the
+    connections and frame order within each (a full slot leaves the rest to the next round, or to the next submit of
+    the same round when the connections do not fit one).  Then each connection that stopped at a frame that is not a
+    plain THROTTLE hands that one frame to the general parser, in list order; a THROTTLE among them is decided there
+    and then, on its own.  That is the order in which decisions are made, so connections that share keys see each
+    other's requests in that order."""
+    from . import RESP_MAX_CONN_BYTES
+    now = int(now_ns)
+    datas = [bytes(b) for b in buffers]
+    n = len(datas)
+    for d in datas:
+        if len(d) > min(RESP_MAX_CONN_BYTES, ring.in_capacity):
+            raise ValueError("a connection buffer of %d bytes: at most %d" % (len(d), min(RESP_MAX_CONN_BYTES,
+                                                                                       ring.in_capacity)))
+    pos, n_thr, close = [0] * n, [0] * n, [None] * n
+    out = [[] for _ in range(n)]
+    parser = RespParser()
+    live = [c for c in range(n) if datas[c]]
+    while live:
+        stops, i = {}, 0
+        while i < len(live):                               # as many submits as the ring's capacity needs
+            group, used = [], 0
+            while i < len(live) and len(group) < ring.max_conns:
+                c = live[i]
+                rest = len(datas[c]) - pos[c]
+                if used + rest > ring.in_capacity:
+                    break
+                ring.input[slot][used:used + rest] = np.frombuffer(datas[c], np.uint8, rest, pos[c])
+                ring.conns[slot][len(group)] = (used, rest)
+                group.append(c)
+                used += rest
+                i += 1
+            ring.submit(slot, len(group), now)
+            ring.wait(slot)
+            for j, c in enumerate(group):
+                o = ring.outcome[slot][j]
+                off, ln = int(o["reply_off"]), int(o["reply_len"])
+                out[c].append(ring.replies[slot][off:off + ln].tobytes())
+                pos[c] += int(o["consumed"])
+                n_thr[c] += int(o["n_frames"])
+                stops[c] = int(o["stop"])
+        nxt = []
+        for c in live:
+            if stops[c] == 3:
+                nxt.append(c)
+                continue
+            if stops[c] != 2:
+                continue                                   # the end of its bytes, or an incomplete frame
+            try:
+                r = parser.parse(datas[c][pos[c]:])
+            except RespError:
+                close[c] = "error"
+                continue
+            if r is None:
+                continue
+            pos[c] += r[1]
+            plan = _plan_command(r[0])
+            if plan[0] == "throttle":
+                kb = plan[1].encode()
+                req = np.empty(1, REQ_DTYPE)
+                req[0] = (limiter.store.hash_key(kb), plan[2], plan[3], plan[4], plan[5], now)
+                res = limiter.rate_limit_batch(req)
+                out[c].append(RespSerializer.serialize(_throttle_reply(res[0], plan[2], plan[5])))
+                n_thr[c] += 1
+            else:
+                out[c].append(RespSerializer.serialize(plan[1]))
+            if _is_quit(r[0]):
+                close[c] = "quit"
+            elif pos[c] < len(datas[c]):
+                nxt.append(c)
+        live = nxt
+    return [(b"".join(out[c]), pos[c], n_thr[c], close[c]) for c in range(n)]
