@@ -501,6 +501,43 @@ gcra_resp_outcome *gcra_resp_ring_outcome(gcra_engine *h, uint32_t slot);  /* pi
 int32_t gcra_resp_ring_rows(gcra_engine *h, uint32_t slot, gcra_request *req_out, gcra_result *res_out, uint32_t cap,
                             uint32_t *n);
 
+/* ---- batch HTTP ingest: POST /throttle requests -> request rows, results -> responses ----------------------------
+ * The HTTP transport's hot request (transport/http.rs:60-73,103-159), the way gcra_resp_parse_throttle takes RESP's.
+ * gcra_http_parse_throttle walks `buf` once and writes one request row per plain request: exactly
+ * "POST /throttle HTTP/1.1" CRLF, at most 64 header lines "name: value" CRLF with Content-Length (1-5 digits,
+ * <= 65536) and Content-Type: application/json once each (names in any case, other headers skipped) and none of
+ * Transfer-Encoding, Connection, Expect, Upgrade, the empty line, then a Content-Length body that is one JSON object
+ * with the members key (a string without escapes or control bytes, UTF-8), max_burst, count_per_period, period and
+ * optionally quantity (null or absent: 1), in any order, each once, integers without fraction or exponent within
+ * (-2^63, 2^63), -0 excluded.  Key hashes under the engine's seed (h may be NULL).  It never consumes part of a
+ * request.  *stop: 0 the buffer ended on a request boundary, 1 an incomplete request follows (read more), 2 a request
+ * follows that is not plain (hand THAT request to a general HTTP parser, e.g. throttlecrab_b200.http, then call
+ * again), 3 max_frames reached. */
+int32_t gcra_http_parse_throttle(gcra_engine *h, const void *buf, uint64_t len, int64_t now_ns, uint32_t max_frames,
+                                 gcra_request *req_out, uint64_t *consumed, uint32_t *n_frames, int32_t *stop);
+/* responses of n decided requests, in order: "HTTP/1.1 200 OK" with the compact JSON body
+ * {"allowed":..,"limit":..,"remaining":..,"reset_after":..,"retry_after":..} (seconds, types.rs:73-97), or
+ * "HTTP/1.1 500 Internal Server Error" with {"error":"Internal server error: Rate limit check failed: ..."}; headers
+ * content-type: application/json, content-length, date (the IMF-fixdate of the row's now_ns, whole seconds).
+ * Returns the bytes written, 0 if cap < GCRA_HTTP_REPLY_MAX n. */
+#define GCRA_HTTP_REPLY_MAX 256u
+uint64_t gcra_http_format_replies(const gcra_request *req, const gcra_result *res, uint32_t n, void *out,
+                                  uint64_t cap);
+/* The engine's ring as an HTTP ring: a RESP ring in everything but its grammar and replies.  Same limits, same
+ * validation and the same calls: gcra_resp_ring_input, _conns, _submit, _replies, _outcome, _rows, gcra_ring_wait and
+ * gcra_ring_poll, with gcra_resp_conn, gcra_resp_outcome and GCRA_RESP_MAX_CONN_BYTES.  Its replies area holds
+ * row_capacity x GCRA_HTTP_REPLY_MAX bytes.  Contract: for connection c, in table order, the GPU takes exactly what
+ *     gcra_http_parse_throttle(h, input + off_c, len_c, now_ns, row_capacity - base_c, rows + base_c, ...)
+ * takes, base_c being the rows of the connections before c; the connection's replies are the bytes
+ * gcra_http_format_replies writes for its rows.  What the caller does at each stop:
+ *   0  every byte was a plain request: send the responses;
+ *   1  an incomplete request follows at `consumed`: keep its bytes and read more;
+ *   2  a request that is not plain follows at `consumed`: hand that ONE request to a general HTTP parser (other
+ *      routes, other headers, escaped keys, malformed input), then submit the rest again;
+ *   3  the slot's row_capacity is used up: submit the rest again. */
+int32_t gcra_http_ring_create(gcra_engine *h, uint32_t slots, uint32_t max_conns, uint64_t in_capacity,
+                              uint32_t row_capacity);
+
 #ifdef __cplusplus
 }
 #endif

@@ -22,7 +22,7 @@ import numpy as np
 from . import _native
 from ._native import (REQ_DTYPE, RES_DTYPE, REQ16_DTYPE, RES16_DTYPE, POLICY_DTYPE, OK, NEGATIVE_QUANTITY,
                       INVALID_RATE_LIMIT, INTERNAL, RESP_CONN_DTYPE, RESP_OUTCOME_DTYPE, RESP_MAX_CONN_BYTES,
-                      RESP_REPLY_MAX)
+                      RESP_REPLY_MAX, HTTP_REPLY_MAX)
 
 __all__ = ["RateLimiter", "RateLimitResult", "Rate", "CellError", "NegativeQuantity", "InvalidRateLimit",
            "Internal", "AdaptiveStore", "PeriodicStore", "ProbabilisticStore", "ManualStore",
@@ -551,20 +551,27 @@ class RespRing:
     Fill input[slot] (uint8, in_capacity bytes) and conns[slot][:n] (RESP_CONN_DTYPE: off, len <= 65536), submit,
     wait; outcome[slot][:n] (RESP_OUTCOME_DTYPE) then says what each connection consumed, how many frames it had
     decided, where it stopped, and where its replies lie in replies[slot].  Contract and stop codes: gcra_b200.h.
-    An engine has one ring: this takes the place of Ring."""
+    An engine has one ring: this takes the place of Ring.
+    protocol="http" makes it an HTTP ring (gcra_http_ring_create): POST /throttle requests in, HTTP responses out,
+    with the same calls and outcome table (HttpRing)."""
 
-    def __init__(self, limiter, slots, max_conns, in_capacity, row_capacity):
+    def __init__(self, limiter, slots, max_conns, in_capacity, row_capacity, protocol="resp"):
+        if protocol not in ("resp", "http"):
+            raise ValueError("protocol must be 'resp' or 'http'")
         self.lim, self.store = limiter, limiter.store
         self._L, self._h = limiter._L, limiter._h
         self.slots, self.max_conns, self.in_capacity, self.row_capacity = slots, max_conns, in_capacity, row_capacity
-        self.store._check(self._L.gcra_resp_ring_create(self._h, slots, max_conns, in_capacity, row_capacity))
+        self.protocol = protocol
+        create = self._L.gcra_http_ring_create if protocol == "http" else self._L.gcra_resp_ring_create
+        self.store._check(create(self._h, slots, max_conns, in_capacity, row_capacity))
+        reply_max = HTTP_REPLY_MAX if protocol == "http" else RESP_REPLY_MAX
 
         def view(ptr, n, dt):
             return np.frombuffer((C.c_char * (n * np.dtype(dt).itemsize)).from_address(ptr), dtype=dt)
         L, h = self._L, self._h
         self.input = [view(L.gcra_resp_ring_input(h, s), in_capacity, np.uint8) for s in range(slots)]
         self.conns = [view(L.gcra_resp_ring_conns(h, s), max_conns, RESP_CONN_DTYPE) for s in range(slots)]
-        self.replies = [view(L.gcra_resp_ring_replies(h, s), row_capacity * RESP_REPLY_MAX, np.uint8)
+        self.replies = [view(L.gcra_resp_ring_replies(h, s), row_capacity * reply_max, np.uint8)
                         for s in range(slots)]
         self.outcome = [view(L.gcra_resp_ring_outcome(h, s), max_conns, RESP_OUTCOME_DTYPE) for s in range(slots)]
 
@@ -582,3 +589,8 @@ class RespRing:
         self.store._check(self._L.gcra_resp_ring_rows(self._h, slot, req.ctypes.data, res.ctypes.data,
                                                       self.row_capacity, C.byref(n)))
         return req[:n.value], res[:n.value]
+
+
+def HttpRing(limiter, slots, max_conns, in_capacity, row_capacity):
+    """The engine's ring as an HTTP ring: RespRing(..., protocol="http")."""
+    return RespRing(limiter, slots, max_conns, in_capacity, row_capacity, protocol="http")

@@ -28,7 +28,7 @@ POLICY_DTYPE = np.dtype([("max_burst", "<i8"), ("count_per_period", "<i8"), ("pe
 RESP_CONN_DTYPE = np.dtype([("off", "<u4"), ("len", "<u4")])                       # gcra_resp_conn
 RESP_OUTCOME_DTYPE = np.dtype([("consumed", "<u4"), ("n_frames", "<u4"), ("stop", "<i4"), ("reserved", "<u4"),
                                ("reply_off", "<u8"), ("reply_len", "<u8")])         # gcra_resp_outcome
-RESP_MAX_CONN_BYTES, RESP_REPLY_MAX = 65536, 160
+RESP_MAX_CONN_BYTES, RESP_REPLY_MAX, HTTP_REPLY_MAX = 65536, 160, 256
 assert REQ_DTYPE.itemsize == 48 and RES_DTYPE.itemsize == 32 and REQ16_DTYPE.itemsize == 16
 assert RES16_DTYPE.itemsize == 16
 
@@ -160,6 +160,9 @@ SYMBOLS = {
     "gcra_resp_ring_replies": (_vp, [_vp, _u32]),
     "gcra_resp_ring_outcome": (_vp, [_vp, _u32]),
     "gcra_resp_ring_rows": (_i32, [_vp, _u32, _vp, _vp, _u32, C.POINTER(_u32)]),
+    "gcra_http_parse_throttle": (_i32, [_vp, C.c_char_p, _u64, _i64, _u32, _vp, _pu64, C.POINTER(_u32), C.POINTER(_i32)]),
+    "gcra_http_format_replies": (_u64, [_vp, _vp, _u32, _vp, _u64]),
+    "gcra_http_ring_create": (_i32, [_vp, _u32, _u32, _u64, _u32]),
     "gcra_owner_of": (_u32, [_u64, _u32]),
     "gcra_route_partition": (_i32, [_vp, _u64, _vp, _u32, _vp, _vp, _vp, _vp]),
     "gcra_route_unpermute": (_i32, [_vp, _u64, _vp, _vp, _vp, _vp]),

@@ -58,7 +58,8 @@ struct RingSlot {
     DevBuf<unsigned char> d_keys;
     Event ev_in, ev_done;
     bool in_flight = false;
-    // RESP ring (gcra_resp_ring_create): the rows are d_req / d_res, viewed as resp_nseg segments
+    // RESP or HTTP ring (gcra_resp_ring_create, gcra_http_ring_create): the rows are d_req / d_res, viewed as
+    // resp_nseg segments
     PinnedBuf<unsigned char> h_in, h_replies;   // (the kernels write h_replies and h_outcome)
     PinnedBuf<gcra_resp_conn> h_conns;
     PinnedBuf<gcra_resp_outcome> h_outcome;
@@ -335,7 +336,7 @@ struct gcra_engine {
     uint32_t ring_cap = 0;
     int ring_fmt = FMT_48_32;        // the slots' RowFmt (gcra_ring_create)
     uint64_t ring_key_cap = 0;       // bytes of every slot's key arena (0: the ring is not keyed)
-    bool ring_resp = false;          // the ring is a RESP ring (gcra_resp_ring_create)
+    RingProto ring_proto = PROTO_NONE;   // the ring is a RESP or HTTP ring (gcra_resp_ring_create, gcra_http_ring_create)
     uint32_t resp_max_conns = 0, resp_nseg = 0, resp_shift = 0;
     uint64_t resp_in_cap = 0;
     DevBuf<unsigned char> d_keys;    // gcra_rate_limit_batch_keys: the caller's key arena on the device
@@ -1577,7 +1578,7 @@ gcra_result16 *gcra_ring_results16(gcra_engine *h, uint32_t slot) {
 static int ring_submit(gcra_engine *h, uint32_t slot, uint32_t n, int64_t now_ns, const uint64_t *keys_len) {
     CK(cudaSetDevice(h->device));
     if (slot >= h->ring.size() || n > h->ring_cap) { h->err = "bad ring slot / size"; return GCRA_INTERNAL; }
-    if (h->ring_resp) { h->err = "a RESP ring takes gcra_resp_ring_submit"; return GCRA_INTERNAL; }
+    if (h->ring_proto) { h->err = "a RESP or HTTP ring takes gcra_resp_ring_submit"; return GCRA_INTERNAL; }
     if (keys_len && *keys_len > h->ring_key_cap) { h->err = "keys_len larger than the ring's key_capacity"; return GCRA_INTERNAL; }
     RingSlot &s = h->ring[slot];
     if (s.in_flight) { h->err = "ring slot still in flight"; return GCRA_INTERNAL; }

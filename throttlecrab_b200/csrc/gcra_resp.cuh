@@ -169,6 +169,25 @@ GCRA_RESP_HD void put_i64(Out &o, int64_t v) {
     for (; p; p /= 10) o.put((char)('0' + u / p % 10));
 }
 
+// the actor's error for a row that was not decided: "Rate limit check failed: {CellError}" (actor.rs:252,
+// core/mod.rs:58-65), which every transport wraps in its own way.  (Literals, so that each reply below is written
+// from one string.)
+#define GCRA_CHECK_FAILED_NEGATIVE "Rate limit check failed: negative quantity: "
+#define GCRA_CHECK_FAILED_INVALID "Rate limit check failed: invalid rate limit parameters"
+#define GCRA_CHECK_FAILED_INTERNAL "Rate limit check failed: internal error"
+
+template <class Out>
+GCRA_RESP_HD void put_check_failed(Out &o, const gcra_request &q, const gcra_result &r) {
+    if (r.status == GCRA_NEGATIVE_QUANTITY) {
+        put_str(o, GCRA_CHECK_FAILED_NEGATIVE);
+        put_i64(o, q.quantity);
+    } else if (r.status == GCRA_INVALID_RATE_LIMIT) {
+        put_str(o, GCRA_CHECK_FAILED_INVALID);
+    } else {
+        put_str(o, GCRA_CHECK_FAILED_INTERNAL);
+    }
+}
+
 // the reply to one decided THROTTLE command: *5 :allowed :limit :remaining :reset_after_s :retry_after_s, or the
 // reference's error line.  At most REPLY_MAX bytes.
 template <class Out>
@@ -182,13 +201,13 @@ GCRA_RESP_HD void put_reply(Out &o, const gcra_request &q, const gcra_result &r)
         put_str(o, "\r\n:"); put_i64(o, r.retry_after_ns / 1000000000LL);
         put_str(o, "\r\n");
     } else if (r.status == GCRA_NEGATIVE_QUANTITY) {
-        put_str(o, "-ERR Rate limit check failed: negative quantity: ");
+        put_str(o, "-ERR " GCRA_CHECK_FAILED_NEGATIVE);
         put_i64(o, q.quantity);
         put_str(o, "\r\n");
     } else if (r.status == GCRA_INVALID_RATE_LIMIT) {
-        put_str(o, "-ERR Rate limit check failed: invalid rate limit parameters\r\n");
+        put_str(o, "-ERR " GCRA_CHECK_FAILED_INVALID "\r\n");
     } else {
-        put_str(o, "-ERR Rate limit check failed: internal error\r\n");
+        put_str(o, "-ERR " GCRA_CHECK_FAILED_INTERNAL "\r\n");
     }
 }
 constexpr uint32_t REPLY_MAX = 160;

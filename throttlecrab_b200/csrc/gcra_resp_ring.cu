@@ -1,16 +1,48 @@
-// gcra_resp_ring.cu -- the RESP ring's kernels (gcra_resp_ring_*): connections' read buffers -> request rows, and
-// results -> reply bytes.  The frame grammar and the reply text are gcra_resp.cuh, the host parser's own.  A
-// translation unit of its own: the parse kernel's dynamic shared memory would pad every kernel's static shared memory
-// in gcra_b200.cu to 16 bytes.  gcra_b200.cu launches these kernels through the functions at the end.
+// gcra_resp_ring.cu -- the RESP and HTTP rings' kernels (gcra_resp_ring_*): connections' read buffers -> request
+// rows, and results -> reply bytes.  The frame grammar and the reply text are the host parser's own: gcra_resp.cuh for
+// RESP, gcra_http.cuh for HTTP, brought in by a protocol traits type that the parse and reply kernels are templates
+// over.  A translation unit of its own: the parse kernel's dynamic shared memory would pad every kernel's static
+// shared memory in gcra_b200.cu to 16 bytes.  gcra_b200.cu launches these kernels through the functions at the end.
 //
-//   resp_parse_kernel    one CTA per connection: rows of the connection's plain-THROTTLE prefix, exactly what
-//                        gcra_resp_parse_throttle writes for it at the row cap that connections before it leave
+//   resp_parse_kernel    one CTA per connection: rows of the connection's plain prefix, exactly what
+//                        gcra_resp_parse_throttle (gcra_http_parse_throttle) writes for it at the row cap that
+//                        connections before it leave
 //   resp_reply_kernel    one thread per row: the reply bytes, packed in row order
 //   resp_outcome_kernel  one thread per connection: where its replies lie
 #include "gcra_resp_ring.cuh"
-#include "gcra_resp.cuh"
+#include "gcra_http.cuh"
 
 namespace gcra {
+
+// What the ring kernels need of a protocol: where a frame may start (`candidate`: every position the parse kernel
+// parses speculatively; `chain_start`: whether the frame that follows the previous one can start here), the grammar,
+// the reply text and its bound, the rows of a reply tile and the parse kernel's candidate room.
+struct RespTraits {
+    static constexpr u32 REPLY_THREADS = RESP_THREADS, REPLY_MAX = gcra_resp::REPLY_MAX, CAND_PER_WORD = 16;
+    __device__ static bool candidate(const unsigned char *s, u32 p, u32) { return s[p] == '*' && (p == 0 || s[p - 1] == '\n'); }
+    // (a frame ends with "\r\n", so the next one starts at a candidate exactly when its first byte is '*')
+    __device__ static bool chain_start(const unsigned char *s, u32 p, u32) { return s[p] == '*'; }
+    __device__ static int parse(gcra_resp::Cursor &c, gcra_resp::Frame &f) { return gcra_resp::parse_frame(c, f); }
+    template <class Out>
+    __device__ static void put_reply(Out &o, const gcra_request &q, const gcra_result &r) { gcra_resp::put_reply(o, q, r); }
+};
+
+struct HttpTraits {
+    static constexpr u32 REPLY_THREADS = reply_tile_rows(PROTO_HTTP), REPLY_MAX = gcra_http::REPLY_MAX, CAND_PER_WORD = 7;
+    // "POST ", or the part of it that fits before the segment's end (a body ends in '}' or whitespace, so there is no
+    // line-start rule as for RESP)
+    __device__ static bool candidate(const unsigned char *s, u32 p, u32 len) {
+        const char *w = "POST ";
+        for (u32 i = 0; i < 5 && p + i < len; i++)
+            if (s[p + i] != (unsigned char)w[i]) return false;
+        return true;
+    }
+    __device__ static bool chain_start(const unsigned char *s, u32 p, u32 len) { return candidate(s, p, len); }
+    __device__ static int parse(gcra_resp::Cursor &c, gcra_resp::Frame &f) { return gcra_http::parse_frame(c, f); }
+    template <class Out>
+    __device__ static void put_reply(Out &o, const gcra_request &q, const gcra_result &r) { gcra_http::put_reply(o, q, r); }
+};
+static_assert(HttpTraits::REPLY_THREADS * HttpTraits::REPLY_MAX <= 48 * 1024, "the reply tile fits static shared memory");
 
 constexpr u32 RESP_KIND_SHIFT = 17;            // a candidate's word: frame end (0 .. 65536) | kind << 17
 constexpr u64 RESP_AGG = 1ULL << 62, RESP_INC = 1ULL << 63, RESP_VAL = RESP_AGG - 1;   // look-back status words
@@ -24,7 +56,8 @@ __device__ __forceinline__ void st_volatile_u64(u64 *p, u64 v) {
     asm volatile("st.volatile.u64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
 }
 
-// exclusive scan of one value per thread over the CTA; *sum receives the total
+// exclusive scan of one value per thread over a CTA of THREADS threads; *sum receives the total
+template <u32 THREADS>
 __device__ __forceinline__ u64 resp_block_scan(u64 v, u64 *warp_sums, u64 *sum) {
     const u32 lane = threadIdx.x & 31, w = threadIdx.x >> 5;
     u64 inc = v;
@@ -36,7 +69,7 @@ __device__ __forceinline__ u64 resp_block_scan(u64 v, u64 *warp_sums, u64 *sum) 
     if (lane == 31) warp_sums[w] = inc;
     __syncthreads();
     u64 before = 0, all = 0;
-    for (u32 i = 0; i < RESP_THREADS / 32; i++) {
+    for (u32 i = 0; i < THREADS / 32; i++) {
         if (i < w) before += warp_sums[i];
         all += warp_sums[i];
     }
@@ -68,10 +101,12 @@ __device__ __forceinline__ u32 resp_rank(const u32 *bits, const u32 *before, u32
 
 // Connection c (taken by ticket, so in table order) = in[conns[c].off, + conns[c].len), len <= 65536.  Its rows go
 // to rows[base_c ...], base_c = the rows of the connections before it; at most row_cap rows in all, cut exactly where
-// gcra_resp_parse_throttle with max_frames = row_cap - base_c stops (stop 3).  Writes the connection's consumed,
+// the protocol's host walk (gcra_resp_parse_throttle, gcra_http_parse_throttle) with max_frames = row_cap - base_c
+// stops (stop 3).  Writes the connection's consumed,
 // n_frames and stop to outcome[c] (pinned host memory), {base_c, n_frames} to conn_rows[c]; the CTA of the last
 // connection writes the row count to *total and the segments' row counts of the batch view (segment s holds rows
 // [s << cap_shift, (s + 1) << cap_shift)).  status[0 .. n_conns) and *ticket are zero at launch.
+template <class P>
 __global__ void __launch_bounds__(RESP_THREADS, 1)
 resp_parse_kernel(const unsigned char *__restrict__ in, const gcra_resp_conn *__restrict__ conns, u32 n_conns,
                   u32 max_len, i64 now_ns, u32 row_cap, u64 k0, u64 k1, gcra_request *__restrict__ rows,
@@ -83,7 +118,7 @@ resp_parse_kernel(const unsigned char *__restrict__ in, const gcra_resp_conn *__
     unsigned char *smem = reinterpret_cast<unsigned char *>((reinterpret_cast<uintptr_t>(resp_dyn) + 15) & ~(uintptr_t)15);
     __shared__ u64 warp_sums[RESP_THREADS / 32];
     __shared__ u32 s_conn, s_base, s_n;
-    const RespSmem L(max_len);
+    const RespSmem L(max_len, P::CAND_PER_WORD);
     u32 *bits = reinterpret_cast<u32 *>(smem + L.bits_off);
     u32 *before = reinterpret_cast<u32 *>(smem + L.before_off);
     u32 *cand = reinterpret_cast<u32 *>(smem + L.cand_off);
@@ -110,35 +145,35 @@ resp_parse_kernel(const unsigned char *__restrict__ in, const gcra_resp_conn *__
         u32 b = 0;
         for (u32 j = 0; j < 32; j++) {
             const u32 p = w * 32 + j;
-            if (p < len && sb[p] == '*' && (p == 0 || sb[p - 1] == '\n')) b |= 1u << j;
+            if (p < len && P::candidate(sb, p, len)) b |= 1u << j;
         }
         bits[w] = b;
         mine += __popc(b);
     }
     u64 ncand;
-    u32 idx = (u32)resp_block_scan(mine, warp_sums, &ncand);
+    u32 idx = (u32)resp_block_scan<RESP_THREADS>(mine, warp_sums, &ncand);
     for (u32 w = w0; w < w1; w++) {
         before[w] = idx;
         for (u32 b = bits[w]; b; b &= b - 1) cand[idx++] = w * 32 + __ffs(b) - 1;
     }
     __syncthreads();
 
-    // every candidate parsed speculatively: its end, or why it is not a plain THROTTLE frame
+    // every candidate parsed speculatively: its end, or why it is not a plain frame
     for (u32 i = threadIdx.x; i < (u32)ncand; i += RESP_THREADS) {
         gcra_resp::Cursor cu = {sb + cand[i], sb + len};
         gcra_resp::Frame fr;
-        const int rc = gcra_resp::parse_frame(cu, fr);
+        const int rc = P::parse(cu, fr);
         cand[i] = rc ? (u32)rc << RESP_KIND_SHIFT : (u32)(cu.p - sb);
     }
     __syncthreads();
 
     if (threadIdx.x == 0) {
-        // The true frames: the chain from the segment start.  A frame ends with "\r\n", so the next one starts at a
-        // candidate exactly when its first byte is '*'.  cand[k] becomes the start of the k-th frame (k <= the index
-        // read, so nothing still to be read is overwritten).
+        // The true frames: the chain from the segment start; a position the protocol cannot start a frame at is a
+        // frame that is not plain.  cand[k] becomes the start of the k-th frame (k <= the index read, so nothing still
+        // to be read is overwritten).
         u32 n = 0, p = 0, why = 0;
         while (p < len) {
-            if (sb[p] != '*') { why = 2; break; }
+            if (!P::chain_start(sb, p, len)) { why = 2; break; }
             const u32 e = cand[resp_rank(bits, before, p)];
             if (e >> RESP_KIND_SHIFT) { why = e >> RESP_KIND_SHIFT; break; }
             cand[n++] = p;
@@ -175,7 +210,7 @@ resp_parse_kernel(const unsigned char *__restrict__ in, const gcra_resp_conn *__
     for (u32 k = threadIdx.x; k < take; k += RESP_THREADS) {
         gcra_resp::Cursor cu = {sb + cand[k], sb + len};
         gcra_resp::Frame fr;
-        gcra_resp::parse_frame(cu, fr);
+        P::parse(cu, fr);
         gcra_request r;
         r.key_hash = hash_key_engine(KeyBytes{fr.key}, fr.klen, k0, k1);
         r.max_burst = fr.a[0];
@@ -191,38 +226,40 @@ resp_parse_kernel(const unsigned char *__restrict__ in, const gcra_resp_conn *__
 // rows by ticket, measures its replies, finds the tile's offset by a look-back over the tiles before it, writes the
 // replies into shared memory and copies the tile's bytes out in one coalesced sweep.  row_off[i] = the offset of row
 // i's reply, row_off[*total] = all the bytes.  status[] and *ticket are zero at launch.
-__global__ void __launch_bounds__(RESP_THREADS)
+template <class P>
+__global__ void __launch_bounds__(P::REPLY_THREADS)
 resp_reply_kernel(const gcra_request *__restrict__ rows, const gcra_result *__restrict__ res, const u32 *total_p,
                   u64 *status, u32 *ticket, u64 *__restrict__ row_off, unsigned char *out) {
-    __shared__ __align__(16) char stage[RESP_THREADS * gcra_resp::REPLY_MAX];
-    __shared__ u64 warp_sums[RESP_THREADS / 32];
+    constexpr u32 T = P::REPLY_THREADS;
+    __shared__ __align__(16) char stage[T * P::REPLY_MAX];
+    __shared__ u64 warp_sums[T / 32];
     __shared__ u64 s_base;
     __shared__ u32 s_tile;
     if (threadIdx.x == 0) s_tile = atomicAdd(ticket, 1u);
     __syncthreads();
     const u32 tile = s_tile, total = *total_p;
-    if ((u64)tile * RESP_THREADS >= total) return;             // uniform over the CTA
-    const u32 row = tile * RESP_THREADS + threadIdx.x;
+    if ((u64)tile * T >= total) return;                        // uniform over the CTA
+    const u32 row = tile * T + threadIdx.x;
     gcra_request q{};
     gcra_result r{};
     gcra_resp::Count cnt;
     if (row < total) {
         q = rows[row];
         r = res[row];
-        gcra_resp::put_reply(cnt, q, r);
+        P::put_reply(cnt, q, r);
     }
     u64 tile_bytes;
-    const u64 at = resp_block_scan(cnt.n, warp_sums, &tile_bytes);
+    const u64 at = resp_block_scan<T>(cnt.n, warp_sums, &tile_bytes);
     if (threadIdx.x == 0) s_base = resp_look_back(status, tile, tile_bytes);
     if (row < total) {
         gcra_resp::Write o{stage + at};
-        gcra_resp::put_reply(o, q, r);
+        P::put_reply(o, q, r);
     }
     __syncthreads();
     const u64 base = s_base;
     if (row < total) row_off[row] = base + at;
     if (row + 1 == total) row_off[total] = base + at + cnt.n;
-    for (u32 i = threadIdx.x; i < (u32)tile_bytes; i += RESP_THREADS) out[base + i] = stage[i];
+    for (u32 i = threadIdx.x; i < (u32)tile_bytes; i += T) out[base + i] = stage[i];
 }
 
 // connection c's replies: rows [base_c, base_c + n_c) -> outcome[c].reply_off, reply_len
@@ -240,24 +277,39 @@ __global__ void resp_outcome_kernel(const uint2 *__restrict__ conn_rows, u32 n_c
 // ---- launches (gcra_resp.inc) ----
 cudaError_t resp_ring_setup() {
     cudaFuncAttributes a;
-    for (const void *k : {(const void *)resp_parse_kernel, (const void *)resp_reply_kernel, (const void *)resp_outcome_kernel}) {
+    for (const void *k : {(const void *)resp_parse_kernel<RespTraits>, (const void *)resp_reply_kernel<RespTraits>,
+                          (const void *)resp_parse_kernel<HttpTraits>, (const void *)resp_reply_kernel<HttpTraits>,
+                          (const void *)resp_outcome_kernel}) {
         const cudaError_t e = cudaFuncGetAttributes(&a, k);    // (loads the code now: see preload in gcra_b200.cu)
         if (e) return e;
     }
-    return cudaFuncSetAttribute(resp_parse_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                (int)RespSmem(RESP_MAX_CONN_BYTES).total);
+    cudaError_t e = cudaFuncSetAttribute(resp_parse_kernel<RespTraits>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         (int)RespSmem(RESP_MAX_CONN_BYTES, RespTraits::CAND_PER_WORD).total);
+    if (e) return e;
+    return cudaFuncSetAttribute(resp_parse_kernel<HttpTraits>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                (int)RespSmem(RESP_MAX_CONN_BYTES, HttpTraits::CAND_PER_WORD).total);
 }
 
-cudaError_t launch_resp_parse(const RespParse &a, cudaStream_t st) {
-    resp_parse_kernel<<<a.n_conns, RESP_THREADS, RespSmem(a.max_len).total, st>>>(
+template <class P>
+static cudaError_t launch_parse(const RespParse &a, cudaStream_t st) {
+    resp_parse_kernel<P><<<a.n_conns, RESP_THREADS, RespSmem(a.max_len, P::CAND_PER_WORD).total, st>>>(
         a.in, a.conns, a.n_conns, a.max_len, a.now_ns, a.row_cap, a.k0, a.k1, a.rows, a.status, a.ticket, a.conn_rows,
         a.outcome, a.total, a.seg_counts, a.nseg, a.cap_shift);
     return cudaGetLastError();
 }
 
-cudaError_t launch_resp_reply(u32 tiles, const gcra_request *rows, const gcra_result *res, const u32 *total, u64 *ctrl,
-                              u64 *row_off, unsigned char *out, cudaStream_t st) {
-    resp_reply_kernel<<<tiles, RESP_THREADS, 0, st>>>(rows, res, total, ctrl + 1, reinterpret_cast<u32 *>(ctrl), row_off, out);
+cudaError_t launch_resp_parse(const RespParse &a, cudaStream_t st) {
+    return a.proto == PROTO_HTTP ? launch_parse<HttpTraits>(a, st) : launch_parse<RespTraits>(a, st);
+}
+
+cudaError_t launch_resp_reply(RingProto proto, u32 tiles, const gcra_request *rows, const gcra_result *res,
+                              const u32 *total, u64 *ctrl, u64 *row_off, unsigned char *out, cudaStream_t st) {
+    if (proto == PROTO_HTTP)
+        resp_reply_kernel<HttpTraits><<<tiles, HttpTraits::REPLY_THREADS, 0, st>>>(rows, res, total, ctrl + 1,
+                                                                                 reinterpret_cast<u32 *>(ctrl), row_off, out);
+    else
+        resp_reply_kernel<RespTraits><<<tiles, RespTraits::REPLY_THREADS, 0, st>>>(rows, res, total, ctrl + 1,
+                                                                                 reinterpret_cast<u32 *>(ctrl), row_off, out);
     return cudaGetLastError();
 }
 

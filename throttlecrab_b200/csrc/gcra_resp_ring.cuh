@@ -11,18 +11,24 @@ namespace gcra {
 constexpr u32 RESP_THREADS = 256;
 constexpr u32 RESP_MAX_CONN_BYTES = 65536;     // MAX_BUFFER_SIZE of the reference's Redis transport (redis/mod.rs:83)
 
+// The ring's protocol: which grammar its parse kernel takes and which replies its reply kernel writes
+// (gcra_resp.cuh for RESP, gcra_http.cuh for HTTP); everything else about a ring slot is shared.
+enum RingProto : u32 { PROTO_NONE = 0, PROTO_RESP = 1, PROTO_HTTP = 2 };
+
 // The dynamic shared memory of resp_parse_kernel for connections of up to `max_len` bytes: the staged bytes (16
 // more for the segment's misalignment), one candidate bit per byte, the candidates before each 32-byte word, and one
-// word per candidate -- a candidate is a '*' that starts the segment or follows a '\n', so at most every other byte.
+// word per candidate, `cand_per_word` per 32 bytes.  A RESP candidate is a '*' that starts the segment or follows a
+// '\n', so at most every other byte (16); an HTTP candidate starts "POST ", which cannot overlap itself, or a prefix
+// of it at the segment's end, so at most len / 5 + 1 (7 per 32 bytes covers that for every len).
 struct RespSmem {
     u32 words, bytes_off, bits_off, before_off, cand_off, total;
-    __host__ __device__ explicit RespSmem(u32 max_len) {
+    __host__ __device__ explicit RespSmem(u32 max_len, u32 cand_per_word = 16) {
         words = (max_len + 31) / 32;
         bytes_off = 0;
         bits_off = (words * 32 + 16 + 15) & ~15u;
         before_off = bits_off + 4 * words;
         cand_off = before_off + 4 * words;
-        total = cand_off + 4 * (words * 16) + 16;   // (+16: the start rounded up to 16 bytes)
+        total = cand_off + 4 * (words * cand_per_word) + 16;   // (+16: the start rounded up to 16 bytes)
     }
 };
 
@@ -41,13 +47,17 @@ struct RespParse {
     gcra_resp_outcome *outcome;  // [n_conns] out (pinned host memory)
     u32 *total, *seg_counts;     // out: rows of the batch, rows of each segment
     u32 nseg, cap_shift;
+    RingProto proto;
 };
+
+// a protocol's rows per reply tile (the reply kernel stages a tile's replies in shared memory)
+constexpr u32 reply_tile_rows(RingProto p) { return p == PROTO_HTTP ? 128 : RESP_THREADS; }
 
 cudaError_t resp_ring_setup();   // once, before the first launch
 cudaError_t launch_resp_parse(const RespParse &a, cudaStream_t st);
-// ctrl: word 0 the ticket, then one status word per tile; all zero
-cudaError_t launch_resp_reply(u32 tiles, const gcra_request *rows, const gcra_result *res, const u32 *total, u64 *ctrl,
-                              u64 *row_off, unsigned char *out, cudaStream_t st);
+// ctrl: word 0 the ticket, then one status word per tile of reply_tile_rows(proto) rows; all zero
+cudaError_t launch_resp_reply(RingProto proto, u32 tiles, const gcra_request *rows, const gcra_result *res,
+                              const u32 *total, u64 *ctrl, u64 *row_off, unsigned char *out, cudaStream_t st);
 cudaError_t launch_resp_outcome(u32 n_conns, const uint2 *conn_rows, const u32 *total, const u64 *row_off,
                                 gcra_resp_outcome *outcome, cudaStream_t st);
 

@@ -389,8 +389,35 @@ def process_connections(buffers, limiter, now_ns, ring, slot=0):
     plain THROTTLE hands that one frame to the general parser, in list order; a THROTTLE among them is decided there
     and then, on its own.  That is the order in which decisions are made, so connections that share keys see each
     other's requests in that order."""
-    from . import RESP_MAX_CONN_BYTES
     now = int(now_ns)
+    parser = RespParser()
+
+    def general(data):
+        try:
+            r = parser.parse(data)
+        except RespError:
+            return 0, b"", 0, "error"
+        if r is None:
+            return None
+        plan = _plan_command(r[0])
+        if plan[0] == "throttle":
+            kb = plan[1].encode()
+            req = np.empty(1, REQ_DTYPE)
+            req[0] = (limiter.store.hash_key(kb), plan[2], plan[3], plan[4], plan[5], now)
+            res = limiter.rate_limit_batch(req)
+            return r[1], RespSerializer.serialize(_throttle_reply(res[0], plan[2], plan[5])), 1, \
+                "quit" if _is_quit(r[0]) else None
+        return r[1], RespSerializer.serialize(plan[1]), 0, "quit" if _is_quit(r[0]) else None
+
+    return ring_rounds(buffers, ring, slot, now, general)
+
+
+def ring_rounds(buffers, ring, slot, now, general):
+    """The round loop of process_connections, shared by the RESP and HTTP rings: GPU prefixes, then one call of
+    `general(bytes from the connection's position)` per connection that stopped at 2, in list order.  `general`
+    returns None (the frame is incomplete: the connection waits for more bytes) or (bytes consumed, reply bytes,
+    THROTTLE decisions, close), where a close other than None ends the connection."""
+    from . import RESP_MAX_CONN_BYTES
     datas = [bytes(b) for b in buffers]
     n = len(datas)
     for d in datas:
@@ -399,7 +426,6 @@ def process_connections(buffers, limiter, now_ns, ring, slot=0):
                                                                                        ring.in_capacity)))
     pos, n_thr, close = [0] * n, [0] * n, [None] * n
     out = [[] for _ in range(n)]
-    parser = RespParser()
     live = [c for c in range(n) if datas[c]]
     while live:
         stops, i = {}, 0
@@ -431,27 +457,14 @@ def process_connections(buffers, limiter, now_ns, ring, slot=0):
                 continue
             if stops[c] != 2:
                 continue                                   # the end of its bytes, or an incomplete frame
-            try:
-                r = parser.parse(datas[c][pos[c]:])
-            except RespError:
-                close[c] = "error"
+            g = general(datas[c][pos[c]:])
+            if g is None:
                 continue
-            if r is None:
-                continue
-            pos[c] += r[1]
-            plan = _plan_command(r[0])
-            if plan[0] == "throttle":
-                kb = plan[1].encode()
-                req = np.empty(1, REQ_DTYPE)
-                req[0] = (limiter.store.hash_key(kb), plan[2], plan[3], plan[4], plan[5], now)
-                res = limiter.rate_limit_batch(req)
-                out[c].append(RespSerializer.serialize(_throttle_reply(res[0], plan[2], plan[5])))
-                n_thr[c] += 1
-            else:
-                out[c].append(RespSerializer.serialize(plan[1]))
-            if _is_quit(r[0]):
-                close[c] = "quit"
-            elif pos[c] < len(datas[c]):
+            used, reply, k, close[c] = g
+            pos[c] += used
+            out[c].append(reply)
+            n_thr[c] += k
+            if close[c] is None and pos[c] < len(datas[c]):
                 nxt.append(c)
         live = nxt
     return [(b"".join(out[c]), pos[c], n_thr[c], close[c]) for c in range(n)]
