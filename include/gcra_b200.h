@@ -538,6 +538,87 @@ uint64_t gcra_http_format_replies(const gcra_request *req, const gcra_result *re
 int32_t gcra_http_ring_create(gcra_engine *h, uint32_t slots, uint32_t max_conns, uint64_t in_capacity,
                               uint32_t row_capacity);
 
+/* ---- batch gRPC ingest: Throttle calls on HTTP/2 connections -> request rows, results -> response frames ---------
+ * The gRPC transport's only call (transport/grpc.rs:148-193, proto/throttlecrab.proto) the way
+ * gcra_resp_parse_throttle takes RESP's hot command.  HTTP/2 keeps state per connection, so a connection is described
+ * by a gcra_grpc_conn: its bytes (for the ring: in the slot's input) and the state the walk needs.  The host's HPACK
+ * decoder owns the dynamic table: dyn_class[k] is the class byte of dynamic index 62 + k (gcra_grpc_header_class of
+ * the entry's name and value | gcra_grpc_header_class of its name alone << 4), and it rewrites them only when the
+ * general path changed the table.  send_window is the connection's send window, init_window the peer's
+ * SETTINGS_INITIAL_WINDOW_SIZE (every new stream's send window).
+ *
+ * gcra_grpc_parse_throttle walks `buf` once and writes one request row per plain call (the grammar: gcra_grpc.cuh):
+ * HEADERS on a new odd stream with an HPACK block of indexed fields and literals that leave the table as it is,
+ * :method POST, :path /throttlecrab.RateLimiter/Throttle and content-type application/grpc[+proto]; then one DATA
+ * frame with an uncompressed ThrottleRequest (END_STREAM, or an empty DATA(END_STREAM) after it); in between only
+ * WINDOW_UPDATE and at most one PING per walk.  The row is the message as prost decodes it: absent fields are 0 (so
+ * quantity defaults to 0, grpc.rs:158-165), int32 fields sign-extended, the key UTF-8.  stream_ids_out[k] is row k's
+ * stream.  WINDOW_UPDATE and PING frames between calls are taken on their own, so `consumed` can cover frames that
+ * make no row.  A call is taken only if the windows can take its response: the peer's stream window (init_window plus
+ * the stream's WINDOW_UPDATEs) and the connection's send window (after the WINDOW_UPDATEs so far) must hold the
+ * largest response DATA (GCRA_GRPC_RESPONSE_DATA_MAX) of this call and of every call before it.  *out receives
+ * consumed, n_frames (calls), stop (0 .. 3 as gcra_resp_parse_throttle), data_octets (the DATA octets taken: the
+ * connection owes the peer one WINDOW_UPDATE of that much), ping / ping_opaque (a PING that wants its ACK), and the
+ * state after the walk: last_stream and send_window before the responses are sent.  The caller subtracts the
+ * responses' data_sent from send_window and writes the WINDOW_UPDATE and PING ACK (at most 30 bytes) after the
+ * responses.  h (may be NULL) supplies the engine's key-hash seed.  GCRA_INTERNAL if n_dyn > 128 or len >= 2^32. */
+#define GCRA_GRPC_MAX_DYN 128u
+#define GCRA_GRPC_RESPONSE_DATA_MAX 51u
+typedef struct {
+    uint32_t off, len;                 /* bytes [off, off + len) of the ring slot's input (the ring only) */
+    uint32_t last_stream;              /* the highest client stream id seen so far */
+    int32_t send_window;               /* the connection's send window */
+    int32_t init_window;               /* the peer's SETTINGS_INITIAL_WINDOW_SIZE */
+    uint32_t n_dyn;                    /* dynamic-table entries, <= GCRA_GRPC_MAX_DYN */
+    uint8_t dyn_class[GCRA_GRPC_MAX_DYN];
+} gcra_grpc_conn;
+typedef struct {
+    uint32_t consumed, n_frames;
+    int32_t stop;
+    uint32_t data_octets;              /* DATA octets taken: owed to the peer as a connection WINDOW_UPDATE */
+    uint64_t reply_off, reply_len;     /* the ring: the connection's responses in gcra_resp_ring_replies */
+    uint32_t last_stream;              /* state out */
+    int32_t send_window;               /* state out, before this walk's responses */
+    uint32_t data_sent;                /* the ring: the DATA octets of the connection's responses */
+    uint32_t ping;                     /* 1: a PING was taken; ACK it with ping_opaque */
+    uint8_t ping_opaque[8];
+} gcra_grpc_outcome;
+int32_t gcra_grpc_parse_throttle(gcra_engine *h, const void *buf, uint64_t len, int64_t now_ns, uint32_t max_frames,
+                                 const gcra_grpc_conn *conn, gcra_request *req_out, uint32_t *stream_ids_out,
+                                 gcra_grpc_outcome *out);
+/* the responses of n decided calls, in order, row k on stream stream_ids[k]: HEADERS(:status 200, content-type:
+ * application/grpc), DATA(ThrottleResponse exactly as prost encodes it: fields in number order, zero values omitted,
+ * each field `as i32`, seconds as types.rs:87-97) and trailers HEADERS(END_STREAM, grpc-status: 0); for a decide
+ * error one trailers-only HEADERS(END_STREAM) with grpc-status: 13 and grpc-message "Rate limiter error: <the
+ * actor's error>", percent-encoded (grpc.rs:177-180).  No HPACK state: literals without indexing.  *data_sent (may be
+ * NULL) receives the DATA octets written.  Returns the bytes written, 0 if cap < GCRA_GRPC_REPLY_MAX n. */
+#define GCRA_GRPC_REPLY_MAX 168u
+uint64_t gcra_grpc_format_replies(const gcra_request *req, const gcra_result *res, const uint32_t *stream_ids,
+                                  uint32_t n, void *out, uint64_t cap, uint32_t *data_sent);
+/* the class of one decoded header field, or of a name alone (value NULL): 0 ignorable, 1 :method POST, 2 the
+ * Throttle :path, 3 :scheme, 4 :authority, 5 a gRPC content-type, 6 grpc-encoding: identity, 7 not plain; for a
+ * name alone, 8 .. 12 name a header whose value decides (:method, :path, content-type, grpc-encoding, te). */
+uint32_t gcra_grpc_header_class(const void *name, uint64_t name_len, const void *value, uint64_t value_len);
+/* The engine's ring as a gRPC ring: the RESP ring's slots, calls and validation (gcra_resp_ring_input, _submit,
+ * _replies, _rows, gcra_ring_wait, gcra_ring_poll), with gcra_grpc_ring_conns and gcra_grpc_ring_outcome in place of
+ * the RESP tables and row_capacity x GCRA_GRPC_REPLY_MAX bytes of replies.  Contract: for connection c, in table
+ * order, the GPU takes exactly what
+ *     gcra_grpc_parse_throttle(h, input + off_c, len_c, now_ns, row_capacity - base_c, &conns[c], rows + base_c, ...)
+ * takes -- the same rows, stream ids, consumed, n_frames, stop, data_octets, ping and state out -- base_c being the
+ * rows of the connections before c; its responses are the bytes gcra_grpc_format_replies writes for those rows, and
+ * data_sent their DATA octets.  What the caller does at each stop (after sending the responses, the WINDOW_UPDATE for
+ * data_octets and the PING ACK, and taking last_stream and send_window - data_sent as the connection's state):
+ *   0  every byte was taken: read more;
+ *   1  an incomplete frame or call follows at `consumed`: keep its bytes and read more;
+ *   2  a frame that is not plain follows at `consumed`: the general HTTP/2 path takes the connection from there and
+ *      keeps it until no stream is open; then it hands back the updated state (and class bytes);
+ *   3  the slot's row_capacity is used up: submit the rest again.
+ * Submit also refuses (GCRA_INTERNAL, nothing enqueued) a connection with n_dyn > GCRA_GRPC_MAX_DYN. */
+int32_t gcra_grpc_ring_create(gcra_engine *h, uint32_t slots, uint32_t max_conns, uint64_t in_capacity,
+                              uint32_t row_capacity);
+gcra_grpc_conn *gcra_grpc_ring_conns(gcra_engine *h, uint32_t slot);       /* pinned [max_conns], caller fills */
+gcra_grpc_outcome *gcra_grpc_ring_outcome(gcra_engine *h, uint32_t slot);  /* pinned [max_conns], valid after wait */
+
 #ifdef __cplusplus
 }
 #endif

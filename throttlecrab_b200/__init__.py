@@ -22,11 +22,12 @@ import numpy as np
 from . import _native
 from ._native import (REQ_DTYPE, RES_DTYPE, REQ16_DTYPE, RES16_DTYPE, POLICY_DTYPE, OK, NEGATIVE_QUANTITY,
                       INVALID_RATE_LIMIT, INTERNAL, RESP_CONN_DTYPE, RESP_OUTCOME_DTYPE, RESP_MAX_CONN_BYTES,
-                      RESP_REPLY_MAX, HTTP_REPLY_MAX)
+                      RESP_REPLY_MAX, HTTP_REPLY_MAX, GRPC_CONN_DTYPE, GRPC_OUTCOME_DTYPE, GRPC_REPLY_MAX,
+                      GRPC_MAX_DYN)
 
 __all__ = ["RateLimiter", "RateLimitResult", "Rate", "CellError", "NegativeQuantity", "InvalidRateLimit",
            "Internal", "AdaptiveStore", "PeriodicStore", "ProbabilisticStore", "ManualStore",
-           "hash_key", "key_ref", "pack_keys", "RespRing", "derive_params", "expand_results16", "REQ_DTYPE", "RES_DTYPE",
+           "hash_key", "key_ref", "pack_keys", "RespRing", "GrpcRing", "derive_params", "expand_results16", "REQ_DTYPE", "RES_DTYPE",
            "REQ16_DTYPE", "RES16_DTYPE", "POLICY_DTYPE"]
 
 NS = 1_000_000_000
@@ -553,27 +554,36 @@ class RespRing:
     decided, where it stopped, and where its replies lie in replies[slot].  Contract and stop codes: gcra_b200.h.
     An engine has one ring: this takes the place of Ring.
     protocol="http" makes it an HTTP ring (gcra_http_ring_create): POST /throttle requests in, HTTP responses out,
-    with the same calls and outcome table (HttpRing)."""
+    with the same calls and outcome table (HttpRing).  protocol="grpc" makes it a gRPC ring (GrpcRing)."""
+
+    # protocol -> (create call, connection table and its dtype, outcome table and its dtype, reply bytes per row)
+    _PROTOCOLS = {
+        "resp": ("gcra_resp_ring_create", "gcra_resp_ring_conns", RESP_CONN_DTYPE, "gcra_resp_ring_outcome",
+                 RESP_OUTCOME_DTYPE, RESP_REPLY_MAX),
+        "http": ("gcra_http_ring_create", "gcra_resp_ring_conns", RESP_CONN_DTYPE, "gcra_resp_ring_outcome",
+                 RESP_OUTCOME_DTYPE, HTTP_REPLY_MAX),
+        "grpc": ("gcra_grpc_ring_create", "gcra_grpc_ring_conns", GRPC_CONN_DTYPE, "gcra_grpc_ring_outcome",
+                 GRPC_OUTCOME_DTYPE, GRPC_REPLY_MAX),
+    }
 
     def __init__(self, limiter, slots, max_conns, in_capacity, row_capacity, protocol="resp"):
-        if protocol not in ("resp", "http"):
-            raise ValueError("protocol must be 'resp' or 'http'")
+        if protocol not in self._PROTOCOLS:
+            raise ValueError("protocol must be 'resp', 'http' or 'grpc'")
+        create, conns, conn_dt, outcome, outcome_dt, reply_max = self._PROTOCOLS[protocol]
         self.lim, self.store = limiter, limiter.store
         self._L, self._h = limiter._L, limiter._h
         self.slots, self.max_conns, self.in_capacity, self.row_capacity = slots, max_conns, in_capacity, row_capacity
         self.protocol = protocol
-        create = self._L.gcra_http_ring_create if protocol == "http" else self._L.gcra_resp_ring_create
-        self.store._check(create(self._h, slots, max_conns, in_capacity, row_capacity))
-        reply_max = HTTP_REPLY_MAX if protocol == "http" else RESP_REPLY_MAX
+        self.store._check(getattr(self._L, create)(self._h, slots, max_conns, in_capacity, row_capacity))
 
         def view(ptr, n, dt):
             return np.frombuffer((C.c_char * (n * np.dtype(dt).itemsize)).from_address(ptr), dtype=dt)
         L, h = self._L, self._h
         self.input = [view(L.gcra_resp_ring_input(h, s), in_capacity, np.uint8) for s in range(slots)]
-        self.conns = [view(L.gcra_resp_ring_conns(h, s), max_conns, RESP_CONN_DTYPE) for s in range(slots)]
+        self.conns = [view(getattr(L, conns)(h, s), max_conns, conn_dt) for s in range(slots)]
         self.replies = [view(L.gcra_resp_ring_replies(h, s), row_capacity * reply_max, np.uint8)
                         for s in range(slots)]
-        self.outcome = [view(L.gcra_resp_ring_outcome(h, s), max_conns, RESP_OUTCOME_DTYPE) for s in range(slots)]
+        self.outcome = [view(getattr(L, outcome)(h, s), max_conns, outcome_dt) for s in range(slots)]
 
     def submit(self, slot, n_conns, now=0):
         self.store._check(self._L.gcra_resp_ring_submit(self._h, slot, n_conns, _ns(now)))
@@ -594,3 +604,12 @@ class RespRing:
 def HttpRing(limiter, slots, max_conns, in_capacity, row_capacity):
     """The engine's ring as an HTTP ring: RespRing(..., protocol="http")."""
     return RespRing(limiter, slots, max_conns, in_capacity, row_capacity, protocol="http")
+
+
+def GrpcRing(limiter, slots, max_conns, in_capacity, row_capacity):
+    """The engine's ring as a gRPC ring (gcra_grpc_ring_create): HTTP/2 connections' bytes in, Throttle responses
+    out.  RespRing(..., protocol="grpc"): conns[slot] is GRPC_CONN_DTYPE (off, len and the connection's HTTP/2 state:
+    last_stream, send_window, init_window and the class bytes of its HPACK dynamic table) and outcome[slot] is
+    GRPC_OUTCOME_DTYPE (RespRing's fields, the DATA octets taken and sent, a PING to acknowledge and the state after
+    the walk).  Contract and stop codes: gcra_b200.h.  throttlecrab_b200.grpc_transport drives one."""
+    return RespRing(limiter, slots, max_conns, in_capacity, row_capacity, protocol="grpc")

@@ -29,6 +29,14 @@ RESP_CONN_DTYPE = np.dtype([("off", "<u4"), ("len", "<u4")])                    
 RESP_OUTCOME_DTYPE = np.dtype([("consumed", "<u4"), ("n_frames", "<u4"), ("stop", "<i4"), ("reserved", "<u4"),
                                ("reply_off", "<u8"), ("reply_len", "<u8")])         # gcra_resp_outcome
 RESP_MAX_CONN_BYTES, RESP_REPLY_MAX, HTTP_REPLY_MAX = 65536, 160, 256
+GRPC_MAX_DYN, GRPC_REPLY_MAX, GRPC_RESPONSE_DATA_MAX = 128, 168, 51
+GRPC_CONN_DTYPE = np.dtype([("off", "<u4"), ("len", "<u4"), ("last_stream", "<u4"), ("send_window", "<i4"),
+                            ("init_window", "<i4"), ("n_dyn", "<u4"), ("dyn_class", "u1", (GRPC_MAX_DYN,))])
+GRPC_OUTCOME_DTYPE = np.dtype([("consumed", "<u4"), ("n_frames", "<u4"), ("stop", "<i4"), ("data_octets", "<u4"),
+                               ("reply_off", "<u8"), ("reply_len", "<u8"), ("last_stream", "<u4"),
+                               ("send_window", "<i4"), ("data_sent", "<u4"), ("ping", "<u4"),
+                               ("ping_opaque", "u1", (8,))])                 # gcra_grpc_outcome
+assert GRPC_CONN_DTYPE.itemsize == 152 and GRPC_OUTCOME_DTYPE.itemsize == 56
 assert REQ_DTYPE.itemsize == 48 and RES_DTYPE.itemsize == 32 and REQ16_DTYPE.itemsize == 16
 assert RES16_DTYPE.itemsize == 16
 
@@ -163,6 +171,12 @@ SYMBOLS = {
     "gcra_http_parse_throttle": (_i32, [_vp, C.c_char_p, _u64, _i64, _u32, _vp, _pu64, C.POINTER(_u32), C.POINTER(_i32)]),
     "gcra_http_format_replies": (_u64, [_vp, _vp, _u32, _vp, _u64]),
     "gcra_http_ring_create": (_i32, [_vp, _u32, _u32, _u64, _u32]),
+    "gcra_grpc_parse_throttle": (_i32, [_vp, C.c_char_p, _u64, _i64, _u32, _vp, _vp, _vp, _vp]),
+    "gcra_grpc_format_replies": (_u64, [_vp, _vp, _vp, _u32, _vp, _u64, C.POINTER(_u32)]),
+    "gcra_grpc_header_class": (_u32, [C.c_char_p, _u64, C.c_char_p, _u64]),
+    "gcra_grpc_ring_create": (_i32, [_vp, _u32, _u32, _u64, _u32]),
+    "gcra_grpc_ring_conns": (_vp, [_vp, _u32]),
+    "gcra_grpc_ring_outcome": (_vp, [_vp, _u32]),
     "gcra_owner_of": (_u32, [_u64, _u32]),
     "gcra_route_partition": (_i32, [_vp, _u64, _vp, _u32, _vp, _vp, _vp, _vp]),
     "gcra_route_unpermute": (_i32, [_vp, _u64, _vp, _vp, _vp, _vp]),

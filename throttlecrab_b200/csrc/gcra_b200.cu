@@ -70,6 +70,12 @@ struct RingSlot {
     DevBuf<u64> row_off;                // [row_capacity + 1] where each row's reply starts
     DevBuf<u32> counts;                 // [0] rows of the batch, [1 + s] rows of segment s
     DevBuf<SegDesc> segs;
+    // gRPC ring (gcra_grpc_ring_create): its connection and outcome tables in place of h_conns / h_outcome, and each
+    // row's stream id
+    PinnedBuf<gcra_grpc_conn> h_gconns;
+    PinnedBuf<gcra_grpc_outcome> h_goutcome;
+    DevBuf<gcra_grpc_conn> d_gconns;
+    DevBuf<u32> stream_ids;
 };
 }  // namespace
 
@@ -336,7 +342,7 @@ struct gcra_engine {
     uint32_t ring_cap = 0;
     int ring_fmt = FMT_48_32;        // the slots' RowFmt (gcra_ring_create)
     uint64_t ring_key_cap = 0;       // bytes of every slot's key arena (0: the ring is not keyed)
-    RingProto ring_proto = PROTO_NONE;   // the ring is a RESP or HTTP ring (gcra_resp_ring_create, gcra_http_ring_create)
+    RingProto ring_proto = PROTO_NONE;   // a RESP, HTTP or gRPC ring (gcra_resp_ring_create, _http_, _grpc_)
     uint32_t resp_max_conns = 0, resp_nseg = 0, resp_shift = 0;
     uint64_t resp_in_cap = 0;
     DevBuf<unsigned char> d_keys;    // gcra_rate_limit_batch_keys: the caller's key arena on the device

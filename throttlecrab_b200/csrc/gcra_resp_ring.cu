@@ -1,4 +1,4 @@
-// gcra_resp_ring.cu -- the RESP and HTTP rings' kernels (gcra_resp_ring_*): connections' read buffers -> request
+// gcra_resp_ring.cu -- the RESP, HTTP and gRPC rings' kernels (gcra_resp_ring_*): connections' read buffers -> request
 // rows, and results -> reply bytes.  The frame grammar and the reply text are the host parser's own: gcra_resp.cuh for
 // RESP, gcra_http.cuh for HTTP, brought in by a protocol traits type that the parse and reply kernels are templates
 // over.  A translation unit of its own: the parse kernel's dynamic shared memory would pad every kernel's static
@@ -9,8 +9,11 @@
 //                        connections before it leave
 //   resp_reply_kernel    one thread per row: the reply bytes, packed in row order
 //   resp_outcome_kernel  one thread per connection: where its replies lie
+// and their gRPC counterparts (grpc_parse_kernel, grpc_reply_kernel, grpc_outcome_kernel), which carry each row's
+// stream id and each connection's HTTP/2 state.
 #include "gcra_resp_ring.cuh"
 #include "gcra_http.cuh"
+#include "gcra_grpc.cuh"
 
 namespace gcra {
 
@@ -274,20 +277,200 @@ __global__ void resp_outcome_kernel(const uint2 *__restrict__ conn_rows, u32 n_c
     outcome[c].reply_len = b - a;
 }
 
+// ---- gRPC ----
+// HTTP/2 has no byte that marks a frame start: the starts are the chain of 9-byte headers from offset 0.  So thread 0
+// hops that chain over the staged bytes and lists every whole frame (one shared-memory word per frame); then every
+// HEADERS and DATA frame is judged in parallel (gcra_grpc::headers_plain, data_plain: the stateless, costly part);
+// then thread 0 runs the host's walk (gcra_grpc::walk) over the list with the connection's state, looking the
+// judgements up instead of making them; the rows are decoded and hashed in parallel.  Connection c is taken by ticket,
+// so in table order; its rows go to rows[base_c ...] and their stream ids to stream_ids[base_c ...], cut exactly
+// where gcra_grpc_parse_throttle with max_frames = row_cap - base_c stops.  outcome[c] receives everything but the
+// reply fields and data_sent (grpc_outcome_kernel).  status[0 .. n_conns) and *ticket are zero at launch.
+__global__ void __launch_bounds__(RESP_THREADS, 1)
+grpc_parse_kernel(const unsigned char *__restrict__ in, const gcra_grpc_conn *__restrict__ conns, u32 n_conns,
+                  u32 max_len, i64 now_ns, u32 row_cap, u64 k0, u64 k1, gcra_request *__restrict__ rows,
+                  u32 *__restrict__ stream_ids, u64 *status, u32 *ticket, uint2 *__restrict__ conn_rows,
+                  gcra_grpc_outcome *outcome, u32 *__restrict__ total, u32 *__restrict__ seg_counts, u32 nseg,
+                  u32 cap_shift) {
+    extern __shared__ unsigned char grpc_dyn[];
+    unsigned char *smem = reinterpret_cast<unsigned char *>((reinterpret_cast<uintptr_t>(grpc_dyn) + 15) & ~(uintptr_t)15);
+    __shared__ unsigned char s_dyn[GCRA_GRPC_MAX_DYN];
+    __shared__ u32 s_conn, s_nf, s_base, s_n;
+    const GrpcSmem L(max_len);
+    u32 *frames = reinterpret_cast<u32 *>(smem + L.frames_off);
+    u32 *calls = reinterpret_cast<u32 *>(smem + L.calls_off);
+
+    if (threadIdx.x == 0) s_conn = atomicAdd(ticket, 1u);
+    __syncthreads();
+    const u32 c = s_conn;
+    const gcra_grpc_conn *cn = conns + c;
+    const u32 len = cn->len, n_dyn = cn->n_dyn;
+    const uintptr_t seg = reinterpret_cast<uintptr_t>(in) + cn->off;
+    const unsigned char *sb = smem + (seg & 15);
+    stage_key_span(seg, len, 0, len, threadIdx.x, RESP_THREADS,
+                   [&](uintptr_t g, u32 o) { *reinterpret_cast<uint4 *>(smem + o) = __ldg(reinterpret_cast<const uint4 *>(g)); },
+                   [&](uintptr_t g, u32 o) { smem[o] = *reinterpret_cast<const unsigned char *>(g); });
+    for (u32 i = threadIdx.x; i < n_dyn; i += RESP_THREADS) s_dyn[i] = cn->dyn_class[i];
+    __syncthreads();
+
+    if (threadIdx.x == 0) {                                    // the hop walk: every whole frame's start
+        u32 p = 0, nf = 0;
+        while (len - p >= 9) {
+            const u32 fl = (u32)sb[p] << 16 | (u32)sb[p + 1] << 8 | sb[p + 2];
+            if (fl > len - p - 9) break;
+            frames[nf++] = p;
+            p += 9 + fl;
+        }
+        s_nf = nf;
+    }
+    __syncthreads();
+    const u32 nf = s_nf;
+    for (u32 i = threadIdx.x; i < nf; i += RESP_THREADS) {   // the judgements: bit 31 of the frame's word
+        const u32 p = frames[i];
+        gcra_grpc::Hdr h;
+        bool ok = false;
+        if (!gcra_grpc::read_frame(sb, p, len, h)) {
+            gcra_resp::Frame fr;
+            if (h.type == gcra_grpc::F_HEADERS) ok = gcra_grpc::headers_plain(sb, p, h, s_dyn, n_dyn);
+            else if (h.type == gcra_grpc::F_DATA) ok = gcra_grpc::data_plain(sb, p, h, fr);
+        }
+        frames[i] = p | (u32)ok << 31;
+    }
+    __syncthreads();
+
+    if (threadIdx.x == 0) {
+        const gcra_grpc::Conn k{cn->last_stream, cn->send_window, cn->init_window, n_dyn, s_dyn};
+        auto plain = [&](u32 i, u32, const gcra_grpc::Hdr &) { return (frames[i] >> 31) != 0; };
+        auto call = [&](u32 j, u32 at) { calls[j] = at; };
+        gcra_grpc::State st;
+        gcra_grpc::WalkEnd e = gcra_grpc::walk(sb, len, k, 0xffffffffu, plain, call, st);
+        const u64 excl = resp_look_back(status, c, e.n);
+        const u32 base = excl < row_cap ? (u32)excl : row_cap, room = row_cap - base;
+        if (e.n >= room) e = gcra_grpc::walk(sb, len, k, room, plain, call, st);   // the cap decides the stop
+        s_base = base; s_n = e.n;
+        gcra_grpc_outcome o;
+        o.consumed = e.consumed;
+        o.n_frames = e.n;
+        o.stop = (int32_t)e.stop;
+        o.data_octets = st.data_octets;
+        o.reply_off = 0;
+        o.reply_len = 0;
+        o.last_stream = st.last_stream;
+        o.send_window = (int32_t)st.send_window;
+        o.data_sent = 0;
+        o.ping = st.ping;
+        for (int i = 0; i < 8; i++) o.ping_opaque[i] = st.ping ? st.opaque[i] : 0;
+        outcome[c] = o;
+        conn_rows[c] = make_uint2(base, e.n);
+        if (c == n_conns - 1) {
+            const u32 t = base + e.n;
+            *total = t;
+            for (u32 s = 0; s < nseg; s++) {
+                const u32 first = s << cap_shift;
+                seg_counts[s] = t <= first ? 0 : min(t - first, 1u << cap_shift);
+            }
+        }
+    }
+    __syncthreads();
+
+    const u32 base = s_base, take = s_n;
+    for (u32 j = threadIdx.x; j < take; j += RESP_THREADS) {
+        const u32 at = calls[j];
+        gcra_grpc::Hdr h;
+        gcra_grpc::read_frame(sb, at, len, h);
+        gcra_resp::Frame fr;
+        gcra_grpc::data_plain(sb, at, h, fr);
+        gcra_request r;
+        r.key_hash = hash_key_engine(KeyBytes{fr.key}, fr.klen, k0, k1);
+        r.max_burst = fr.a[0];
+        r.count_per_period = fr.a[1];
+        r.period = fr.a[2];
+        r.quantity = fr.a[3];
+        r.now_ns = now_ns;
+        rows[base + j] = r;
+        stream_ids[base + j] = h.sid;
+    }
+}
+
+// resp_reply_kernel for gRPC: row i's response goes on stream stream_ids[i]
+__global__ void __launch_bounds__(RESP_THREADS)
+grpc_reply_kernel(const gcra_request *__restrict__ rows, const gcra_result *__restrict__ res,
+                  const u32 *__restrict__ stream_ids, const u32 *total_p, u64 *status, u32 *ticket,
+                  u64 *__restrict__ row_off, unsigned char *out) {
+    constexpr u32 T = RESP_THREADS;
+    __shared__ __align__(16) char stage[T * gcra_grpc::REPLY_MAX];
+    __shared__ u64 warp_sums[T / 32];
+    __shared__ u64 s_base;
+    __shared__ u32 s_tile;
+    if (threadIdx.x == 0) s_tile = atomicAdd(ticket, 1u);
+    __syncthreads();
+    const u32 tile = s_tile, total = *total_p;
+    if ((u64)tile * T >= total) return;                        // uniform over the CTA
+    const u32 row = tile * T + threadIdx.x;
+    gcra_request q{};
+    gcra_result r{};
+    u32 sid = 0;
+    gcra_resp::Count cnt;
+    if (row < total) {
+        q = rows[row];
+        r = res[row];
+        sid = stream_ids[row];
+        gcra_grpc::put_reply(cnt, q, r, sid);
+    }
+    u64 tile_bytes;
+    const u64 at = resp_block_scan<T>(cnt.n, warp_sums, &tile_bytes);
+    if (threadIdx.x == 0) s_base = resp_look_back(status, tile, tile_bytes);
+    if (row < total) {
+        gcra_resp::Write o{stage + at};
+        gcra_grpc::put_reply(o, q, r, sid);
+    }
+    __syncthreads();
+    const u64 base = s_base;
+    if (row < total) row_off[row] = base + at;
+    if (row + 1 == total) row_off[total] = base + at + cnt.n;
+    for (u32 i = threadIdx.x; i < (u32)tile_bytes; i += T) out[base + i] = stage[i];
+}
+static_assert(RESP_THREADS * gcra_grpc::REPLY_MAX <= 48 * 1024, "the reply tile fits static shared memory");
+
+// one warp per connection: where its responses lie, and their DATA octets
+__global__ void grpc_outcome_kernel(const uint2 *__restrict__ conn_rows, u32 n_conns,
+                                    const gcra_request *__restrict__ rows, const gcra_result *__restrict__ res,
+                                    const u32 *total_p, const u64 *__restrict__ row_off, gcra_grpc_outcome *outcome) {
+    const u32 c = (blockIdx.x * blockDim.x + threadIdx.x) / 32, lane = threadIdx.x & 31;
+    if (c >= n_conns) return;                                  // uniform over the warp
+    const u32 total = *total_p;
+    const uint2 br = conn_rows[c];
+    const u32 lo = min(br.x, total), hi = min(br.x + br.y, total);
+    u32 sent = 0;
+    for (u32 i = lo + lane; i < hi; i += 32) sent += gcra_grpc::data_len(rows[i], res[i]);
+#pragma unroll
+    for (u32 o = 16; o; o >>= 1) sent += __shfl_xor_sync(0xffffffffu, sent, o);
+    if (lane == 0) {
+        const u64 a = total ? row_off[lo] : 0, b = total ? row_off[hi] : 0;
+        outcome[c].reply_off = a;
+        outcome[c].reply_len = b - a;
+        outcome[c].data_sent = sent;
+    }
+}
+
 // ---- launches (gcra_resp.inc) ----
 cudaError_t resp_ring_setup() {
     cudaFuncAttributes a;
     for (const void *k : {(const void *)resp_parse_kernel<RespTraits>, (const void *)resp_reply_kernel<RespTraits>,
                           (const void *)resp_parse_kernel<HttpTraits>, (const void *)resp_reply_kernel<HttpTraits>,
-                          (const void *)resp_outcome_kernel}) {
+                          (const void *)resp_outcome_kernel, (const void *)grpc_parse_kernel,
+                          (const void *)grpc_reply_kernel, (const void *)grpc_outcome_kernel}) {
         const cudaError_t e = cudaFuncGetAttributes(&a, k);    // (loads the code now: see preload in gcra_b200.cu)
         if (e) return e;
     }
     cudaError_t e = cudaFuncSetAttribute(resp_parse_kernel<RespTraits>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                          (int)RespSmem(RESP_MAX_CONN_BYTES, RespTraits::CAND_PER_WORD).total);
     if (e) return e;
-    return cudaFuncSetAttribute(resp_parse_kernel<HttpTraits>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                (int)RespSmem(RESP_MAX_CONN_BYTES, HttpTraits::CAND_PER_WORD).total);
+    e = cudaFuncSetAttribute(resp_parse_kernel<HttpTraits>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                             (int)RespSmem(RESP_MAX_CONN_BYTES, HttpTraits::CAND_PER_WORD).total);
+    if (e) return e;
+    return cudaFuncSetAttribute(grpc_parse_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                (int)GrpcSmem(RESP_MAX_CONN_BYTES).total);
 }
 
 template <class P>
@@ -317,6 +500,26 @@ cudaError_t launch_resp_outcome(u32 n_conns, const uint2 *conn_rows, const u32 *
                                 gcra_resp_outcome *outcome, cudaStream_t st) {
     resp_outcome_kernel<<<(n_conns + RESP_THREADS - 1) / RESP_THREADS, RESP_THREADS, 0, st>>>(conn_rows, n_conns, total,
                                                                                             row_off, outcome);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_grpc_parse(const GrpcParse &a, cudaStream_t st) {
+    grpc_parse_kernel<<<a.n_conns, RESP_THREADS, GrpcSmem(a.max_len).total, st>>>(
+        a.in, a.conns, a.n_conns, a.max_len, a.now_ns, a.row_cap, a.k0, a.k1, a.rows, a.stream_ids, a.status, a.ticket,
+        a.conn_rows, a.outcome, a.total, a.seg_counts, a.nseg, a.cap_shift);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_grpc_reply(u32 tiles, const gcra_request *rows, const gcra_result *res, const u32 *stream_ids,
+                              const u32 *total, u64 *ctrl, u64 *row_off, unsigned char *out, cudaStream_t st) {
+    grpc_reply_kernel<<<tiles, RESP_THREADS, 0, st>>>(rows, res, stream_ids, total, ctrl + 1,
+                                                     reinterpret_cast<u32 *>(ctrl), row_off, out);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_grpc_outcome(u32 n_conns, const uint2 *conn_rows, const gcra_request *rows, const gcra_result *res,
+                                const u32 *total, const u64 *row_off, gcra_grpc_outcome *outcome, cudaStream_t st) {
+    grpc_outcome_kernel<<<(n_conns + 7) / 8, 256, 0, st>>>(conn_rows, n_conns, rows, res, total, row_off, outcome);
     return cudaGetLastError();
 }
 

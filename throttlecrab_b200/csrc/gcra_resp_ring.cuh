@@ -12,8 +12,9 @@ constexpr u32 RESP_THREADS = 256;
 constexpr u32 RESP_MAX_CONN_BYTES = 65536;     // MAX_BUFFER_SIZE of the reference's Redis transport (redis/mod.rs:83)
 
 // The ring's protocol: which grammar its parse kernel takes and which replies its reply kernel writes
-// (gcra_resp.cuh for RESP, gcra_http.cuh for HTTP); everything else about a ring slot is shared.
-enum RingProto : u32 { PROTO_NONE = 0, PROTO_RESP = 1, PROTO_HTTP = 2 };
+// (gcra_resp.cuh for RESP, gcra_http.cuh for HTTP, gcra_grpc.cuh for gRPC); everything else about a ring slot is
+// shared.  A gRPC ring has its own connection and outcome tables (gcra_grpc_conn, gcra_grpc_outcome).
+enum RingProto : u32 { PROTO_NONE = 0, PROTO_RESP = 1, PROTO_HTTP = 2, PROTO_GRPC = 3 };
 
 // The dynamic shared memory of resp_parse_kernel for connections of up to `max_len` bytes: the staged bytes (16
 // more for the segment's misalignment), one candidate bit per byte, the candidates before each 32-byte word, and one
@@ -52,6 +53,41 @@ struct RespParse {
 
 // a protocol's rows per reply tile (the reply kernel stages a tile's replies in shared memory)
 constexpr u32 reply_tile_rows(RingProto p) { return p == PROTO_HTTP ? 128 : RESP_THREADS; }
+
+// The dynamic shared memory of grpc_parse_kernel for connections of up to `max_len` bytes: the staged bytes (16 more
+// for the segment's misalignment), one word per frame (a frame has at least 9 bytes) and one per call (a call has at
+// least gcra_grpc::MIN_CALL_BYTES = 26).
+struct GrpcSmem {
+    u32 frames_off, calls_off, total;
+    __host__ __device__ explicit GrpcSmem(u32 max_len) {
+        frames_off = (max_len + 16 + 15) & ~15u;
+        calls_off = frames_off + 4 * (max_len / 9 + 1);
+        total = calls_off + 4 * (max_len / 26 + 1) + 16;        // (+16: the start rounded up to 16 bytes)
+    }
+};
+
+// grpc_parse_kernel's arguments: RespParse's, with the gRPC connection and outcome tables and the rows' stream ids
+struct GrpcParse {
+    const unsigned char *in;
+    const gcra_grpc_conn *conns;
+    u32 n_conns, max_len;
+    i64 now_ns;
+    u32 row_cap;
+    u64 k0, k1;
+    gcra_request *rows;
+    u32 *stream_ids;             // [row_capacity] out
+    u64 *status;
+    u32 *ticket;
+    uint2 *conn_rows;
+    gcra_grpc_outcome *outcome;  // [n_conns] out (pinned host memory)
+    u32 *total, *seg_counts;
+    u32 nseg, cap_shift;
+};
+cudaError_t launch_grpc_parse(const GrpcParse &a, cudaStream_t st);
+cudaError_t launch_grpc_reply(u32 tiles, const gcra_request *rows, const gcra_result *res, const u32 *stream_ids,
+                              const u32 *total, u64 *ctrl, u64 *row_off, unsigned char *out, cudaStream_t st);
+cudaError_t launch_grpc_outcome(u32 n_conns, const uint2 *conn_rows, const gcra_request *rows, const gcra_result *res,
+                                const u32 *total, const u64 *row_off, gcra_grpc_outcome *outcome, cudaStream_t st);
 
 cudaError_t resp_ring_setup();   // once, before the first launch
 cudaError_t launch_resp_parse(const RespParse &a, cudaStream_t st);
