@@ -453,7 +453,8 @@ uint64_t gcra_resp_format_replies(const gcra_request *req, const gcra_result *re
                                   uint64_t cap);
 
 /* ---- RESP ring: connections' read buffers in, reply bytes out -------------------------------------------------
- * The engine's ring (one per engine: it takes the place of gcra_ring_create), whose slots carry bytes instead of
+ * The engine's ring (one per engine: it takes the place of gcra_ring_create; the mixed ring below serves RESP, HTTP
+ * and gRPC connections from one ring), whose slots carry bytes instead of
  * rows.  The caller reads its sockets into gcra_resp_ring_input(h, slot) and describes each connection's bytes in
  * gcra_resp_ring_conns(h, slot)[c] = {off, len}, len <= GCRA_RESP_MAX_CONN_BYTES (the reference's MAX_BUFFER_SIZE,
  * redis/mod.rs:83).  Submit parses every connection on the GPU, decides the rows as one batch and writes the replies;
@@ -618,6 +619,50 @@ int32_t gcra_grpc_ring_create(gcra_engine *h, uint32_t slots, uint32_t max_conns
                               uint32_t row_capacity);
 gcra_grpc_conn *gcra_grpc_ring_conns(gcra_engine *h, uint32_t slot);       /* pinned [max_conns], caller fills */
 gcra_grpc_outcome *gcra_grpc_ring_outcome(gcra_engine *h, uint32_t slot);  /* pinned [max_conns], valid after wait */
+
+/* ---- mixed ring: RESP, HTTP and gRPC connections in one slot, decided as one batch --------------------------------
+ * The engine's ring as all three at once, so that one server serves every transport against one table, one submit
+ * per tick: every connection parsed in one launch, whatever its protocol, all rows decided as ONE batch, all replies
+ * written in one launch.  The caller describes connection c in gcra_mixed_ring_conns(h, slot)[c]: its bytes in
+ * gcra_resp_ring_input, its protocol and, for a gRPC connection, grpc_state = k, the row of gcra_grpc_ring_conns
+ * (h, slot) that holds its HTTP/2 state (whose off and len are not read) and of gcra_grpc_ring_outcome(h, slot) that
+ * receives its outcome.  Every other call is the rings' own: gcra_resp_ring_input, _submit, _replies, _outcome, _rows,
+ * gcra_ring_wait and gcra_ring_poll.
+ *
+ * Contract: for connection c, in table order, with base_c the rows of the connections before it, the GPU takes
+ * exactly what its protocol's host walk takes at max_frames = row_capacity - base_c:
+ *     GCRA_PROTO_RESP  gcra_resp_parse_throttle,
+ *     GCRA_PROTO_HTTP  gcra_http_parse_throttle,
+ *     GCRA_PROTO_GRPC  gcra_grpc_parse_throttle with gcra_grpc_ring_conns(h, slot)[grpc_state]
+ * -- the same rows (key hashes under the engine's seed, so one key string is one entry from every transport),
+ * consumed, n_frames and stop.  All rows of a submit form one batch, in table order.  After wait,
+ * gcra_resp_ring_outcome(h, slot)[c] gives every connection's consumed, n_frames, stop, reply_off and reply_len; its
+ * replies are the bytes its protocol's formatter writes for its rows (gcra_resp_format_replies,
+ * gcra_http_format_replies, or gcra_grpc_format_replies with the stream ids).  gcra_grpc_ring_outcome(h, slot)[k] gets
+ * everything a gRPC ring writes for the gRPC connection whose grpc_state is k (data_octets, data_sent, ping, the state
+ * out).  Stop codes are each protocol's ring's.  A stop 3 in any connection leaves no rows to every later connection,
+ * whatever its protocol: a RESP or HTTP connection with bytes stops with 3, and a gRPC connection where its walk at
+ * max_frames 0 stops (3 at its first call, or 2 at a frame that is not plain before it).  The replies area holds
+ * row_capacity x GCRA_HTTP_REPLY_MAX bytes (the longest reply).
+ *
+ * Submit validates everything before it enqueues anything, and returns GCRA_INTERNAL leaving the engine usable, for:
+ * a protocol outside 1 .. 3; grpc_state values that are not 0, 1, 2, ... in table order among the gRPC connections;
+ * a gRPC state with n_dyn > GCRA_GRPC_MAX_DYN; n_conns > max_conns; a connection past in_capacity or longer than
+ * GCRA_RESP_MAX_CONN_BYTES; a slot in flight.  gcra_ring_submit refuses a mixed ring, gcra_resp_ring_conns returns
+ * NULL on it, and a second ring create on the engine is refused as always. */
+#define GCRA_PROTO_RESP 1u
+#define GCRA_PROTO_HTTP 2u
+#define GCRA_PROTO_GRPC 3u
+typedef struct {
+    uint32_t off, len;                 /* bytes [off, off + len) of the slot's input, len <= GCRA_RESP_MAX_CONN_BYTES */
+    uint32_t protocol;                 /* GCRA_PROTO_* */
+    uint32_t grpc_state;               /* gRPC only: its row in gcra_grpc_ring_conns / gcra_grpc_ring_outcome */
+} gcra_mixed_conn;
+/* slots x (in_capacity bytes of input (1 .. 2^32), max_conns connections (1 .. 65536) of any protocol, as many gRPC
+ * state and outcome rows, row_capacity rows (1 .. max_batch) and row_capacity x GCRA_HTTP_REPLY_MAX bytes of replies) */
+int32_t gcra_mixed_ring_create(gcra_engine *h, uint32_t slots, uint32_t max_conns, uint64_t in_capacity,
+                               uint32_t row_capacity);
+gcra_mixed_conn *gcra_mixed_ring_conns(gcra_engine *h, uint32_t slot);     /* pinned [max_conns], caller fills */
 
 #ifdef __cplusplus
 }

@@ -23,11 +23,11 @@ from . import _native
 from ._native import (REQ_DTYPE, RES_DTYPE, REQ16_DTYPE, RES16_DTYPE, POLICY_DTYPE, OK, NEGATIVE_QUANTITY,
                       INVALID_RATE_LIMIT, INTERNAL, RESP_CONN_DTYPE, RESP_OUTCOME_DTYPE, RESP_MAX_CONN_BYTES,
                       RESP_REPLY_MAX, HTTP_REPLY_MAX, GRPC_CONN_DTYPE, GRPC_OUTCOME_DTYPE, GRPC_REPLY_MAX,
-                      GRPC_MAX_DYN)
+                      GRPC_MAX_DYN, PROTO_RESP, PROTO_HTTP, PROTO_GRPC, MIXED_CONN_DTYPE)
 
 __all__ = ["RateLimiter", "RateLimitResult", "Rate", "CellError", "NegativeQuantity", "InvalidRateLimit",
            "Internal", "AdaptiveStore", "PeriodicStore", "ProbabilisticStore", "ManualStore",
-           "hash_key", "key_ref", "pack_keys", "RespRing", "GrpcRing", "derive_params", "expand_results16", "REQ_DTYPE", "RES_DTYPE",
+           "hash_key", "key_ref", "pack_keys", "RespRing", "GrpcRing", "MixedRing", "derive_params", "expand_results16", "REQ_DTYPE", "RES_DTYPE",
            "REQ16_DTYPE", "RES16_DTYPE", "POLICY_DTYPE"]
 
 NS = 1_000_000_000
@@ -554,7 +554,8 @@ class RespRing:
     decided, where it stopped, and where its replies lie in replies[slot].  Contract and stop codes: gcra_b200.h.
     An engine has one ring: this takes the place of Ring.
     protocol="http" makes it an HTTP ring (gcra_http_ring_create): POST /throttle requests in, HTTP responses out,
-    with the same calls and outcome table (HttpRing).  protocol="grpc" makes it a gRPC ring (GrpcRing)."""
+    with the same calls and outcome table (HttpRing).  protocol="grpc" makes it a gRPC ring (GrpcRing), and
+    protocol="mixed" a ring that takes all three in one slot (MixedRing)."""
 
     # protocol -> (create call, connection table and its dtype, outcome table and its dtype, reply bytes per row)
     _PROTOCOLS = {
@@ -564,11 +565,13 @@ class RespRing:
                  RESP_OUTCOME_DTYPE, HTTP_REPLY_MAX),
         "grpc": ("gcra_grpc_ring_create", "gcra_grpc_ring_conns", GRPC_CONN_DTYPE, "gcra_grpc_ring_outcome",
                  GRPC_OUTCOME_DTYPE, GRPC_REPLY_MAX),
+        "mixed": ("gcra_mixed_ring_create", "gcra_mixed_ring_conns", MIXED_CONN_DTYPE, "gcra_resp_ring_outcome",
+                  RESP_OUTCOME_DTYPE, HTTP_REPLY_MAX),
     }
 
     def __init__(self, limiter, slots, max_conns, in_capacity, row_capacity, protocol="resp"):
         if protocol not in self._PROTOCOLS:
-            raise ValueError("protocol must be 'resp', 'http' or 'grpc'")
+            raise ValueError("protocol must be 'resp', 'http', 'grpc' or 'mixed'")
         create, conns, conn_dt, outcome, outcome_dt, reply_max = self._PROTOCOLS[protocol]
         self.lim, self.store = limiter, limiter.store
         self._L, self._h = limiter._L, limiter._h
@@ -584,6 +587,10 @@ class RespRing:
         self.replies = [view(L.gcra_resp_ring_replies(h, s), row_capacity * reply_max, np.uint8)
                         for s in range(slots)]
         self.outcome = [view(getattr(L, outcome)(h, s), max_conns, outcome_dt) for s in range(slots)]
+        if protocol == "mixed":                            # the gRPC connections' state and outcome rows
+            self.grpc_conns = [view(L.gcra_grpc_ring_conns(h, s), max_conns, GRPC_CONN_DTYPE) for s in range(slots)]
+            self.grpc_outcome = [view(L.gcra_grpc_ring_outcome(h, s), max_conns, GRPC_OUTCOME_DTYPE)
+                                 for s in range(slots)]
 
     def submit(self, slot, n_conns, now=0):
         self.store._check(self._L.gcra_resp_ring_submit(self._h, slot, n_conns, _ns(now)))
@@ -613,3 +620,14 @@ def GrpcRing(limiter, slots, max_conns, in_capacity, row_capacity):
     GRPC_OUTCOME_DTYPE (RespRing's fields, the DATA octets taken and sent, a PING to acknowledge and the state after
     the walk).  Contract and stop codes: gcra_b200.h.  throttlecrab_b200.grpc_transport drives one."""
     return RespRing(limiter, slots, max_conns, in_capacity, row_capacity, protocol="grpc")
+
+
+def MixedRing(limiter, slots, max_conns, in_capacity, row_capacity):
+    """The engine's ring as a mixed ring (gcra_mixed_ring_create): RESP, HTTP and gRPC connections in one slot, all
+    their rows decided as one batch on the engine's one table.  RespRing(..., protocol="mixed"): conns[slot] is
+    MIXED_CONN_DTYPE (off, len, protocol PROTO_RESP / PROTO_HTTP / PROTO_GRPC and, for gRPC, grpc_state: 0, 1, 2, ...
+    in table order among the gRPC connections); grpc_conns[slot][grpc_state] (GRPC_CONN_DTYPE, off and len unused)
+    holds a gRPC connection's HTTP/2 state and grpc_outcome[slot][grpc_state] (GRPC_OUTCOME_DTYPE) receives its
+    outcome; outcome[slot] (RESP_OUTCOME_DTYPE) has every connection's.  replies[slot] has HTTP_REPLY_MAX bytes per
+    row.  Contract: gcra_b200.h.  throttlecrab_b200.mixed drives one."""
+    return RespRing(limiter, slots, max_conns, in_capacity, row_capacity, protocol="mixed")

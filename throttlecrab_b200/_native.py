@@ -36,7 +36,10 @@ GRPC_OUTCOME_DTYPE = np.dtype([("consumed", "<u4"), ("n_frames", "<u4"), ("stop"
                                ("reply_off", "<u8"), ("reply_len", "<u8"), ("last_stream", "<u4"),
                                ("send_window", "<i4"), ("data_sent", "<u4"), ("ping", "<u4"),
                                ("ping_opaque", "u1", (8,))])                 # gcra_grpc_outcome
-assert GRPC_CONN_DTYPE.itemsize == 152 and GRPC_OUTCOME_DTYPE.itemsize == 56
+PROTO_RESP, PROTO_HTTP, PROTO_GRPC = 1, 2, 3                                       # GCRA_PROTO_*
+MIXED_CONN_DTYPE = np.dtype([("off", "<u4"), ("len", "<u4"), ("protocol", "<u4"),
+                             ("grpc_state", "<u4")])                                # gcra_mixed_conn
+assert GRPC_CONN_DTYPE.itemsize == 152 and GRPC_OUTCOME_DTYPE.itemsize == 56 and MIXED_CONN_DTYPE.itemsize == 16
 assert REQ_DTYPE.itemsize == 48 and RES_DTYPE.itemsize == 32 and REQ16_DTYPE.itemsize == 16
 assert RES16_DTYPE.itemsize == 16
 
@@ -177,6 +180,8 @@ SYMBOLS = {
     "gcra_grpc_ring_create": (_i32, [_vp, _u32, _u32, _u64, _u32]),
     "gcra_grpc_ring_conns": (_vp, [_vp, _u32]),
     "gcra_grpc_ring_outcome": (_vp, [_vp, _u32]),
+    "gcra_mixed_ring_create": (_i32, [_vp, _u32, _u32, _u64, _u32]),
+    "gcra_mixed_ring_conns": (_vp, [_vp, _u32]),
     "gcra_owner_of": (_u32, [_u64, _u32]),
     "gcra_route_partition": (_i32, [_vp, _u64, _vp, _u32, _vp, _vp, _vp, _vp]),
     "gcra_route_unpermute": (_i32, [_vp, _u64, _vp, _vp, _vp, _vp]),

@@ -76,6 +76,11 @@ struct RingSlot {
     PinnedBuf<gcra_grpc_outcome> h_goutcome;
     DevBuf<gcra_grpc_conn> d_gconns;
     DevBuf<u32> stream_ids;
+    // mixed ring (gcra_mixed_ring_create): its connection table, with h_outcome and the gRPC tables above, and each
+    // row's protocol
+    PinnedBuf<gcra_mixed_conn> h_mconns;
+    DevBuf<gcra_mixed_conn> d_mconns;
+    DevBuf<unsigned char> row_proto;
 };
 }  // namespace
 
@@ -342,7 +347,7 @@ struct gcra_engine {
     uint32_t ring_cap = 0;
     int ring_fmt = FMT_48_32;        // the slots' RowFmt (gcra_ring_create)
     uint64_t ring_key_cap = 0;       // bytes of every slot's key arena (0: the ring is not keyed)
-    RingProto ring_proto = PROTO_NONE;   // a RESP, HTTP or gRPC ring (gcra_resp_ring_create, _http_, _grpc_)
+    RingProto ring_proto = PROTO_NONE;   // a RESP, HTTP, gRPC or mixed ring (gcra_resp_ring_create, _http_, _grpc_, _mixed_)
     uint32_t resp_max_conns = 0, resp_nseg = 0, resp_shift = 0;
     uint64_t resp_in_cap = 0;
     DevBuf<unsigned char> d_keys;    // gcra_rate_limit_batch_keys: the caller's key arena on the device
@@ -1584,7 +1589,7 @@ gcra_result16 *gcra_ring_results16(gcra_engine *h, uint32_t slot) {
 static int ring_submit(gcra_engine *h, uint32_t slot, uint32_t n, int64_t now_ns, const uint64_t *keys_len) {
     CK(cudaSetDevice(h->device));
     if (slot >= h->ring.size() || n > h->ring_cap) { h->err = "bad ring slot / size"; return GCRA_INTERNAL; }
-    if (h->ring_proto) { h->err = "a RESP or HTTP ring takes gcra_resp_ring_submit"; return GCRA_INTERNAL; }
+    if (h->ring_proto) { h->err = "a RESP, HTTP, gRPC or mixed ring takes gcra_resp_ring_submit"; return GCRA_INTERNAL; }
     if (keys_len && *keys_len > h->ring_key_cap) { h->err = "keys_len larger than the ring's key_capacity"; return GCRA_INTERNAL; }
     RingSlot &s = h->ring[slot];
     if (s.in_flight) { h->err = "ring slot still in flight"; return GCRA_INTERNAL; }

@@ -10,7 +10,9 @@
 //   resp_reply_kernel    one thread per row: the reply bytes, packed in row order
 //   resp_outcome_kernel  one thread per connection: where its replies lie
 // and their gRPC counterparts (grpc_parse_kernel, grpc_reply_kernel, grpc_outcome_kernel), which carry each row's
-// stream id and each connection's HTTP/2 state.
+// stream id and each connection's HTTP/2 state.  The mixed ring's kernels (mixed_parse_kernel, mixed_reply_kernel,
+// mixed_outcome_kernel) take connections of all three protocols in one slot: the parse kernel runs the same parse
+// bodies (resp_parse_conn, grpc_parse_conn), the reply kernel the same reply writers.
 #include "gcra_resp_ring.cuh"
 #include "gcra_http.cuh"
 #include "gcra_grpc.cuh"
@@ -109,31 +111,24 @@ __device__ __forceinline__ u32 resp_rank(const u32 *bits, const u32 *before, u32
 // n_frames and stop to outcome[c] (pinned host memory), {base_c, n_frames} to conn_rows[c]; the CTA of the last
 // connection writes the row count to *total and the segments' row counts of the batch view (segment s holds rows
 // [s << cap_shift, (s + 1) << cap_shift)).  status[0 .. n_conns) and *ticket are zero at launch.
+// The body of resp_parse_kernel for connection c = in[off, + len) (a CTA's whole work; mixed_parse_kernel runs it
+// too): smem is the dynamic shared memory rounded up to 16 bytes, laid out as RespSmem(max_len, P::CAND_PER_WORD),
+// len <= max_len.  Returns {base_c, the rows taken} to every thread.
 template <class P>
-__global__ void __launch_bounds__(RESP_THREADS, 1)
-resp_parse_kernel(const unsigned char *__restrict__ in, const gcra_resp_conn *__restrict__ conns, u32 n_conns,
-                  u32 max_len, i64 now_ns, u32 row_cap, u64 k0, u64 k1, gcra_request *__restrict__ rows,
-                  u64 *status, u32 *ticket, uint2 *__restrict__ conn_rows, gcra_resp_outcome *outcome,
-                  u32 *__restrict__ total, u32 *__restrict__ seg_counts, u32 nseg, u32 cap_shift) {
-    // (no alignment is declared for the dynamic shared memory: that would pad every kernel's; RespSmem leaves room to
-    // round its start up to 16 bytes)
-    extern __shared__ unsigned char resp_dyn[];
-    unsigned char *smem = reinterpret_cast<unsigned char *>((reinterpret_cast<uintptr_t>(resp_dyn) + 15) & ~(uintptr_t)15);
+__device__ __forceinline__ uint2
+resp_parse_conn(unsigned char *smem, u32 c, u32 off, u32 len, const unsigned char *__restrict__ in, u32 n_conns,
+                u32 max_len, i64 now_ns, u32 row_cap, u64 k0, u64 k1, gcra_request *__restrict__ rows, u64 *status,
+                uint2 *__restrict__ conn_rows, gcra_resp_outcome *outcome, u32 *__restrict__ total,
+                u32 *__restrict__ seg_counts, u32 nseg, u32 cap_shift) {
     __shared__ u64 warp_sums[RESP_THREADS / 32];
-    __shared__ u32 s_conn, s_base, s_n;
+    __shared__ u32 s_base, s_n;
     const RespSmem L(max_len, P::CAND_PER_WORD);
     u32 *bits = reinterpret_cast<u32 *>(smem + L.bits_off);
     u32 *before = reinterpret_cast<u32 *>(smem + L.before_off);
     u32 *cand = reinterpret_cast<u32 *>(smem + L.cand_off);
 
-    if (threadIdx.x == 0) s_conn = atomicAdd(ticket, 1u);
-    __syncthreads();
-    const u32 c = s_conn;
-    const gcra_resp_conn cn = conns[c];
-    const u32 len = cn.len;
-
     // stage the segment: 16-byte loads of the chunks wholly inside it, single bytes at its ends (nothing outside it)
-    const uintptr_t seg = reinterpret_cast<uintptr_t>(in) + cn.off;
+    const uintptr_t seg = reinterpret_cast<uintptr_t>(in) + off;
     const unsigned char *sb = smem + (seg & 15);
     stage_key_span(seg, len, 0, len, threadIdx.x, RESP_THREADS,
                    [&](uintptr_t g, u32 o) { *reinterpret_cast<uint4 *>(smem + o) = __ldg(reinterpret_cast<const uint4 *>(g)); },
@@ -223,6 +218,26 @@ resp_parse_kernel(const unsigned char *__restrict__ in, const gcra_resp_conn *__
         r.now_ns = now_ns;
         rows[base + k] = r;
     }
+    return make_uint2(base, take);
+}
+
+template <class P>
+__global__ void __launch_bounds__(RESP_THREADS, 1)
+resp_parse_kernel(const unsigned char *__restrict__ in, const gcra_resp_conn *__restrict__ conns, u32 n_conns,
+                  u32 max_len, i64 now_ns, u32 row_cap, u64 k0, u64 k1, gcra_request *__restrict__ rows,
+                  u64 *status, u32 *ticket, uint2 *__restrict__ conn_rows, gcra_resp_outcome *outcome,
+                  u32 *__restrict__ total, u32 *__restrict__ seg_counts, u32 nseg, u32 cap_shift) {
+    // (no alignment is declared for the dynamic shared memory: that would pad every kernel's; RespSmem leaves room to
+    // round its start up to 16 bytes)
+    extern __shared__ unsigned char resp_dyn[];
+    unsigned char *smem = reinterpret_cast<unsigned char *>((reinterpret_cast<uintptr_t>(resp_dyn) + 15) & ~(uintptr_t)15);
+    __shared__ u32 s_conn;
+    if (threadIdx.x == 0) s_conn = atomicAdd(ticket, 1u);
+    __syncthreads();
+    const u32 c = s_conn;
+    const gcra_resp_conn cn = conns[c];
+    resp_parse_conn<P>(smem, c, cn.off, cn.len, in, n_conns, max_len, now_ns, row_cap, k0, k1, rows, status, conn_rows,
+                       outcome, total, seg_counts, nseg, cap_shift);
 }
 
 // The replies of rows [0, *total) in row order, straight into `out` (pinned host memory): each CTA takes a tile of
@@ -286,26 +301,25 @@ __global__ void resp_outcome_kernel(const uint2 *__restrict__ conn_rows, u32 n_c
 // so in table order; its rows go to rows[base_c ...] and their stream ids to stream_ids[base_c ...], cut exactly
 // where gcra_grpc_parse_throttle with max_frames = row_cap - base_c stops.  outcome[c] receives everything but the
 // reply fields and data_sent (grpc_outcome_kernel).  status[0 .. n_conns) and *ticket are zero at launch.
-__global__ void __launch_bounds__(RESP_THREADS, 1)
-grpc_parse_kernel(const unsigned char *__restrict__ in, const gcra_grpc_conn *__restrict__ conns, u32 n_conns,
-                  u32 max_len, i64 now_ns, u32 row_cap, u64 k0, u64 k1, gcra_request *__restrict__ rows,
-                  u32 *__restrict__ stream_ids, u64 *status, u32 *ticket, uint2 *__restrict__ conn_rows,
-                  gcra_grpc_outcome *outcome, u32 *__restrict__ total, u32 *__restrict__ seg_counts, u32 nseg,
-                  u32 cap_shift) {
-    extern __shared__ unsigned char grpc_dyn[];
-    unsigned char *smem = reinterpret_cast<unsigned char *>((reinterpret_cast<uintptr_t>(grpc_dyn) + 15) & ~(uintptr_t)15);
+//
+// grpc_parse_conn is that CTA's work for connection c = in[off, + len) with the HTTP/2 state *cn (whose off and len it
+// does not read), the dynamic shared memory laid out as GrpcSmem(max_len), len <= max_len; mixed_parse_kernel runs it
+// too.  emit(o) stores the connection's outcome (thread 0).  Returns {base_c, the rows taken} to every thread.
+template <class Emit>
+__device__ __forceinline__ uint2
+grpc_parse_conn(unsigned char *smem, u32 c, u32 off, u32 len, const gcra_grpc_conn *cn,
+                const unsigned char *__restrict__ in, u32 n_conns, u32 max_len, i64 now_ns, u32 row_cap, u64 k0,
+                u64 k1, gcra_request *__restrict__ rows, u32 *__restrict__ stream_ids, u64 *status,
+                uint2 *__restrict__ conn_rows, Emit emit, u32 *__restrict__ total, u32 *__restrict__ seg_counts,
+                u32 nseg, u32 cap_shift) {
     __shared__ unsigned char s_dyn[GCRA_GRPC_MAX_DYN];
-    __shared__ u32 s_conn, s_nf, s_base, s_n;
+    __shared__ u32 s_nf, s_base, s_n;
     const GrpcSmem L(max_len);
     u32 *frames = reinterpret_cast<u32 *>(smem + L.frames_off);
     u32 *calls = reinterpret_cast<u32 *>(smem + L.calls_off);
 
-    if (threadIdx.x == 0) s_conn = atomicAdd(ticket, 1u);
-    __syncthreads();
-    const u32 c = s_conn;
-    const gcra_grpc_conn *cn = conns + c;
-    const u32 len = cn->len, n_dyn = cn->n_dyn;
-    const uintptr_t seg = reinterpret_cast<uintptr_t>(in) + cn->off;
+    const u32 n_dyn = cn->n_dyn;
+    const uintptr_t seg = reinterpret_cast<uintptr_t>(in) + off;
     const unsigned char *sb = smem + (seg & 15);
     stage_key_span(seg, len, 0, len, threadIdx.x, RESP_THREADS,
                    [&](uintptr_t g, u32 o) { *reinterpret_cast<uint4 *>(smem + o) = __ldg(reinterpret_cast<const uint4 *>(g)); },
@@ -360,7 +374,7 @@ grpc_parse_kernel(const unsigned char *__restrict__ in, const gcra_grpc_conn *__
         o.data_sent = 0;
         o.ping = st.ping;
         for (int i = 0; i < 8; i++) o.ping_opaque[i] = st.ping ? st.opaque[i] : 0;
-        outcome[c] = o;
+        emit(o);
         conn_rows[c] = make_uint2(base, e.n);
         if (c == n_conns - 1) {
             const u32 t = base + e.n;
@@ -390,6 +404,25 @@ grpc_parse_kernel(const unsigned char *__restrict__ in, const gcra_grpc_conn *__
         rows[base + j] = r;
         stream_ids[base + j] = h.sid;
     }
+    return make_uint2(base, take);
+}
+
+__global__ void __launch_bounds__(RESP_THREADS, 1)
+grpc_parse_kernel(const unsigned char *__restrict__ in, const gcra_grpc_conn *__restrict__ conns, u32 n_conns,
+                  u32 max_len, i64 now_ns, u32 row_cap, u64 k0, u64 k1, gcra_request *__restrict__ rows,
+                  u32 *__restrict__ stream_ids, u64 *status, u32 *ticket, uint2 *__restrict__ conn_rows,
+                  gcra_grpc_outcome *outcome, u32 *__restrict__ total, u32 *__restrict__ seg_counts, u32 nseg,
+                  u32 cap_shift) {
+    extern __shared__ unsigned char grpc_dyn[];
+    unsigned char *smem = reinterpret_cast<unsigned char *>((reinterpret_cast<uintptr_t>(grpc_dyn) + 15) & ~(uintptr_t)15);
+    __shared__ u32 s_conn;
+    if (threadIdx.x == 0) s_conn = atomicAdd(ticket, 1u);
+    __syncthreads();
+    const u32 c = s_conn;
+    const gcra_grpc_conn *cn = conns + c;
+    grpc_parse_conn(smem, c, cn->off, cn->len, cn, in, n_conns, max_len, now_ns, row_cap, k0, k1, rows, stream_ids,
+                    status, conn_rows, [&](const gcra_grpc_outcome &o) { outcome[c] = o; }, total, seg_counts, nseg,
+                    cap_shift);
 }
 
 // resp_reply_kernel for gRPC: row i's response goes on stream stream_ids[i]
@@ -453,13 +486,151 @@ __global__ void grpc_outcome_kernel(const uint2 *__restrict__ conn_rows, u32 n_c
     }
 }
 
+// ---- mixed: RESP, HTTP and gRPC connections in one slot ----
+// One CTA per connection, taken by ticket, with one look-back chain over all connections: base_c is the rows of the
+// connections before c in table order, whatever their protocols.  The CTA runs its connection's protocol's parse body
+// (uniform over the CTA), so connection c's rows are exactly what its protocol's host walk takes at row_cap - base_c.
+// Every connection's consumed, n_frames and stop go to outcome[c]; a gRPC connection's whole outcome also goes to
+// goutcome[grpc_state] (its state is gconns[grpc_state]).  row_proto[i] receives row i's protocol, for the reply
+// kernel.  The dynamic shared memory is the largest layout of the protocols present; max_len[p - 1] is the longest
+// connection of protocol p.  (3 CTAs per SM: the registers of resp_parse_kernel<RespTraits>, so that short connections
+// keep its occupancy.)
+__global__ void __launch_bounds__(RESP_THREADS, 3)
+mixed_parse_kernel(const unsigned char *__restrict__ in, const gcra_mixed_conn *__restrict__ conns, u32 n_conns,
+                   const gcra_grpc_conn *__restrict__ gconns, uint3 max_len, i64 now_ns, u32 row_cap, u64 k0, u64 k1,
+                   gcra_request *__restrict__ rows, u32 *__restrict__ stream_ids, unsigned char *__restrict__ row_proto,
+                   u64 *status, u32 *ticket, uint2 *__restrict__ conn_rows, gcra_resp_outcome *outcome,
+                   gcra_grpc_outcome *goutcome, u32 *__restrict__ total, u32 *__restrict__ seg_counts, u32 nseg,
+                   u32 cap_shift) {
+    extern __shared__ unsigned char mixed_dyn[];
+    unsigned char *smem = reinterpret_cast<unsigned char *>((reinterpret_cast<uintptr_t>(mixed_dyn) + 15) & ~(uintptr_t)15);
+    __shared__ u32 s_conn;
+    if (threadIdx.x == 0) s_conn = atomicAdd(ticket, 1u);
+    __syncthreads();
+    const u32 c = s_conn;
+    const gcra_mixed_conn mc = conns[c];
+    uint2 br;
+    if (mc.protocol == GCRA_PROTO_GRPC) {
+        gcra_grpc_outcome *go = goutcome + mc.grpc_state;
+        auto emit = [&](const gcra_grpc_outcome &o) {
+            *go = o;
+            gcra_resp_outcome r;
+            r.consumed = o.consumed;
+            r.n_frames = o.n_frames;
+            r.stop = o.stop;
+            r.reserved = 0;
+            r.reply_off = 0;
+            r.reply_len = 0;
+            outcome[c] = r;
+        };
+        br = grpc_parse_conn(smem, c, mc.off, mc.len, gconns + mc.grpc_state, in, n_conns, max_len.z, now_ns, row_cap,
+                             k0, k1, rows, stream_ids, status, conn_rows, emit, total, seg_counts, nseg, cap_shift);
+    } else if (mc.protocol == GCRA_PROTO_HTTP) {
+        br = resp_parse_conn<HttpTraits>(smem, c, mc.off, mc.len, in, n_conns, max_len.y, now_ns, row_cap, k0, k1, rows,
+                                         status, conn_rows, outcome, total, seg_counts, nseg, cap_shift);
+    } else {
+        br = resp_parse_conn<RespTraits>(smem, c, mc.off, mc.len, in, n_conns, max_len.x, now_ns, row_cap, k0, k1, rows,
+                                         status, conn_rows, outcome, total, seg_counts, nseg, cap_shift);
+    }
+    for (u32 k = threadIdx.x; k < br.y; k += RESP_THREADS) row_proto[br.x + k] = (unsigned char)mc.protocol;
+}
+
+// row i's reply in its protocol: gcra_resp::put_reply, gcra_http::put_reply, or gcra_grpc::put_reply on its stream
+template <class Out>
+__device__ __forceinline__ void mixed_put_reply(Out &o, u32 proto, const gcra_request &q, const gcra_result &r, u32 sid) {
+    if (proto == GCRA_PROTO_GRPC) gcra_grpc::put_reply(o, q, r, sid);
+    else if (proto == GCRA_PROTO_HTTP) gcra_http::put_reply(o, q, r);
+    else gcra_resp::put_reply(o, q, r);
+}
+
+// resp_reply_kernel for a mixed slot: tiles of MIXED_REPLY_THREADS rows (a tile stages up to GCRA_HTTP_REPLY_MAX bytes
+// per row), each row in its protocol.  A connection's rows are contiguous, so most warps take one branch.
+__global__ void __launch_bounds__(MIXED_REPLY_THREADS)
+mixed_reply_kernel(const gcra_request *__restrict__ rows, const gcra_result *__restrict__ res,
+                   const u32 *__restrict__ stream_ids, const unsigned char *__restrict__ row_proto, const u32 *total_p,
+                   u64 *status, u32 *ticket, u64 *__restrict__ row_off, unsigned char *out) {
+    constexpr u32 T = MIXED_REPLY_THREADS;
+    __shared__ __align__(16) char stage[T * gcra_http::REPLY_MAX];
+    __shared__ u64 warp_sums[T / 32];
+    __shared__ u64 s_base;
+    __shared__ u32 s_tile;
+    if (threadIdx.x == 0) s_tile = atomicAdd(ticket, 1u);
+    __syncthreads();
+    const u32 tile = s_tile, total = *total_p;
+    if ((u64)tile * T >= total) return;                        // uniform over the CTA
+    const u32 row = tile * T + threadIdx.x;
+    gcra_request q{};
+    gcra_result r{};
+    u32 sid = 0, proto = 0;
+    gcra_resp::Count cnt;
+    if (row < total) {
+        q = rows[row];
+        r = res[row];
+        proto = row_proto[row];
+        if (proto == GCRA_PROTO_GRPC) sid = stream_ids[row];
+        mixed_put_reply(cnt, proto, q, r, sid);
+    }
+    u64 tile_bytes;
+    const u64 at = resp_block_scan<T>(cnt.n, warp_sums, &tile_bytes);
+    if (threadIdx.x == 0) s_base = resp_look_back(status, tile, tile_bytes);
+    if (row < total) {
+        gcra_resp::Write o{stage + at};
+        mixed_put_reply(o, proto, q, r, sid);
+    }
+    __syncthreads();
+    const u64 base = s_base;
+    if (row < total) row_off[row] = base + at;
+    if (row + 1 == total) row_off[total] = base + at + cnt.n;
+    for (u32 i = threadIdx.x; i < (u32)tile_bytes; i += T) out[base + i] = stage[i];
+}
+static_assert(MIXED_REPLY_THREADS * gcra_http::REPLY_MAX <= 48 * 1024, "the reply tile fits static shared memory");
+static_assert(gcra_http::REPLY_MAX >= gcra_resp::REPLY_MAX && gcra_http::REPLY_MAX >= gcra_grpc::REPLY_MAX,
+              "HTTP's replies are the longest");
+
+// one warp per connection: where its replies lie (outcome[c]); for a gRPC connection also in its gRPC outcome row,
+// with the DATA octets of its responses
+__global__ void mixed_outcome_kernel(const uint2 *__restrict__ conn_rows, const gcra_mixed_conn *__restrict__ conns,
+                                     u32 n_conns, const gcra_request *__restrict__ rows,
+                                     const gcra_result *__restrict__ res, const u32 *total_p,
+                                     const u64 *__restrict__ row_off, gcra_resp_outcome *outcome,
+                                     gcra_grpc_outcome *goutcome) {
+    const u32 c = (blockIdx.x * blockDim.x + threadIdx.x) / 32, lane = threadIdx.x & 31;
+    if (c >= n_conns) return;                                  // uniform over the warp
+    const u32 total = *total_p;
+    const gcra_mixed_conn mc = conns[c];
+    const uint2 br = conn_rows[c];
+    const u32 lo = min(br.x, total), hi = min(br.x + br.y, total);
+    const u64 a = total ? row_off[lo] : 0, b = total ? row_off[hi] : 0;
+    if (mc.protocol != GCRA_PROTO_GRPC) {
+        if (lane == 0) {
+            outcome[c].reply_off = a;
+            outcome[c].reply_len = b - a;
+        }
+        return;
+    }
+    u32 sent = 0;
+    for (u32 i = lo + lane; i < hi; i += 32) sent += gcra_grpc::data_len(rows[i], res[i]);
+#pragma unroll
+    for (u32 o = 16; o; o >>= 1) sent += __shfl_xor_sync(0xffffffffu, sent, o);
+    if (lane == 0) {
+        outcome[c].reply_off = a;
+        outcome[c].reply_len = b - a;
+        gcra_grpc_outcome *go = goutcome + mc.grpc_state;
+        go->reply_off = a;
+        go->reply_len = b - a;
+        go->data_sent = sent;
+    }
+}
+
 // ---- launches (gcra_resp.inc) ----
 cudaError_t resp_ring_setup() {
     cudaFuncAttributes a;
     for (const void *k : {(const void *)resp_parse_kernel<RespTraits>, (const void *)resp_reply_kernel<RespTraits>,
                           (const void *)resp_parse_kernel<HttpTraits>, (const void *)resp_reply_kernel<HttpTraits>,
                           (const void *)resp_outcome_kernel, (const void *)grpc_parse_kernel,
-                          (const void *)grpc_reply_kernel, (const void *)grpc_outcome_kernel}) {
+                          (const void *)grpc_reply_kernel, (const void *)grpc_outcome_kernel,
+                          (const void *)mixed_parse_kernel, (const void *)mixed_reply_kernel,
+                          (const void *)mixed_outcome_kernel}) {
         const cudaError_t e = cudaFuncGetAttributes(&a, k);    // (loads the code now: see preload in gcra_b200.cu)
         if (e) return e;
     }
@@ -469,8 +640,11 @@ cudaError_t resp_ring_setup() {
     e = cudaFuncSetAttribute(resp_parse_kernel<HttpTraits>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                              (int)RespSmem(RESP_MAX_CONN_BYTES, HttpTraits::CAND_PER_WORD).total);
     if (e) return e;
-    return cudaFuncSetAttribute(grpc_parse_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                (int)GrpcSmem(RESP_MAX_CONN_BYTES).total);
+    e = cudaFuncSetAttribute(grpc_parse_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                             (int)GrpcSmem(RESP_MAX_CONN_BYTES).total);
+    if (e) return e;
+    return cudaFuncSetAttribute(mixed_parse_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                (int)mixed_parse_smem(RESP_MAX_CONN_BYTES, RESP_MAX_CONN_BYTES, RESP_MAX_CONN_BYTES));
 }
 
 template <class P>
@@ -520,6 +694,31 @@ cudaError_t launch_grpc_reply(u32 tiles, const gcra_request *rows, const gcra_re
 cudaError_t launch_grpc_outcome(u32 n_conns, const uint2 *conn_rows, const gcra_request *rows, const gcra_result *res,
                                 const u32 *total, const u64 *row_off, gcra_grpc_outcome *outcome, cudaStream_t st) {
     grpc_outcome_kernel<<<(n_conns + 7) / 8, 256, 0, st>>>(conn_rows, n_conns, rows, res, total, row_off, outcome);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_mixed_parse(const MixedParse &a, cudaStream_t st) {
+    mixed_parse_kernel<<<a.n_conns, RESP_THREADS, mixed_parse_smem(a.max_len[0], a.max_len[1], a.max_len[2]), st>>>(
+        a.in, a.conns, a.n_conns, a.gconns, make_uint3(a.max_len[0], a.max_len[1], a.max_len[2]), a.now_ns, a.row_cap,
+        a.k0, a.k1, a.rows, a.stream_ids, a.row_proto, a.status, a.ticket, a.conn_rows, a.outcome, a.goutcome, a.total,
+        a.seg_counts, a.nseg, a.cap_shift);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_mixed_reply(u32 tiles, const gcra_request *rows, const gcra_result *res, const u32 *stream_ids,
+                               const unsigned char *row_proto, const u32 *total, u64 *ctrl, u64 *row_off,
+                               unsigned char *out, cudaStream_t st) {
+    mixed_reply_kernel<<<tiles, MIXED_REPLY_THREADS, 0, st>>>(rows, res, stream_ids, row_proto, total, ctrl + 1,
+                                                            reinterpret_cast<u32 *>(ctrl), row_off, out);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_mixed_outcome(u32 n_conns, const uint2 *conn_rows, const gcra_mixed_conn *conns,
+                                 const gcra_request *rows, const gcra_result *res, const u32 *total,
+                                 const u64 *row_off, gcra_resp_outcome *outcome, gcra_grpc_outcome *goutcome,
+                                 cudaStream_t st) {
+    mixed_outcome_kernel<<<(n_conns + 7) / 8, 256, 0, st>>>(conn_rows, conns, n_conns, rows, res, total, row_off,
+                                                            outcome, goutcome);
     return cudaGetLastError();
 }
 

@@ -13,8 +13,12 @@ constexpr u32 RESP_MAX_CONN_BYTES = 65536;     // MAX_BUFFER_SIZE of the referen
 
 // The ring's protocol: which grammar its parse kernel takes and which replies its reply kernel writes
 // (gcra_resp.cuh for RESP, gcra_http.cuh for HTTP, gcra_grpc.cuh for gRPC); everything else about a ring slot is
-// shared.  A gRPC ring has its own connection and outcome tables (gcra_grpc_conn, gcra_grpc_outcome).
-enum RingProto : u32 { PROTO_NONE = 0, PROTO_RESP = 1, PROTO_HTTP = 2, PROTO_GRPC = 3 };
+// shared.  A gRPC ring has its own connection and outcome tables (gcra_grpc_conn, gcra_grpc_outcome).  A mixed ring
+// takes all three in one slot: its connection table (gcra_mixed_conn) names each connection's protocol, and its
+// gRPC connections' state and outcome rows are the gRPC ring's tables.
+enum RingProto : u32 { PROTO_NONE = 0, PROTO_RESP = 1, PROTO_HTTP = 2, PROTO_GRPC = 3, PROTO_MIXED = 4 };
+static_assert(PROTO_RESP == GCRA_PROTO_RESP && PROTO_HTTP == GCRA_PROTO_HTTP && PROTO_GRPC == GCRA_PROTO_GRPC,
+              "a ring's protocol is a mixed connection's protocol");
 
 // The dynamic shared memory of resp_parse_kernel for connections of up to `max_len` bytes: the staged bytes (16
 // more for the segment's misalignment), one candidate bit per byte, the candidates before each 32-byte word, and one
@@ -51,8 +55,12 @@ struct RespParse {
     RingProto proto;
 };
 
-// a protocol's rows per reply tile (the reply kernel stages a tile's replies in shared memory)
-constexpr u32 reply_tile_rows(RingProto p) { return p == PROTO_HTTP ? 128 : RESP_THREADS; }
+// a protocol's rows per reply tile (the reply kernel stages a tile's replies in shared memory); a mixed ring's tile
+// has room for HTTP's replies, the longest
+constexpr u32 MIXED_REPLY_THREADS = 128;
+constexpr u32 reply_tile_rows(RingProto p) {
+    return p == PROTO_HTTP ? 128 : p == PROTO_MIXED ? MIXED_REPLY_THREADS : RESP_THREADS;
+}
 
 // The dynamic shared memory of grpc_parse_kernel for connections of up to `max_len` bytes: the staged bytes (16 more
 // for the segment's misalignment), one word per frame (a frame has at least 9 bytes) and one per call (a call has at
@@ -88,6 +96,46 @@ cudaError_t launch_grpc_reply(u32 tiles, const gcra_request *rows, const gcra_re
                               const u32 *total, u64 *ctrl, u64 *row_off, unsigned char *out, cudaStream_t st);
 cudaError_t launch_grpc_outcome(u32 n_conns, const uint2 *conn_rows, const gcra_request *rows, const gcra_result *res,
                                 const u32 *total, const u64 *row_off, gcra_grpc_outcome *outcome, cudaStream_t st);
+
+// The dynamic shared memory of mixed_parse_kernel: the largest layout that a present protocol needs, for the longest
+// connection of each protocol (0 where none)
+inline u32 mixed_parse_smem(u32 max_len_resp, u32 max_len_http, u32 max_len_grpc) {
+    u32 b = RespSmem(max_len_resp, 16).total;
+    b = b > RespSmem(max_len_http, 7).total ? b : RespSmem(max_len_http, 7).total;
+    return b > GrpcSmem(max_len_grpc).total ? b : GrpcSmem(max_len_grpc).total;
+}
+
+// mixed_parse_kernel's arguments: GrpcParse's with the mixed connection table, the gRPC state table (row k: the
+// connection whose grpc_state is k), the gRPC outcome table and each row's protocol
+struct MixedParse {
+    const unsigned char *in;
+    const gcra_mixed_conn *conns;
+    u32 n_conns;
+    u32 max_len[3];              // the longest connection of RESP, HTTP and gRPC
+    const gcra_grpc_conn *gconns;
+    i64 now_ns;
+    u32 row_cap;
+    u64 k0, k1;
+    gcra_request *rows;
+    u32 *stream_ids;             // [row_capacity] out (gRPC rows)
+    unsigned char *row_proto;    // [row_capacity] out: each row's GCRA_PROTO_*
+    u64 *status;
+    u32 *ticket;
+    uint2 *conn_rows;
+    gcra_resp_outcome *outcome;  // [n_conns] out (pinned host memory)
+    gcra_grpc_outcome *goutcome; // [gRPC connections] out (pinned host memory)
+    u32 *total, *seg_counts;
+    u32 nseg, cap_shift;
+};
+cudaError_t launch_mixed_parse(const MixedParse &a, cudaStream_t st);
+// ctrl: word 0 the ticket, then one status word per tile of MIXED_REPLY_THREADS rows; all zero
+cudaError_t launch_mixed_reply(u32 tiles, const gcra_request *rows, const gcra_result *res, const u32 *stream_ids,
+                               const unsigned char *row_proto, const u32 *total, u64 *ctrl, u64 *row_off,
+                               unsigned char *out, cudaStream_t st);
+cudaError_t launch_mixed_outcome(u32 n_conns, const uint2 *conn_rows, const gcra_mixed_conn *conns,
+                                 const gcra_request *rows, const gcra_result *res, const u32 *total,
+                                 const u64 *row_off, gcra_resp_outcome *outcome, gcra_grpc_outcome *goutcome,
+                                 cudaStream_t st);
 
 cudaError_t resp_ring_setup();   // once, before the first launch
 cudaError_t launch_resp_parse(const RespParse &a, cudaStream_t st);

@@ -531,12 +531,15 @@ def process_connections(buffers, limiter, now_ns, ring, slot=0, metrics=None):
     GPU takes every open connection's plain prefix, then each connection stopped at a request that is not plain hands
     that one request to parse_request / handle_request, in list order."""
     now = int(now_ns)
+    return ring_rounds(buffers, ring, slot, now, lambda data: general(data, limiter, now, metrics))
 
-    def general(data):
-        req = parse_request(data)
-        if req is None:
-            return None
-        out, n, close = handle_request(req, limiter, now, metrics)
-        return req.consumed, out, n, ("error" if req.bad is not None else "close") if close else None
 
-    return ring_rounds(buffers, ring, slot, now, general)
+def general(data, limiter, now, metrics=None):
+    """The general path of a connection stopped at a request that is not plain (stop 2): that one request, at the start
+    of `data`, parsed by parse_request and answered by handle_request.  Returns None (the request is incomplete) or
+    (bytes consumed, response bytes, THROTTLE decisions, close), close being None, "close" or "error"."""
+    req = parse_request(data)
+    if req is None:
+        return None
+    out, n, close = handle_request(req, limiter, now, metrics)
+    return req.consumed, out, n, ("error" if req.bad is not None else "close") if close else None

@@ -390,26 +390,29 @@ def process_connections(buffers, limiter, now_ns, ring, slot=0):
     and then, on its own.  That is the order in which decisions are made, so connections that share keys see each
     other's requests in that order."""
     now = int(now_ns)
-    parser = RespParser()
+    return ring_rounds(buffers, ring, slot, now, lambda data: general(data, limiter, now))
 
-    def general(data):
-        try:
-            r = parser.parse(data)
-        except RespError:
-            return 0, b"", 0, "error"
-        if r is None:
-            return None
-        plan = _plan_command(r[0])
-        if plan[0] == "throttle":
-            kb = plan[1].encode()
-            req = np.empty(1, REQ_DTYPE)
-            req[0] = (limiter.store.hash_key(kb), plan[2], plan[3], plan[4], plan[5], now)
-            res = limiter.rate_limit_batch(req)
-            return r[1], RespSerializer.serialize(_throttle_reply(res[0], plan[2], plan[5])), 1, \
-                "quit" if _is_quit(r[0]) else None
-        return r[1], RespSerializer.serialize(plan[1]), 0, "quit" if _is_quit(r[0]) else None
 
-    return ring_rounds(buffers, ring, slot, now, general)
+def general(data, limiter, now):
+    """The general path of a connection that the batch walk stopped at a frame that is not a plain THROTTLE (stop 2):
+    that one frame, at the start of `data`, parsed by RespParser and answered; a THROTTLE among them is decided there
+    and then, on its own, with the key hashed by limiter.store.hash_key.  Returns None (the frame is incomplete) or
+    (bytes consumed, reply bytes, THROTTLE decisions, close), close being None, "quit" or "error"."""
+    try:
+        r = RespParser().parse(data)
+    except RespError:
+        return 0, b"", 0, "error"
+    if r is None:
+        return None
+    plan = _plan_command(r[0])
+    if plan[0] == "throttle":
+        kb = plan[1].encode()
+        req = np.empty(1, REQ_DTYPE)
+        req[0] = (limiter.store.hash_key(kb), plan[2], plan[3], plan[4], plan[5], now)
+        res = limiter.rate_limit_batch(req)
+        return r[1], RespSerializer.serialize(_throttle_reply(res[0], plan[2], plan[5])), 1, \
+            "quit" if _is_quit(r[0]) else None
+    return r[1], RespSerializer.serialize(plan[1]), 0, "quit" if _is_quit(r[0]) else None
 
 
 def ring_rounds(buffers, ring, slot, now, general):
