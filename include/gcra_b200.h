@@ -271,7 +271,7 @@ int32_t gcra_get_stats(gcra_engine *h, gcra_stats *out);
  * per key hash in a device table; gcra_top_denied returns the k most denied (hash, count) pairs, most denied first
  * (ties: smaller hash first), and prunes the table to its max_keys top entries once more than 3 x max_keys keys have
  * accumulated (the reference's cleanup rule).  Keys are hashes here -- the caller of the batch entry points owns the
- * strings.  max_keys = 0 switches tracking off.  max_keys is at most 2^27 (the table holds 16 entries per key, at
+ * strings; the rings name theirs on the GPU (gcra_ring_metrics, gcra_denied_names).  max_keys = 0 switches tracking off.  max_keys is at most 2^27 (the table holds 16 entries per key, at
  * most 2^31); a larger value, or a failed allocation, returns GCRA_INTERNAL and leaves the previous setting and its
  * counts as they were.
  *   - Multi-GPU: every pipeline counts a denied request on the engine that owns its key (gcra_owner_of): the owner's
@@ -663,6 +663,39 @@ typedef struct {
 int32_t gcra_mixed_ring_create(gcra_engine *h, uint32_t slots, uint32_t max_conns, uint64_t in_capacity,
                                uint32_t row_capacity);
 gcra_mixed_conn *gcra_mixed_ring_conns(gcra_engine *h, uint32_t slot);     /* pinned [max_conns], caller fills */
+
+/* ---- ring metrics: the server's GET /metrics counts and top denied keys by name (metrics.rs:233-310) -------------
+ * Only the rings know which transport a row came from, and they never hand key strings to the host.  With ring
+ * metrics on, every ring submit (RESP, HTTP, gRPC or mixed ring, created before or after) launches one more kernel on
+ * its reply stream, after the replies: it counts the slot's rows per transport by the reference's rules, and names
+ * the denied keys of the denied-key table (gcra_track_denied) from the slot's input.
+ *   - RESP ("redis"): a row is denied when its status is GCRA_OK and allowed is 0, else allowed -- an -ERR reply
+ *     counts as allowed (redis/mod.rs:193-205).  RESP rows are never errors.
+ *   - HTTP and gRPC: status != GCRA_OK is an error (the 500 response, grpc-status 13), else allowed or denied.
+ *   - A denied row's key hash found in the denied table takes the row's key bytes as its name, once (the first row
+ *     to name it wins); a key longer than GCRA_DENIED_NAME_MAX bytes is marked GCRA_NAME_TOO_LONG, as the reference
+ *     never tracks such keys (metrics.rs:11,39-41).  A hash that found the table full has no entry to name.
+ *   - gcra_top_denied's pruning keeps the surviving keys' names and forgets the rest.
+ * Names cost GCRA_DENIED_NAME_MAX + 4 bytes per denied-table entry while both ring metrics and denied tracking are
+ * on, so max_keys is then at most GCRA_RING_METRICS_MAX_KEYS (10,000, the reference's MAX_DENIED_KEYS_LIMIT, about
+ * 68 MB): gcra_ring_metrics(h, 1) refuses while tracking runs with more, gcra_track_denied refuses more while ring
+ * metrics are on.  Both return GCRA_INTERNAL and leave the engine as it was.  Every call here and gcra_top_denied
+ * wait for the ring slots in flight and the engine's batches. */
+typedef struct { uint64_t allowed, denied, errors; } gcra_transport_counts;
+#define GCRA_DENIED_NAME_MAX 256u
+#define GCRA_RING_METRICS_MAX_KEYS 10000u
+#define GCRA_NAME_UNKNOWN  0xFFFFFFFFu   /* no ring row has named this hash */
+#define GCRA_NAME_TOO_LONG 0xFFFFFFFEu   /* the key is longer than GCRA_DENIED_NAME_MAX bytes */
+/* on: every later ring submit counts its rows per transport and names its denied keys; switching on zeroes the
+ * counts and the names.  off: no kernel is launched and the parse kernels write no key positions; the counts stay
+ * readable, the names are released. */
+int32_t gcra_ring_metrics(gcra_engine *h, uint32_t on);
+/* [0] RESP, [1] HTTP, [2] gRPC: the ring rows counted since ring metrics were switched on */
+int32_t gcra_ring_transport_counts(gcra_engine *h, gcra_transport_counts out[3]);
+/* for each of n hashes (from gcra_top_denied): lens[i] = its name's length, with the bytes at names + 256 i, or one of
+ * the two markers (GCRA_NAME_UNKNOWN also for a hash not in the table, or while ring metrics are off).  Needs denied
+ * tracking on. */
+int32_t gcra_denied_names(gcra_engine *h, uint32_t n, const uint64_t *key_hashes, char *names, uint32_t *lens);
 
 #ifdef __cplusplus
 }

@@ -23,7 +23,8 @@ from . import _native
 from ._native import (REQ_DTYPE, RES_DTYPE, REQ16_DTYPE, RES16_DTYPE, POLICY_DTYPE, OK, NEGATIVE_QUANTITY,
                       INVALID_RATE_LIMIT, INTERNAL, RESP_CONN_DTYPE, RESP_OUTCOME_DTYPE, RESP_MAX_CONN_BYTES,
                       RESP_REPLY_MAX, HTTP_REPLY_MAX, GRPC_CONN_DTYPE, GRPC_OUTCOME_DTYPE, GRPC_REPLY_MAX,
-                      GRPC_MAX_DYN, PROTO_RESP, PROTO_HTTP, PROTO_GRPC, MIXED_CONN_DTYPE)
+                      GRPC_MAX_DYN, PROTO_RESP, PROTO_HTTP, PROTO_GRPC, MIXED_CONN_DTYPE, DENIED_NAME_MAX,
+                      RING_METRICS_MAX_KEYS, NAME_UNKNOWN, NAME_TOO_LONG)
 
 __all__ = ["RateLimiter", "RateLimitResult", "Rate", "CellError", "NegativeQuantity", "InvalidRateLimit",
            "Internal", "AdaptiveStore", "PeriodicStore", "ProbabilisticStore", "ManualStore",
@@ -270,6 +271,27 @@ class _GpuStore:
         n, dropped = C.c_uint32(), C.c_uint64()
         self._check(self._L.gcra_top_denied(self._h, k, keys.ctypes.data, cnts.ctypes.data, C.byref(n), C.byref(dropped)))
         return [(int(keys[i]), int(cnts[i])) for i in range(n.value)], int(dropped.value)
+
+    def ring_metrics(self, on):
+        """gcra_ring_metrics: every later ring submit counts its rows per transport and names its denied keys (on
+        zeroes both); off launches nothing more.  Refused while denied tracking runs with more than 10,000 keys."""
+        self._check(self._L.gcra_ring_metrics(self._h, 1 if on else 0))
+
+    def ring_transport_counts(self):
+        """the ring rows counted so far: uint64 [3, 3], rows RESP, HTTP, gRPC and columns allowed, denied, errors"""
+        out = np.zeros((3, 3), np.uint64)
+        self._check(self._L.gcra_ring_transport_counts(self._h, out.ctypes.data))
+        return out
+
+    def denied_names(self, key_hashes):
+        """gcra_denied_names: per hash (from top_denied) its key's bytes as a ring named them, or the marker
+        NAME_UNKNOWN or NAME_TOO_LONG (an int)"""
+        hs = np.ascontiguousarray(key_hashes, np.uint64)
+        names = np.zeros((max(len(hs), 1), DENIED_NAME_MAX), np.uint8)
+        lens = np.zeros(max(len(hs), 1), np.uint32)
+        self._check(self._L.gcra_denied_names(self._h, len(hs), hs.ctypes.data, names.ctypes.data, lens.ctypes.data))
+        return [names[i, :int(lens[i])].tobytes() if lens[i] <= DENIED_NAME_MAX else int(lens[i])
+                for i in range(len(hs))]
 
     def policy_tick(self, now):
         """The store kind's sweep policy against the caller's clock (for device-resident / pipelined / sharded

@@ -43,6 +43,9 @@ assert GRPC_CONN_DTYPE.itemsize == 152 and GRPC_OUTCOME_DTYPE.itemsize == 56 and
 assert REQ_DTYPE.itemsize == 48 and RES_DTYPE.itemsize == 32 and REQ16_DTYPE.itemsize == 16
 assert RES16_DTYPE.itemsize == 16
 
+# ring metrics (gcra_ring_metrics, gcra_denied_names)
+DENIED_NAME_MAX, RING_METRICS_MAX_KEYS, NAME_UNKNOWN, NAME_TOO_LONG = 256, 10_000, 0xFFFFFFFF, 0xFFFFFFFE
+
 OK, NEGATIVE_QUANTITY, INVALID_RATE_LIMIT, INTERNAL = 0, 1, 2, 3
 STORE_PERIODIC, STORE_PROBABILISTIC, STORE_ADAPTIVE, STORE_MANUAL = 0, 1, 2, 3
 FLAG_TIGHT_TABLE, FLAG_INDEX_PATH, FLAG_SORT_PATH, FLAG_RANDOM_SEED = 1, 2, 4, 8
@@ -182,6 +185,9 @@ SYMBOLS = {
     "gcra_grpc_ring_outcome": (_vp, [_vp, _u32]),
     "gcra_mixed_ring_create": (_i32, [_vp, _u32, _u32, _u64, _u32]),
     "gcra_mixed_ring_conns": (_vp, [_vp, _u32]),
+    "gcra_ring_metrics": (_i32, [_vp, _u32]),
+    "gcra_ring_transport_counts": (_i32, [_vp, _vp]),
+    "gcra_denied_names": (_i32, [_vp, _u32, _vp, _vp, _vp]),
     "gcra_owner_of": (_u32, [_u64, _u32]),
     "gcra_route_partition": (_i32, [_vp, _u64, _vp, _u32, _vp, _vp, _vp, _vp]),
     "gcra_route_unpermute": (_i32, [_vp, _u64, _vp, _vp, _vp, _vp]),

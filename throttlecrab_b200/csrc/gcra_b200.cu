@@ -81,6 +81,8 @@ struct RingSlot {
     PinnedBuf<gcra_mixed_conn> h_mconns;
     DevBuf<gcra_mixed_conn> d_mconns;
     DevBuf<unsigned char> row_proto;
+    // ring metrics (gcra_ring_metrics): each row's key {offset in d_in, length}, written by the parse kernels
+    DevBuf<uint2> key_ref;
 };
 }  // namespace
 
@@ -225,8 +227,13 @@ struct HostTable {
     uint32_t lines() const { return view.null_slot / 4 + 1; }
 };
 
-// the arrays of the denied-key table: gcra_engine::denied is the view the kernels take
-struct DeniedArrays { DevBuf<u64> keys, counts, dropped; };
+// the arrays of the denied-key table: gcra_engine::denied is the view the kernels take.  names / name_len: the keys'
+// names (GCRA_DENIED_NAME_MAX bytes, and a length word, per entry), while ring metrics are on
+struct DeniedArrays {
+    DevBuf<u64> keys, counts, dropped;
+    DevBuf<unsigned char> names;
+    DevBuf<u32> name_len;
+};
 
 // the header of a snapshot file (gcra_snapshot_save, gcra_snapshot_begin)
 namespace {
@@ -357,6 +364,9 @@ struct gcra_engine {
     DeniedTable denied{};
     uint32_t denied_max = 0;
     uint64_t denied_cap = 0;
+    // ring metrics (gcra_ring_metrics): ring rows per transport [3][allowed, denied, errors]
+    bool ring_metrics = false;
+    DevBuf<u64> ring_counts;
     uint64_t hash_seed[2] = {0, 0};  // SipHash key of the string-keyed entry points ((0,0): the unkeyed gcra_hash_key)
     // background saves (gcra_snapshot_begin); gcra_destroy joins the writer thread before anything is released
     std::unique_ptr<SnapshotStaging> snap;
@@ -382,6 +392,14 @@ static int order_after_batches(gcra_engine *h, cudaStream_t st) {
 }
 static int wait_for_batches(gcra_engine *h) {
     for (auto &o : h->scr) if (o.back_recorded) CK(cudaEventSynchronize(o.ev_back.get()));
+    return GCRA_OK;
+}
+// What reads or rewrites the denied table or the ring counts waits for the batches and for the ring slots in flight:
+// a ring slot counts and names on its reply stream, after its batch's ev_back.  (The slots stay in flight for
+// gcra_ring_wait.)
+static int wait_for_metrics_writers(gcra_engine *h) {
+    RC(wait_for_batches(h));
+    for (auto &s : h->ring) if (s.in_flight) CK(cudaEventSynchronize(s.ev_done.get()));
     return GCRA_OK;
 }
 
@@ -1703,10 +1721,23 @@ int32_t gcra_peek(gcra_engine *h, uint64_t key_hash, int64_t *tat, int64_t *expi
 }
 
 // ---- metrics bridge: top denied keys (throttlecrab-server/src/metrics.rs:24-64,162-173) --------------------------
+// the names of a denied table of `cap` entries (ring metrics), none known
+static int make_denied_names(gcra_engine *h, DeniedArrays &a, uint64_t cap) {
+    CK(a.names.make((size_t)cap * GCRA_DENIED_NAME_MAX));
+    CK(a.name_len.make(cap));
+    CK(cudaMemset(a.name_len.get(), 0xff, cap * sizeof(u32)));           // GCRA_NAME_UNKNOWN
+    return GCRA_OK;
+}
+
 int32_t gcra_track_denied(gcra_engine *h, uint32_t max_keys) {
     CK(cudaSetDevice(h->device));
     // the table holds 16 entries per tracked key: at most 2^31
     if (max_keys > (1u << 27)) { h->err = "track_denied: max_keys must be at most 2^27"; return GCRA_INTERNAL; }
+    if (h->ring_metrics && max_keys > GCRA_RING_METRICS_MAX_KEYS) {
+        h->err = "track_denied: max_keys must be at most 10,000 while ring metrics are on";
+        return GCRA_INTERNAL;
+    }
+    RC(wait_for_metrics_writers(h));
     CK(cudaDeviceSynchronize());
     DeniedArrays a;
     const uint64_t cap = max_keys ? 1ULL << ceil_log2(std::max<uint64_t>(16ULL * max_keys, 1024)) : 0;
@@ -1717,6 +1748,7 @@ int32_t gcra_track_denied(gcra_engine *h, uint32_t max_keys) {
         CK(cudaMemset(a.keys.get(), 0, cap * sizeof(u64)));
         CK(cudaMemset(a.counts.get(), 0, cap * sizeof(u64)));
         CK(cudaMemset(a.dropped.get(), 0, sizeof(u64)));
+        if (h->ring_metrics) RC(make_denied_names(h, a, cap));
     }
     h->denied = max_keys ? DeniedTable{a.keys.get(), a.counts.get(), (u32)(cap - 1), a.dropped.get()} : DeniedTable{};
     h->denied_arrays = std::move(a);
@@ -1726,6 +1758,7 @@ int32_t gcra_track_denied(gcra_engine *h, uint32_t max_keys) {
 }
 
 // the k most denied keys (hash, count), most denied first; *dropped = denials of keys that found the table full.
+// The pruning moves each surviving key's name (ring metrics) with it and forgets the others'.
 // Like the reference's cleanup (metrics.rs:52-64) the table is pruned to its `max_keys` top entries when more than
 // three times as many have accumulated.  Waits for every scratch set's ev_back, which a peer-memory tick records
 // after its count and before it publishes its results: multi-GPU callers query between ticks, after joining them.
@@ -1733,30 +1766,113 @@ int32_t gcra_top_denied(gcra_engine *h, uint32_t k, uint64_t *key_hashes, uint64
     CK(cudaSetDevice(h->device));
     if (n_out) *n_out = 0;
     if (!h->denied_max) { h->err = "gcra_track_denied first"; return GCRA_INTERNAL; }
-    RC(wait_for_batches(h));
+    RC(wait_for_metrics_writers(h));
     std::vector<u64> keys(h->denied_cap), cnts(h->denied_cap);
     CK(cudaMemcpy(keys.data(), h->denied.keys, keys.size() * sizeof(u64), cudaMemcpyDeviceToHost));
     CK(cudaMemcpy(cnts.data(), h->denied.counts, cnts.size() * sizeof(u64), cudaMemcpyDeviceToHost));
     if (dropped) CK(cudaMemcpy(dropped, h->denied.dropped, sizeof(u64), cudaMemcpyDeviceToHost));
-    std::vector<std::pair<u64, u64>> top;      // (count, key)
-    for (uint32_t i = 0; i < h->denied_cap; i++) if (keys[i]) top.emplace_back(cnts[i], keys[i]);
-    std::sort(top.begin(), top.end(), [](const std::pair<u64, u64> &a, const std::pair<u64, u64> &b) {
-        return a.first != b.first ? a.first > b.first : a.second < b.second;
+    struct Entry { u64 count, key; uint32_t at; };
+    std::vector<Entry> top;
+    for (uint32_t i = 0; i < h->denied_cap; i++) if (keys[i]) top.push_back({cnts[i], keys[i], i});
+    std::sort(top.begin(), top.end(), [](const Entry &a, const Entry &b) {
+        return a.count != b.count ? a.count > b.count : a.key < b.key;
     });
     const uint32_t n = (uint32_t)std::min<size_t>(k, top.size());
-    for (uint32_t i = 0; i < n; i++) { key_hashes[i] = top[i].second; counts[i] = top[i].first; }
+    for (uint32_t i = 0; i < n; i++) { key_hashes[i] = top[i].key; counts[i] = top[i].count; }
     if (n_out) *n_out = n;
     if (top.size() > (size_t)3 * h->denied_max) {
+        DeniedArrays &a = h->denied_arrays;
+        const bool named = a.name_len.get() != nullptr;
+        const size_t nb = named ? (size_t)h->denied_cap * GCRA_DENIED_NAME_MAX : 0;
+        std::vector<u32> len(named ? h->denied_cap : 0), new_len(len.size(), GCRA_NAME_UNKNOWN);
+        std::vector<unsigned char> names(nb), new_names(nb);
+        if (named) {
+            CK(cudaMemcpy(len.data(), a.name_len.get(), len.size() * sizeof(u32), cudaMemcpyDeviceToHost));
+            CK(cudaMemcpy(names.data(), a.names.get(), nb, cudaMemcpyDeviceToHost));
+        }
         std::fill(keys.begin(), keys.end(), 0);
         std::fill(cnts.begin(), cnts.end(), 0);
         for (uint32_t i = 0; i < h->denied_max; i++) {
-            uint32_t s = (uint32_t)(mix64(top[i].second ^ 0x9E3779B97F4A7C15ULL)) & h->denied.mask;
+            uint32_t s = (uint32_t)(mix64(top[i].key ^ 0x9E3779B97F4A7C15ULL)) & h->denied.mask;
             while (keys[s]) s = (s + 1) & h->denied.mask;
-            keys[s] = top[i].second;
-            cnts[s] = top[i].first;
+            keys[s] = top[i].key;
+            cnts[s] = top[i].count;
+            if (named) {
+                const uint32_t from = top[i].at;
+                new_len[s] = len[from];
+                if (len[from] <= GCRA_DENIED_NAME_MAX)
+                    memcpy(&new_names[(size_t)s * GCRA_DENIED_NAME_MAX], &names[(size_t)from * GCRA_DENIED_NAME_MAX], len[from]);
+            }
         }
         CK(cudaMemcpy(h->denied.keys, keys.data(), keys.size() * sizeof(u64), cudaMemcpyHostToDevice));
         CK(cudaMemcpy(h->denied.counts, cnts.data(), cnts.size() * sizeof(u64), cudaMemcpyHostToDevice));
+        if (named) {
+            CK(cudaMemcpy(a.name_len.get(), new_len.data(), new_len.size() * sizeof(u32), cudaMemcpyHostToDevice));
+            CK(cudaMemcpy(a.names.get(), new_names.data(), nb, cudaMemcpyHostToDevice));
+        }
+    }
+    return GCRA_OK;
+}
+
+// ---- ring metrics (metrics.rs:233-310: requests by transport, top denied keys by name) ------------------------------
+int32_t gcra_ring_metrics(gcra_engine *h, uint32_t on) {
+    CK(cudaSetDevice(h->device));
+    if (on && h->denied_max > GCRA_RING_METRICS_MAX_KEYS) {
+        h->err = "ring metrics: denied tracking runs with max_keys above 10,000";
+        return GCRA_INTERNAL;
+    }
+    RC(wait_for_metrics_writers(h));
+    if (!on) {
+        h->ring_metrics = false;
+        h->denied_arrays.names.reset();
+        h->denied_arrays.name_len.reset();
+        return GCRA_OK;
+    }
+    DevBuf<u64> counts;                                 // (built whole before anything is swapped in)
+    CK(counts.make(9));
+    CK(cudaMemset(counts.get(), 0, 9 * sizeof(u64)));
+    DeniedArrays named;
+    if (h->denied_max) RC(make_denied_names(h, named, h->denied_cap));
+    h->ring_counts = std::move(counts);
+    h->denied_arrays.names = std::move(named.names);
+    h->denied_arrays.name_len = std::move(named.name_len);
+    h->ring_metrics = true;
+    return GCRA_OK;
+}
+
+int32_t gcra_ring_transport_counts(gcra_engine *h, gcra_transport_counts out[3]) {
+    CK(cudaSetDevice(h->device));
+    if (!h->ring_counts.get()) { memset(out, 0, 3 * sizeof(gcra_transport_counts)); return GCRA_OK; }
+    RC(wait_for_metrics_writers(h));
+    static_assert(sizeof(gcra_transport_counts) == 3 * sizeof(u64), "three counters per transport");
+    CK(cudaMemcpy(out, h->ring_counts.get(), 9 * sizeof(u64), cudaMemcpyDeviceToHost));
+    return GCRA_OK;
+}
+
+int32_t gcra_denied_names(gcra_engine *h, uint32_t n, const uint64_t *key_hashes, char *names, uint32_t *lens) {
+    CK(cudaSetDevice(h->device));
+    if (!h->denied_max) { h->err = "gcra_track_denied first"; return GCRA_INTERNAL; }
+    RC(wait_for_metrics_writers(h));
+    for (uint32_t i = 0; i < n; i++) lens[i] = GCRA_NAME_UNKNOWN;
+    const DeniedArrays &a = h->denied_arrays;
+    if (!a.name_len.get() || !n) return GCRA_OK;
+    // (the whole table in three copies: a scrape asks for every entry gcra_top_denied returns)
+    std::vector<u64> keys(h->denied_cap);
+    std::vector<u32> len(h->denied_cap);
+    std::vector<unsigned char> all((size_t)h->denied_cap * GCRA_DENIED_NAME_MAX);
+    CK(cudaMemcpy(keys.data(), h->denied.keys, keys.size() * sizeof(u64), cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(len.data(), a.name_len.get(), len.size() * sizeof(u32), cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(all.data(), a.names.get(), all.size(), cudaMemcpyDeviceToHost));
+    for (uint32_t i = 0; i < n; i++) {
+        const u64 k = key_hashes[i] ? key_hashes[i] : 1;                     // (as the table stores it)
+        uint32_t s = (uint32_t)(mix64(k ^ 0x9E3779B97F4A7C15ULL)) & h->denied.mask;
+        for (uint32_t probe = 0; probe < 64 && keys[s]; probe++, s = (s + 1) & h->denied.mask) {
+            if (keys[s] != k) continue;
+            lens[i] = len[s];
+            if (len[s] <= GCRA_DENIED_NAME_MAX)
+                memcpy(names + (size_t)i * GCRA_DENIED_NAME_MAX, &all[(size_t)s * GCRA_DENIED_NAME_MAX], len[s]);
+            break;
+        }
     }
     return GCRA_OK;
 }

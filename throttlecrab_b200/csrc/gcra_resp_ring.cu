@@ -12,7 +12,8 @@
 // and their gRPC counterparts (grpc_parse_kernel, grpc_reply_kernel, grpc_outcome_kernel), which carry each row's
 // stream id and each connection's HTTP/2 state.  The mixed ring's kernels (mixed_parse_kernel, mixed_reply_kernel,
 // mixed_outcome_kernel) take connections of all three protocols in one slot: the parse kernel runs the same parse
-// bodies (resp_parse_conn, grpc_parse_conn), the reply kernel the same reply writers.
+// bodies (resp_parse_conn, grpc_parse_conn), the reply kernel the same reply writers.  ring_metrics_kernel counts a
+// finished slot's rows per transport and names its denied keys (gcra_ring_metrics).
 #include "gcra_resp_ring.cuh"
 #include "gcra_http.cuh"
 #include "gcra_grpc.cuh"
@@ -113,13 +114,15 @@ __device__ __forceinline__ u32 resp_rank(const u32 *bits, const u32 *before, u32
 // [s << cap_shift, (s + 1) << cap_shift)).  status[0 .. n_conns) and *ticket are zero at launch.
 // The body of resp_parse_kernel for connection c = in[off, + len) (a CTA's whole work; mixed_parse_kernel runs it
 // too): smem is the dynamic shared memory rounded up to 16 bytes, laid out as RespSmem(max_len, P::CAND_PER_WORD),
-// len <= max_len.  Returns {base_c, the rows taken} to every thread.
+// len <= max_len.  Returns {base_c, the rows taken} to every thread.  key_ref (null: not written) receives each row's
+// key as {its offset in `in`, its length}: a plain key is raw contiguous bytes (a RESP bulk string, a JSON string
+// without escapes), which ring_metrics_kernel names denied keys from.
 template <class P>
 __device__ __forceinline__ uint2
 resp_parse_conn(unsigned char *smem, u32 c, u32 off, u32 len, const unsigned char *__restrict__ in, u32 n_conns,
                 u32 max_len, i64 now_ns, u32 row_cap, u64 k0, u64 k1, gcra_request *__restrict__ rows, u64 *status,
                 uint2 *__restrict__ conn_rows, gcra_resp_outcome *outcome, u32 *__restrict__ total,
-                u32 *__restrict__ seg_counts, u32 nseg, u32 cap_shift) {
+                u32 *__restrict__ seg_counts, u32 nseg, u32 cap_shift, uint2 *__restrict__ key_ref) {
     __shared__ u64 warp_sums[RESP_THREADS / 32];
     __shared__ u32 s_base, s_n;
     const RespSmem L(max_len, P::CAND_PER_WORD);
@@ -217,16 +220,20 @@ resp_parse_conn(unsigned char *smem, u32 c, u32 off, u32 len, const unsigned cha
         r.quantity = fr.a[3];
         r.now_ns = now_ns;
         rows[base + k] = r;
+        if (key_ref) key_ref[base + k] = make_uint2(off + (u32)(fr.key - sb), (u32)fr.klen);
     }
     return make_uint2(base, take);
 }
 
+// (3 CTAs per SM: the key_ref store would take the RESP instantiation from 80 to 84 registers, and 2 CTAs per SM,
+// for short connections; bounded, it fits 80 with no spills)
 template <class P>
-__global__ void __launch_bounds__(RESP_THREADS, 1)
+__global__ void __launch_bounds__(RESP_THREADS, 3)
 resp_parse_kernel(const unsigned char *__restrict__ in, const gcra_resp_conn *__restrict__ conns, u32 n_conns,
                   u32 max_len, i64 now_ns, u32 row_cap, u64 k0, u64 k1, gcra_request *__restrict__ rows,
                   u64 *status, u32 *ticket, uint2 *__restrict__ conn_rows, gcra_resp_outcome *outcome,
-                  u32 *__restrict__ total, u32 *__restrict__ seg_counts, u32 nseg, u32 cap_shift) {
+                  u32 *__restrict__ total, u32 *__restrict__ seg_counts, u32 nseg, u32 cap_shift,
+                  uint2 *__restrict__ key_ref) {
     // (no alignment is declared for the dynamic shared memory: that would pad every kernel's; RespSmem leaves room to
     // round its start up to 16 bytes)
     extern __shared__ unsigned char resp_dyn[];
@@ -237,7 +244,7 @@ resp_parse_kernel(const unsigned char *__restrict__ in, const gcra_resp_conn *__
     const u32 c = s_conn;
     const gcra_resp_conn cn = conns[c];
     resp_parse_conn<P>(smem, c, cn.off, cn.len, in, n_conns, max_len, now_ns, row_cap, k0, k1, rows, status, conn_rows,
-                       outcome, total, seg_counts, nseg, cap_shift);
+                       outcome, total, seg_counts, nseg, cap_shift, key_ref);
 }
 
 // The replies of rows [0, *total) in row order, straight into `out` (pinned host memory): each CTA takes a tile of
@@ -305,13 +312,14 @@ __global__ void resp_outcome_kernel(const uint2 *__restrict__ conn_rows, u32 n_c
 // grpc_parse_conn is that CTA's work for connection c = in[off, + len) with the HTTP/2 state *cn (whose off and len it
 // does not read), the dynamic shared memory laid out as GrpcSmem(max_len), len <= max_len; mixed_parse_kernel runs it
 // too.  emit(o) stores the connection's outcome (thread 0).  Returns {base_c, the rows taken} to every thread.
+// key_ref: as in resp_parse_conn (a protobuf string is raw contiguous bytes too).
 template <class Emit>
 __device__ __forceinline__ uint2
 grpc_parse_conn(unsigned char *smem, u32 c, u32 off, u32 len, const gcra_grpc_conn *cn,
                 const unsigned char *__restrict__ in, u32 n_conns, u32 max_len, i64 now_ns, u32 row_cap, u64 k0,
                 u64 k1, gcra_request *__restrict__ rows, u32 *__restrict__ stream_ids, u64 *status,
                 uint2 *__restrict__ conn_rows, Emit emit, u32 *__restrict__ total, u32 *__restrict__ seg_counts,
-                u32 nseg, u32 cap_shift) {
+                u32 nseg, u32 cap_shift, uint2 *__restrict__ key_ref) {
     __shared__ unsigned char s_dyn[GCRA_GRPC_MAX_DYN];
     __shared__ u32 s_nf, s_base, s_n;
     const GrpcSmem L(max_len);
@@ -403,6 +411,7 @@ grpc_parse_conn(unsigned char *smem, u32 c, u32 off, u32 len, const gcra_grpc_co
         r.now_ns = now_ns;
         rows[base + j] = r;
         stream_ids[base + j] = h.sid;
+        if (key_ref) key_ref[base + j] = make_uint2(off + (u32)(fr.key - sb), (u32)fr.klen);
     }
     return make_uint2(base, take);
 }
@@ -412,7 +421,7 @@ grpc_parse_kernel(const unsigned char *__restrict__ in, const gcra_grpc_conn *__
                   u32 max_len, i64 now_ns, u32 row_cap, u64 k0, u64 k1, gcra_request *__restrict__ rows,
                   u32 *__restrict__ stream_ids, u64 *status, u32 *ticket, uint2 *__restrict__ conn_rows,
                   gcra_grpc_outcome *outcome, u32 *__restrict__ total, u32 *__restrict__ seg_counts, u32 nseg,
-                  u32 cap_shift) {
+                  u32 cap_shift, uint2 *__restrict__ key_ref) {
     extern __shared__ unsigned char grpc_dyn[];
     unsigned char *smem = reinterpret_cast<unsigned char *>((reinterpret_cast<uintptr_t>(grpc_dyn) + 15) & ~(uintptr_t)15);
     __shared__ u32 s_conn;
@@ -422,7 +431,7 @@ grpc_parse_kernel(const unsigned char *__restrict__ in, const gcra_grpc_conn *__
     const gcra_grpc_conn *cn = conns + c;
     grpc_parse_conn(smem, c, cn->off, cn->len, cn, in, n_conns, max_len, now_ns, row_cap, k0, k1, rows, stream_ids,
                     status, conn_rows, [&](const gcra_grpc_outcome &o) { outcome[c] = o; }, total, seg_counts, nseg,
-                    cap_shift);
+                    cap_shift, key_ref);
 }
 
 // resp_reply_kernel for gRPC: row i's response goes on stream stream_ids[i]
@@ -501,7 +510,7 @@ mixed_parse_kernel(const unsigned char *__restrict__ in, const gcra_mixed_conn *
                    gcra_request *__restrict__ rows, u32 *__restrict__ stream_ids, unsigned char *__restrict__ row_proto,
                    u64 *status, u32 *ticket, uint2 *__restrict__ conn_rows, gcra_resp_outcome *outcome,
                    gcra_grpc_outcome *goutcome, u32 *__restrict__ total, u32 *__restrict__ seg_counts, u32 nseg,
-                   u32 cap_shift) {
+                   u32 cap_shift, uint2 *__restrict__ key_ref) {
     extern __shared__ unsigned char mixed_dyn[];
     unsigned char *smem = reinterpret_cast<unsigned char *>((reinterpret_cast<uintptr_t>(mixed_dyn) + 15) & ~(uintptr_t)15);
     __shared__ u32 s_conn;
@@ -524,13 +533,14 @@ mixed_parse_kernel(const unsigned char *__restrict__ in, const gcra_mixed_conn *
             outcome[c] = r;
         };
         br = grpc_parse_conn(smem, c, mc.off, mc.len, gconns + mc.grpc_state, in, n_conns, max_len.z, now_ns, row_cap,
-                             k0, k1, rows, stream_ids, status, conn_rows, emit, total, seg_counts, nseg, cap_shift);
+                             k0, k1, rows, stream_ids, status, conn_rows, emit, total, seg_counts, nseg, cap_shift,
+                             key_ref);
     } else if (mc.protocol == GCRA_PROTO_HTTP) {
         br = resp_parse_conn<HttpTraits>(smem, c, mc.off, mc.len, in, n_conns, max_len.y, now_ns, row_cap, k0, k1, rows,
-                                         status, conn_rows, outcome, total, seg_counts, nseg, cap_shift);
+                                         status, conn_rows, outcome, total, seg_counts, nseg, cap_shift, key_ref);
     } else {
         br = resp_parse_conn<RespTraits>(smem, c, mc.off, mc.len, in, n_conns, max_len.x, now_ns, row_cap, k0, k1, rows,
-                                         status, conn_rows, outcome, total, seg_counts, nseg, cap_shift);
+                                         status, conn_rows, outcome, total, seg_counts, nseg, cap_shift, key_ref);
     }
     for (u32 k = threadIdx.x; k < br.y; k += RESP_THREADS) row_proto[br.x + k] = (unsigned char)mc.protocol;
 }
@@ -622,6 +632,64 @@ __global__ void mixed_outcome_kernel(const uint2 *__restrict__ conn_rows, const 
     }
 }
 
+// ---- ring metrics: counts per transport and denied keys' names (gcra_ring_metrics) ----
+// One thread per row.  A row's class follows the reference's transports: RESP counts an -ERR reply as allowed and
+// never an error (redis/mod.rs:193-205); HTTP and gRPC answer status != OK with an error (http.rs:148-151,
+// grpc.rs:177-179).  A warp's rows go to the CTA's 9 counters by ballot, the CTA's to HBM in at most 9 atomic adds.
+// A denied row finds its key's entry in the denied table, which finish_batch counted this batch into before the reply
+// stream went on: the probe of denied_tile_flush (an empty word or 64 probes: the key found the table full).  The
+// first row to CAS the entry's length word from GCRA_NAME_UNKNOWN copies its key bytes.
+constexpr u32 RING_METRICS_THREADS = 256, DENIED_PROBES = 64;
+
+__device__ __forceinline__ void ring_metrics_name(const RingMetrics &a, u32 i) {
+    u64 k = a.rows[i].key_hash;
+    if (k == 0) k = 1;                                          // (as denied_tile_add stores it)
+    u32 h = (u32)(mix64(k ^ 0x9E3779B97F4A7C15ULL)) & a.denied_mask;
+    for (u32 probe = 0; probe < DENIED_PROBES; probe++) {
+        const u64 cur = a.denied_keys[h];
+        if (cur == 0) return;
+        if (cur == k) {
+            if (a.name_len[h] != GCRA_NAME_UNKNOWN) return;     // (most denials are of keys named already)
+            const uint2 kr = a.key_ref[i];
+            const u32 len = kr.y > GCRA_DENIED_NAME_MAX ? GCRA_NAME_TOO_LONG : kr.y;
+            if (atomicCAS(&a.name_len[h], GCRA_NAME_UNKNOWN, len) != GCRA_NAME_UNKNOWN || len == GCRA_NAME_TOO_LONG) return;
+            unsigned char *dst = a.names + (size_t)h * GCRA_DENIED_NAME_MAX;
+            for (u32 b = 0; b < len; b++) dst[b] = a.in[kr.x + b];
+            return;
+        }
+        h = (h + 1) & a.denied_mask;
+    }
+}
+
+__global__ void __launch_bounds__(RING_METRICS_THREADS) ring_metrics_kernel(RingMetrics a) {
+    __shared__ u32 cnt[9];
+    if (threadIdx.x < 9) cnt[threadIdx.x] = 0;
+    __syncthreads();
+    const u32 i = blockIdx.x * RING_METRICS_THREADS + threadIdx.x, total = *a.total;
+    u32 cls = 9;                                                // (no row)
+    if (i < total) {
+        const u32 proto = a.row_proto ? a.row_proto[i] : a.proto;
+        // status | allowed << 32: the second half of the 32-byte result row
+        const longlong2 tail = reinterpret_cast<const longlong2 *>(a.res + i)[1];
+        const bool ok = (u32)tail.y == GCRA_OK, denied = ok && ((tail.y >> 32) & 0xff) == 0;
+        cls = (proto - 1) * 3 + (denied ? 1 : ok || proto == GCRA_PROTO_RESP ? 0 : 2);
+        if (denied && a.denied_keys) ring_metrics_name(a, i);
+    }
+#pragma unroll
+    for (u32 k = 0; k < 9; k++) {
+        const u32 b = __ballot_sync(0xffffffffu, cls == k);
+        if ((threadIdx.x & 31) == 0 && b) atomicAdd(&cnt[k], (u32)__popc(b));
+    }
+    __syncthreads();
+    if (threadIdx.x < 9 && cnt[threadIdx.x])
+        atomicAdd(reinterpret_cast<unsigned long long *>(a.counts + threadIdx.x), (unsigned long long)cnt[threadIdx.x]);
+}
+
+cudaError_t launch_ring_metrics(const RingMetrics &a, u32 max_rows, cudaStream_t st) {
+    ring_metrics_kernel<<<(max_rows + RING_METRICS_THREADS - 1) / RING_METRICS_THREADS, RING_METRICS_THREADS, 0, st>>>(a);
+    return cudaGetLastError();
+}
+
 // ---- launches (gcra_resp.inc) ----
 cudaError_t resp_ring_setup() {
     cudaFuncAttributes a;
@@ -630,7 +698,7 @@ cudaError_t resp_ring_setup() {
                           (const void *)resp_outcome_kernel, (const void *)grpc_parse_kernel,
                           (const void *)grpc_reply_kernel, (const void *)grpc_outcome_kernel,
                           (const void *)mixed_parse_kernel, (const void *)mixed_reply_kernel,
-                          (const void *)mixed_outcome_kernel}) {
+                          (const void *)mixed_outcome_kernel, (const void *)ring_metrics_kernel}) {
         const cudaError_t e = cudaFuncGetAttributes(&a, k);    // (loads the code now: see preload in gcra_b200.cu)
         if (e) return e;
     }
@@ -651,7 +719,7 @@ template <class P>
 static cudaError_t launch_parse(const RespParse &a, cudaStream_t st) {
     resp_parse_kernel<P><<<a.n_conns, RESP_THREADS, RespSmem(a.max_len, P::CAND_PER_WORD).total, st>>>(
         a.in, a.conns, a.n_conns, a.max_len, a.now_ns, a.row_cap, a.k0, a.k1, a.rows, a.status, a.ticket, a.conn_rows,
-        a.outcome, a.total, a.seg_counts, a.nseg, a.cap_shift);
+        a.outcome, a.total, a.seg_counts, a.nseg, a.cap_shift, a.key_ref);
     return cudaGetLastError();
 }
 
@@ -680,7 +748,7 @@ cudaError_t launch_resp_outcome(u32 n_conns, const uint2 *conn_rows, const u32 *
 cudaError_t launch_grpc_parse(const GrpcParse &a, cudaStream_t st) {
     grpc_parse_kernel<<<a.n_conns, RESP_THREADS, GrpcSmem(a.max_len).total, st>>>(
         a.in, a.conns, a.n_conns, a.max_len, a.now_ns, a.row_cap, a.k0, a.k1, a.rows, a.stream_ids, a.status, a.ticket,
-        a.conn_rows, a.outcome, a.total, a.seg_counts, a.nseg, a.cap_shift);
+        a.conn_rows, a.outcome, a.total, a.seg_counts, a.nseg, a.cap_shift, a.key_ref);
     return cudaGetLastError();
 }
 
@@ -701,7 +769,7 @@ cudaError_t launch_mixed_parse(const MixedParse &a, cudaStream_t st) {
     mixed_parse_kernel<<<a.n_conns, RESP_THREADS, mixed_parse_smem(a.max_len[0], a.max_len[1], a.max_len[2]), st>>>(
         a.in, a.conns, a.n_conns, a.gconns, make_uint3(a.max_len[0], a.max_len[1], a.max_len[2]), a.now_ns, a.row_cap,
         a.k0, a.k1, a.rows, a.stream_ids, a.row_proto, a.status, a.ticket, a.conn_rows, a.outcome, a.goutcome, a.total,
-        a.seg_counts, a.nseg, a.cap_shift);
+        a.seg_counts, a.nseg, a.cap_shift, a.key_ref);
     return cudaGetLastError();
 }
 

@@ -53,6 +53,7 @@ struct RespParse {
     u32 *total, *seg_counts;     // out: rows of the batch, rows of each segment
     u32 nseg, cap_shift;
     RingProto proto;
+    uint2 *key_ref;              // [row_capacity] out, or null: each row's key {offset in `in`, length}
 };
 
 // a protocol's rows per reply tile (the reply kernel stages a tile's replies in shared memory); a mixed ring's tile
@@ -90,6 +91,7 @@ struct GrpcParse {
     gcra_grpc_outcome *outcome;  // [n_conns] out (pinned host memory)
     u32 *total, *seg_counts;
     u32 nseg, cap_shift;
+    uint2 *key_ref;              // as in RespParse
 };
 cudaError_t launch_grpc_parse(const GrpcParse &a, cudaStream_t st);
 cudaError_t launch_grpc_reply(u32 tiles, const gcra_request *rows, const gcra_result *res, const u32 *stream_ids,
@@ -126,6 +128,7 @@ struct MixedParse {
     gcra_grpc_outcome *goutcome; // [gRPC connections] out (pinned host memory)
     u32 *total, *seg_counts;
     u32 nseg, cap_shift;
+    uint2 *key_ref;              // as in RespParse
 };
 cudaError_t launch_mixed_parse(const MixedParse &a, cudaStream_t st);
 // ctrl: word 0 the ticket, then one status word per tile of MIXED_REPLY_THREADS rows; all zero
@@ -136,6 +139,25 @@ cudaError_t launch_mixed_outcome(u32 n_conns, const uint2 *conn_rows, const gcra
                                  const gcra_request *rows, const gcra_result *res, const u32 *total,
                                  const u64 *row_off, gcra_resp_outcome *outcome, gcra_grpc_outcome *goutcome,
                                  cudaStream_t st);
+
+// ring_metrics_kernel's arguments (gcra_ring_metrics): a finished slot's rows, counted per transport into
+// counts[3 transports][allowed, denied, errors], and their denied keys named from the slot's input
+struct RingMetrics {
+    const gcra_request *rows;
+    const gcra_result *res;
+    const unsigned char *row_proto;  // each row's GCRA_PROTO_* (mixed ring), or null: every row is `proto`'s
+    u32 proto;
+    const u32 *total;                // rows of the batch
+    const uint2 *key_ref;            // each row's key {offset in `in`, length} (the parse kernel's key_ref)
+    const unsigned char *in;         // the slot's device input
+    u64 *counts;                     // [9]
+    const u64 *denied_keys;          // the denied table's keys (DeniedTable::keys), or null: no names
+    u32 denied_mask;                 // its entries - 1
+    u32 *name_len;                   // [entries] GCRA_NAME_UNKNOWN, GCRA_NAME_TOO_LONG or the name's length
+    unsigned char *names;            // [entries][GCRA_DENIED_NAME_MAX]
+};
+// one thread per row of [0, *total), max_rows >= *total
+cudaError_t launch_ring_metrics(const RingMetrics &a, u32 max_rows, cudaStream_t st);
 
 cudaError_t resp_ring_setup();   // once, before the first launch
 cudaError_t launch_resp_parse(const RespParse &a, cudaStream_t st);

@@ -21,7 +21,8 @@ import struct
 
 import numpy as np
 
-from . import REQ_DTYPE, RES_DTYPE, GRPC_REPLY_MAX, GRPC_MAX_DYN, _native
+from . import REQ_DTYPE, RES_DTYPE, GRPC_REPLY_MAX, GRPC_MAX_DYN, OK, _native
+from .metrics import Metrics
 
 PREFACE = b"PRI * HTTP/2.0\r\n\r\nSM\r\n\r\n"
 PATH = b"/throttlecrab.RateLimiter/Throttle"
@@ -372,6 +373,7 @@ class Connection:
         self.closed = False
         self.first_settings = False    # the client's SETTINGS have arrived
         self.n_throttle = 0
+        self.metrics = None            # (general's `metrics`, for the calls it decides)
 
     def state(self, row):
         """write this connection's state into a GRPC_CONN_DTYPE row (not off / len)"""
@@ -403,9 +405,11 @@ class Connection:
             self.out += frame(PING, ACK, 0, bytes(o["ping_opaque"]))
 
     # -- the general path --
-    def general(self, limiter, now_ns):
+    def general(self, limiter, now_ns, metrics=None):
         """Take frames off `buf` until no stream is open and nothing is pending (at least one frame, or the preface).
-        Returns the Throttle decisions made."""
+        Returns the Throttle decisions made.  A metrics.Metrics as `metrics` records each Throttle call decided here
+        as grpc.rs:170-180 does: an error when the engine returns a status other than OK, else allowed or denied."""
+        self.metrics = metrics
         before = self.n_throttle
         try:
             if not self.preface:
@@ -612,6 +616,11 @@ class Connection:
         row[0] = (limiter.store.hash_key(key), b, c, p, q, now_ns)
         res = limiter.rate_limit_batch(row)
         self.n_throttle += 1
+        if isinstance(self.metrics, Metrics):
+            if int(res[0]["status"]) != OK:
+                self.metrics.record_error("grpc")
+            else:
+                self.metrics.record_request("grpc", bool(res[0]["allowed"]), key)
         out, _ = format_replies(row, res, [sid])
         frames, i = [], 0
         while i < len(out):
@@ -660,14 +669,18 @@ def host_walk(cn, limiter, now_ns, max_calls=1 << 20):
     return o, out, req[:n], res, sids[:n]
 
 
-def process_connections(conns, limiter, now_ns, ring, slot=0):
+def process_connections(conns, limiter, now_ns, ring, slot=0, metrics=None):
     """Serve every Connection in `conns` from its received bytes: rounds in which the GPU (`ring`, a GrpcRing of
     `limiter`'s engine; None: the host walk, gcra_grpc_parse_throttle, one connection at a time, with keys hashed as
     limiter.store.hash_key hashes them) takes every ready connection's plain prefix, in list order, one batch per submit; then each
     connection that stopped at a frame that is not plain (or has not yet finished its preface, or has a stream open)
     takes the general path until no stream is open, in list order, deciding its calls there and then.  Each
-    connection's `buf` must hold at most 65,536 bytes.  Returns the Throttle decisions made per connection."""
+    connection's `buf` must hold at most 65,536 bytes.  Returns the Throttle decisions made per connection.
+    `metrics`, a metrics.Metrics of `limiter`'s engine, records the calls of the general path; the GPU counts the
+    ring's rows.  It needs a ring: the host walk has no key positions to name denied keys from (ValueError)."""
     from . import RESP_MAX_CONN_BYTES
+    if ring is None and isinstance(metrics, Metrics):
+        raise ValueError("metrics need a ring: the host walk does not name denied keys")
     now = int(now_ns)
     for cn in conns:
         if len(cn.buf) > (RESP_MAX_CONN_BYTES if ring is None else min(RESP_MAX_CONN_BYTES, ring.in_capacity)):
@@ -719,7 +732,7 @@ def process_connections(conns, limiter, now_ns, ring, slot=0):
             if st != 2:
                 continue
             had = len(cn.buf)
-            cn.general(limiter, now)
+            cn.general(limiter, now, metrics)
             if not cn.closed and cn.buf and len(cn.buf) < had and cn.plain_ready:
                 nxt.append(cn)
         live = nxt

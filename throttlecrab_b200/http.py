@@ -25,7 +25,8 @@ import ctypes as C
 
 import numpy as np
 
-from . import REQ_DTYPE, RES_DTYPE, HTTP_REPLY_MAX, _native
+from . import REQ_DTYPE, RES_DTYPE, HTTP_REPLY_MAX, OK, _native
+from .metrics import Metrics
 from .resp import ring_rounds
 
 I64_MIN, I64_MAX = -2**63, 2**63 - 1
@@ -489,7 +490,8 @@ def format_replies(req, res):
 def handle_request(req, limiter, now_ns, metrics=None):
     """Answer one Request -> (response bytes, n_throttle, close).  A THROTTLE is decided on its own through
     limiter.rate_limit_batch with the key hashed by limiter.store.hash_key; `metrics` (a callable returning text)
-    serves GET /metrics, which is 404 without it."""
+    serves GET /metrics, which is 404 without it.  A metrics.Metrics also records the THROTTLE: an error when the
+    engine returns a status other than OK (the 500 response), else allowed or denied with its key."""
     now = int(now_ns)
     close = req.close
     if req.bad is not None:
@@ -517,7 +519,13 @@ def handle_request(req, limiter, now_ns, metrics=None):
         return response(e.status, (prefix + str(e)).encode(), now, TEXT, close=close), 0, close
     row = np.zeros(1, REQ_DTYPE)
     row[0] = (limiter.store.hash_key(key.encode()), b, c, p, q, now)
-    out = format_replies(row, limiter.rate_limit_batch(row))
+    res = limiter.rate_limit_batch(row)
+    if isinstance(metrics, Metrics):                       # (http.rs:146-160)
+        if int(res[0]["status"]) != OK:
+            metrics.record_error("http")
+        else:
+            metrics.record_request("http", bool(res[0]["allowed"]), key)
+    out = format_replies(row, res)
     if close:                                              # hyper's connection header, after the handler's
         i = out.index(b"\r\n", out.index(b"\r\n") + 2) + 2
         out = out[:i] + b"connection: close\r\n" + out[i:]

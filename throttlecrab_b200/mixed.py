@@ -14,6 +14,7 @@ from . import REQ_DTYPE, RES_DTYPE, RESP_MAX_CONN_BYTES, RESP_REPLY_MAX, HTTP_RE
 from . import grpc_transport as _gt
 from . import http as _http
 from . import resp as _resp
+from .metrics import Metrics
 
 PROTOCOLS = {"resp": PROTO_RESP, "http": PROTO_HTTP, "grpc": PROTO_GRPC}
 # the smallest plain frame of RESP and HTTP (gcra_resp.cuh, gcra_http.cuh MIN_FRAME_BYTES): room for a walk's rows
@@ -60,7 +61,13 @@ def process_connections(conns, limiter, now_ns, ring, slot=0, metrics=None):
     request that is not plain takes its own protocol's general path: a RESP or HTTP connection for that one request,
     a gRPC connection (also one that was not ready) until no stream is open.  A Throttle request there is decided there
     and then, on its own.  Connections that share keys see each other's requests in that order, whatever their
-    transports."""
+    transports.
+
+    A metrics.Metrics as `metrics` is GET /metrics for the HTTP connections, and records every request the general
+    paths decide as the reference's transports do (the GPU counts the ring's rows).  It needs a ring: the host walks
+    have no key positions to name denied keys from (ValueError)."""
+    if ring is None and isinstance(metrics, Metrics):
+        raise ValueError("metrics need a ring: the host walks do not name denied keys")
     now = int(now_ns)
     room = RESP_MAX_CONN_BYTES if ring is None else min(RESP_MAX_CONN_BYTES, ring.in_capacity)
     for p, cn in conns:
@@ -147,12 +154,12 @@ def process_connections(conns, limiter, now_ns, ring, slot=0, metrics=None):
             p, cn = conns[c]
             if p == "grpc":
                 had = len(cn.buf)
-                cn.general(limiter, now)
+                cn.general(limiter, now, metrics)
                 if not cn.closed and cn.buf and len(cn.buf) < had and cn.plain_ready:
                     nxt.append(c)
                 continue
             data = datas[c][pos[c]:]
-            g = _resp.general(data, limiter, now) if p == "resp" else _http.general(data, limiter, now, metrics)
+            g = _resp.general(data, limiter, now, metrics) if p == "resp" else _http.general(data, limiter, now, metrics)
             if g is None:
                 continue
             used, reply, k, close[c] = g

@@ -11,6 +11,7 @@ replies in command order.  Host-side glue only: no decision is made here.
 import numpy as np
 
 from . import REQ_DTYPE, NS, hash_key, OK, NEGATIVE_QUANTITY, INVALID_RATE_LIMIT
+from .metrics import Metrics
 
 MAX_BULK_STRING_SIZE = 512 * 1024 * 1024      # resp.rs:8
 MAX_ARRAY_SIZE = 1024 * 1024                  # resp.rs:9
@@ -213,6 +214,12 @@ def _is_quit(value):
             and value[1][0][1] is not None and value[1][0][1].upper() == "QUIT")
 
 
+def _counted(value):
+    """whether process_command reaches its command match and records the command (redis/mod.rs:156-169,201-205): an
+    array whose first element is a bulk string"""
+    return value[0] == "array" and len(value[1]) > 0 and value[1][0][0] == "bulk" and value[1][0][1] is not None
+
+
 def _throttle_reply(o, limit, quantity):
     st = int(o["status"])
     if st == OK:                                                                 # mod.rs:274-283, types.rs:87-97
@@ -376,7 +383,7 @@ def process_pipeline_native(buffer, limiter, now_ns, ring=None, slot=0):
     return b"".join(out), consumed, n, close
 
 
-def process_connections(buffers, limiter, now_ns, ring, slot=0):
+def process_connections(buffers, limiter, now_ns, ring, slot=0, metrics=None):
     """process_pipeline for many connections at once, with the parsing and the reply formatting of plain THROTTLE
     frames on the GPU: `ring` is a RespRing of `limiter`'s engine.  Returns one (reply_bytes, bytes_consumed,
     n_throttle, close) per buffer, with process_pipeline's meaning; an error or a QUIT closes only its own connection.
@@ -388,16 +395,19 @@ def process_connections(buffers, limiter, now_ns, ring, slot=0):
     the same round when the connections do not fit one).  Then each connection that stopped at a frame that is not a
     plain THROTTLE hands that one frame to the general parser, in list order; a THROTTLE among them is decided there
     and then, on its own.  That is the order in which decisions are made, so connections that share keys see each
-    other's requests in that order."""
+    other's requests in that order.  `metrics` (a metrics.Metrics of `limiter`'s engine) records the commands of the
+    general path as the reference's Redis transport does; the GPU counts the ring's rows."""
     now = int(now_ns)
-    return ring_rounds(buffers, ring, slot, now, lambda data: general(data, limiter, now))
+    return ring_rounds(buffers, ring, slot, now, lambda data: general(data, limiter, now, metrics))
 
 
-def general(data, limiter, now):
+def general(data, limiter, now, metrics=None):
     """The general path of a connection that the batch walk stopped at a frame that is not a plain THROTTLE (stop 2):
     that one frame, at the start of `data`, parsed by RespParser and answered; a THROTTLE among them is decided there
     and then, on its own, with the key hashed by limiter.store.hash_key.  Returns None (the frame is incomplete) or
-    (bytes consumed, reply bytes, THROTTLE decisions, close), close being None, "quit" or "error"."""
+    (bytes consumed, reply bytes, THROTTLE decisions, close), close being None, "quit" or "error".  A Metrics as
+    `metrics` records the command as redis/mod.rs:193-205 does: every command that reaches the command match, allowed
+    unless its THROTTLE reply is an array that starts with 0 (an -ERR reply counts as allowed)."""
     try:
         r = RespParser().parse(data)
     except RespError:
@@ -410,8 +420,12 @@ def general(data, limiter, now):
         req = np.empty(1, REQ_DTYPE)
         req[0] = (limiter.store.hash_key(kb), plan[2], plan[3], plan[4], plan[5], now)
         res = limiter.rate_limit_batch(req)
+        if isinstance(metrics, Metrics):
+            metrics.record_request("redis", not (int(res[0]["status"]) == OK and not res[0]["allowed"]), plan[1])
         return r[1], RespSerializer.serialize(_throttle_reply(res[0], plan[2], plan[5])), 1, \
             "quit" if _is_quit(r[0]) else None
+    if isinstance(metrics, Metrics) and _counted(r[0]):
+        metrics.record_request("redis", True)
     return r[1], RespSerializer.serialize(plan[1]), 0, "quit" if _is_quit(r[0]) else None
 
 
