@@ -394,7 +394,9 @@ int32_t gcra_shard_wait_tick(gcra_engine *h, uint32_t ticks_back, void *stream);
  * gcra_shard_*: within a tick rank r's rows precede rank r+1's; ticks are decided in submission order; every rank
  * submits every tick.  gcra_p2p_prepare allocates the window (cap_rows = most rows a rank submits per tick) and
  * returns its CUDA IPC handle (64 bytes) and its address; the caller hands all ranks' handles (other processes) or
- * addresses (engines of one process) to gcra_p2p_connect. */
+ * addresses (engines of one process) to gcra_p2p_connect.  Given addresses, connect enables peer access to each
+ * window's device that is not the engine's own, so that one process can drive engines on several GPUs.  World 1 is a
+ * valid world: the owner decides its one sender's rows (its inbox is viewed as that segment and an empty one). */
 int32_t gcra_p2p_prepare(gcra_engine *h, int32_t rank, int32_t world, uint32_t cap_rows, void *ipc_handle_out_64,
                          void **window_out);
 int32_t gcra_p2p_connect(gcra_engine *h, const void *ipc_handles_world_x_64, void *const *windows);
@@ -663,6 +665,37 @@ typedef struct {
 int32_t gcra_mixed_ring_create(gcra_engine *h, uint32_t slots, uint32_t max_conns, uint64_t in_capacity,
                                uint32_t row_capacity);
 gcra_mixed_conn *gcra_mixed_ring_conns(gcra_engine *h, uint32_t slot);     /* pinned [max_conns], caller fills */
+
+/* ---- rings over peer memory: N engines' connections served against one hash-sharded table ------------------------
+ * gcra_ring_p2p(h, 1) makes every later submit of the engine's RESP, HTTP, gRPC or mixed ring a peer-memory tick
+ * (gcra_p2p_*): the slot is parsed on this engine's GPU as always, its rows (their count known only on the device)
+ * go to their keys' owners, each owner decides its inbox as one batch, and the results come back into the slot's row
+ * order, where the reply and outcome kernels write replies and outcomes as for any ring.  It refuses (GCRA_INTERNAL,
+ * the engine as it was) when the engine is not gcra_p2p_connect-ed or has no such ring, when row_capacity exceeds the
+ * peer-memory cap (the power of two >= cap_rows), when ring metrics are on, or when any rank's key-hash seed differs
+ * from this engine's (gcra_p2p_prepare publishes each rank's seed in its window).  gcra_ring_metrics(h, 1) refuses
+ * while it is on.  gcra_ring_p2p(h, 0) returns the ring to the engine's own table.
+ *
+ * Contract:
+ *   - Ring ticks and gcra_p2p_submit ticks form ONE tick sequence per rank.  Every rank submits every tick; a ring
+ *     tick of 0 connections is a tick of 0 rows, and rank r's t-th tick may be a ring submit while rank s's is a
+ *     gcra_p2p_submit.
+ *   - Within a tick, rank r's rows precede rank r+1's, and a rank's rows are in its connection table's order.
+ *   - Every connection takes what its protocol's host walk takes at the row cap of ITS OWN rank's slot (the ring
+ *     contracts above); its replies are its protocol's formatter applied to the results decided in that order.
+ *   - A refused submit enqueues nothing.  The caller must still submit that tick (e.g. again, or with 0 connections),
+ *     or the peers' waits give up (gcra_p2p_error).
+ * gcra_resp_ring_submit on such a ring is gcra_resp_ring_submit_route + gcra_resp_ring_submit_finish.  Engines of ONE
+ * process (sharded.connect_local, one GPU or several) use the halves, as with gcra_p2p_submit_route / _finish: every
+ * engine's route of a tick is enqueued before the first finish, and every engine's finish of a tick before the first
+ * route of the next (a route may wait for the device while it makes room in the table, and the device then waits for
+ * the finishes already enqueued; a missing one would leave a wait to give up).  Route validates and parses the slot
+ * and routes its rows; finish decides this rank's inbox, brings the slot's results back and enqueues the replies and outcomes.  No
+ * other tick may be routed on the engine between the two.  gcra_ring_wait / gcra_ring_poll complete the slot after
+ * finish.  The engine's store sweep policy is not applied on these ticks (as on gcra_p2p_submit's). */
+int32_t gcra_ring_p2p(gcra_engine *h, uint32_t on);
+int32_t gcra_resp_ring_submit_route(gcra_engine *h, uint32_t slot, uint32_t n_conns, int64_t now_ns);
+int32_t gcra_resp_ring_submit_finish(gcra_engine *h, uint32_t slot);
 
 /* ---- ring metrics: the server's GET /metrics counts and top denied keys by name (metrics.rs:233-310) -------------
  * Only the rings know which transport a row came from, and they never hand key strings to the host.  With ring

@@ -617,6 +617,20 @@ class RespRing:
     def submit(self, slot, n_conns, now=0):
         self.store._check(self._L.gcra_resp_ring_submit(self._h, slot, n_conns, _ns(now)))
 
+    def peer_memory(self, on=True):
+        """on: every later submit is a peer-memory tick of the engine's gcra_p2p_* ranks (gcra_ring_p2p): the rows
+        are decided on their keys' owners, against the ranks' one sharded table.  Contract: gcra_b200.h."""
+        self.store._check(self._L.gcra_ring_p2p(self._h, 1 if on else 0))
+
+    def submit_route(self, slot, n_conns, now=0):
+        """First half of a peer-memory submit: parse the slot and route its rows to their owners.  Engines of one
+        process route every engine's tick before the first submit_finish."""
+        self.store._check(self._L.gcra_resp_ring_submit_route(self._h, slot, n_conns, _ns(now)))
+
+    def submit_finish(self, slot):
+        """Second half: decide this rank's inbox, bring the slot's results back, write its replies and outcomes."""
+        self.store._check(self._L.gcra_resp_ring_submit_finish(self._h, slot))
+
     def wait(self, slot):
         self.store._check(self._L.gcra_ring_wait(self._h, slot))
 

@@ -185,6 +185,9 @@ SYMBOLS = {
     "gcra_grpc_ring_outcome": (_vp, [_vp, _u32]),
     "gcra_mixed_ring_create": (_i32, [_vp, _u32, _u32, _u64, _u32]),
     "gcra_mixed_ring_conns": (_vp, [_vp, _u32]),
+    "gcra_ring_p2p": (_i32, [_vp, _u32]),
+    "gcra_resp_ring_submit_route": (_i32, [_vp, _u32, _u32, _i64]),
+    "gcra_resp_ring_submit_finish": (_i32, [_vp, _u32]),
     "gcra_ring_metrics": (_i32, [_vp, _u32]),
     "gcra_ring_transport_counts": (_i32, [_vp, _vp]),
     "gcra_denied_names": (_i32, [_vp, _u32, _vp, _vp, _vp]),

@@ -83,6 +83,8 @@ struct RingSlot {
     DevBuf<unsigned char> row_proto;
     // ring metrics (gcra_ring_metrics): each row's key {offset in d_in, length}, written by the parse kernels
     DevBuf<uint2> key_ref;
+    // a peer-memory tick routed from this slot (gcra_resp_ring_submit_route): its connections and the bound of its rows
+    uint32_t routed_conns = 0, routed_rows = 0;
 };
 }  // namespace
 
@@ -172,7 +174,9 @@ struct P2PSlot {
     DevBuf<SegDesc> segs_dev;          // [world] segment r of this inbox slot: sender r's rows, sender r's outbox
     Event ev_ready, ev_wait, ev_done;
     bool used = false;
-    uint32_t n = 0;
+    uint32_t n = 0;                    // rows routed, or (dev_n) a bound of them
+    const u32 *dev_n = nullptr;        // a ring tick's row count on the device (gcra_resp_ring_submit_route)
+    bool room_reserved = false;        // a ring tick made its room in the table before its route (p2p_room)
 };
 
 struct P2P {
@@ -182,6 +186,8 @@ struct P2P {
     size_t window_bytes = 0, inbox_off = 0, outbox_off = 0;
     IpcMapping peer_map[P2P_MAX_WORLD];    // the windows of other processes' ranks (gcra_p2p_connect with IPC handles)
     bool connected = false, routed_pending = false;
+    int ring_slot_pending = -1;            // the ring slot whose tick was routed (gcra_resp_ring_submit_route)
+    P2PPeers peers_host;                   // peers_dev as this process addresses it
     DevBuf<P2PPeers> peers_dev;
     DevBuf<u32> tile_counts;
     Stream s_part, s_wait, s_sig, s_return;
@@ -367,6 +373,7 @@ struct gcra_engine {
     // ring metrics (gcra_ring_metrics): ring rows per transport [3][allowed, denied, errors]
     bool ring_metrics = false;
     DevBuf<u64> ring_counts;
+    bool ring_p2p = false;           // gcra_ring_p2p: every ring submit is a peer-memory tick
     uint64_t hash_seed[2] = {0, 0};  // SipHash key of the string-keyed entry points ((0,0): the unkeyed gcra_hash_key)
     // background saves (gcra_snapshot_begin); gcra_destroy joins the writer thread before anything is released
     std::unique_ptr<SnapshotStaging> snap;
@@ -1075,11 +1082,12 @@ static BatchPlan plan_pipelined(gcra_engine *h, uint32_t k, const BatchView &v, 
 // ingest + sort, stage 2 = decide, after every earlier batch has completely finished.
 // `ready` (may be null) is an event after which the requests may be read; `*done` is set to an event after which
 // the results are complete.
+// room_reserved: the caller has made room in the table for n_rows already (ensure_room).
 static int launch_pipelined_view(gcra_engine *h, const BatchView &v, uint32_t n_rows, int fmt, int64_t now_batch,
-                                 cudaEvent_t ready, cudaEvent_t *done) {
+                                 cudaEvent_t ready, cudaEvent_t *done, bool room_reserved = false) {
     // 16-byte results are a single-GPU format: the multi-GPU ticks return 32-byte rows into peers' outboxes
     if (res_bytes(fmt) == sizeof(gcra_result16) && v.nseg != 1) { h->err = "16-byte results need a single-segment batch"; return GCRA_INTERNAL; }
-    RC(check_batch(h, n_rows, fmt));
+    if (!room_reserved) RC(check_batch(h, n_rows, fmt));
     const uint32_t k = h->scr_next;
     h->scr_next = (h->scr_next + 1) % gcra_engine::N_SCR;
     const Lanes on = {h->front_stream.get(), h->back_stream.get(), h->tail_stream.get()};   // (all sets share one front stream, see gcra_create)
@@ -1144,6 +1152,7 @@ static void preload_kernels() {
     preload(route_count_kernel); preload(route_scan_kernel); preload(route_scatter_kernel); preload(route_unpermute_kernel);
     preload(p2p_scan_kernel); preload(p2p_scatter_kernel); preload(p2p_signal_req_kernel); preload(p2p_signal_res_kernel);
     preload(p2p_wait_kernel); preload(p2p_unpermute_kernel);
+    preload(route_count_dev_kernel); preload(p2p_scatter_dev_kernel); preload(p2p_unpermute_dev_kernel);
     preload(snapshot_capture_kernel); preload(denied_count_seg_kernel); preload(hash_keys_kernel);
 }
 
@@ -1817,6 +1826,7 @@ int32_t gcra_top_denied(gcra_engine *h, uint32_t k, uint64_t *key_hashes, uint64
 // ---- ring metrics (metrics.rs:233-310: requests by transport, top denied keys by name) ------------------------------
 int32_t gcra_ring_metrics(gcra_engine *h, uint32_t on) {
     CK(cudaSetDevice(h->device));
+    if (on && h->ring_p2p) { h->err = "ring metrics: the ring's ticks are peer-memory ticks (gcra_ring_p2p)"; return GCRA_INTERNAL; }
     if (on && h->denied_max > GCRA_RING_METRICS_MAX_KEYS) {
         h->err = "ring metrics: denied tracking runs with max_keys above 10,000";
         return GCRA_INTERNAL;
@@ -2505,6 +2515,11 @@ int32_t gcra_shard_join(gcra_engine *h, void *stream) {
 // ---- multi-GPU over NVLink peer memory: the whole sharded tick without NCCL and without a host sync ------------
 static size_t align_up(size_t x, size_t a) { return (x + a - 1) / a * a; }
 
+// segments of the owner's view of an inbox slot: one per sender, and at least 2 -- a view of one segment is a batch
+// whose row count the host knows (BatchView), so world 1 adds an empty second segment (its count stays 0).  Without
+// it a world-1 tick, bulk (gcra_p2p_submit) or ring, ran the single-segment path over a view with no rows and failed.
+static uint32_t p2p_segs(int world) { return (uint32_t)std::max(world, 2); }
+
 int32_t gcra_p2p_prepare(gcra_engine *h, int32_t rank, int32_t world, uint32_t cap_rows, void *ipc_handle_out_64,
                          void **window_out) {
     CK(cudaSetDevice(h->device));
@@ -2522,6 +2537,8 @@ int32_t gcra_p2p_prepare(gcra_engine *h, int32_t rank, int32_t world, uint32_t c
     p->window_bytes = align_up(p->outbox_off + seg_rows * sizeof(gcra_result), 256);
     CK(p->window.make(p->window_bytes));
     CK(cudaMemset(p->window.get(), 0, p->inbox_off));
+    CK(cudaMemcpy((char *)p->window.get() + offsetof(P2PHeader, seed), h->hash_seed, sizeof(h->hash_seed),
+                  cudaMemcpyHostToDevice));
     if (ipc_handle_out_64) {
         cudaIpcMemHandle_t hd;
         CK(cudaIpcGetMemHandle(&hd, p->window.get()));
@@ -2541,13 +2558,13 @@ int32_t gcra_p2p_prepare(gcra_engine *h, int32_t rank, int32_t world, uint32_t c
     }
     // the engine's per-row buffers now span the row-id space of a whole inbox slot
     CK(cudaDeviceSynchronize());
-    RC(alloc_index_scratch(h, (uint32_t)world << p->cap_shift));
+    RC(alloc_index_scratch(h, (uint32_t)p2p_segs(world) << p->cap_shift));
     h->p2p = std::move(p);
     return GCRA_OK;
 }
 
 // every rank's window: `ipc_handles` (world x 64 bytes, other processes) or `windows` (world pointers valid in THIS
-// process: engines that share a process, e.g. the single-GPU loop-back test)
+// process: engines that share a process, on one GPU or several -- a window on another device gets peer access)
 int32_t gcra_p2p_connect(gcra_engine *h, const void *ipc_handles, void *const *windows) {
     CK(cudaSetDevice(h->device));
     P2P *p = h->p2p.get();
@@ -2557,8 +2574,16 @@ int32_t gcra_p2p_connect(gcra_engine *h, const void *ipc_handles, void *const *w
     for (int r = 0; r < p->world; r++) {
         void *base = nullptr;
         if (r == p->rank) base = p->window.get();
-        else if (windows) base = windows[r];
-        else {
+        else if (windows) {
+            base = windows[r];
+            cudaPointerAttributes at;
+            CK(cudaPointerGetAttributes(&at, base));
+            if (at.type == cudaMemoryTypeDevice && at.device != h->device) {
+                const cudaError_t e = cudaDeviceEnablePeerAccess(at.device, 0);
+                if (e == cudaErrorPeerAccessAlreadyEnabled) (void)cudaGetLastError();
+                else CK(e);
+            }
+        } else {
             cudaIpcMemHandle_t hd;
             memcpy(&hd, (const char *)ipc_handles + 64 * r, 64);
             CK(p->peer_map[r].make(hd));
@@ -2569,6 +2594,7 @@ int32_t gcra_p2p_connect(gcra_engine *h, const void *ipc_handles, void *const *w
         peers.outbox[r] = (unsigned char *)base + p->outbox_off;
     }
     CK(cudaMemcpy(p->peers_dev.get(), &peers, sizeof(peers), cudaMemcpyHostToDevice));
+    p->peers_host = peers;
     for (int d = 0; d < P2P_DEPTH; d++) {
         SegDesc segs[P2P_MAX_WORLD] = {};
         for (int r = 0; r < p->world; r++) {
@@ -2577,20 +2603,30 @@ int32_t gcra_p2p_connect(gcra_engine *h, const void *ipc_handles, void *const *w
             segs[r].req = peers.inbox[p->rank] + (((size_t)d * p->world + r) << p->cap_shift) * sizeof(gcra_request);
             segs[r].res = (gcra_result *)(peers.outbox[r] + (((size_t)d * p->world + p->rank) << p->cap_shift) * sizeof(gcra_result));
         }
+        for (int r = p->world; r < (int)p2p_segs(p->world); r++) segs[r] = segs[0];   // (world 1: 0 rows)
         CK(cudaMemcpy(p->slots[d].segs_dev.get(), segs, sizeof(segs), cudaMemcpyHostToDevice));
     }
     p->connected = true;
     return GCRA_OK;
 }
 
-// first half of a tick: the sender's side (partition + transfer + flags)
-int32_t gcra_p2p_submit_route(gcra_engine *h, uint64_t n64, const gcra_request *d_req, void *ready_stream) {
-    CK(cudaSetDevice(h->device));
+// Room in the table for the keys a tick of n rows from this rank may insert.  How many rows arrive is only known on the
+// device; with a hash-sharded key space it is about what this rank submitted itself, so 1.25 x that (+ slack) is
+// reserved -- a reservation of the full inbox would make the host wait for the device every tick.  Should a tick bring
+// more NEW keys than the table has room for, the surplus rows are answered with GCRA_INTERNAL ("table full"), as
+// find_or_claim always does; the next tick's check then sees the real occupancy and grows the table.  (A ring tick's n
+// is the host's bound of its rows.)
+static uint32_t p2p_room(gcra_engine *h, uint32_t n) {
+    const P2P *p = h->p2p.get();
+    return (uint32_t)std::min<uint64_t>((uint64_t)n + n / 4 + 4096, std::min<uint64_t>((uint64_t)p->world << p->cap_shift, h->max_batch));
+}
+
+// first half of a tick: the sender's side (partition + transfer + flags).  n rows at d_req, or, with dev_n, the
+// *dev_n <= n rows there (a ring slot's parsed rows: the grids are sized from the bound n).  s_part starts after
+// `ready`.
+static int p2p_route(gcra_engine *h, uint32_t n, const u32 *dev_n, const gcra_request *d_req, cudaEvent_t ready,
+                     bool room_reserved = false) {
     P2P *p = h->p2p.get();
-    if (!p || !p->connected) { h->err = "gcra_p2p_prepare / gcra_p2p_connect first"; return GCRA_INTERNAL; }
-    if (p->routed_pending) { h->err = "gcra_p2p_submit_finish the previous tick first"; return GCRA_INTERNAL; }
-    if (n64 > p->cap) { h->err = "tick larger than cap_rows"; return GCRA_INTERNAL; }
-    const uint32_t n = (uint32_t)n64;
     const uint32_t W = (uint32_t)p->world, me = (uint32_t)p->rank;
     const uint64_t tick = ++p->next_tick;
     const uint32_t d = (uint32_t)((tick - 1) % P2P_DEPTH);
@@ -2598,19 +2634,23 @@ int32_t gcra_p2p_submit_route(gcra_engine *h, uint64_t n64, const gcra_request *
     // slot d again: its previous tick has been un-permuted here, i.e. every owner is through with my rows of that
     // tick and with my outbox slot
     if (sl.used) CK(cudaStreamWaitEvent(p->s_part.get(), sl.ev_done.get(), 0));
-    sl.used = true; sl.n = n;
-    if (ready_stream) {
-        CK(cudaEventRecord(sl.ev_ready.get(), (cudaStream_t)ready_stream));
-        CK(cudaStreamWaitEvent(p->s_part.get(), sl.ev_ready.get(), 0));
-    }
+    sl.used = true; sl.n = n; sl.dev_n = dev_n; sl.room_reserved = room_reserved;
+    if (ready) CK(cudaStreamWaitEvent(p->s_part.get(), ready, 0));
     // stable partition by owner, rows stored straight into the owners' inboxes, then the flags
     const uint32_t tiles = (n + TILE_THREADS - 1) / TILE_THREADS;
     if (p->timed) CK(cudaEventRecord(p->ev_t[0].get(), p->s_part.get()));
     if (n) {
-        route_count_kernel<<<tiles, TILE_THREADS, 0, p->s_part.get()>>>(d_req, n, W, tiles, p->tile_counts.get());
+        if (dev_n)
+            route_count_dev_kernel<<<tiles, TILE_THREADS, 0, p->s_part.get()>>>(d_req, n, dev_n, W, tiles, p->tile_counts.get());
+        else
+            route_count_kernel<<<tiles, TILE_THREADS, 0, p->s_part.get()>>>(d_req, n, W, tiles, p->tile_counts.get());
         p2p_scan_kernel<<<W, TILE_THREADS, 0, p->s_part.get()>>>(p->tile_counts.get(), tiles, sl.counts_dev.get());
-        p2p_scatter_kernel<<<tiles, TILE_THREADS, 0, p->s_part.get()>>>(d_req, n, W, me, d, p->cap_shift, tiles, p->tile_counts.get(),
-                                                                 p->peers_dev.get(), sl.res_loc.get());
+        if (dev_n)
+            p2p_scatter_dev_kernel<<<tiles, TILE_THREADS, 0, p->s_part.get()>>>(d_req, n, dev_n, W, me, d, p->cap_shift, tiles,
+                                                                         p->tile_counts.get(), p->peers_dev.get(), sl.res_loc.get());
+        else
+            p2p_scatter_kernel<<<tiles, TILE_THREADS, 0, p->s_part.get()>>>(d_req, n, W, me, d, p->cap_shift, tiles, p->tile_counts.get(),
+                                                                     p->peers_dev.get(), sl.res_loc.get());
         h->launches += 3;
     } else {
         CK(cudaMemsetAsync(sl.counts_dev.get(), 0, W * sizeof(u32), p->s_part.get()));
@@ -2623,12 +2663,25 @@ int32_t gcra_p2p_submit_route(gcra_engine *h, uint64_t n64, const gcra_request *
     return GCRA_OK;
 }
 
-// second half: the owner's side (wait for every sender, decide, results into the senders' outboxes, flags) and the
-// way back (wait for every owner, results into input order)
-int32_t gcra_p2p_submit_finish(gcra_engine *h, gcra_result *d_res) {
+int32_t gcra_p2p_submit_route(gcra_engine *h, uint64_t n64, const gcra_request *d_req, void *ready_stream) {
     CK(cudaSetDevice(h->device));
     P2P *p = h->p2p.get();
-    if (!p || !p->routed_pending) { h->err = "gcra_p2p_submit_route first"; return GCRA_INTERNAL; }
+    if (!p || !p->connected) { h->err = "gcra_p2p_prepare / gcra_p2p_connect first"; return GCRA_INTERNAL; }
+    if (p->routed_pending) { h->err = "gcra_p2p_submit_finish the previous tick first"; return GCRA_INTERNAL; }
+    if (n64 > p->cap) { h->err = "tick larger than cap_rows"; return GCRA_INTERNAL; }
+    cudaEvent_t ready = nullptr;
+    if (ready_stream) {
+        P2PSlot &sl = p->slots[p->next_tick % P2P_DEPTH];     // (the slot this tick takes)
+        CK(cudaEventRecord(sl.ev_ready.get(), (cudaStream_t)ready_stream));
+        ready = sl.ev_ready.get();
+    }
+    return p2p_route(h, (uint32_t)n64, nullptr, d_req, ready);
+}
+
+// second half: the owner's side (wait for every sender, decide, results into the senders' outboxes, flags) and the
+// way back (wait for every owner, results into input order, into d_res); the tick's ev_done follows the last
+static int p2p_finish(gcra_engine *h, gcra_result *d_res) {
+    P2P *p = h->p2p.get();
     p->routed_pending = false;
     const uint32_t W = (uint32_t)p->world, me = (uint32_t)p->rank;
     const uint64_t tick = p->next_tick;
@@ -2644,17 +2697,12 @@ int32_t gcra_p2p_submit_finish(gcra_engine *h, gcra_result *d_res) {
     v.segs = sl.segs_dev.get();
     v.dev_counts = &hdr->counts[d][0];
     v.n = 0;
-    v.nseg = W;
+    v.nseg = p2p_segs(p->world);
     v.cap_shift = p->cap_shift;
     cudaEvent_t done = nullptr;
-    // Room in the table for the keys this tick may insert.  How many rows arrive is only known on the device; with a
-    // hash-sharded key space it is about what this rank submitted itself, so 1.25 x that (+ slack) is reserved -- a
-    // reservation of the full inbox would make the host wait for the device every tick.  Should a tick bring more
-    // NEW keys than the table has room for, the surplus rows are answered with GCRA_INTERNAL ("table full"), as
-    // find_or_claim always does; the next tick's check then sees the real occupancy and grows the table.
-    const uint32_t n_rows = (uint32_t)std::min<uint64_t>((uint64_t)sl.n + sl.n / 4 + 4096, std::min<uint64_t>((uint64_t)W << p->cap_shift, h->max_batch));
+    const uint32_t n_rows = p2p_room(h, sl.n);
     if (p->timed) CK(cudaEventRecord(p->ev_t[2].get(), p->s_wait.get()));
-    RC(launch_pipelined_view(h, v, n_rows, FMT_48_32, 0, sl.ev_wait.get(), &done));
+    RC(launch_pipelined_view(h, v, n_rows, FMT_48_32, 0, sl.ev_wait.get(), &done, sl.room_reserved));
     CK(cudaStreamWaitEvent(p->s_sig.get(), done, 0));
     if (p->timed) CK(cudaEventRecord(p->ev_t[3].get(), p->s_sig.get()));
     p2p_signal_res_kernel<<<1, 32, 0, p->s_sig.get()>>>(p->peers_dev.get(), W, me, tick);
@@ -2663,8 +2711,13 @@ int32_t gcra_p2p_submit_finish(gcra_engine *h, gcra_result *d_res) {
     if (p->timed) CK(cudaEventRecord(p->ev_t[4].get(), p->s_return.get()));
     if (sl.n) {
         const uint32_t tiles = (sl.n + TILE_THREADS - 1) / TILE_THREADS;
-        p2p_unpermute_kernel<<<tiles, TILE_THREADS, 0, p->s_return.get()>>>((const unsigned char *)p->window.get() + p->outbox_off, sl.res_loc.get(),
-                                                                     sl.n, W, d, p->cap_shift, d_res);
+        const unsigned char *outbox = (const unsigned char *)p->window.get() + p->outbox_off;
+        if (sl.dev_n)
+            p2p_unpermute_dev_kernel<<<tiles, TILE_THREADS, 0, p->s_return.get()>>>(outbox, sl.res_loc.get(), sl.n, sl.dev_n, W, d,
+                                                                                 p->cap_shift, d_res);
+        else
+            p2p_unpermute_kernel<<<tiles, TILE_THREADS, 0, p->s_return.get()>>>(outbox, sl.res_loc.get(), sl.n, W, d, p->cap_shift,
+                                                                             d_res);
         h->launches++;
     }
     CK(cudaEventRecord(sl.ev_done.get(), p->s_return.get()));
@@ -2672,6 +2725,13 @@ int32_t gcra_p2p_submit_finish(gcra_engine *h, gcra_result *d_res) {
     h->launches += 3;
     CK(cudaGetLastError());
     return GCRA_OK;
+}
+
+int32_t gcra_p2p_submit_finish(gcra_engine *h, gcra_result *d_res) {
+    CK(cudaSetDevice(h->device));
+    P2P *p = h->p2p.get();
+    if (!p || !p->routed_pending || p->ring_slot_pending >= 0) { h->err = "gcra_p2p_submit_route first"; return GCRA_INTERNAL; }
+    return p2p_finish(h, d_res);
 }
 
 // stage times (ms) of the most recent tick submitted with timing on (gcra_p2p_set_timing(h, 1)) -- meaningful when

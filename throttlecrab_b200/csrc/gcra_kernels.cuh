@@ -1307,9 +1307,9 @@ __host__ __device__ __forceinline__ u32 owner_of(u64 key_hash, u32 n_shards) {
 
 constexpr int ROUTE_MAX_SHARDS = 16;
 
-__global__ void __launch_bounds__(TILE_THREADS)
-route_count_kernel(const gcra_request *__restrict__ req, u32 n, u32 n_shards, u32 num_tiles,
-                   u32 *__restrict__ tile_counts) {
+// (tiles at or past n count zero rows: route_count_dev_kernel sizes its grid from a bound of the device count)
+__device__ __forceinline__ void route_count_tile(const gcra_request *__restrict__ req, u32 n, u32 n_shards,
+                                                 u32 num_tiles, u32 *__restrict__ tile_counts) {
     __shared__ u32 c[ROUTE_MAX_SHARDS];
     if (threadIdx.x < ROUTE_MAX_SHARDS) c[threadIdx.x] = 0;
     __syncthreads();
@@ -1317,6 +1317,19 @@ route_count_kernel(const gcra_request *__restrict__ req, u32 n, u32 n_shards, u3
     if (i < n) atomicAdd(&c[owner_of(req[i].key_hash, n_shards)], 1u);
     __syncthreads();
     if (threadIdx.x < n_shards) tile_counts[threadIdx.x * num_tiles + blockIdx.x] = c[threadIdx.x];
+}
+
+__global__ void __launch_bounds__(TILE_THREADS)
+route_count_kernel(const gcra_request *__restrict__ req, u32 n, u32 n_shards, u32 num_tiles,
+                   u32 *__restrict__ tile_counts) {
+    route_count_tile(req, n, n_shards, num_tiles, tile_counts);
+}
+
+// the row count on the device (a ring slot's parsed rows): min(*dev_n, n_bound) rows, grid sized from n_bound
+__global__ void __launch_bounds__(TILE_THREADS)
+route_count_dev_kernel(const gcra_request *__restrict__ req, u32 n_bound, const u32 *__restrict__ dev_n, u32 n_shards,
+                       u32 num_tiles, u32 *__restrict__ tile_counts) {
+    route_count_tile(req, min(*dev_n, n_bound), n_shards, num_tiles, tile_counts);
 }
 
 // single CTA: exclusive scan of tile_counts in (shard, tile) order; per-shard totals to counts

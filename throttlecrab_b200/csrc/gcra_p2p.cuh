@@ -21,6 +21,8 @@
 // buffer in input order.  Slot d of tick t is reused by tick t + DEPTH; a sender only routes tick t + DEPTH after
 // it has un-permuted tick t, i.e. after every owner published res_tick >= t -- which the owner does after its last
 // read of inbox slot d and its last write to my outbox slot d -- so one flag orders both reuses.
+// A ring tick (gcra_resp_ring_submit_route) knows its row count only on the device: the *_dev_kernel variants read it
+// there and size their grids from the host's bound of it.
 #pragma once
 #include "gcra_index_path.cuh"
 
@@ -34,7 +36,9 @@ struct P2PHeader {
     u64 res_tick[P2P_MAX_WORLD];
     u32 counts[P2P_DEPTH][P2P_MAX_WORLD];
     u32 error;                       // a wait gave up (a peer never arrived): results of that tick are garbage
-    u32 pad[31];
+    u32 pad0;
+    u64 seed[2];                     // the rank's key-hash seed (gcra_p2p_prepare): gcra_ring_p2p checks every rank's
+    u32 pad[26];
 };
 
 // what a rank knows about everybody's window (device memory; index = rank)
@@ -73,10 +77,10 @@ p2p_scan_kernel(u32 *__restrict__ tile_counts, u32 num_tiles, u32 *__restrict__ 
 // will arrive in my outbox.  The tile's rows are first grouped by owner in shared memory, then written out as
 // contiguous 16-byte pieces -- a warp's store covers 512 consecutive bytes of one inbox, which is what NVLink wants
 // (a lane storing the three pieces of its own row would send 16-byte packets).
-__global__ void __launch_bounds__(TILE_THREADS)
-p2p_scatter_kernel(const gcra_request *__restrict__ req, u32 n, u32 world, u32 me, u32 slot, u32 cap_shift,
-                   u32 num_tiles, const u32 *__restrict__ tile_offsets, const P2PPeers *__restrict__ peers,
-                   u32 *__restrict__ res_loc) {
+__device__ __forceinline__ void p2p_scatter_tile(const gcra_request *__restrict__ req, u32 n, u32 world, u32 me,
+                                                 u32 slot, u32 cap_shift, u32 num_tiles,
+                                                 const u32 *__restrict__ tile_offsets,
+                                                 const P2PPeers *__restrict__ peers, u32 *__restrict__ res_loc) {
     constexpr int NW = TILE_THREADS / 32;
     __shared__ u32 wc[NW][ROUTE_MAX_SHARDS];
     __shared__ u32 lbase[ROUTE_MAX_SHARDS + 1];              // first tile-local position of every owner's rows
@@ -133,6 +137,24 @@ p2p_scatter_kernel(const gcra_request *__restrict__ req, u32 n, u32 world, u32 m
     }
 }
 
+__global__ void __launch_bounds__(TILE_THREADS)
+p2p_scatter_kernel(const gcra_request *__restrict__ req, u32 n, u32 world, u32 me, u32 slot, u32 cap_shift,
+                   u32 num_tiles, const u32 *__restrict__ tile_offsets, const P2PPeers *__restrict__ peers,
+                   u32 *__restrict__ res_loc) {
+    p2p_scatter_tile(req, n, world, me, slot, cap_shift, num_tiles, tile_offsets, peers, res_loc);
+}
+
+// the row count on the device (a ring slot's parsed rows, gcra_resp_ring_submit_route): min(*dev_n, n_bound) rows
+// over a grid sized from n_bound; a tile past the count stores nothing (route_count_dev_kernel counted it as empty)
+__global__ void __launch_bounds__(TILE_THREADS)
+p2p_scatter_dev_kernel(const gcra_request *__restrict__ req, u32 n_bound, const u32 *__restrict__ dev_n, u32 world,
+                       u32 me, u32 slot, u32 cap_shift, u32 num_tiles, const u32 *__restrict__ tile_offsets,
+                       const P2PPeers *__restrict__ peers, u32 *__restrict__ res_loc) {
+    const u32 n = min(*dev_n, n_bound);
+    if (blockIdx.x * TILE_THREADS >= n) return;
+    p2p_scatter_tile(req, n, world, me, slot, cap_shift, num_tiles, tile_offsets, peers, res_loc);
+}
+
 // after the scatter kernel: lane p tells owner p how many rows it got and that tick `tick` is complete
 __global__ void p2p_signal_req_kernel(const P2PPeers *__restrict__ peers, const u32 *__restrict__ counts, u32 world,
                                       u32 me, u32 slot, u64 tick) {
@@ -167,9 +189,9 @@ __global__ void p2p_wait_kernel(P2PHeader *__restrict__ hdr, int which, u32 worl
 }
 
 // results back into input order: row i's result sits at outbox segment (slot, owner) position pos
-__global__ void __launch_bounds__(TILE_THREADS)
-p2p_unpermute_kernel(const unsigned char *__restrict__ outbox, const u32 *__restrict__ res_loc, u32 n, u32 world,
-                     u32 slot, u32 cap_shift, gcra_result *__restrict__ out) {
+__device__ __forceinline__ void p2p_unpermute_row(const unsigned char *__restrict__ outbox,
+                                                  const u32 *__restrict__ res_loc, u32 n, u32 world, u32 slot,
+                                                  u32 cap_shift, gcra_result *__restrict__ out) {
     const u32 i = blockIdx.x * TILE_THREADS + threadIdx.x;
     if (i >= n) return;
     const u32 loc = res_loc[i];
@@ -178,6 +200,20 @@ p2p_unpermute_kernel(const unsigned char *__restrict__ outbox, const u32 *__rest
     const ulonglong2 *s = reinterpret_cast<const ulonglong2 *>(outbox + (seg + pos) * sizeof(gcra_result));
     ulonglong2 *d = reinterpret_cast<ulonglong2 *>(out + i);
     d[0] = s[0]; d[1] = s[1];
+}
+
+__global__ void __launch_bounds__(TILE_THREADS)
+p2p_unpermute_kernel(const unsigned char *__restrict__ outbox, const u32 *__restrict__ res_loc, u32 n, u32 world,
+                     u32 slot, u32 cap_shift, gcra_result *__restrict__ out) {
+    p2p_unpermute_row(outbox, res_loc, n, world, slot, cap_shift, out);
+}
+
+// the row count on the device: rows past min(*dev_n, n_bound) are not un-permuted
+__global__ void __launch_bounds__(TILE_THREADS)
+p2p_unpermute_dev_kernel(const unsigned char *__restrict__ outbox, const u32 *__restrict__ res_loc, u32 n_bound,
+                         const u32 *__restrict__ dev_n, u32 world, u32 slot, u32 cap_shift,
+                         gcra_result *__restrict__ out) {
+    p2p_unpermute_row(outbox, res_loc, min(*dev_n, n_bound), world, slot, cap_shift, out);
 }
 
 }  // namespace gcra
