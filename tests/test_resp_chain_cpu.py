@@ -1,4 +1,4 @@
-"""A CPU model of how resp_parse_kernel (csrc/gcra_resp_ring.cu) finds a connection's frames, against the sequential
+"""A CPU model of how ring_parse_kernel<RespTraits> (csrc/gcra_resp_ring.cu) finds a connection's frames, against the sequential
 host walk (gcra_resp_parse_throttle).  The kernel marks every candidate frame start (a '*' at the segment start or
 right after a '\\n'), parses every candidate on its own, then follows the chain of frame ends from the segment start,
 and cuts it at the row cap.  Here each candidate is parsed by the host parser with max_frames = 1, which is the same

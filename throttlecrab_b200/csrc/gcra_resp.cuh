@@ -115,6 +115,18 @@ struct Frame {
     int64_t a[4];
 };
 
+// the request row of a plain frame whose key hashes to key_hash (or is the reference key_hash)
+GCRA_RESP_HD gcra_request request_row(const Frame &fr, uint64_t key_hash, int64_t now_ns) {
+    gcra_request r;
+    r.key_hash = key_hash;
+    r.max_burst = fr.a[0];
+    r.count_per_period = fr.a[1];
+    r.period = fr.a[2];
+    r.quantity = fr.a[3];
+    r.now_ns = now_ns;
+    return r;
+}
+
 // The frame at c.p (c.p < c.end): 0 a plain THROTTLE frame (c.p moves past it, `fr` is filled), 1 it is incomplete
 // (read more), 2 it is anything else (the general parser).  A frame is consumed completely or not at all.
 GCRA_RESP_HD int parse_frame(Cursor &c, Frame &fr) {

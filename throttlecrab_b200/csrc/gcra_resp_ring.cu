@@ -1,40 +1,42 @@
-// gcra_resp_ring.cu -- the RESP, HTTP and gRPC rings' kernels (gcra_resp_ring_*): connections' read buffers -> request
-// rows, and results -> reply bytes.  The frame grammar and the reply text are the host parser's own: gcra_resp.cuh for
-// RESP, gcra_http.cuh for HTTP, brought in by a protocol traits type that the parse and reply kernels are templates
-// over.  A translation unit of its own: the parse kernel's dynamic shared memory would pad every kernel's static
-// shared memory in gcra_b200.cu to 16 bytes.  gcra_b200.cu launches these kernels through the functions at the end.
+// gcra_resp_ring.cu -- the rings' kernels (gcra_resp_ring_*): connections' read buffers -> request rows, and results
+// -> reply bytes.  The frame grammar and the reply text are the host parser's own: gcra_resp.cuh for RESP,
+// gcra_http.cuh for HTTP, gcra_grpc.cuh for gRPC.  A translation unit of its own: the parse kernel's dynamic shared
+// memory would pad every kernel's static shared memory in gcra_b200.cu to 16 bytes.  gcra_b200.cu launches these
+// kernels through the functions at the end.
 //
-//   resp_parse_kernel    one CTA per connection: rows of the connection's plain prefix, exactly what
-//                        gcra_resp_parse_throttle (gcra_http_parse_throttle) writes for it at the row cap that
-//                        connections before it leave
-//   resp_reply_kernel    one thread per row: the reply bytes, packed in row order
-//   resp_outcome_kernel  one thread per connection: where its replies lie
-// and their gRPC counterparts (grpc_parse_kernel, grpc_reply_kernel, grpc_outcome_kernel), which carry each row's
-// stream id and each connection's HTTP/2 state.  The mixed ring's kernels (mixed_parse_kernel, mixed_reply_kernel,
-// mixed_outcome_kernel) take connections of all three protocols in one slot: the parse kernel runs the same parse
-// bodies (resp_parse_conn, grpc_parse_conn), the reply kernel the same reply writers.  ring_metrics_kernel counts a
-// finished slot's rows per transport and names its denied keys (gcra_ring_metrics).
+//   ring_parse_kernel<K>    one CTA per connection: rows of the connection's plain prefix, exactly what its
+//                           protocol's host walk (gcra_resp_parse_throttle, gcra_http_parse_throttle,
+//                           gcra_grpc_parse_throttle) writes for it at the row cap that connections before it leave
+//   ring_reply_kernel<K>    one thread per row: the reply bytes, packed in row order
+//   ring_outcome_kernel<K>  one warp per connection: where its replies lie (and a gRPC connection's DATA octets)
+// Every ring kind -- RespTraits, HttpTraits, GrpcTraits, MixedTraits -- is an instantiation of these three templates.
+// A mixed ring takes connections of all three protocols in one slot: its parse kernel picks each connection's parse
+// body, its reply kernel each row's reply writer.  ring_metrics_kernel counts a finished slot's rows per transport and
+// names its denied keys (gcra_ring_metrics).
 #include "gcra_resp_ring.cuh"
-#include "gcra_http.cuh"
-#include "gcra_grpc.cuh"
 
 namespace gcra {
 
-// What the ring kernels need of a protocol: where a frame may start (`candidate`: every position the parse kernel
-// parses speculatively; `chain_start`: whether the frame that follows the previous one can start here), the grammar,
-// the reply text and its bound, the rows of a reply tile and the parse kernel's candidate room.
+// A ring kind: its protocol, and the parse kernel's CTAs per SM (its min-blocks bound).  Everything else the kernels
+// take of a kind follows from the protocol: the reply tile and bound (reply_tile_rows, reply_max), each connection's
+// parse body (ring_conn: constant but for a mixed ring), each row's reply writer (put_reply: constant but for a mixed
+// ring), and whether the outcome kernel sums DATA octets (where gRPC rows can occur).  RESP and HTTP also carry the
+// grammar of their parse body: where a frame may start (`candidate`: every position the parse kernel parses
+// speculatively; `chain_start`: whether the frame that follows the previous one can start here) and the frame's parse.
 struct RespTraits {
-    static constexpr u32 REPLY_THREADS = RESP_THREADS, REPLY_MAX = gcra_resp::REPLY_MAX, CAND_PER_WORD = 16;
+    // (3 CTAs per SM: the key_ref store would take the parse kernel from 80 to 84 registers, and 2 CTAs per SM, for
+    // short connections; bounded, it fits 80 with no spills)
+    static constexpr RingProto PROTO = PROTO_RESP;
+    static constexpr u32 PARSE_CTAS = 3;
     __device__ static bool candidate(const unsigned char *s, u32 p, u32) { return s[p] == '*' && (p == 0 || s[p - 1] == '\n'); }
     // (a frame ends with "\r\n", so the next one starts at a candidate exactly when its first byte is '*')
     __device__ static bool chain_start(const unsigned char *s, u32 p, u32) { return s[p] == '*'; }
     __device__ static int parse(gcra_resp::Cursor &c, gcra_resp::Frame &f) { return gcra_resp::parse_frame(c, f); }
-    template <class Out>
-    __device__ static void put_reply(Out &o, const gcra_request &q, const gcra_result &r) { gcra_resp::put_reply(o, q, r); }
 };
 
 struct HttpTraits {
-    static constexpr u32 REPLY_THREADS = reply_tile_rows(PROTO_HTTP), REPLY_MAX = gcra_http::REPLY_MAX, CAND_PER_WORD = 7;
+    static constexpr RingProto PROTO = PROTO_HTTP;
+    static constexpr u32 PARSE_CTAS = 3;
     // "POST ", or the part of it that fits before the segment's end (a body ends in '}' or whitespace, so there is no
     // line-start rule as for RESP)
     __device__ static bool candidate(const unsigned char *s, u32 p, u32 len) {
@@ -45,10 +47,18 @@ struct HttpTraits {
     }
     __device__ static bool chain_start(const unsigned char *s, u32 p, u32 len) { return candidate(s, p, len); }
     __device__ static int parse(gcra_resp::Cursor &c, gcra_resp::Frame &f) { return gcra_http::parse_frame(c, f); }
-    template <class Out>
-    __device__ static void put_reply(Out &o, const gcra_request &q, const gcra_result &r) { gcra_http::put_reply(o, q, r); }
 };
-static_assert(HttpTraits::REPLY_THREADS * HttpTraits::REPLY_MAX <= 48 * 1024, "the reply tile fits static shared memory");
+
+struct GrpcTraits {
+    static constexpr RingProto PROTO = PROTO_GRPC;
+    static constexpr u32 PARSE_CTAS = 1;
+};
+
+// (3 CTAs per SM: the RESP parse kernel's, so that short connections keep its occupancy)
+struct MixedTraits {
+    static constexpr RingProto PROTO = PROTO_MIXED;
+    static constexpr u32 PARSE_CTAS = 3;
+};
 
 constexpr u32 RESP_KIND_SHIFT = 17;            // a candidate's word: frame end (0 .. 65536) | kind << 17
 constexpr u64 RESP_AGG = 1ULL << 62, RESP_INC = 1ULL << 63, RESP_VAL = RESP_AGG - 1;   // look-back status words
@@ -105,37 +115,78 @@ __device__ __forceinline__ u32 resp_rank(const u32 *bits, const u32 *before, u32
     return before[p >> 5] + __popc(bits[p >> 5] & ((1u << (p & 31)) - 1));
 }
 
-// Connection c (taken by ticket, so in table order) = in[conns[c].off, + conns[c].len), len <= 65536.  Its rows go
-// to rows[base_c ...], base_c = the rows of the connections before it; at most row_cap rows in all, cut exactly where
-// the protocol's host walk (gcra_resp_parse_throttle, gcra_http_parse_throttle) with max_frames = row_cap - base_c
-// stops (stop 3).  Writes the connection's consumed,
-// n_frames and stop to outcome[c] (pinned host memory), {base_c, n_frames} to conn_rows[c]; the CTA of the last
-// connection writes the row count to *total and the segments' row counts of the batch view (segment s holds rows
-// [s << cap_shift, (s + 1) << cap_shift)).  status[0 .. n_conns) and *ticket are zero at launch.
-// The body of resp_parse_kernel for connection c = in[off, + len) (a CTA's whole work; mixed_parse_kernel runs it
-// too): smem is the dynamic shared memory rounded up to 16 bytes, laid out as RespSmem(max_len, P::CAND_PER_WORD),
-// len <= max_len.  Returns {base_c, the rows taken} to every thread.  key_ref (null: not written) receives each row's
-// key as {its offset in `in`, its length}: a plain key is raw contiguous bytes (a RESP bulk string, a JSON string
-// without escapes), which ring_metrics_kernel names denied keys from.
+// ---- the parse bodies: connection c = in[off, + len), taken by ticket, so in table order ----
+// Its rows go to rows[base_c ...], base_c = the rows of the connections before it, whatever their protocols; at most
+// row_cap rows in all, cut exactly where its protocol's host walk with max_frames = row_cap - base_c stops (stop 3).
+// A body writes the connection's end state to its outcome rows, {base_c, n_frames} to
+// conn_rows[c]; the CTA of the last connection writes the row count to *total and the segments' row counts of the
+// batch view (segment s holds rows [s << cap_shift, (s + 1) << cap_shift)).  status[0 .. n_conns) and *ticket are zero
+// at launch.  smem is the dynamic shared memory rounded up to 16 bytes.  A body returns {base_c, the rows taken} to
+// every thread.  key_ref (null: not written) receives each row's key as {its offset in `in`, its length}: a plain key
+// is raw contiguous bytes (a RESP bulk string, a JSON string without escapes, a protobuf string), which
+// ring_metrics_kernel names denied keys from.
+
+// the connection's bytes into smem: 16-byte loads of the chunks wholly inside it, single bytes at its ends (nothing
+// outside it); returns where its first byte lands
+__device__ __forceinline__ const unsigned char *stage_conn(unsigned char *smem, const unsigned char *in, u32 off, u32 len) {
+    const uintptr_t seg = reinterpret_cast<uintptr_t>(in) + off;
+    stage_key_span(seg, len, 0, len, threadIdx.x, RESP_THREADS,
+                   [&](uintptr_t g, u32 o) { *reinterpret_cast<uint4 *>(smem + o) = __ldg(reinterpret_cast<const uint4 *>(g)); },
+                   [&](uintptr_t g, u32 o) { smem[o] = *reinterpret_cast<const unsigned char *>(g); });
+    return smem + (seg & 15);
+}
+
+// (thread 0) connection c's first row, its walk having found n: the rows of the connections before it, at most row_cap
+__device__ __forceinline__ u32 claim_rows(const RingParse &a, u32 c, u32 n) {
+    const u64 excl = resp_look_back(a.status, c, n);
+    return excl < a.row_cap ? (u32)excl : a.row_cap;
+}
+
+// (thread 0) connection c's rows [base, + n): conn_rows[c]; after the last connection's, the batch's row counts
+__device__ __forceinline__ void publish_rows(const RingParse &a, u32 c, u32 base, u32 n) {
+    a.conn_rows[c] = make_uint2(base, n);
+    if (c == a.n_conns - 1) {
+        const u32 t = base + n;
+        *a.total = t;
+        for (u32 s = 0; s < a.nseg; s++) {
+            const u32 first = s << a.cap_shift;
+            a.seg_counts[s] = t <= first ? 0 : min(t - first, 1u << a.cap_shift);
+        }
+    }
+}
+
+// row i: frame fr of the connection at in[off ...], staged at sb; its key hashed from shared memory with the engine's
+// hash
+__device__ __forceinline__ void put_row(const RingParse &a, u32 i, const gcra_resp::Frame &fr, const unsigned char *sb,
+                                        u32 off) {
+    a.rows[i] = gcra_resp::request_row(fr, hash_key_engine(KeyBytes{fr.key}, fr.klen, a.k0, a.k1), a.now_ns);
+    if (a.key_ref) a.key_ref[i] = make_uint2(off + (u32)(fr.key - sb), (u32)fr.klen);
+}
+
+__device__ __forceinline__ gcra_resp_outcome resp_outcome(u32 consumed, u32 n_frames, int32_t stop) {
+    gcra_resp_outcome o;
+    o.consumed = consumed;
+    o.n_frames = n_frames;
+    o.stop = stop;
+    o.reserved = 0;
+    o.reply_off = 0;
+    o.reply_len = 0;
+    return o;
+}
+
+// RESP and HTTP (grammar P): the dynamic shared memory laid out as RespSmem(max_len, cand_per_word(P::PROTO)).  Every
+// candidate frame start is parsed speculatively in parallel; thread 0 chains the true frames from the segment start.
+// The end state goes to outcome[c].
 template <class P>
-__device__ __forceinline__ uint2
-resp_parse_conn(unsigned char *smem, u32 c, u32 off, u32 len, const unsigned char *__restrict__ in, u32 n_conns,
-                u32 max_len, i64 now_ns, u32 row_cap, u64 k0, u64 k1, gcra_request *__restrict__ rows, u64 *status,
-                uint2 *__restrict__ conn_rows, gcra_resp_outcome *outcome, u32 *__restrict__ total,
-                u32 *__restrict__ seg_counts, u32 nseg, u32 cap_shift, uint2 *__restrict__ key_ref) {
+__device__ __forceinline__ uint2 resp_parse_conn(unsigned char *smem, const RingParse &a, u32 c, u32 off, u32 len) {
     __shared__ u64 warp_sums[RESP_THREADS / 32];
     __shared__ u32 s_base, s_n;
-    const RespSmem L(max_len, P::CAND_PER_WORD);
+    const RespSmem L(a.max_len[P::PROTO - 1], cand_per_word(P::PROTO));
     u32 *bits = reinterpret_cast<u32 *>(smem + L.bits_off);
     u32 *before = reinterpret_cast<u32 *>(smem + L.before_off);
     u32 *cand = reinterpret_cast<u32 *>(smem + L.cand_off);
 
-    // stage the segment: 16-byte loads of the chunks wholly inside it, single bytes at its ends (nothing outside it)
-    const uintptr_t seg = reinterpret_cast<uintptr_t>(in) + off;
-    const unsigned char *sb = smem + (seg & 15);
-    stage_key_span(seg, len, 0, len, threadIdx.x, RESP_THREADS,
-                   [&](uintptr_t g, u32 o) { *reinterpret_cast<uint4 *>(smem + o) = __ldg(reinterpret_cast<const uint4 *>(g)); },
-                   [&](uintptr_t g, u32 o) { smem[o] = *reinterpret_cast<const unsigned char *>(g); });
+    const unsigned char *sb = stage_conn(smem, a.in, off, len);
     __syncthreads();
 
     // candidate frame starts: one bit per byte; each thread takes a run of 32-byte words
@@ -180,158 +231,48 @@ resp_parse_conn(unsigned char *smem, u32 c, u32 off, u32 len, const unsigned cha
             cand[n++] = p;
             p = e;
         }
-        // rows of the connections before this one; the cap cuts this one as max_frames = row_cap - base would
-        const u64 excl = resp_look_back(status, c, n);
-        const u32 base = excl < row_cap ? (u32)excl : row_cap, room = row_cap - base;
+        // the cap cuts this connection as max_frames = row_cap - base would
+        const u32 base = claim_rows(a, c, n), room = a.row_cap - base;
         u32 take = n, stop_at = p;
         if (n > room || (n == room && p < len)) { take = room; why = 3; stop_at = take < n ? cand[take] : p; }
         s_base = base; s_n = take;
-        gcra_resp_outcome o;
-        o.consumed = stop_at;
-        o.n_frames = take;
-        o.stop = (int32_t)why;
-        o.reserved = 0;
-        o.reply_off = 0;
-        o.reply_len = 0;
-        outcome[c] = o;
-        conn_rows[c] = make_uint2(base, take);
-        if (c == n_conns - 1) {
-            const u32 t = base + take;
-            *total = t;
-            for (u32 s = 0; s < nseg; s++) {
-                const u32 first = s << cap_shift;
-                seg_counts[s] = t <= first ? 0 : min(t - first, 1u << cap_shift);
-            }
-        }
+        a.outcome[c] = resp_outcome(stop_at, take, (int32_t)why);
+        publish_rows(a, c, base, take);
     }
     __syncthreads();
 
-    // the rows: each frame parsed again, its key hashed from shared memory with the engine's hash
+    // the rows: each frame parsed again
     const u32 base = s_base, take = s_n;
     for (u32 k = threadIdx.x; k < take; k += RESP_THREADS) {
         gcra_resp::Cursor cu = {sb + cand[k], sb + len};
         gcra_resp::Frame fr;
         P::parse(cu, fr);
-        gcra_request r;
-        r.key_hash = hash_key_engine(KeyBytes{fr.key}, fr.klen, k0, k1);
-        r.max_burst = fr.a[0];
-        r.count_per_period = fr.a[1];
-        r.period = fr.a[2];
-        r.quantity = fr.a[3];
-        r.now_ns = now_ns;
-        rows[base + k] = r;
-        if (key_ref) key_ref[base + k] = make_uint2(off + (u32)(fr.key - sb), (u32)fr.klen);
+        put_row(a, base + k, fr, sb, off);
     }
     return make_uint2(base, take);
 }
 
-// (3 CTAs per SM: the key_ref store would take the RESP instantiation from 80 to 84 registers, and 2 CTAs per SM,
-// for short connections; bounded, it fits 80 with no spills)
-template <class P>
-__global__ void __launch_bounds__(RESP_THREADS, 3)
-resp_parse_kernel(const unsigned char *__restrict__ in, const gcra_resp_conn *__restrict__ conns, u32 n_conns,
-                  u32 max_len, i64 now_ns, u32 row_cap, u64 k0, u64 k1, gcra_request *__restrict__ rows,
-                  u64 *status, u32 *ticket, uint2 *__restrict__ conn_rows, gcra_resp_outcome *outcome,
-                  u32 *__restrict__ total, u32 *__restrict__ seg_counts, u32 nseg, u32 cap_shift,
-                  uint2 *__restrict__ key_ref) {
-    // (no alignment is declared for the dynamic shared memory: that would pad every kernel's; RespSmem leaves room to
-    // round its start up to 16 bytes)
-    extern __shared__ unsigned char resp_dyn[];
-    unsigned char *smem = reinterpret_cast<unsigned char *>((reinterpret_cast<uintptr_t>(resp_dyn) + 15) & ~(uintptr_t)15);
-    __shared__ u32 s_conn;
-    if (threadIdx.x == 0) s_conn = atomicAdd(ticket, 1u);
-    __syncthreads();
-    const u32 c = s_conn;
-    const gcra_resp_conn cn = conns[c];
-    resp_parse_conn<P>(smem, c, cn.off, cn.len, in, n_conns, max_len, now_ns, row_cap, k0, k1, rows, status, conn_rows,
-                       outcome, total, seg_counts, nseg, cap_shift, key_ref);
-}
-
-// The replies of rows [0, *total) in row order, straight into `out` (pinned host memory): each CTA takes a tile of
-// rows by ticket, measures its replies, finds the tile's offset by a look-back over the tiles before it, writes the
-// replies into shared memory and copies the tile's bytes out in one coalesced sweep.  row_off[i] = the offset of row
-// i's reply, row_off[*total] = all the bytes.  status[] and *ticket are zero at launch.
-template <class P>
-__global__ void __launch_bounds__(P::REPLY_THREADS)
-resp_reply_kernel(const gcra_request *__restrict__ rows, const gcra_result *__restrict__ res, const u32 *total_p,
-                  u64 *status, u32 *ticket, u64 *__restrict__ row_off, unsigned char *out) {
-    constexpr u32 T = P::REPLY_THREADS;
-    __shared__ __align__(16) char stage[T * P::REPLY_MAX];
-    __shared__ u64 warp_sums[T / 32];
-    __shared__ u64 s_base;
-    __shared__ u32 s_tile;
-    if (threadIdx.x == 0) s_tile = atomicAdd(ticket, 1u);
-    __syncthreads();
-    const u32 tile = s_tile, total = *total_p;
-    if ((u64)tile * T >= total) return;                        // uniform over the CTA
-    const u32 row = tile * T + threadIdx.x;
-    gcra_request q{};
-    gcra_result r{};
-    gcra_resp::Count cnt;
-    if (row < total) {
-        q = rows[row];
-        r = res[row];
-        P::put_reply(cnt, q, r);
-    }
-    u64 tile_bytes;
-    const u64 at = resp_block_scan<T>(cnt.n, warp_sums, &tile_bytes);
-    if (threadIdx.x == 0) s_base = resp_look_back(status, tile, tile_bytes);
-    if (row < total) {
-        gcra_resp::Write o{stage + at};
-        P::put_reply(o, q, r);
-    }
-    __syncthreads();
-    const u64 base = s_base;
-    if (row < total) row_off[row] = base + at;
-    if (row + 1 == total) row_off[total] = base + at + cnt.n;
-    for (u32 i = threadIdx.x; i < (u32)tile_bytes; i += T) out[base + i] = stage[i];
-}
-
-// connection c's replies: rows [base_c, base_c + n_c) -> outcome[c].reply_off, reply_len
-__global__ void resp_outcome_kernel(const uint2 *__restrict__ conn_rows, u32 n_conns, const u32 *total_p,
-                                    const u64 *__restrict__ row_off, gcra_resp_outcome *outcome) {
-    const u32 c = blockIdx.x * blockDim.x + threadIdx.x;
-    if (c >= n_conns) return;
-    const u32 total = *total_p;
-    const uint2 br = conn_rows[c];
-    const u64 a = total ? row_off[min(br.x, total)] : 0, b = total ? row_off[min(br.x + br.y, total)] : 0;
-    outcome[c].reply_off = a;
-    outcome[c].reply_len = b - a;
-}
-
-// ---- gRPC ----
-// HTTP/2 has no byte that marks a frame start: the starts are the chain of 9-byte headers from offset 0.  So thread 0
-// hops that chain over the staged bytes and lists every whole frame (one shared-memory word per frame); then every
-// HEADERS and DATA frame is judged in parallel (gcra_grpc::headers_plain, data_plain: the stateless, costly part);
-// then thread 0 runs the host's walk (gcra_grpc::walk) over the list with the connection's state, looking the
-// judgements up instead of making them; the rows are decoded and hashed in parallel.  Connection c is taken by ticket,
-// so in table order; its rows go to rows[base_c ...] and their stream ids to stream_ids[base_c ...], cut exactly
-// where gcra_grpc_parse_throttle with max_frames = row_cap - base_c stops.  outcome[c] receives everything but the
-// reply fields and data_sent (grpc_outcome_kernel).  status[0 .. n_conns) and *ticket are zero at launch.
-//
-// grpc_parse_conn is that CTA's work for connection c = in[off, + len) with the HTTP/2 state *cn (whose off and len it
-// does not read), the dynamic shared memory laid out as GrpcSmem(max_len), len <= max_len; mixed_parse_kernel runs it
-// too.  emit(o) stores the connection's outcome (thread 0).  Returns {base_c, the rows taken} to every thread.
-// key_ref: as in resp_parse_conn (a protobuf string is raw contiguous bytes too).
-template <class Emit>
-__device__ __forceinline__ uint2
-grpc_parse_conn(unsigned char *smem, u32 c, u32 off, u32 len, const gcra_grpc_conn *cn,
-                const unsigned char *__restrict__ in, u32 n_conns, u32 max_len, i64 now_ns, u32 row_cap, u64 k0,
-                u64 k1, gcra_request *__restrict__ rows, u32 *__restrict__ stream_ids, u64 *status,
-                uint2 *__restrict__ conn_rows, Emit emit, u32 *__restrict__ total, u32 *__restrict__ seg_counts,
-                u32 nseg, u32 cap_shift, uint2 *__restrict__ key_ref) {
+// gRPC: the HTTP/2 state gconns[gs] (whose off and len it does not read), the dynamic shared memory laid out as
+// GrpcSmem(max_len).  HTTP/2 has no byte that marks a frame start: the starts are the chain of 9-byte headers from
+// offset 0.  So thread 0 hops that chain over the staged bytes and lists every whole frame (one shared-memory word per
+// frame); then every HEADERS and DATA frame is judged in parallel (gcra_grpc::headers_plain, data_plain: the
+// stateless, costly part); then thread 0 runs the host's walk (gcra_grpc::walk) over the list with the connection's
+// state, looking the judgements up instead of making them; the rows are decoded and hashed in parallel, their stream
+// ids to stream_ids[base_c ...].  The end state goes to the connection's gRPC outcome row goutcome[gs], all but the
+// reply fields and data_sent (the outcome kernel's); on a mixed ring (K) its consumed, n_frames and stop also go to
+// outcome[c].
+template <class K>
+__device__ __forceinline__ uint2 grpc_parse_conn(unsigned char *smem, const RingParse &a, u32 c, u32 off, u32 len,
+                                                 u32 gs) {
     __shared__ unsigned char s_dyn[GCRA_GRPC_MAX_DYN];
     __shared__ u32 s_nf, s_base, s_n;
-    const GrpcSmem L(max_len);
+    const GrpcSmem L(a.max_len[PROTO_GRPC - 1]);
     u32 *frames = reinterpret_cast<u32 *>(smem + L.frames_off);
     u32 *calls = reinterpret_cast<u32 *>(smem + L.calls_off);
 
+    const gcra_grpc_conn *cn = a.gconns + gs;
     const u32 n_dyn = cn->n_dyn;
-    const uintptr_t seg = reinterpret_cast<uintptr_t>(in) + off;
-    const unsigned char *sb = smem + (seg & 15);
-    stage_key_span(seg, len, 0, len, threadIdx.x, RESP_THREADS,
-                   [&](uintptr_t g, u32 o) { *reinterpret_cast<uint4 *>(smem + o) = __ldg(reinterpret_cast<const uint4 *>(g)); },
-                   [&](uintptr_t g, u32 o) { smem[o] = *reinterpret_cast<const unsigned char *>(g); });
+    const unsigned char *sb = stage_conn(smem, a.in, off, len);
     for (u32 i = threadIdx.x; i < n_dyn; i += RESP_THREADS) s_dyn[i] = cn->dyn_class[i];
     __syncthreads();
 
@@ -366,8 +307,7 @@ grpc_parse_conn(unsigned char *smem, u32 c, u32 off, u32 len, const gcra_grpc_co
         auto call = [&](u32 j, u32 at) { calls[j] = at; };
         gcra_grpc::State st;
         gcra_grpc::WalkEnd e = gcra_grpc::walk(sb, len, k, 0xffffffffu, plain, call, st);
-        const u64 excl = resp_look_back(status, c, e.n);
-        const u32 base = excl < row_cap ? (u32)excl : row_cap, room = row_cap - base;
+        const u32 base = claim_rows(a, c, e.n), room = a.row_cap - base;
         if (e.n >= room) e = gcra_grpc::walk(sb, len, k, room, plain, call, st);   // the cap decides the stop
         s_base = base; s_n = e.n;
         gcra_grpc_outcome o;
@@ -382,16 +322,9 @@ grpc_parse_conn(unsigned char *smem, u32 c, u32 off, u32 len, const gcra_grpc_co
         o.data_sent = 0;
         o.ping = st.ping;
         for (int i = 0; i < 8; i++) o.ping_opaque[i] = st.ping ? st.opaque[i] : 0;
-        emit(o);
-        conn_rows[c] = make_uint2(base, e.n);
-        if (c == n_conns - 1) {
-            const u32 t = base + e.n;
-            *total = t;
-            for (u32 s = 0; s < nseg; s++) {
-                const u32 first = s << cap_shift;
-                seg_counts[s] = t <= first ? 0 : min(t - first, 1u << cap_shift);
-            }
-        }
+        a.goutcome[gs] = o;
+        if (K::PROTO == PROTO_MIXED) a.outcome[c] = resp_outcome(o.consumed, o.n_frames, o.stop);
+        publish_rows(a, c, base, e.n);
     }
     __syncthreads();
 
@@ -402,165 +335,60 @@ grpc_parse_conn(unsigned char *smem, u32 c, u32 off, u32 len, const gcra_grpc_co
         gcra_grpc::read_frame(sb, at, len, h);
         gcra_resp::Frame fr;
         gcra_grpc::data_plain(sb, at, h, fr);
-        gcra_request r;
-        r.key_hash = hash_key_engine(KeyBytes{fr.key}, fr.klen, k0, k1);
-        r.max_burst = fr.a[0];
-        r.count_per_period = fr.a[1];
-        r.period = fr.a[2];
-        r.quantity = fr.a[3];
-        r.now_ns = now_ns;
-        rows[base + j] = r;
-        stream_ids[base + j] = h.sid;
-        if (key_ref) key_ref[base + j] = make_uint2(off + (u32)(fr.key - sb), (u32)fr.klen);
+        put_row(a, base + j, fr, sb, off);
+        a.stream_ids[base + j] = h.sid;
     }
     return make_uint2(base, take);
 }
 
-__global__ void __launch_bounds__(RESP_THREADS, 1)
-grpc_parse_kernel(const unsigned char *__restrict__ in, const gcra_grpc_conn *__restrict__ conns, u32 n_conns,
-                  u32 max_len, i64 now_ns, u32 row_cap, u64 k0, u64 k1, gcra_request *__restrict__ rows,
-                  u32 *__restrict__ stream_ids, u64 *status, u32 *ticket, uint2 *__restrict__ conn_rows,
-                  gcra_grpc_outcome *outcome, u32 *__restrict__ total, u32 *__restrict__ seg_counts, u32 nseg,
-                  u32 cap_shift, uint2 *__restrict__ key_ref) {
-    extern __shared__ unsigned char grpc_dyn[];
-    unsigned char *smem = reinterpret_cast<unsigned char *>((reinterpret_cast<uintptr_t>(grpc_dyn) + 15) & ~(uintptr_t)15);
+// ---- the kernels ----
+// The parse kernel: connection c's protocol's body (uniform over the CTA; a compile-time choice but for a mixed ring),
+// whose end state goes to outcome[c] (every ring but a gRPC one) and, for a gRPC connection, to its gRPC outcome row.
+// A mixed ring's row i also gets its protocol in row_proto[i], for the reply kernel.
+template <class K>
+__global__ void __launch_bounds__(RESP_THREADS, K::PARSE_CTAS) ring_parse_kernel(const __grid_constant__ RingParse a) {
+    // (no alignment is declared for the dynamic shared memory: that would pad every kernel's; RespSmem and GrpcSmem
+    // leave room to round its start up to 16 bytes)
+    extern __shared__ unsigned char ring_dyn[];
+    unsigned char *smem = reinterpret_cast<unsigned char *>((reinterpret_cast<uintptr_t>(ring_dyn) + 15) & ~(uintptr_t)15);
     __shared__ u32 s_conn;
-    if (threadIdx.x == 0) s_conn = atomicAdd(ticket, 1u);
+    if (threadIdx.x == 0) s_conn = atomicAdd(a.ticket, 1u);
     __syncthreads();
     const u32 c = s_conn;
-    const gcra_grpc_conn *cn = conns + c;
-    grpc_parse_conn(smem, c, cn->off, cn->len, cn, in, n_conns, max_len, now_ns, row_cap, k0, k1, rows, stream_ids,
-                    status, conn_rows, [&](const gcra_grpc_outcome &o) { outcome[c] = o; }, total, seg_counts, nseg,
-                    cap_shift, key_ref);
-}
-
-// resp_reply_kernel for gRPC: row i's response goes on stream stream_ids[i]
-__global__ void __launch_bounds__(RESP_THREADS)
-grpc_reply_kernel(const gcra_request *__restrict__ rows, const gcra_result *__restrict__ res,
-                  const u32 *__restrict__ stream_ids, const u32 *total_p, u64 *status, u32 *ticket,
-                  u64 *__restrict__ row_off, unsigned char *out) {
-    constexpr u32 T = RESP_THREADS;
-    __shared__ __align__(16) char stage[T * gcra_grpc::REPLY_MAX];
-    __shared__ u64 warp_sums[T / 32];
-    __shared__ u64 s_base;
-    __shared__ u32 s_tile;
-    if (threadIdx.x == 0) s_tile = atomicAdd(ticket, 1u);
-    __syncthreads();
-    const u32 tile = s_tile, total = *total_p;
-    if ((u64)tile * T >= total) return;                        // uniform over the CTA
-    const u32 row = tile * T + threadIdx.x;
-    gcra_request q{};
-    gcra_result r{};
-    u32 sid = 0;
-    gcra_resp::Count cnt;
-    if (row < total) {
-        q = rows[row];
-        r = res[row];
-        sid = stream_ids[row];
-        gcra_grpc::put_reply(cnt, q, r, sid);
-    }
-    u64 tile_bytes;
-    const u64 at = resp_block_scan<T>(cnt.n, warp_sums, &tile_bytes);
-    if (threadIdx.x == 0) s_base = resp_look_back(status, tile, tile_bytes);
-    if (row < total) {
-        gcra_resp::Write o{stage + at};
-        gcra_grpc::put_reply(o, q, r, sid);
-    }
-    __syncthreads();
-    const u64 base = s_base;
-    if (row < total) row_off[row] = base + at;
-    if (row + 1 == total) row_off[total] = base + at + cnt.n;
-    for (u32 i = threadIdx.x; i < (u32)tile_bytes; i += T) out[base + i] = stage[i];
-}
-static_assert(RESP_THREADS * gcra_grpc::REPLY_MAX <= 48 * 1024, "the reply tile fits static shared memory");
-
-// one warp per connection: where its responses lie, and their DATA octets
-__global__ void grpc_outcome_kernel(const uint2 *__restrict__ conn_rows, u32 n_conns,
-                                    const gcra_request *__restrict__ rows, const gcra_result *__restrict__ res,
-                                    const u32 *total_p, const u64 *__restrict__ row_off, gcra_grpc_outcome *outcome) {
-    const u32 c = (blockIdx.x * blockDim.x + threadIdx.x) / 32, lane = threadIdx.x & 31;
-    if (c >= n_conns) return;                                  // uniform over the warp
-    const u32 total = *total_p;
-    const uint2 br = conn_rows[c];
-    const u32 lo = min(br.x, total), hi = min(br.x + br.y, total);
-    u32 sent = 0;
-    for (u32 i = lo + lane; i < hi; i += 32) sent += gcra_grpc::data_len(rows[i], res[i]);
-#pragma unroll
-    for (u32 o = 16; o; o >>= 1) sent += __shfl_xor_sync(0xffffffffu, sent, o);
-    if (lane == 0) {
-        const u64 a = total ? row_off[lo] : 0, b = total ? row_off[hi] : 0;
-        outcome[c].reply_off = a;
-        outcome[c].reply_len = b - a;
-        outcome[c].data_sent = sent;
-    }
-}
-
-// ---- mixed: RESP, HTTP and gRPC connections in one slot ----
-// One CTA per connection, taken by ticket, with one look-back chain over all connections: base_c is the rows of the
-// connections before c in table order, whatever their protocols.  The CTA runs its connection's protocol's parse body
-// (uniform over the CTA), so connection c's rows are exactly what its protocol's host walk takes at row_cap - base_c.
-// Every connection's consumed, n_frames and stop go to outcome[c]; a gRPC connection's whole outcome also goes to
-// goutcome[grpc_state] (its state is gconns[grpc_state]).  row_proto[i] receives row i's protocol, for the reply
-// kernel.  The dynamic shared memory is the largest layout of the protocols present; max_len[p - 1] is the longest
-// connection of protocol p.  (3 CTAs per SM: the registers of resp_parse_kernel<RespTraits>, so that short connections
-// keep its occupancy.)
-__global__ void __launch_bounds__(RESP_THREADS, 3)
-mixed_parse_kernel(const unsigned char *__restrict__ in, const gcra_mixed_conn *__restrict__ conns, u32 n_conns,
-                   const gcra_grpc_conn *__restrict__ gconns, uint3 max_len, i64 now_ns, u32 row_cap, u64 k0, u64 k1,
-                   gcra_request *__restrict__ rows, u32 *__restrict__ stream_ids, unsigned char *__restrict__ row_proto,
-                   u64 *status, u32 *ticket, uint2 *__restrict__ conn_rows, gcra_resp_outcome *outcome,
-                   gcra_grpc_outcome *goutcome, u32 *__restrict__ total, u32 *__restrict__ seg_counts, u32 nseg,
-                   u32 cap_shift, uint2 *__restrict__ key_ref) {
-    extern __shared__ unsigned char mixed_dyn[];
-    unsigned char *smem = reinterpret_cast<unsigned char *>((reinterpret_cast<uintptr_t>(mixed_dyn) + 15) & ~(uintptr_t)15);
-    __shared__ u32 s_conn;
-    if (threadIdx.x == 0) s_conn = atomicAdd(ticket, 1u);
-    __syncthreads();
-    const u32 c = s_conn;
-    const gcra_mixed_conn mc = conns[c];
+    const RingConn cn = ring_conn(K::PROTO, a.conns, a.gconns, a.mconns, c);
     uint2 br;
-    if (mc.protocol == GCRA_PROTO_GRPC) {
-        gcra_grpc_outcome *go = goutcome + mc.grpc_state;
-        auto emit = [&](const gcra_grpc_outcome &o) {
-            *go = o;
-            gcra_resp_outcome r;
-            r.consumed = o.consumed;
-            r.n_frames = o.n_frames;
-            r.stop = o.stop;
-            r.reserved = 0;
-            r.reply_off = 0;
-            r.reply_len = 0;
-            outcome[c] = r;
-        };
-        br = grpc_parse_conn(smem, c, mc.off, mc.len, gconns + mc.grpc_state, in, n_conns, max_len.z, now_ns, row_cap,
-                             k0, k1, rows, stream_ids, status, conn_rows, emit, total, seg_counts, nseg, cap_shift,
-                             key_ref);
-    } else if (mc.protocol == GCRA_PROTO_HTTP) {
-        br = resp_parse_conn<HttpTraits>(smem, c, mc.off, mc.len, in, n_conns, max_len.y, now_ns, row_cap, k0, k1, rows,
-                                         status, conn_rows, outcome, total, seg_counts, nseg, cap_shift, key_ref);
-    } else {
-        br = resp_parse_conn<RespTraits>(smem, c, mc.off, mc.len, in, n_conns, max_len.x, now_ns, row_cap, k0, k1, rows,
-                                         status, conn_rows, outcome, total, seg_counts, nseg, cap_shift, key_ref);
-    }
-    for (u32 k = threadIdx.x; k < br.y; k += RESP_THREADS) row_proto[br.x + k] = (unsigned char)mc.protocol;
+    if (cn.proto == PROTO_GRPC)
+        br = grpc_parse_conn<K>(smem, a, c, cn.off, cn.len, cn.grpc_state);
+    else if (cn.proto == PROTO_HTTP)
+        br = resp_parse_conn<HttpTraits>(smem, a, c, cn.off, cn.len);
+    else
+        br = resp_parse_conn<RespTraits>(smem, a, c, cn.off, cn.len);
+    if (K::PROTO == PROTO_MIXED)
+        for (u32 k = threadIdx.x; k < br.y; k += RESP_THREADS) a.row_proto[br.x + k] = (unsigned char)cn.proto;
 }
 
 // row i's reply in its protocol: gcra_resp::put_reply, gcra_http::put_reply, or gcra_grpc::put_reply on its stream
 template <class Out>
-__device__ __forceinline__ void mixed_put_reply(Out &o, u32 proto, const gcra_request &q, const gcra_result &r, u32 sid) {
-    if (proto == GCRA_PROTO_GRPC) gcra_grpc::put_reply(o, q, r, sid);
-    else if (proto == GCRA_PROTO_HTTP) gcra_http::put_reply(o, q, r);
+__device__ __forceinline__ void put_reply(Out &o, u32 proto, const gcra_request &q, const gcra_result &r, u32 sid) {
+    if (proto == PROTO_GRPC) gcra_grpc::put_reply(o, q, r, sid);
+    else if (proto == PROTO_HTTP) gcra_http::put_reply(o, q, r);
     else gcra_resp::put_reply(o, q, r);
 }
 
-// resp_reply_kernel for a mixed slot: tiles of MIXED_REPLY_THREADS rows (a tile stages up to GCRA_HTTP_REPLY_MAX bytes
-// per row), each row in its protocol.  A connection's rows are contiguous, so most warps take one branch.
-__global__ void __launch_bounds__(MIXED_REPLY_THREADS)
-mixed_reply_kernel(const gcra_request *__restrict__ rows, const gcra_result *__restrict__ res,
-                   const u32 *__restrict__ stream_ids, const unsigned char *__restrict__ row_proto, const u32 *total_p,
-                   u64 *status, u32 *ticket, u64 *__restrict__ row_off, unsigned char *out) {
-    constexpr u32 T = MIXED_REPLY_THREADS;
-    __shared__ __align__(16) char stage[T * gcra_http::REPLY_MAX];
+// The replies of rows [0, *total) in row order, straight into `out` (pinned host memory): each CTA takes a tile of
+// rows by ticket, measures its replies, finds the tile's offset by a look-back over the tiles before it, writes the
+// replies into shared memory and copies the tile's bytes out in one coalesced sweep.  row_off[i] = the offset of row
+// i's reply, row_off[*total] = all the bytes.  status[] and *ticket are zero at launch.  A gRPC row's response goes on
+// stream stream_ids[i]; a mixed ring's row i is in protocol row_proto[i] (a connection's rows are contiguous, so most
+// warps take one branch).
+template <class K>
+__global__ void __launch_bounds__(reply_tile_rows(K::PROTO))
+ring_reply_kernel(const gcra_request *__restrict__ rows, const gcra_result *__restrict__ res,
+                  const u32 *__restrict__ stream_ids, const unsigned char *__restrict__ row_proto, const u32 *total_p,
+                  u64 *status, u32 *ticket, u64 *__restrict__ row_off, unsigned char *out) {
+    constexpr u32 T = reply_tile_rows(K::PROTO);
+    static_assert(T * reply_max(K::PROTO) <= 48 * 1024, "the reply tile fits static shared memory");
+    __shared__ __align__(16) char stage[T * reply_max(K::PROTO)];
     __shared__ u64 warp_sums[T / 32];
     __shared__ u64 s_base;
     __shared__ u32 s_tile;
@@ -571,21 +399,21 @@ mixed_reply_kernel(const gcra_request *__restrict__ rows, const gcra_result *__r
     const u32 row = tile * T + threadIdx.x;
     gcra_request q{};
     gcra_result r{};
-    u32 sid = 0, proto = 0;
+    u32 sid = 0, proto = K::PROTO;
     gcra_resp::Count cnt;
     if (row < total) {
         q = rows[row];
         r = res[row];
-        proto = row_proto[row];
-        if (proto == GCRA_PROTO_GRPC) sid = stream_ids[row];
-        mixed_put_reply(cnt, proto, q, r, sid);
+        if (K::PROTO == PROTO_MIXED) proto = row_proto[row];
+        if (proto == PROTO_GRPC) sid = stream_ids[row];
+        put_reply(cnt, proto, q, r, sid);
     }
     u64 tile_bytes;
     const u64 at = resp_block_scan<T>(cnt.n, warp_sums, &tile_bytes);
     if (threadIdx.x == 0) s_base = resp_look_back(status, tile, tile_bytes);
     if (row < total) {
         gcra_resp::Write o{stage + at};
-        mixed_put_reply(o, proto, q, r, sid);
+        put_reply(o, proto, q, r, sid);
     }
     __syncthreads();
     const u64 base = s_base;
@@ -593,39 +421,40 @@ mixed_reply_kernel(const gcra_request *__restrict__ rows, const gcra_result *__r
     if (row + 1 == total) row_off[total] = base + at + cnt.n;
     for (u32 i = threadIdx.x; i < (u32)tile_bytes; i += T) out[base + i] = stage[i];
 }
-static_assert(MIXED_REPLY_THREADS * gcra_http::REPLY_MAX <= 48 * 1024, "the reply tile fits static shared memory");
-static_assert(gcra_http::REPLY_MAX >= gcra_resp::REPLY_MAX && gcra_http::REPLY_MAX >= gcra_grpc::REPLY_MAX,
-              "HTTP's replies are the longest");
 
-// one warp per connection: where its replies lie (outcome[c]); for a gRPC connection also in its gRPC outcome row,
-// with the DATA octets of its responses
-__global__ void mixed_outcome_kernel(const uint2 *__restrict__ conn_rows, const gcra_mixed_conn *__restrict__ conns,
-                                     u32 n_conns, const gcra_request *__restrict__ rows,
-                                     const gcra_result *__restrict__ res, const u32 *total_p,
-                                     const u64 *__restrict__ row_off, gcra_resp_outcome *outcome,
-                                     gcra_grpc_outcome *goutcome) {
+// one warp per connection: where its replies lie, in outcome[c] (every ring but a gRPC one) and in a gRPC
+// connection's gRPC outcome row (on a mixed ring: row mconns[c].grpc_state), with the DATA octets of its responses
+template <class K>
+__global__ void ring_outcome_kernel(const uint2 *__restrict__ conn_rows, const gcra_mixed_conn *__restrict__ mconns,
+                                    u32 n_conns, const gcra_request *__restrict__ rows,
+                                    const gcra_result *__restrict__ res, const u32 *total_p,
+                                    const u64 *__restrict__ row_off, gcra_resp_outcome *outcome,
+                                    gcra_grpc_outcome *goutcome) {
     const u32 c = (blockIdx.x * blockDim.x + threadIdx.x) / 32, lane = threadIdx.x & 31;
     if (c >= n_conns) return;                                  // uniform over the warp
     const u32 total = *total_p;
-    const gcra_mixed_conn mc = conns[c];
+    u32 proto = K::PROTO, grpc_state = c;
+    if (K::PROTO == PROTO_MIXED) {
+        const gcra_mixed_conn mc = mconns[c];
+        proto = mc.protocol;
+        grpc_state = mc.grpc_state;
+    }
     const uint2 br = conn_rows[c];
     const u32 lo = min(br.x, total), hi = min(br.x + br.y, total);
     const u64 a = total ? row_off[lo] : 0, b = total ? row_off[hi] : 0;
-    if (mc.protocol != GCRA_PROTO_GRPC) {
-        if (lane == 0) {
-            outcome[c].reply_off = a;
-            outcome[c].reply_len = b - a;
-        }
-        return;
-    }
     u32 sent = 0;
-    for (u32 i = lo + lane; i < hi; i += 32) sent += gcra_grpc::data_len(rows[i], res[i]);
+    if (proto == PROTO_GRPC) {                                 // uniform over the warp
+        for (u32 i = lo + lane; i < hi; i += 32) sent += gcra_grpc::data_len(rows[i], res[i]);
 #pragma unroll
-    for (u32 o = 16; o; o >>= 1) sent += __shfl_xor_sync(0xffffffffu, sent, o);
-    if (lane == 0) {
+        for (u32 o = 16; o; o >>= 1) sent += __shfl_xor_sync(0xffffffffu, sent, o);
+    }
+    if (lane) return;
+    if (K::PROTO != PROTO_GRPC) {
         outcome[c].reply_off = a;
         outcome[c].reply_len = b - a;
-        gcra_grpc_outcome *go = goutcome + mc.grpc_state;
+    }
+    if (proto == PROTO_GRPC) {
+        gcra_grpc_outcome *go = goutcome + grpc_state;
         go->reply_off = a;
         go->reply_len = b - a;
         go->data_sent = sent;
@@ -691,103 +520,63 @@ cudaError_t launch_ring_metrics(const RingMetrics &a, u32 max_rows, cudaStream_t
 }
 
 // ---- launches (gcra_resp.inc) ----
-cudaError_t resp_ring_setup() {
-    cudaFuncAttributes a;
-    for (const void *k : {(const void *)resp_parse_kernel<RespTraits>, (const void *)resp_reply_kernel<RespTraits>,
-                          (const void *)resp_parse_kernel<HttpTraits>, (const void *)resp_reply_kernel<HttpTraits>,
-                          (const void *)resp_outcome_kernel, (const void *)grpc_parse_kernel,
-                          (const void *)grpc_reply_kernel, (const void *)grpc_outcome_kernel,
-                          (const void *)mixed_parse_kernel, (const void *)mixed_reply_kernel,
-                          (const void *)mixed_outcome_kernel, (const void *)ring_metrics_kernel}) {
-        const cudaError_t e = cudaFuncGetAttributes(&a, k);    // (loads the code now: see preload in gcra_b200.cu)
-        if (e) return e;
+// f(K()) for the ring kind K of `proto`
+template <class F>
+static cudaError_t for_kind(RingProto proto, F f) {
+    switch (proto) {
+    case PROTO_RESP: return f(RespTraits());
+    case PROTO_HTTP: return f(HttpTraits());
+    case PROTO_GRPC: return f(GrpcTraits());
+    case PROTO_MIXED: return f(MixedTraits());
+    default: return cudaErrorInvalidValue;
     }
-    cudaError_t e = cudaFuncSetAttribute(resp_parse_kernel<RespTraits>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                         (int)RespSmem(RESP_MAX_CONN_BYTES, RespTraits::CAND_PER_WORD).total);
-    if (e) return e;
-    e = cudaFuncSetAttribute(resp_parse_kernel<HttpTraits>, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                             (int)RespSmem(RESP_MAX_CONN_BYTES, HttpTraits::CAND_PER_WORD).total);
-    if (e) return e;
-    e = cudaFuncSetAttribute(grpc_parse_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                             (int)GrpcSmem(RESP_MAX_CONN_BYTES).total);
-    if (e) return e;
-    return cudaFuncSetAttribute(mixed_parse_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize,
-                                (int)mixed_parse_smem(RESP_MAX_CONN_BYTES, RESP_MAX_CONN_BYTES, RESP_MAX_CONN_BYTES));
 }
 
-template <class P>
-static cudaError_t launch_parse(const RespParse &a, cudaStream_t st) {
-    resp_parse_kernel<P><<<a.n_conns, RESP_THREADS, RespSmem(a.max_len, P::CAND_PER_WORD).total, st>>>(
-        a.in, a.conns, a.n_conns, a.max_len, a.now_ns, a.row_cap, a.k0, a.k1, a.rows, a.status, a.ticket, a.conn_rows,
-        a.outcome, a.total, a.seg_counts, a.nseg, a.cap_shift, a.key_ref);
-    return cudaGetLastError();
+cudaError_t resp_ring_setup() {
+    cudaFuncAttributes fa;
+    cudaError_t e = cudaFuncGetAttributes(&fa, ring_metrics_kernel);  // (loads the code now: see preload in gcra_b200.cu)
+    for (RingProto p : {PROTO_RESP, PROTO_HTTP, PROTO_GRPC, PROTO_MIXED}) {
+        if (!e) e = for_kind(p, [&](auto k) {
+            using K = decltype(k);
+            for (const void *f : {(const void *)ring_parse_kernel<K>, (const void *)ring_reply_kernel<K>,
+                                  (const void *)ring_outcome_kernel<K>}) {
+                const cudaError_t r = cudaFuncGetAttributes(&fa, f);
+                if (r) return r;
+            }
+            const u32 max_len[3] = {RESP_MAX_CONN_BYTES, RESP_MAX_CONN_BYTES, RESP_MAX_CONN_BYTES};
+            return cudaFuncSetAttribute(ring_parse_kernel<K>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                        (int)parse_smem(K::PROTO, max_len));
+        });
+    }
+    return e;
 }
 
-cudaError_t launch_resp_parse(const RespParse &a, cudaStream_t st) {
-    return a.proto == PROTO_HTTP ? launch_parse<HttpTraits>(a, st) : launch_parse<RespTraits>(a, st);
+cudaError_t launch_ring_parse(RingProto proto, const RingParse &a, cudaStream_t st) {
+    return for_kind(proto, [&](auto k) {
+        ring_parse_kernel<decltype(k)><<<a.n_conns, RESP_THREADS, parse_smem(proto, a.max_len), st>>>(a);
+        return cudaGetLastError();
+    });
 }
 
-cudaError_t launch_resp_reply(RingProto proto, u32 tiles, const gcra_request *rows, const gcra_result *res,
-                              const u32 *total, u64 *ctrl, u64 *row_off, unsigned char *out, cudaStream_t st) {
-    if (proto == PROTO_HTTP)
-        resp_reply_kernel<HttpTraits><<<tiles, HttpTraits::REPLY_THREADS, 0, st>>>(rows, res, total, ctrl + 1,
-                                                                                 reinterpret_cast<u32 *>(ctrl), row_off, out);
-    else
-        resp_reply_kernel<RespTraits><<<tiles, RespTraits::REPLY_THREADS, 0, st>>>(rows, res, total, ctrl + 1,
-                                                                                 reinterpret_cast<u32 *>(ctrl), row_off, out);
-    return cudaGetLastError();
+cudaError_t launch_ring_reply(RingProto proto, u32 tiles, const gcra_request *rows, const gcra_result *res,
+                              const u32 *stream_ids, const unsigned char *row_proto, const u32 *total, u64 *ctrl,
+                              u64 *row_off, unsigned char *out, cudaStream_t st) {
+    return for_kind(proto, [&](auto k) {
+        ring_reply_kernel<decltype(k)><<<tiles, reply_tile_rows(proto), 0, st>>>(
+            rows, res, stream_ids, row_proto, total, ctrl + 1, reinterpret_cast<u32 *>(ctrl), row_off, out);
+        return cudaGetLastError();
+    });
 }
 
-cudaError_t launch_resp_outcome(u32 n_conns, const uint2 *conn_rows, const u32 *total, const u64 *row_off,
-                                gcra_resp_outcome *outcome, cudaStream_t st) {
-    resp_outcome_kernel<<<(n_conns + RESP_THREADS - 1) / RESP_THREADS, RESP_THREADS, 0, st>>>(conn_rows, n_conns, total,
-                                                                                            row_off, outcome);
-    return cudaGetLastError();
-}
-
-cudaError_t launch_grpc_parse(const GrpcParse &a, cudaStream_t st) {
-    grpc_parse_kernel<<<a.n_conns, RESP_THREADS, GrpcSmem(a.max_len).total, st>>>(
-        a.in, a.conns, a.n_conns, a.max_len, a.now_ns, a.row_cap, a.k0, a.k1, a.rows, a.stream_ids, a.status, a.ticket,
-        a.conn_rows, a.outcome, a.total, a.seg_counts, a.nseg, a.cap_shift, a.key_ref);
-    return cudaGetLastError();
-}
-
-cudaError_t launch_grpc_reply(u32 tiles, const gcra_request *rows, const gcra_result *res, const u32 *stream_ids,
-                              const u32 *total, u64 *ctrl, u64 *row_off, unsigned char *out, cudaStream_t st) {
-    grpc_reply_kernel<<<tiles, RESP_THREADS, 0, st>>>(rows, res, stream_ids, total, ctrl + 1,
-                                                     reinterpret_cast<u32 *>(ctrl), row_off, out);
-    return cudaGetLastError();
-}
-
-cudaError_t launch_grpc_outcome(u32 n_conns, const uint2 *conn_rows, const gcra_request *rows, const gcra_result *res,
-                                const u32 *total, const u64 *row_off, gcra_grpc_outcome *outcome, cudaStream_t st) {
-    grpc_outcome_kernel<<<(n_conns + 7) / 8, 256, 0, st>>>(conn_rows, n_conns, rows, res, total, row_off, outcome);
-    return cudaGetLastError();
-}
-
-cudaError_t launch_mixed_parse(const MixedParse &a, cudaStream_t st) {
-    mixed_parse_kernel<<<a.n_conns, RESP_THREADS, mixed_parse_smem(a.max_len[0], a.max_len[1], a.max_len[2]), st>>>(
-        a.in, a.conns, a.n_conns, a.gconns, make_uint3(a.max_len[0], a.max_len[1], a.max_len[2]), a.now_ns, a.row_cap,
-        a.k0, a.k1, a.rows, a.stream_ids, a.row_proto, a.status, a.ticket, a.conn_rows, a.outcome, a.goutcome, a.total,
-        a.seg_counts, a.nseg, a.cap_shift, a.key_ref);
-    return cudaGetLastError();
-}
-
-cudaError_t launch_mixed_reply(u32 tiles, const gcra_request *rows, const gcra_result *res, const u32 *stream_ids,
-                               const unsigned char *row_proto, const u32 *total, u64 *ctrl, u64 *row_off,
-                               unsigned char *out, cudaStream_t st) {
-    mixed_reply_kernel<<<tiles, MIXED_REPLY_THREADS, 0, st>>>(rows, res, stream_ids, row_proto, total, ctrl + 1,
-                                                            reinterpret_cast<u32 *>(ctrl), row_off, out);
-    return cudaGetLastError();
-}
-
-cudaError_t launch_mixed_outcome(u32 n_conns, const uint2 *conn_rows, const gcra_mixed_conn *conns,
-                                 const gcra_request *rows, const gcra_result *res, const u32 *total,
-                                 const u64 *row_off, gcra_resp_outcome *outcome, gcra_grpc_outcome *goutcome,
-                                 cudaStream_t st) {
-    mixed_outcome_kernel<<<(n_conns + 7) / 8, 256, 0, st>>>(conn_rows, conns, n_conns, rows, res, total, row_off,
-                                                            outcome, goutcome);
-    return cudaGetLastError();
+cudaError_t launch_ring_outcome(RingProto proto, u32 n_conns, const uint2 *conn_rows, const gcra_mixed_conn *mconns,
+                                const gcra_request *rows, const gcra_result *res, const u32 *total,
+                                const u64 *row_off, gcra_resp_outcome *outcome, gcra_grpc_outcome *goutcome,
+                                cudaStream_t st) {
+    return for_kind(proto, [&](auto k) {
+        ring_outcome_kernel<decltype(k)><<<(n_conns + 7) / 8, 256, 0, st>>>(conn_rows, mconns, n_conns, rows, res,
+                                                                             total, row_off, outcome, goutcome);
+        return cudaGetLastError();
+    });
 }
 
 }  // namespace gcra

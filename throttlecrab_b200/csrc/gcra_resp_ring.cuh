@@ -1,9 +1,11 @@
-// gcra_resp_ring.cuh -- what gcra_b200.cu needs of the RESP ring's kernels (gcra_resp_ring.cu, a translation unit
-// of its own): their shared-memory layout and their launches.
+// gcra_resp_ring.cuh -- what gcra_b200.cu needs of the rings' kernels (gcra_resp_ring.cu, a translation unit of its
+// own): the protocols' bounds, the kernels' shared-memory layout, their arguments and their launches.
 #pragma once
 #include <cuda_runtime.h>
 
 #include "gcra_device.cuh"
+#include "gcra_http.cuh"
+#include "gcra_grpc.cuh"
 #include "../../include/gcra_b200.h"
 
 namespace gcra {
@@ -20,14 +22,31 @@ enum RingProto : u32 { PROTO_NONE = 0, PROTO_RESP = 1, PROTO_HTTP = 2, PROTO_GRP
 static_assert(PROTO_RESP == GCRA_PROTO_RESP && PROTO_HTTP == GCRA_PROTO_HTTP && PROTO_GRPC == GCRA_PROTO_GRPC,
               "a ring's protocol is a mixed connection's protocol");
 
-// The dynamic shared memory of resp_parse_kernel for connections of up to `max_len` bytes: the staged bytes (16
+// What the host and the kernels both need of a protocol (a ring's kind for the reply room and tile): the reply bound
+// (a mixed ring's is HTTP's, the longest), the rows of a reply tile (the reply kernel stages a tile's replies in shared
+// memory, at most 48 KiB), and the smallest plain frame (a connection of len bytes holds at most len / that).
+__host__ __device__ constexpr u32 reply_max(RingProto p) {
+    return p == PROTO_HTTP || p == PROTO_MIXED ? gcra_http::REPLY_MAX : p == PROTO_GRPC ? gcra_grpc::REPLY_MAX
+                                                                                         : gcra_resp::REPLY_MAX;
+}
+__host__ __device__ constexpr u32 reply_tile_rows(RingProto p) { return p == PROTO_HTTP || p == PROTO_MIXED ? 128 : RESP_THREADS; }
+static_assert(gcra_http::REPLY_MAX >= gcra_resp::REPLY_MAX && gcra_http::REPLY_MAX >= gcra_grpc::REPLY_MAX,
+              "HTTP's replies are the longest");
+__host__ __device__ constexpr u32 min_frame_bytes(RingProto p) {
+    return p == PROTO_HTTP ? gcra_http::MIN_FRAME_BYTES : p == PROTO_GRPC ? gcra_grpc::MIN_CALL_BYTES
+                                                                          : gcra_resp::MIN_FRAME_BYTES;
+}
+// The RESP and HTTP parse body's candidate room: candidates per 32 bytes.  A RESP candidate is a '*' that starts the
+// segment or follows a '\n', so at most every other byte (16); an HTTP candidate starts "POST ", which cannot overlap
+// itself, or a prefix of it at the segment's end, so at most len / 5 + 1 (7 per 32 bytes covers that for every len).
+__host__ __device__ constexpr u32 cand_per_word(RingProto p) { return p == PROTO_HTTP ? 7 : 16; }
+
+// The RESP and HTTP parse body's dynamic shared memory for connections of up to `max_len` bytes: the staged bytes (16
 // more for the segment's misalignment), one candidate bit per byte, the candidates before each 32-byte word, and one
-// word per candidate, `cand_per_word` per 32 bytes.  A RESP candidate is a '*' that starts the segment or follows a
-// '\n', so at most every other byte (16); an HTTP candidate starts "POST ", which cannot overlap itself, or a prefix
-// of it at the segment's end, so at most len / 5 + 1 (7 per 32 bytes covers that for every len).
+// word per candidate, `cand_per_word` per 32 bytes.
 struct RespSmem {
     u32 words, bytes_off, bits_off, before_off, cand_off, total;
-    __host__ __device__ explicit RespSmem(u32 max_len, u32 cand_per_word = 16) {
+    __host__ __device__ RespSmem(u32 max_len, u32 cand_per_word) {
         words = (max_len + 31) / 32;
         bytes_off = 0;
         bits_off = (words * 32 + 16 + 15) & ~15u;
@@ -37,33 +56,7 @@ struct RespSmem {
     }
 };
 
-// resp_parse_kernel's arguments: connection c is in[conns[c].off, + conns[c].len)
-struct RespParse {
-    const unsigned char *in;
-    const gcra_resp_conn *conns;
-    u32 n_conns, max_len;
-    i64 now_ns;
-    u32 row_cap;
-    u64 k0, k1;                  // the engine's hash seed
-    gcra_request *rows;          // the slot's flat row array
-    u64 *status;                 // [n_conns] look-back status words, zero
-    u32 *ticket;                 // zero
-    uint2 *conn_rows;            // [n_conns] out: first row, rows
-    gcra_resp_outcome *outcome;  // [n_conns] out (pinned host memory)
-    u32 *total, *seg_counts;     // out: rows of the batch, rows of each segment
-    u32 nseg, cap_shift;
-    RingProto proto;
-    uint2 *key_ref;              // [row_capacity] out, or null: each row's key {offset in `in`, length}
-};
-
-// a protocol's rows per reply tile (the reply kernel stages a tile's replies in shared memory); a mixed ring's tile
-// has room for HTTP's replies, the longest
-constexpr u32 MIXED_REPLY_THREADS = 128;
-constexpr u32 reply_tile_rows(RingProto p) {
-    return p == PROTO_HTTP ? 128 : p == PROTO_MIXED ? MIXED_REPLY_THREADS : RESP_THREADS;
-}
-
-// The dynamic shared memory of grpc_parse_kernel for connections of up to `max_len` bytes: the staged bytes (16 more
+// The gRPC parse body's dynamic shared memory for connections of up to `max_len` bytes: the staged bytes (16 more
 // for the segment's misalignment), one word per frame (a frame has at least 9 bytes) and one per call (a call has at
 // least gcra_grpc::MIN_CALL_BYTES = 26).
 struct GrpcSmem {
@@ -75,70 +68,60 @@ struct GrpcSmem {
     }
 };
 
-// grpc_parse_kernel's arguments: RespParse's, with the gRPC connection and outcome tables and the rows' stream ids
-struct GrpcParse {
-    const unsigned char *in;
-    const gcra_grpc_conn *conns;
-    u32 n_conns, max_len;
-    i64 now_ns;
-    u32 row_cap;
-    u64 k0, k1;
-    gcra_request *rows;
-    u32 *stream_ids;             // [row_capacity] out
-    u64 *status;
-    u32 *ticket;
-    uint2 *conn_rows;
-    gcra_grpc_outcome *outcome;  // [n_conns] out (pinned host memory)
-    u32 *total, *seg_counts;
-    u32 nseg, cap_shift;
-    uint2 *key_ref;              // as in RespParse
-};
-cudaError_t launch_grpc_parse(const GrpcParse &a, cudaStream_t st);
-cudaError_t launch_grpc_reply(u32 tiles, const gcra_request *rows, const gcra_result *res, const u32 *stream_ids,
-                              const u32 *total, u64 *ctrl, u64 *row_off, unsigned char *out, cudaStream_t st);
-cudaError_t launch_grpc_outcome(u32 n_conns, const uint2 *conn_rows, const gcra_request *rows, const gcra_result *res,
-                                const u32 *total, const u64 *row_off, gcra_grpc_outcome *outcome, cudaStream_t st);
-
-// The dynamic shared memory of mixed_parse_kernel: the largest layout that a present protocol needs, for the longest
-// connection of each protocol (0 where none)
-inline u32 mixed_parse_smem(u32 max_len_resp, u32 max_len_http, u32 max_len_grpc) {
-    u32 b = RespSmem(max_len_resp, 16).total;
-    b = b > RespSmem(max_len_http, 7).total ? b : RespSmem(max_len_http, 7).total;
-    return b > GrpcSmem(max_len_grpc).total ? b : GrpcSmem(max_len_grpc).total;
+// The parse kernel's dynamic shared memory for a ring of kind `ring`: the largest layout of its protocols, for the
+// longest connection of each (max_len[p - 1] for protocol p, 0 where none)
+inline u32 parse_smem(RingProto ring, const u32 max_len[3]) {
+    u32 b = 0;
+    for (u32 p = PROTO_RESP; p <= PROTO_GRPC; p++) {
+        if (ring != PROTO_MIXED && ring != p) continue;
+        const u32 t = p == PROTO_GRPC ? GrpcSmem(max_len[p - 1]).total
+                                      : RespSmem(max_len[p - 1], cand_per_word((RingProto)p)).total;
+        b = b > t ? b : t;
+    }
+    return b;
 }
 
-// mixed_parse_kernel's arguments: GrpcParse's with the mixed connection table, the gRPC state table (row k: the
-// connection whose grpc_state is k), the gRPC outcome table and each row's protocol
-struct MixedParse {
+// Connection c of a ring of kind `ring`, read from the kind's own table: in[off, + len), its protocol and, for a gRPC
+// connection, its row in the gRPC state and outcome tables (c on a gRPC ring)
+struct RingConn {
+    u32 off, len, proto, grpc_state;
+};
+__host__ __device__ __forceinline__ RingConn ring_conn(RingProto ring, const gcra_resp_conn *conns,
+                                                       const gcra_grpc_conn *gconns, const gcra_mixed_conn *mconns,
+                                                       u32 c) {
+    if (ring == PROTO_MIXED) {
+        const gcra_mixed_conn m = mconns[c];
+        return {m.off, m.len, m.protocol, m.grpc_state};
+    }
+    if (ring == PROTO_GRPC) return {gconns[c].off, gconns[c].len, PROTO_GRPC, c};
+    const gcra_resp_conn r = conns[c];
+    return {r.off, r.len, ring, 0};
+}
+
+// The parse kernel's arguments.  Only the ring kind's own connection table is set: conns (RESP, HTTP), gconns (gRPC)
+// or mconns with gconns (mixed: row k of gconns is the connection whose grpc_state is k).
+struct RingParse {
     const unsigned char *in;
-    const gcra_mixed_conn *conns;
+    const gcra_resp_conn *conns;
+    const gcra_grpc_conn *gconns;
+    const gcra_mixed_conn *mconns;
     u32 n_conns;
     u32 max_len[3];              // the longest connection of RESP, HTTP and gRPC
-    const gcra_grpc_conn *gconns;
     i64 now_ns;
     u32 row_cap;
-    u64 k0, k1;
-    gcra_request *rows;
-    u32 *stream_ids;             // [row_capacity] out (gRPC rows)
-    unsigned char *row_proto;    // [row_capacity] out: each row's GCRA_PROTO_*
-    u64 *status;
-    u32 *ticket;
-    uint2 *conn_rows;
-    gcra_resp_outcome *outcome;  // [n_conns] out (pinned host memory)
+    u64 k0, k1;                  // the engine's hash seed
+    gcra_request *rows;          // the slot's flat row array
+    u32 *stream_ids;             // [row_capacity] out: gRPC rows' stream ids
+    unsigned char *row_proto;    // [row_capacity] out (mixed): each row's GCRA_PROTO_*
+    u64 *status;                 // [n_conns] look-back status words, zero
+    u32 *ticket;                 // zero
+    uint2 *conn_rows;            // [n_conns] out: first row, rows
+    gcra_resp_outcome *outcome;  // [n_conns] out (pinned host memory; not on a gRPC ring)
     gcra_grpc_outcome *goutcome; // [gRPC connections] out (pinned host memory)
-    u32 *total, *seg_counts;
+    u32 *total, *seg_counts;     // out: rows of the batch, rows of each segment
     u32 nseg, cap_shift;
-    uint2 *key_ref;              // as in RespParse
+    uint2 *key_ref;              // [row_capacity] out, or null: each row's key {offset in `in`, length}
 };
-cudaError_t launch_mixed_parse(const MixedParse &a, cudaStream_t st);
-// ctrl: word 0 the ticket, then one status word per tile of MIXED_REPLY_THREADS rows; all zero
-cudaError_t launch_mixed_reply(u32 tiles, const gcra_request *rows, const gcra_result *res, const u32 *stream_ids,
-                               const unsigned char *row_proto, const u32 *total, u64 *ctrl, u64 *row_off,
-                               unsigned char *out, cudaStream_t st);
-cudaError_t launch_mixed_outcome(u32 n_conns, const uint2 *conn_rows, const gcra_mixed_conn *conns,
-                                 const gcra_request *rows, const gcra_result *res, const u32 *total,
-                                 const u64 *row_off, gcra_resp_outcome *outcome, gcra_grpc_outcome *goutcome,
-                                 cudaStream_t st);
 
 // ring_metrics_kernel's arguments (gcra_ring_metrics): a finished slot's rows, counted per transport into
 // counts[3 transports][allowed, denied, errors], and their denied keys named from the slot's input
@@ -160,11 +143,18 @@ struct RingMetrics {
 cudaError_t launch_ring_metrics(const RingMetrics &a, u32 max_rows, cudaStream_t st);
 
 cudaError_t resp_ring_setup();   // once, before the first launch
-cudaError_t launch_resp_parse(const RespParse &a, cudaStream_t st);
-// ctrl: word 0 the ticket, then one status word per tile of reply_tile_rows(proto) rows; all zero
-cudaError_t launch_resp_reply(RingProto proto, u32 tiles, const gcra_request *rows, const gcra_result *res,
-                              const u32 *total, u64 *ctrl, u64 *row_off, unsigned char *out, cudaStream_t st);
-cudaError_t launch_resp_outcome(u32 n_conns, const uint2 *conn_rows, const u32 *total, const u64 *row_off,
-                                gcra_resp_outcome *outcome, cudaStream_t st);
+// one CTA per connection of a.n_conns
+cudaError_t launch_ring_parse(RingProto proto, const RingParse &a, cudaStream_t st);
+// ctrl: word 0 the ticket, then one status word per tile of reply_tile_rows(proto) rows; all zero.  stream_ids: gRPC
+// and mixed rings; row_proto: mixed rings.
+cudaError_t launch_ring_reply(RingProto proto, u32 tiles, const gcra_request *rows, const gcra_result *res,
+                              const u32 *stream_ids, const unsigned char *row_proto, const u32 *total, u64 *ctrl,
+                              u64 *row_off, unsigned char *out, cudaStream_t st);
+// where each connection's replies lie: outcome[c] (not on a gRPC ring), and a gRPC connection's in its gRPC outcome
+// row with the DATA octets of its responses
+cudaError_t launch_ring_outcome(RingProto proto, u32 n_conns, const uint2 *conn_rows, const gcra_mixed_conn *mconns,
+                                const gcra_request *rows, const gcra_result *res, const u32 *total,
+                                const u64 *row_off, gcra_resp_outcome *outcome, gcra_grpc_outcome *goutcome,
+                                cudaStream_t st);
 
 }  // namespace gcra

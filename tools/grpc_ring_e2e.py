@@ -107,6 +107,9 @@ class GpuPath:
                                           for x in o]
 
 
+KERNELS = tuple("%s<gcra::GrpcTraits>" % k for k in ("ring_parse_kernel", "ring_reply_kernel", "ring_outcome_kernel"))
+
+
 def kernel_ms(gpu, conns, iters=5):
     import torch
     from torch.profiler import ProfilerActivity, profile
@@ -116,7 +119,7 @@ def kernel_ms(gpu, conns, iters=5):
         torch.cuda.synchronize()
     tot = {}
     for e in prof.events():
-        for name in ("grpc_parse_kernel", "grpc_reply_kernel", "grpc_outcome_kernel"):
+        for name in KERNELS:
             if name in e.name and e.device_type.name == "CUDA":
                 tot[name] = tot.get(name, 0.0) + e.device_time / 1000.0
     return {k: v / iters for k, v in tot.items()}

@@ -188,14 +188,13 @@ def kernel_ms(path, conns, names, iters=5):
             continue
         for name in names:
             if name in e.name:
-                key = "%s:%s" % (name, e.name.split("<")[1].split(">")[0]) if "<" in e.name else name
-                tot[key] = tot.get(key, 0.0) + e.device_time / 1000.0
+                tot[name] = tot.get(name, 0.0) + e.device_time / 1000.0
     return {k: round(v / iters, 4) for k, v in tot.items()}
 
 
-RING_KERNELS = ("mixed_parse_kernel", "mixed_reply_kernel", "mixed_outcome_kernel", "resp_parse_kernel",
-                "resp_reply_kernel", "resp_outcome_kernel", "grpc_parse_kernel", "grpc_reply_kernel",
-                "grpc_outcome_kernel")
+# (with the template argument: variant (c)'s single-protocol rings must not count the mixed instantiation's time)
+RING_KERNELS = tuple("%s<gcra::%s>" % (k, t) for t in ("MixedTraits", "RespTraits", "HttpTraits", "GrpcTraits")
+                     for k in ("ring_parse_kernel", "ring_reply_kernel", "ring_outcome_kernel"))
 
 
 def main():

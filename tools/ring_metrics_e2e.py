@@ -24,8 +24,8 @@ from throttlecrab_b200.metrics import Metrics  # noqa: E402
 from mixed_ring_e2e import MixedPath, connections, kernel_ms  # noqa: E402
 from resp_ring_e2e import card  # noqa: E402
 
-KERNELS = ("ring_metrics_kernel", "denied_count_seg_kernel", "mixed_parse_kernel", "mixed_reply_kernel",
-           "mixed_outcome_kernel")
+KERNELS = ("ring_metrics_kernel", "denied_count_seg_kernel", "ring_parse_kernel<gcra::MixedTraits>",
+           "ring_reply_kernel<gcra::MixedTraits>", "ring_outcome_kernel<gcra::MixedTraits>")
 
 
 def main():
