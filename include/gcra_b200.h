@@ -674,7 +674,8 @@ gcra_mixed_conn *gcra_mixed_ring_conns(gcra_engine *h, uint32_t slot);     /* pi
  * the engine as it was) when the engine is not gcra_p2p_connect-ed or has no such ring, when row_capacity exceeds the
  * peer-memory cap (the power of two >= cap_rows), when ring metrics are on, or when any rank's key-hash seed differs
  * from this engine's (gcra_p2p_prepare publishes each rank's seed in its window).  gcra_ring_metrics(h, 1) refuses
- * while it is on.  gcra_ring_p2p(h, 0) returns the ring to the engine's own table.
+ * while it is on; sharded ring metrics (gcra_ring_metrics_sharded) run with it.  gcra_ring_p2p(h, 0) returns the ring
+ * to the engine's own table.
  *
  * Contract:
  *   - Ring ticks and gcra_p2p_submit ticks form ONE tick sequence per rank.  Every rank submits every tick; a ring
@@ -727,8 +728,37 @@ int32_t gcra_ring_metrics(gcra_engine *h, uint32_t on);
 int32_t gcra_ring_transport_counts(gcra_engine *h, gcra_transport_counts out[3]);
 /* for each of n hashes (from gcra_top_denied): lens[i] = its name's length, with the bytes at names + 256 i, or one of
  * the two markers (GCRA_NAME_UNKNOWN also for a hash not in the table, or while ring metrics are off).  Needs denied
- * tracking on. */
+ * tracking on.  With sharded ring metrics on (below) it reads that mode's name table instead, and needs no denied
+ * tracking. */
 int32_t gcra_denied_names(gcra_engine *h, uint32_t n, const uint64_t *key_hashes, char *names, uint32_t *lens);
+
+/* ---- ring metrics for rings whose ticks may be peer-memory ticks (gcra_ring_p2p) ------------------------------------
+ * On a peer-memory tick a denied request is counted on its key's owner (gcra_track_denied / gcra_top_denied on every
+ * rank), but the key's bytes are only in the input of the rank that parsed the connection.  So this mode keeps three
+ * things apart, and the caller joins them at a scrape:
+ *   - counts per transport of THIS rank's ring slots (gcra_ring_transport_counts), by gcra_ring_metrics' rules;
+ *   - names of the keys this rank's connections saw denied, in a name table of this rank keyed by key hash: a denied
+ *     row inserts its key (linear probing from the denied table's home slot, at most 64 probes) and the first row to
+ *     name it copies its bytes; a key over GCRA_DENIED_NAME_MAX bytes is marked GCRA_NAME_TOO_LONG.  A key that finds
+ *     the table full is not stored, and every denied row of such a key is counted in `full` (rows, not keys: the
+ *     table has no room to remember which keys it turned away, so a hot key left out counts once per denial);
+ *   - the denied counts, on the owners.
+ * Every ring submit runs the metrics kernel after the replies whether ring p2p is on or off (on a peer-memory tick,
+ * once the results are back in the slot's row order).  gcra_ring_p2p(h, 1) is accepted in this mode.
+ * gcra_ring_metrics(h, 1) and gcra_ring_metrics_sharded(h, 1, .) each refuse while the other is on, max_keys above
+ * GCRA_RING_METRICS_MAX_KEYS is refused, and gcra_ring_metrics_sharded refuses between a slot's
+ * gcra_resp_ring_submit_route and its _finish (the route decided whether key positions are written); every refusal
+ * returns GCRA_INTERNAL and leaves the engine as it was.  Every
+ * call here, and gcra_denied_names in this mode, waits for the ring slots in flight and the engine's batches: as with
+ * gcra_top_denied, multi-GPU callers query between ticks, after every rank's gcra_ring_wait or join. */
+/* on: counts per transport of this rank's slots, names of the keys this rank's connections saw denied in a name table
+ * of as many entries as a denied table of max_keys (the power of two >= max(16 max_keys, 1024)); max_keys = 0 counts
+ * without names.  Switching on zeroes the counts and empties the table.  off: no kernel is launched, the names are
+ * released, the counts stay readable. */
+int32_t gcra_ring_metrics_sharded(gcra_engine *h, uint32_t on, uint32_t max_keys);
+/* keep the names of these hashes, forget every other (the table is rebuilt, and replaces the old one once complete:
+ * a failed call leaves it as it was); *full = denied rows whose key found the table full since the last keep */
+int32_t gcra_ring_names_keep(gcra_engine *h, uint32_t n, const uint64_t *key_hashes, uint64_t *full);
 
 #ifdef __cplusplus
 }

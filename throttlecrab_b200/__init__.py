@@ -293,6 +293,21 @@ class _GpuStore:
         return [names[i, :int(lens[i])].tobytes() if lens[i] <= DENIED_NAME_MAX else int(lens[i])
                 for i in range(len(hs))]
 
+    def ring_metrics_sharded(self, on, max_keys):
+        """gcra_ring_metrics_sharded: ring metrics for rings whose ticks may be peer-memory ticks: every later ring
+        submit counts its rows per transport on this engine and names the keys its connections saw denied in a name
+        table of this engine (max_keys as track_denied's; 0: no names); the denied counts stay on the keys' owners.
+        Switching on zeroes the counts and empties the table.  Refused while ring_metrics is on."""
+        self._check(self._L.gcra_ring_metrics_sharded(self._h, 1 if on else 0, max_keys))
+
+    def ring_names_keep(self, key_hashes):
+        """gcra_ring_names_keep: keep the name table's names of these hashes and forget the others -> the denied rows
+        whose key found the table full since the last keep"""
+        hs = np.ascontiguousarray(key_hashes, np.uint64)
+        full = C.c_uint64()
+        self._check(self._L.gcra_ring_names_keep(self._h, len(hs), hs.ctypes.data, C.byref(full)))
+        return int(full.value)
+
     def policy_tick(self, now):
         """The store kind's sweep policy against the caller's clock (for device-resident / pipelined / sharded
         submissions, which never sweep by themselves); returns the number of entries removed."""

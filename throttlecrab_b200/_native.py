@@ -191,6 +191,8 @@ SYMBOLS = {
     "gcra_ring_metrics": (_i32, [_vp, _u32]),
     "gcra_ring_transport_counts": (_i32, [_vp, _vp]),
     "gcra_denied_names": (_i32, [_vp, _u32, _vp, _vp, _vp]),
+    "gcra_ring_metrics_sharded": (_i32, [_vp, _u32, _u32]),
+    "gcra_ring_names_keep": (_i32, [_vp, _u32, _vp, _pu64]),
     "gcra_owner_of": (_u32, [_u64, _u32]),
     "gcra_route_partition": (_i32, [_vp, _u64, _vp, _u32, _vp, _vp, _vp, _vp]),
     "gcra_route_unpermute": (_i32, [_vp, _u64, _vp, _vp, _vp, _vp]),

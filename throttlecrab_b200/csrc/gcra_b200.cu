@@ -241,6 +241,16 @@ struct DeniedArrays {
     DevBuf<u32> name_len;
 };
 
+// the name table of sharded ring metrics (gcra_ring_metrics_sharded): keys by hash, each with its name, and the
+// denied rows whose key found the table full since it was made.  Replaced whole by gcra_ring_names_keep.
+struct NameTable {
+    DevBuf<u64> keys, full;
+    DevBuf<u32> name_len;
+    DevBuf<unsigned char> names;
+    uint64_t cap = 0;                // entries (0: counts without names)
+    NameTableView view() const { return {keys.get(), (u32)(cap - 1), name_len.get(), names.get()}; }
+};
+
 // the header of a snapshot file (gcra_snapshot_save, gcra_snapshot_begin)
 namespace {
 struct SnapshotHeader {
@@ -373,6 +383,9 @@ struct gcra_engine {
     // ring metrics (gcra_ring_metrics): ring rows per transport [3][allowed, denied, errors]
     bool ring_metrics = false;
     DevBuf<u64> ring_counts;
+    // sharded ring metrics (gcra_ring_metrics_sharded): the same counts, names in a table of this rank's own
+    bool ring_metrics_sharded = false;
+    NameTable ring_names;
     bool ring_p2p = false;           // gcra_ring_p2p: every ring submit is a peer-memory tick
     uint64_t hash_seed[2] = {0, 0};  // SipHash key of the string-keyed entry points ((0,0): the unkeyed gcra_hash_key)
     // background saves (gcra_snapshot_begin); gcra_destroy joins the writer thread before anything is released
@@ -1730,12 +1743,20 @@ int32_t gcra_peek(gcra_engine *h, uint64_t key_hash, int64_t *tat, int64_t *expi
 }
 
 // ---- metrics bridge: top denied keys (throttlecrab-server/src/metrics.rs:24-64,162-173) --------------------------
-// the names of a denied table of `cap` entries (ring metrics), none known
-static int make_denied_names(gcra_engine *h, DeniedArrays &a, uint64_t cap) {
-    CK(a.names.make((size_t)cap * GCRA_DENIED_NAME_MAX));
-    CK(a.name_len.make(cap));
-    CK(cudaMemset(a.name_len.get(), 0xff, cap * sizeof(u32)));           // GCRA_NAME_UNKNOWN
+// the names of a table of `cap` entries (ring metrics), none known
+static int make_names(gcra_engine *h, DevBuf<unsigned char> &names, DevBuf<u32> &name_len, uint64_t cap) {
+    CK(names.make((size_t)cap * GCRA_DENIED_NAME_MAX));
+    CK(name_len.make(cap));
+    CK(cudaMemset(name_len.get(), 0xff, cap * sizeof(u32)));           // GCRA_NAME_UNKNOWN
     return GCRA_OK;
+}
+static int make_denied_names(gcra_engine *h, DeniedArrays &a, uint64_t cap) {
+    return make_names(h, a.names, a.name_len, cap);
+}
+
+// entries of a denied table, or of a name table, for max_keys > 0 keys: 16 per key, at least 1024, a power of two
+static uint64_t denied_entries(uint32_t max_keys) {
+    return 1ULL << ceil_log2(std::max<uint64_t>(16ULL * max_keys, 1024));
 }
 
 int32_t gcra_track_denied(gcra_engine *h, uint32_t max_keys) {
@@ -1749,7 +1770,7 @@ int32_t gcra_track_denied(gcra_engine *h, uint32_t max_keys) {
     RC(wait_for_metrics_writers(h));
     CK(cudaDeviceSynchronize());
     DeniedArrays a;
-    const uint64_t cap = max_keys ? 1ULL << ceil_log2(std::max<uint64_t>(16ULL * max_keys, 1024)) : 0;
+    const uint64_t cap = max_keys ? denied_entries(max_keys) : 0;
     if (max_keys) {
         CK(a.keys.make(cap));
         CK(a.counts.make(cap));
@@ -1827,6 +1848,7 @@ int32_t gcra_top_denied(gcra_engine *h, uint32_t k, uint64_t *key_hashes, uint64
 int32_t gcra_ring_metrics(gcra_engine *h, uint32_t on) {
     CK(cudaSetDevice(h->device));
     if (on && h->ring_p2p) { h->err = "ring metrics: the ring's ticks are peer-memory ticks (gcra_ring_p2p)"; return GCRA_INTERNAL; }
+    if (on && h->ring_metrics_sharded) { h->err = "ring metrics: sharded ring metrics are on"; return GCRA_INTERNAL; }
     if (on && h->denied_max > GCRA_RING_METRICS_MAX_KEYS) {
         h->err = "ring metrics: denied tracking runs with max_keys above 10,000";
         return GCRA_INTERNAL;
@@ -1859,8 +1881,100 @@ int32_t gcra_ring_transport_counts(gcra_engine *h, gcra_transport_counts out[3])
     return GCRA_OK;
 }
 
+// ---- sharded ring metrics: names in a table of this rank's own (the denied counts are on the keys' owners) ---------
+// an empty name table of `cap` entries, built on the engine's stream
+static int make_name_table(gcra_engine *h, NameTable &t, uint64_t cap) {
+    const cudaStream_t st = h->stream.get();
+    CK(t.keys.make(cap));
+    CK(t.full.make(1));
+    RC(make_names(h, t.names, t.name_len, cap));
+    CK(cudaMemsetAsync(t.keys.get(), 0, cap * sizeof(u64), st));
+    CK(cudaMemsetAsync(t.full.get(), 0, sizeof(u64), st));
+    CK(cudaStreamSynchronize(st));
+    t.cap = cap;
+    return GCRA_OK;
+}
+
+int32_t gcra_ring_metrics_sharded(gcra_engine *h, uint32_t on, uint32_t max_keys) {
+    CK(cudaSetDevice(h->device));
+    // (a routed slot's parse chose whether to write key positions; its finish must launch what the parse chose for)
+    if (h->p2p && h->p2p->ring_slot_pending >= 0) { h->err = "a routed ring tick is not finished yet"; return GCRA_INTERNAL; }
+    if (on && h->ring_metrics) { h->err = "sharded ring metrics: ring metrics are on (gcra_ring_metrics)"; return GCRA_INTERNAL; }
+    if (on && max_keys > GCRA_RING_METRICS_MAX_KEYS) {
+        h->err = "sharded ring metrics: max_keys must be at most 10,000";
+        return GCRA_INTERNAL;
+    }
+    RC(wait_for_metrics_writers(h));
+    if (!on) {
+        h->ring_metrics_sharded = false;
+        h->ring_names = NameTable();
+        return GCRA_OK;
+    }
+    DevBuf<u64> counts;                                 // (built whole before anything is swapped in)
+    CK(counts.make(9));
+    CK(cudaMemset(counts.get(), 0, 9 * sizeof(u64)));
+    NameTable t;
+    if (max_keys) RC(make_name_table(h, t, denied_entries(max_keys)));
+    h->ring_counts = std::move(counts);
+    h->ring_names = std::move(t);
+    h->ring_metrics_sharded = true;
+    return GCRA_OK;
+}
+
+int32_t gcra_ring_names_keep(gcra_engine *h, uint32_t n, const uint64_t *key_hashes, uint64_t *full) {
+    CK(cudaSetDevice(h->device));
+    if (full) *full = 0;
+    if (!h->ring_metrics_sharded) { h->err = "gcra_ring_metrics_sharded first"; return GCRA_INTERNAL; }
+    RC(wait_for_metrics_writers(h));
+    const NameTable &old = h->ring_names;
+    if (!old.cap) return GCRA_OK;
+    uint64_t was_full = 0;
+    CK(cudaMemcpy(&was_full, old.full.get(), sizeof(u64), cudaMemcpyDeviceToHost));
+    NameTable t;                                        // (built whole before it replaces the old one)
+    RC(make_name_table(h, t, old.cap));
+    if (n) {
+        const cudaStream_t st = h->stream.get();
+        DevBuf<u64> d_hashes;
+        CK(d_hashes.make(n));
+        CK(cudaMemcpyAsync(d_hashes.get(), key_hashes, n * sizeof(u64), cudaMemcpyHostToDevice, st));
+        CK(launch_ring_names_keep(old.view(), t.view(), d_hashes.get(), n, t.full.get(), st));
+        h->launches++;
+        CK(cudaStreamSynchronize(st));
+    }
+    h->ring_names = std::move(t);
+    if (full) *full = was_full;
+    return GCRA_OK;
+}
+
+// gcra_denied_names on sharded ring metrics: the lookup kernel over the name table, only the n names copied back
+static int ring_names_lookup(gcra_engine *h, uint32_t n, const uint64_t *key_hashes, char *names, uint32_t *lens) {
+    RC(wait_for_metrics_writers(h));
+    for (uint32_t i = 0; i < n; i++) lens[i] = GCRA_NAME_UNKNOWN;
+    const NameTable &t = h->ring_names;
+    if (!t.cap || !n) return GCRA_OK;
+    const cudaStream_t st = h->stream.get();
+    DevBuf<u64> d_hashes;
+    DevBuf<u32> d_len;
+    DevBuf<unsigned char> d_names;
+    CK(d_hashes.make(n));
+    CK(d_len.make(n));
+    CK(d_names.make((size_t)n * GCRA_DENIED_NAME_MAX));
+    CK(cudaMemcpyAsync(d_hashes.get(), key_hashes, n * sizeof(u64), cudaMemcpyHostToDevice, st));
+    CK(launch_ring_names_lookup(t.view(), d_hashes.get(), n, d_len.get(), d_names.get(), st));
+    h->launches++;
+    std::vector<unsigned char> all((size_t)n * GCRA_DENIED_NAME_MAX);
+    CK(cudaMemcpyAsync(lens, d_len.get(), n * sizeof(u32), cudaMemcpyDeviceToHost, st));
+    CK(cudaMemcpyAsync(all.data(), d_names.get(), all.size(), cudaMemcpyDeviceToHost, st));
+    CK(cudaStreamSynchronize(st));
+    for (uint32_t i = 0; i < n; i++)        // (each name's bytes, and no more, as from the denied table)
+        if (lens[i] <= GCRA_DENIED_NAME_MAX)
+            memcpy(names + (size_t)i * GCRA_DENIED_NAME_MAX, &all[(size_t)i * GCRA_DENIED_NAME_MAX], lens[i]);
+    return GCRA_OK;
+}
+
 int32_t gcra_denied_names(gcra_engine *h, uint32_t n, const uint64_t *key_hashes, char *names, uint32_t *lens) {
     CK(cudaSetDevice(h->device));
+    if (h->ring_metrics_sharded) return ring_names_lookup(h, n, key_hashes, names, lens);
     if (!h->denied_max) { h->err = "gcra_track_denied first"; return GCRA_INTERNAL; }
     RC(wait_for_metrics_writers(h));
     for (uint32_t i = 0; i < n; i++) lens[i] = GCRA_NAME_UNKNOWN;

@@ -466,28 +466,38 @@ __global__ void ring_outcome_kernel(const uint2 *__restrict__ conn_rows, const g
 // never an error (redis/mod.rs:193-205); HTTP and gRPC answer status != OK with an error (http.rs:148-151,
 // grpc.rs:177-179).  A warp's rows go to the CTA's 9 counters by ballot, the CTA's to HBM in at most 9 atomic adds.
 // A denied row finds its key's entry in the denied table, which finish_batch counted this batch into before the reply
-// stream went on: the probe of denied_tile_flush (an empty word or 64 probes: the key found the table full).  The
-// first row to CAS the entry's length word from GCRA_NAME_UNKNOWN copies its key bytes.
+// stream went on: the probe of denied_tile_flush (an empty word or 64 probes: the key found the table full).  On a
+// name table (gcra_ring_metrics_sharded: the denied count is on the key's owner, maybe another GPU) the row inserts its
+// key instead, by a CAS of an empty word, and a key that finds the table full is counted in `full`.  The first row to
+// CAS the entry's length word from GCRA_NAME_UNKNOWN copies its key bytes.
 constexpr u32 RING_METRICS_THREADS = 256, DENIED_PROBES = 64;
 
+__device__ __forceinline__ u32 name_home(u64 k, u32 mask) { return (u32)(mix64(k ^ 0x9E3779B97F4A7C15ULL)) & mask; }
+
 __device__ __forceinline__ void ring_metrics_name(const RingMetrics &a, u32 i) {
+    const NameTableView &t = a.names;
     u64 k = a.rows[i].key_hash;
     if (k == 0) k = 1;                                          // (as denied_tile_add stores it)
-    u32 h = (u32)(mix64(k ^ 0x9E3779B97F4A7C15ULL)) & a.denied_mask;
+    u32 h = name_home(k, t.mask);
     for (u32 probe = 0; probe < DENIED_PROBES; probe++) {
-        const u64 cur = a.denied_keys[h];
-        if (cur == 0) return;
+        u64 cur = t.keys[h];
+        if (cur == 0) {
+            if (!a.full) return;
+            cur = atomicCAS(reinterpret_cast<unsigned long long *>(t.keys + h), 0ULL, (unsigned long long)k);
+            if (cur == 0) cur = k;                              // (claimed)
+        }
         if (cur == k) {
-            if (a.name_len[h] != GCRA_NAME_UNKNOWN) return;     // (most denials are of keys named already)
+            if (t.name_len[h] != GCRA_NAME_UNKNOWN) return;     // (most denials are of keys named already)
             const uint2 kr = a.key_ref[i];
             const u32 len = kr.y > GCRA_DENIED_NAME_MAX ? GCRA_NAME_TOO_LONG : kr.y;
-            if (atomicCAS(&a.name_len[h], GCRA_NAME_UNKNOWN, len) != GCRA_NAME_UNKNOWN || len == GCRA_NAME_TOO_LONG) return;
-            unsigned char *dst = a.names + (size_t)h * GCRA_DENIED_NAME_MAX;
+            if (atomicCAS(&t.name_len[h], GCRA_NAME_UNKNOWN, len) != GCRA_NAME_UNKNOWN || len == GCRA_NAME_TOO_LONG) return;
+            unsigned char *dst = t.names + (size_t)h * GCRA_DENIED_NAME_MAX;
             for (u32 b = 0; b < len; b++) dst[b] = a.in[kr.x + b];
             return;
         }
-        h = (h + 1) & a.denied_mask;
+        h = (h + 1) & t.mask;
     }
+    if (a.full) atomicAdd(reinterpret_cast<unsigned long long *>(a.full), 1ULL);
 }
 
 __global__ void __launch_bounds__(RING_METRICS_THREADS) ring_metrics_kernel(RingMetrics a) {
@@ -502,7 +512,7 @@ __global__ void __launch_bounds__(RING_METRICS_THREADS) ring_metrics_kernel(Ring
         const longlong2 tail = reinterpret_cast<const longlong2 *>(a.res + i)[1];
         const bool ok = (u32)tail.y == GCRA_OK, denied = ok && ((tail.y >> 32) & 0xff) == 0;
         cls = (proto - 1) * 3 + (denied ? 1 : ok || proto == GCRA_PROTO_RESP ? 0 : 2);
-        if (denied && a.denied_keys) ring_metrics_name(a, i);
+        if (denied && a.names.keys) ring_metrics_name(a, i);
     }
 #pragma unroll
     for (u32 k = 0; k < 9; k++) {
@@ -516,6 +526,81 @@ __global__ void __launch_bounds__(RING_METRICS_THREADS) ring_metrics_kernel(Ring
 
 cudaError_t launch_ring_metrics(const RingMetrics &a, u32 max_rows, cudaStream_t st) {
     ring_metrics_kernel<<<(max_rows + RING_METRICS_THREADS - 1) / RING_METRICS_THREADS, RING_METRICS_THREADS, 0, st>>>(a);
+    return cudaGetLastError();
+}
+
+// ---- a name table's lookup and rebuild (gcra_denied_names, gcra_ring_names_keep on gcra_ring_metrics_sharded) ----
+// One warp per hash.  The warp reads 32 probes of ring_metrics_name's sequence at a time; the sequence ends at the
+// key's entry or an empty word (entries are never emptied: the table is rebuilt whole), or after 64 probes.
+constexpr u32 NAME_WARPS = 8;
+
+// the entry of key k (0 stored as 1) in t, or -1; warp-uniform
+__device__ __forceinline__ int warp_find_name(const NameTableView &t, u64 k) {
+    const u32 lane = threadIdx.x & 31, home = name_home(k, t.mask);
+    for (u32 base = 0; base < DENIED_PROBES; base += 32) {
+        const u64 cur = t.keys[(home + base + lane) & t.mask];
+        const u32 hit = __ballot_sync(0xffffffffu, cur == k), stop = hit | __ballot_sync(0xffffffffu, cur == 0);
+        if (stop) {
+            const u32 f = __ffs(stop) - 1;
+            return (hit >> f) & 1 ? (int)((home + base + f) & t.mask) : -1;
+        }
+    }
+    return -1;
+}
+
+// a name's bytes, GCRA_DENIED_NAME_MAX-aligned rows: 8 bytes per lane (len <= GCRA_DENIED_NAME_MAX)
+__device__ __forceinline__ void warp_copy_name(unsigned char *dst, const unsigned char *src, u32 len) {
+    static_assert(GCRA_DENIED_NAME_MAX == 32 * 8, "one 8-byte word per lane");
+    const u32 lane = threadIdx.x & 31;
+    if (lane * 8 < len) reinterpret_cast<u64 *>(dst)[lane] = reinterpret_cast<const u64 *>(src)[lane];
+}
+
+__global__ void __launch_bounds__(NAME_WARPS * 32) ring_names_lookup_kernel(NameTableView t, const u64 *hashes, u32 n,
+                                                                             u32 *out_len, unsigned char *out_names) {
+    const u32 w = blockIdx.x * NAME_WARPS + (threadIdx.x >> 5);
+    if (w >= n) return;
+    const int e = warp_find_name(t, hashes[w] ? hashes[w] : 1);
+    const u32 len = e < 0 ? GCRA_NAME_UNKNOWN : t.name_len[e];
+    if ((threadIdx.x & 31) == 0) out_len[w] = len;
+    if (len <= GCRA_DENIED_NAME_MAX)
+        warp_copy_name(out_names + (size_t)w * GCRA_DENIED_NAME_MAX, t.names + (size_t)e * GCRA_DENIED_NAME_MAX, len);
+}
+
+__global__ void __launch_bounds__(NAME_WARPS * 32) ring_names_keep_kernel(NameTableView from, NameTableView to,
+                                                                           const u64 *hashes, u32 n, u64 *full) {
+    const u32 w = blockIdx.x * NAME_WARPS + (threadIdx.x >> 5), lane = threadIdx.x & 31;
+    if (w >= n) return;
+    const u64 k = hashes[w] ? hashes[w] : 1;
+    const int e = warp_find_name(from, k);
+    if (e < 0) return;
+    int d = -1;                                                 // the entry in `to` (-2: a repeated hash)
+    if (lane == 0) {
+        u32 s = name_home(k, to.mask);
+        for (u32 probe = 0; probe < DENIED_PROBES && d == -1; probe++, s = (s + 1) & to.mask) {
+            const u64 cur = atomicCAS(reinterpret_cast<unsigned long long *>(to.keys + s), 0ULL, (unsigned long long)k);
+            if (cur == 0) d = (int)s;
+            else if (cur == k) d = -2;
+        }
+        if (d == -1) atomicAdd(reinterpret_cast<unsigned long long *>(full), 1ULL);
+    }
+    d = __shfl_sync(0xffffffffu, d, 0);
+    if (d < 0) return;
+    const u32 len = from.name_len[e];
+    if (lane == 0) to.name_len[d] = len;
+    if (len <= GCRA_DENIED_NAME_MAX)
+        warp_copy_name(to.names + (size_t)d * GCRA_DENIED_NAME_MAX, from.names + (size_t)e * GCRA_DENIED_NAME_MAX, len);
+}
+
+cudaError_t launch_ring_names_lookup(const NameTableView &t, const u64 *hashes, u32 n, u32 *out_len,
+                                     unsigned char *out_names, cudaStream_t st) {
+    ring_names_lookup_kernel<<<(n + NAME_WARPS - 1) / NAME_WARPS, NAME_WARPS * 32, 0, st>>>(t, hashes, n, out_len,
+                                                                                           out_names);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_ring_names_keep(const NameTableView &from, const NameTableView &to, const u64 *hashes, u32 n,
+                                   u64 *full, cudaStream_t st) {
+    ring_names_keep_kernel<<<(n + NAME_WARPS - 1) / NAME_WARPS, NAME_WARPS * 32, 0, st>>>(from, to, hashes, n, full);
     return cudaGetLastError();
 }
 

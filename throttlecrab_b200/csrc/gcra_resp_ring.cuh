@@ -123,8 +123,18 @@ struct RingParse {
     uint2 *key_ref;              // [row_capacity] out, or null: each row's key {offset in `in`, length}
 };
 
-// ring_metrics_kernel's arguments (gcra_ring_metrics): a finished slot's rows, counted per transport into
-// counts[3 transports][allowed, denied, errors], and their denied keys named from the slot's input
+// A table of key names by key hash: the denied table's keys with their names (gcra_ring_metrics), or a name table of
+// its own (gcra_ring_metrics_sharded), whose keys the rows insert.  Both probe linearly from
+// mix64(k ^ 0x9E3779B97F4A7C15) & mask for at most 64 entries, with key hash 0 stored as 1.
+struct NameTableView {
+    u64 *keys;                       // [entries], 0: empty
+    u32 mask;                        // entries - 1
+    u32 *name_len;                   // [entries] GCRA_NAME_UNKNOWN, GCRA_NAME_TOO_LONG or the name's length
+    unsigned char *names;            // [entries][GCRA_DENIED_NAME_MAX]
+};
+
+// ring_metrics_kernel's arguments (gcra_ring_metrics, gcra_ring_metrics_sharded): a finished slot's rows, counted per
+// transport into counts[3 transports][allowed, denied, errors], and their denied keys named from the slot's input
 struct RingMetrics {
     const gcra_request *rows;
     const gcra_result *res;
@@ -134,13 +144,20 @@ struct RingMetrics {
     const uint2 *key_ref;            // each row's key {offset in `in`, length} (the parse kernel's key_ref)
     const unsigned char *in;         // the slot's device input
     u64 *counts;                     // [9]
-    const u64 *denied_keys;          // the denied table's keys (DeniedTable::keys), or null: no names
-    u32 denied_mask;                 // its entries - 1
-    u32 *name_len;                   // [entries] GCRA_NAME_UNKNOWN, GCRA_NAME_TOO_LONG or the name's length
-    unsigned char *names;            // [entries][GCRA_DENIED_NAME_MAX]
+    NameTableView names;             // keys null: no names
+    u64 *full;                       // null: names' keys are the denied table's (looked up, never inserted); else the
+                                     // name table's, and the denied rows whose key found it full are counted here
 };
 // one thread per row of [0, *total), max_rows >= *total
 cudaError_t launch_ring_metrics(const RingMetrics &a, u32 max_rows, cudaStream_t st);
+// gcra_denied_names on a name table: one warp per hash; out_len[i] its length word (GCRA_NAME_UNKNOWN when absent),
+// out_names[i] its bytes (GCRA_DENIED_NAME_MAX per hash)
+cudaError_t launch_ring_names_lookup(const NameTableView &t, const u64 *hashes, u32 n, u32 *out_len,
+                                     unsigned char *out_names, cudaStream_t st);
+// gcra_ring_names_keep: one warp per hash; each of `hashes` found in `from` is inserted with its name into `to`
+// (empty); a hash that finds `to` full is counted in *full
+cudaError_t launch_ring_names_keep(const NameTableView &from, const NameTableView &to, const u64 *hashes, u32 n,
+                                   u64 *full, cudaStream_t st);
 
 cudaError_t resp_ring_setup();   // once, before the first launch
 // one CTA per connection of a.n_conns

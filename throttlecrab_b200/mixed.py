@@ -14,7 +14,7 @@ from . import REQ_DTYPE, RES_DTYPE, RESP_MAX_CONN_BYTES, RESP_REPLY_MAX, HTTP_RE
 from . import grpc_transport as _gt
 from . import http as _http
 from . import resp as _resp
-from .metrics import Metrics
+from .metrics import Metrics, ShardedMetrics
 
 PROTOCOLS = {"resp": PROTO_RESP, "http": PROTO_HTTP, "grpc": PROTO_GRPC}
 # the smallest plain frame of RESP and HTTP (gcra_resp.cuh, gcra_http.cuh MIN_FRAME_BYTES): room for a walk's rows
@@ -107,9 +107,12 @@ def process_connections_sharded(ranks, now_ns, slot=0, metrics=None):
     goes to its key's owner engine (OwnerRouter).  When no slot's row capacity fills (stop 3), every connection gets
     the bytes process_connections(ring=None) gives on ONE engine over the joined list.
 
-    `metrics` is refused (ValueError): ring metrics do not run on peer-memory rings."""
-    if metrics is not None:
-        raise ValueError("metrics are not served by the sharded driver")
+    `metrics` may be a metrics.ShardedMetrics over the ranks' limiters in rank order: it is GET /metrics for the HTTP
+    connections, and records every request the general paths decide as process_connections does (each rank's GPU
+    counts its ring's rows and names their denied keys).  Anything else is refused (ValueError)."""
+    if metrics is not None and not (isinstance(metrics, ShardedMetrics) and len(metrics.limiters) == len(ranks) and
+                                    all(m is lim for m, (_, lim, _) in zip(metrics.limiters, ranks))):
+        raise ValueError("the sharded driver serves metrics only from a ShardedMetrics of its ranks' limiters")
     now = int(now_ns)
     conns, rank_of = [], []
     for r, (cs, _, ring) in enumerate(ranks):
@@ -142,7 +145,7 @@ def process_connections_sharded(ranks, now_ns, slot=0, metrics=None):
             if all(a == len(m) for a, m in zip(at, mine)):
                 break
 
-    got = _Rounds(conns).run(router, now, None, gpu)
+    got = _Rounds(conns).run(router, now, metrics, gpu)
     out, a = [], 0
     for cs, _, _ in ranks:
         out.append(got[a:a + len(cs)])
