@@ -760,6 +760,84 @@ int32_t gcra_ring_metrics_sharded(gcra_engine *h, uint32_t on, uint32_t max_keys
  * a failed call leaves it as it was); *full = denied rows whose key found the table full since the last keep */
 int32_t gcra_ring_names_keep(gcra_engine *h, uint32_t n, const uint64_t *key_hashes, uint64_t *full);
 
+/* ---- the server: listeners and connections served through the engine's mixed ring ------------------------------
+ * replaces throttlecrab-server's transports (transport/{redis,http,grpc}.rs, main.rs): one loop in the caller's
+ * thread listens on up to three ports, reads every connection's bytes, and serves them through the engine's mixed ring
+ * (gcra_mixed_ring_create, slot 0) with the caller's general path beside it.  It creates no thread and no process.
+ *
+ * gcra_server_create(h, listens, n, general, ctx, &srv): listens[0 .. n) give up to three (protocol, host, port), a
+ * protocol at most once; port 0 binds an ephemeral port (gcra_server_port tells it).  The sockets are non-blocking,
+ * SO_REUSEADDR, backlog 1024.  It refuses (GCRA_INTERNAL, nothing left open, gcra_last_error(h) says why) when the
+ * engine's ring is not a mixed ring or its in_capacity is below GCRA_RESP_MAX_CONN_BYTES, a protocol is outside 1 .. 3
+ * or listed twice, or a bind fails (e.g. the port is in use).  While the server exists the engine's ring slot 0 is
+ * its own.
+ *
+ * gcra_server_read(srv, timeout_ms) waits up to timeout_ms for the sockets, accepts new connections (their ids are
+ * 0, 1, 2, ... in accept order), and reads into each connection's pending bytes, at most GCRA_RESP_MAX_CONN_BYTES
+ * (the rings' per-connection limit).  An EOF is recorded.  It sends pending output the sockets now take.
+ *
+ * gcra_server_serve(srv, now_ns) serves the pending bytes at one clock: exactly mixed.process_connections(conns,
+ * limiter, now_ns, ring) over the open connections with pending bytes, in accept order -- the same rounds, submits
+ * and general-path calls -- then sends what the sockets take.  Per connection afterwards:
+ *   - a general path's close (QUIT, a RESP protocol error, HTTP/1.0 or Connection: close, a gRPC GOAWAY), or an EOF
+ *     received before this serve: its replies are sent, then the socket closes; nothing more is read;
+ *   - GCRA_RESP_MAX_CONN_BYTES pending bytes on which the serve made no progress (a request longer than the rings
+ *     take): the connection closes (counters.full_closed);
+ *   - more than GCRA_SERVER_READ_PAUSE bytes of unsent output: it is not read until they drain below (one serve adds at
+ *     most the replies of 65,536 bytes of requests, so unsent output stays under GCRA_SERVER_OUT_BOUND); unsent
+ *     output waits for the socket to take it.
+ * A gRPC connection's ring state (gcra_grpc_conn: last_stream, send_window, init_window, class bytes) is kept here:
+ * after a ring walk last_stream and send_window - data_sent, and the WINDOW_UPDATE and PING ACK frames appended after
+ * its responses; after a general call, what the callback wrote into the row.
+ *
+ * The general callback runs inside serve, between ring submits, for a connection the ring stopped at a request that
+ * is not plain (stop 2), or a gRPC connection that is not plain_ready: general(ctx, conn_id, protocol, data, len,
+ * now_ns, grpc, out) with the connection's pending bytes; grpc = its gcra_grpc_conn row for a gRPC connection (read
+ * last_stream and send_window from it, write the state back), else NULL.  It fills *out: consumed (<= len), out/out_len
+ * (bytes to send, copied before the callback's next call), close, and for gRPC plain_ready.  Consuming nothing means
+ * an incomplete request.  It returns 0; anything else, or consumed > len, closes that connection without its unsent
+ * output, and serve finishes every other connection's work and then returns GCRA_INTERNAL ("the general path failed on
+ * connection N").  When a connection that has had a general call closes, the callback is called once more with data
+ * and out NULL: forget its state.
+ *
+ * gcra_server_poll = read, then serve.  gcra_server_destroy closes every socket and frees the server (the engine and
+ * its ring stay).  Known differences from the reference: one clock per serve, where the reference stamps each request;
+ * a request longer than 65,536 bytes is not taken (the connection closes), where the reference accepts larger frames. */
+#define GCRA_SERVER_READ_PAUSE (512u << 10)
+#define GCRA_SERVER_OUT_BOUND (1u << 20)
+typedef struct gcra_server gcra_server;
+typedef struct {
+    uint32_t protocol;                 /* GCRA_PROTO_RESP, _HTTP or _GRPC */
+    uint16_t port;                     /* 0: an ephemeral port */
+    uint16_t reserved;
+    const char *host;                  /* numeric address, e.g. "0.0.0.0" or "127.0.0.1" */
+} gcra_listen;
+typedef struct {
+    uint64_t consumed;                 /* bytes of data taken */
+    const void *out;                   /* bytes to send */
+    uint64_t out_len;
+    uint32_t close;                    /* 1: close after out is sent */
+    uint32_t plain_ready;              /* gRPC: 1 the ring may take the connection */
+} gcra_server_general;
+typedef int32_t (*gcra_server_general_fn)(void *ctx, uint64_t conn_id, uint32_t protocol, const void *data,
+                                          uint64_t len, int64_t now_ns, gcra_grpc_conn *grpc,
+                                          gcra_server_general *out);
+typedef struct {
+    uint64_t open, accepted, closed;   /* connections */
+    uint64_t bytes_read, bytes_written;
+    uint64_t rounds, submits, general_calls, general_errors;
+    uint64_t full_closed;              /* closed with a full buffer on which a serve made no progress */
+    uint64_t peak_unsent;              /* the most unsent output any connection held after a serve */
+} gcra_server_counters;
+int32_t gcra_server_create(gcra_engine *h, const gcra_listen *listens, uint32_t n, gcra_server_general_fn general,
+                           void *ctx, gcra_server **out);
+uint16_t gcra_server_port(gcra_server *srv, uint32_t protocol);      /* the bound port, 0 if not listening */
+int32_t gcra_server_read(gcra_server *srv, int32_t timeout_ms);
+int32_t gcra_server_serve(gcra_server *srv, int64_t now_ns);
+int32_t gcra_server_poll(gcra_server *srv, int32_t timeout_ms, int64_t now_ns);
+int32_t gcra_server_stats(gcra_server *srv, gcra_server_counters *out);
+void gcra_server_destroy(gcra_server *srv);
+
 #ifdef __cplusplus
 }
 #endif

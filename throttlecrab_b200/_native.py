@@ -196,6 +196,13 @@ SYMBOLS = {
     "gcra_owner_of": (_u32, [_u64, _u32]),
     "gcra_route_partition": (_i32, [_vp, _u64, _vp, _u32, _vp, _vp, _vp, _vp]),
     "gcra_route_unpermute": (_i32, [_vp, _u64, _vp, _vp, _vp, _vp]),
+    "gcra_server_create": (_i32, [_vp, _vp, _u32, _vp, _vp, C.POINTER(_vp)]),
+    "gcra_server_port": (C.c_uint16, [_vp, _u32]),
+    "gcra_server_read": (_i32, [_vp, _i32]),
+    "gcra_server_serve": (_i32, [_vp, _i64]),
+    "gcra_server_poll": (_i32, [_vp, _i32, _i64]),
+    "gcra_server_stats": (_i32, [_vp, _vp]),
+    "gcra_server_destroy": (None, [_vp]),
 }
 
 _lib = None

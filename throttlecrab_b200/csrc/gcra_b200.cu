@@ -2939,3 +2939,4 @@ int32_t gcra_route_unpermute(gcra_engine *h, uint64_t n, const gcra_result *d_re
 
 #include "gcra_actor.inc"
 #include "gcra_resp.inc"
+#include "gcra_server.inc"

@@ -384,6 +384,11 @@ class Connection:
         row["n_dyn"] = len(cls)
         row["dyn_class"][:len(cls)] = cls
 
+    def take_state(self, row):
+        """take last_stream and send_window from a GRPC_CONN_DTYPE row: what the ring walks since the last general
+        call left (they never change the HPACK table, init_window or the streams, which stay here)"""
+        self.last_stream, self.send_window = int(row["last_stream"]), int(row["send_window"])
+
     def conn_row(self):
         from . import GRPC_CONN_DTYPE
         row = np.zeros((), GRPC_CONN_DTYPE)
