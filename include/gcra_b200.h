@@ -802,7 +802,30 @@ int32_t gcra_ring_names_keep(gcra_engine *h, uint32_t n, const uint64_t *key_has
  *
  * gcra_server_poll = read, then serve.  gcra_server_destroy closes every socket and frees the server (the engine and
  * its ring stay).  Known differences from the reference: one clock per serve, where the reference stamps each request;
- * a request longer than 65,536 bytes is not taken (the connection closes), where the reference accepts larger frames. */
+ * a request longer than 65,536 bytes is not taken (the connection closes), where the reference accepts larger frames.
+ *
+ * gcra_server_create_sharded(hs, world, listens, n, general, ctx, &srv): the same server over `world` engines of ONE
+ * process that share one hash-sharded table (sharded.connect_local, on one GPU or several), hs[r] the engine of rank r.
+ * Read, serve, poll, port, stats and destroy are the same calls.  Besides gcra_server_create's refusals it refuses
+ * (GCRA_INTERNAL, nothing left open, gcra_last_error(hs[0]) says why, naming the rank) when world is 0, when any
+ * engine's ring is not a mixed ring or its in_capacity is below GCRA_RESP_MAX_CONN_BYTES, when any engine is not
+ * gcra_p2p_connect-ed with this world, when hs[r]'s peer-memory rank is not r, or when any engine's ring is not
+ * switched to peer-memory ticks (gcra_ring_p2p(h, 1)).  While the server exists every engine's ring slot 0 is its own.
+ *   - Placement: connection id (accept order, as above) belongs to rank id % world: its bytes go into that rank's slot
+ *     0 input, and its replies come from that rank's output.
+ *   - gcra_server_serve first runs gcra_policy_tick(hs[r], now_ns) on every rank, in rank order (peer-memory ticks do
+ *     not sweep by themselves), then exactly mixed.process_connections_sharded(ranks, now_ns) with ranks[r] rank r's
+ *     open connections with pending bytes, in accept order: every tick routes every rank before the first finish and
+ *     finishes every rank before the next route; a rank whose connections do not all fit its slot leaves the later
+ *     ranks empty ticks; the general paths run after a round's ticks, in the joined order.
+ *   - A refused route (e.g. the table cannot grow) still owes the peers its tick: that rank routes 0 connections, every
+ *     rank finishes and waits, the connections the other ranks placed get their replies, and serve returns the error.
+ *     No connection loses pending bytes, and no peer's wait gives up.
+ *   - counters.submits counts ticks.
+ * Known differences from one engine: connections are placed round-robin by accept order; within a serve decisions run
+ * rank-major (every connection of rank 0, then of rank 1, ...), where one engine decides in accept order; and each
+ * engine applies the store's sweep policy to the keys it owns, so the adaptive and probabilistic stores count
+ * operations per engine. */
 #define GCRA_SERVER_READ_PAUSE (512u << 10)
 #define GCRA_SERVER_OUT_BOUND (1u << 20)
 typedef struct gcra_server gcra_server;
@@ -831,6 +854,8 @@ typedef struct {
 } gcra_server_counters;
 int32_t gcra_server_create(gcra_engine *h, const gcra_listen *listens, uint32_t n, gcra_server_general_fn general,
                            void *ctx, gcra_server **out);
+int32_t gcra_server_create_sharded(gcra_engine *const *hs, uint32_t world, const gcra_listen *listens, uint32_t n,
+                                   gcra_server_general_fn general, void *ctx, gcra_server **out);
 uint16_t gcra_server_port(gcra_server *srv, uint32_t protocol);      /* the bound port, 0 if not listening */
 int32_t gcra_server_read(gcra_server *srv, int32_t timeout_ms);
 int32_t gcra_server_serve(gcra_server *srv, int64_t now_ns);

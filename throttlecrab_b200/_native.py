@@ -197,6 +197,7 @@ SYMBOLS = {
     "gcra_route_partition": (_i32, [_vp, _u64, _vp, _u32, _vp, _vp, _vp, _vp]),
     "gcra_route_unpermute": (_i32, [_vp, _u64, _vp, _vp, _vp, _vp]),
     "gcra_server_create": (_i32, [_vp, _vp, _u32, _vp, _vp, C.POINTER(_vp)]),
+    "gcra_server_create_sharded": (_i32, [_vp, _u32, _vp, _u32, _vp, _vp, C.POINTER(_vp)]),
     "gcra_server_port": (C.c_uint16, [_vp, _u32]),
     "gcra_server_read": (_i32, [_vp, _i32]),
     "gcra_server_serve": (_i32, [_vp, _i64]),

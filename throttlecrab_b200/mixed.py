@@ -110,9 +110,7 @@ def process_connections_sharded(ranks, now_ns, slot=0, metrics=None):
     `metrics` may be a metrics.ShardedMetrics over the ranks' limiters in rank order: it is GET /metrics for the HTTP
     connections, and records every request the general paths decide as process_connections does (each rank's GPU
     counts its ring's rows and names their denied keys).  Anything else is refused (ValueError)."""
-    if metrics is not None and not (isinstance(metrics, ShardedMetrics) and len(metrics.limiters) == len(ranks) and
-                                    all(m is lim for m, (_, lim, _) in zip(metrics.limiters, ranks))):
-        raise ValueError("the sharded driver serves metrics only from a ShardedMetrics of its ranks' limiters")
+    check_sharded_metrics(metrics, [lim for _, lim, _ in ranks])
     now = int(now_ns)
     conns, rank_of = [], []
     for r, (cs, _, ring) in enumerate(ranks):
@@ -151,6 +149,13 @@ def process_connections_sharded(ranks, now_ns, slot=0, metrics=None):
         out.append(got[a:a + len(cs)])
         a += len(cs)
     return out
+
+
+def check_sharded_metrics(metrics, limiters):
+    """ValueError unless `metrics` is None or a metrics.ShardedMetrics over exactly `limiters`, in their order"""
+    if metrics is not None and not (isinstance(metrics, ShardedMetrics) and len(metrics.limiters) == len(limiters) and
+                                    all(m is lim for m, lim in zip(metrics.limiters, limiters))):
+        raise ValueError("the sharded driver serves metrics only from a ShardedMetrics of its ranks' limiters")
 
 
 class OwnerRouter:

@@ -10,6 +10,11 @@ QUIT, GET /health, GET /metrics, a gRPC connection's preface, SETTINGS and HPACK
 back here through one callback, to the general paths the Python drivers use: resp.general, http.general and
 grpc_transport.Connection.general.  A serve is exactly mixed.process_connections over the connections' pending bytes.
 
+With several devices (--device 0,1,...) the server runs one engine per entry, the engines sharing one hash-sharded
+table over peer memory (sharded.connect_local): connections are placed round-robin by accept order, each engine's
+mixed ring parses its own connections and routes their rows to their keys' owners, and a serve is exactly
+mixed.process_connections_sharded over the engines' connections (gcra_server_create_sharded).
+
 Configuration mirrors config.rs: the same flags, THROTTLECRAB_* environment variables and defaults, CLI over env over
 default; one addition, --device / THROTTLECRAB_DEVICE.  --buffer-size bounds the reference's actor channel; here it is
 the ring's row_capacity, the most requests one submit decides.
@@ -29,13 +34,17 @@ from . import (AdaptiveStore, PeriodicStore, ProbabilisticStore, RateLimiter, Mi
                PROTO_RESP, PROTO_HTTP, PROTO_GRPC)
 from . import grpc_transport as _gt
 from . import http as _http
+from . import mixed as _mixed
 from . import resp as _resp
-from .metrics import Metrics, MAX_DENIED_KEYS_LIMIT
+from .metrics import Metrics, ShardedMetrics, MAX_DENIED_KEYS_LIMIT
 
 MAX_CONNS = 16384             # connections per ring submit: more open connections take several submits per round
 IN_CAPACITY = 16 << 20        # bytes of requests per ring submit (256 full connection buffers)
 MAX_BUFFER_SIZE = 1 << 20     # the largest row_capacity: the engine's default max_batch
 READ_PAUSE, OUT_BOUND = 512 << 10, 1 << 20     # GCRA_SERVER_READ_PAUSE, GCRA_SERVER_OUT_BOUND
+# Engines of one process wait for each other in kernels, and a wait kernel must not sit in a hardware queue ahead of
+# the kernel it waits for: several engines need at least this many (INTEGRATION.md, "Serving from N engines")
+MIN_DEVICE_CONNECTIONS = 32
 
 PROTOCOLS = {"redis": PROTO_RESP, "http": PROTO_HTTP, "grpc": PROTO_GRPC}
 _NAMES = {"redis": "Redis", "http": "HTTP", "grpc": "gRPC"}
@@ -68,7 +77,8 @@ FLAGS = [
     ("--max-denied-keys", "THROTTLECRAB_MAX_DENIED_KEYS", 100,
      "Maximum number of denied keys to track in metrics (0 to disable, max: 10000)"),
     ("--log-level", "THROTTLECRAB_LOG_LEVEL", "info", "Log level: error, warn, info, debug, trace"),
-    ("--device", "THROTTLECRAB_DEVICE", 0, "CUDA device of the engine"),
+    ("--device", "THROTTLECRAB_DEVICE", 0,
+     "CUDA device of the engine, or a comma-separated list: one engine per entry (repeats allowed)"),
 ]
 STORE_TYPES = ("periodic", "probabilistic", "adaptive")
 NO_TRANSPORT = ("At least one transport must be specified.\n\n"
@@ -112,7 +122,11 @@ class Config:
     buffer_size: int
     max_denied_keys: int
     log_level: str
-    device: int
+    device: object                    # an int, or a tuple of them for several engines (--device 0,1)
+
+    def devices(self):
+        """the engines' devices, one per engine"""
+        return self.device if isinstance(self.device, tuple) else (self.device,)
 
     def listens(self):
         """[(transport, host, port)] of the enabled transports"""
@@ -124,7 +138,25 @@ def _dest(flag):
     return flag[2:].replace("-", "_")
 
 
+def _devices(text, origin):
+    """--device with a comma-separated list: a tuple of device indices"""
+    out = []
+    for part in text.split(","):
+        if not part.strip():
+            raise ConfigError("invalid value '%s' for '--device': an empty entry (%s)" % (text, origin), 2)
+        try:
+            v = int(part)
+        except ValueError:
+            raise ConfigError("invalid value '%s' for '--device': '%s' is not a number (%s)" % (text, part, origin), 2)
+        if v < 0:
+            raise ConfigError("invalid value '%s' for '--device': %d is out of range (%s)" % (text, v, origin), 2)
+        out.append(v)
+    return tuple(out)
+
+
 def _value(flag, default, text, origin):
+    if flag == "--device" and "," in text:
+        return _devices(text, origin)
     if isinstance(default, bool):
         return text.strip().lower() not in _FALSEY
     if isinstance(default, int):
@@ -186,11 +218,18 @@ def parse_config(argv=None, environ=None):
                           % (cfg.buffer_size, MAX_BUFFER_SIZE), 2)
     if not (cfg.http or cfg.grpc or cfg.redis):
         raise ConfigError(NO_TRANSPORT, 1)
+    conns = environ.get("CUDA_DEVICE_MAX_CONNECTIONS")
+    if len(cfg.devices()) > 1 and conns is not None and not (conns.strip().isdigit() and
+                                                              int(conns) >= MIN_DEVICE_CONNECTIONS):
+        raise ConfigError("CUDA_DEVICE_MAX_CONNECTIONS=%s: several engines need at least %d (their kernels wait for "
+                          "each other, and a waiting kernel must not hold the hardware queue of the one it waits for)"
+                          % (conns, MIN_DEVICE_CONNECTIONS), 2)
     return cfg
 
 
-def make_store(cfg):
-    """store.rs create_rate_limiter: the configured store type, built by its builder"""
+def make_store(cfg, device=None, capacity=None):
+    """store.rs create_rate_limiter: the configured store type, built by its builder (on `device` with `capacity`,
+    default cfg's)"""
     if cfg.store == "periodic":
         b = PeriodicStore.builder().cleanup_interval(cfg.store_cleanup_interval)
     elif cfg.store == "probabilistic":
@@ -198,7 +237,8 @@ def make_store(cfg):
     else:
         b = AdaptiveStore.builder().min_interval(cfg.store_min_interval).max_interval(cfg.store_max_interval) \
             .max_operations(cfg.store_max_operations)
-    return b.capacity(cfg.store_capacity).device(cfg.device).build()
+    return b.capacity(cfg.store_capacity if capacity is None else capacity) \
+        .device(cfg.device if device is None else device).build()
 
 
 class GeneralPathError(RuntimeError):
@@ -225,12 +265,27 @@ class Server:
     paths deciding on the ring's limiter and `metrics` (a metrics.Metrics of the same engine, or None) serving GET
     /metrics.  `listens` is a list of (transport, host, port), transport "redis", "http" or "grpc"; port 0 binds an
     ephemeral port (port(transport) tells it).  read / serve / poll run in the caller's thread; see gcra_server_* in
-    include/gcra_b200.h for what each does."""
+    include/gcra_b200.h for what each does.
+
+    `ring` may also be a list of MixedRings in rank order, of engines connected over peer memory
+    (sharded.connect_local) whose rings are switched to peer-memory ticks (peer_memory(True)): the server then places
+    connection id on rank id % len(rings), a serve is mixed.process_connections_sharded over the ranks' connections,
+    the general paths decide on mixed.OwnerRouter of the rings' limiters, and `metrics` must be None or a
+    metrics.ShardedMetrics of those limiters in rank order (ValueError otherwise)."""
 
     def __init__(self, ring, listens, metrics=None):
-        self.ring, self.limiter, self.metrics = ring, ring.lim, metrics
-        self.store = ring.store
-        self._L, self._h = ring._L, ring._h
+        rings = list(ring) if isinstance(ring, (list, tuple)) else None
+        if rings is not None:
+            if not rings:
+                raise ValueError("no ring")
+            limiters = [r.lim for r in rings]
+            _mixed.check_sharded_metrics(metrics, limiters)
+            self.rings, self.ring, self.limiter = rings, rings[0], _mixed.OwnerRouter(limiters)
+        else:
+            self.rings, self.ring, self.limiter = [ring], ring, ring.lim
+        self.metrics = metrics
+        self.store = self.ring.store
+        self._L, self._h = self.ring._L, self.ring._h
         self._grpc = {}                                     # connection id -> grpc_transport.Connection
         self._keep, self._error = None, None
         self._cb = _GENERAL_FN(self._general)
@@ -241,7 +296,12 @@ class Server:
             arr[i].protocol, arr[i].port, arr[i].host = PROTOCOLS[t], int(port), host.encode()
         srv = C.c_void_p()
         self._srv = None
-        self.store._check(self._L.gcra_server_create(self._h, arr, len(listens), self._cb, None, C.byref(srv)))
+        if rings is None:
+            self.store._check(self._L.gcra_server_create(self._h, arr, len(listens), self._cb, None, C.byref(srv)))
+        else:
+            hs = (C.c_void_p * len(rings))(*[r._h.value for r in rings])
+            self.store._check(self._L.gcra_server_create_sharded(hs, len(rings), arr, len(listens), self._cb, None,
+                                                                 C.byref(srv)))
         self._srv = srv
 
     def port(self, transport):
@@ -315,21 +375,53 @@ class Server:
 
 
 def serve_config(cfg, log):
-    """build the store, the ring, the metrics and the server of `cfg` -> (server, store)"""
-    store = make_store(cfg)
-    try:
-        lim = RateLimiter(store)
-        ring = MixedRing(lim, 1, MAX_CONNS, IN_CAPACITY, cfg.buffer_size)
-        metrics = Metrics(lim, cfg.max_denied_keys)
-        srv = Server(ring, cfg.listens(), metrics)
-    except Exception:
-        store.close()
-        raise
+    """build the stores, the rings, the metrics and the server of `cfg` -> (server, [store per engine])"""
+    devices = cfg.devices()
+    if len(devices) == 1:
+        store = make_store(cfg)
+        try:
+            lim = RateLimiter(store)
+            ring = MixedRing(lim, 1, MAX_CONNS, IN_CAPACITY, cfg.buffer_size)
+            metrics = Metrics(lim, cfg.max_denied_keys)
+            srv = Server(ring, cfg.listens(), metrics)
+        except Exception:
+            store.close()
+            raise
+        stores = [store]
+    else:
+        srv, stores = _serve_sharded(cfg, devices)
     for t, host, _ in cfg.listens():
         log.info("Starting %s transport on %s:%d", _NAMES[t], host, srv.port(t))
     log.info("ThrottleCrab server started with store type: %s", cfg.store.capitalize())
     log.info("Store capacity: %d, Buffer size: %d", cfg.store_capacity, cfg.buffer_size)
-    return srv, store
+    if len(devices) > 1:
+        log.info("Engines: %d, one table sharded over peer memory (%s)", len(devices),
+                 ", ".join("rank %d on cuda:%d" % (r, d) for r, d in enumerate(devices)))
+    return srv, stores
+
+
+def _serve_sharded(cfg, devices):
+    """one engine per device, each with a 1/world share of the capacity, connected over peer memory, each with its
+    mixed ring switched to peer-memory ticks; ShardedMetrics; the server -> (server, stores).  A failed step closes
+    what was made, in reverse order."""
+    from .sharded import connect_local                 # (sharded imports torch: only several engines need it)
+    world = len(devices)
+    made = []                                          # what has a close(), in the order made
+    try:
+        for d in devices:
+            made.append(make_store(cfg, d, -(-cfg.store_capacity // world)))
+        limiters = [RateLimiter(st) for st in made]
+        connect_local(limiters, cfg.buffer_size)
+        rings = [MixedRing(lim, 1, MAX_CONNS, IN_CAPACITY, cfg.buffer_size) for lim in limiters]
+        for ring in rings:
+            ring.peer_memory(True)
+        metrics = ShardedMetrics(limiters, cfg.max_denied_keys)
+        srv = Server(rings, cfg.listens(), metrics)
+    except Exception:
+        for x in reversed(made):
+            x.close()
+        raise
+    return srv, made
 
 
 def main(argv=None):
@@ -340,6 +432,10 @@ def main(argv=None):
         return e.status
     if cfg is None:
         return 0
+    if len(cfg.devices()) > 1:
+        # read when the process first touches CUDA, which nothing imported so far has done (parse_config refused a
+        # value below MIN_DEVICE_CONNECTIONS)
+        os.environ.setdefault("CUDA_DEVICE_MAX_CONNECTIONS", str(MIN_DEVICE_CONNECTIONS))
     level = {"trace": logging.DEBUG, "warn": logging.WARNING}.get(cfg.log_level.lower(),
                                                                      getattr(logging, cfg.log_level.upper(), None))
     logging.basicConfig(stream=sys.stdout, level=level if isinstance(level, int) else logging.INFO,
@@ -348,8 +444,10 @@ def main(argv=None):
     stop = []
     for sig in (signal.SIGINT, signal.SIGTERM):
         signal.signal(sig, lambda s, _f: stop.append(s))
-    srv, store = serve_config(cfg, log)
+    srv, stores = serve_config(cfg, log)
     try:
+        # A signal is seen here, between polls, never inside one: a poll ends every tick it started on every engine,
+        # so no engine is left owing its peers a tick at exit.
         while not stop:
             try:
                 srv.poll(100, time.time_ns())
@@ -357,8 +455,9 @@ def main(argv=None):
                 log.warning("%s", e)
         log.info("Received %s, initiating graceful shutdown...", signal.Signals(stop[0]).name)
     finally:
-        srv.close()
-        store.close()
+        srv.close()                                    # (the server before the engines whose rings it drives)
+        for store in reversed(stores):
+            store.close()
     log.info("ThrottleCrab server shutdown complete")
     return 0
 

@@ -7,6 +7,8 @@ Two client shapes, each client a process of its own:
   - pipelined: 3 x --conns connections (RESP, HTTP, gRPC), each sending --depth requests at once and reading the replies.
 Every request must get exactly one reply.  Prints the GPU, its power limit and the host CPU count, one JSON line per
 run.  Usage: python tools/server_e2e.py [--reps 2] [--requests 10000] [--conns 4096] [--depth 8]
+[--device 0 --device 0,1 ...]: with --device, the native server at each of the given --device values instead, the
+servers alternated as above (rep 0 in the given order, rep 1 reversed, ...).
 """
 import argparse
 import json
@@ -204,9 +206,9 @@ def baseline_server(buffer_size):
 
 # ---- runs --------------------------------------------------------------------------------------------------------------
 def start(kind, buffer_size):
-    if kind == "native":
+    if kind != "python":                                   # "native", or "native --device D"
         cmd = [sys.executable, "-m", "throttlecrab_b200.server", "--redis", "--http", "--grpc",
-               "--buffer-size", str(buffer_size)]
+               "--buffer-size", str(buffer_size)] + kind.split()[1:]
         for t in ("redis", "http", "grpc"):
             cmd += ["--%s-host" % t, "127.0.0.1", "--%s-port" % t, "0"]
     else:
@@ -273,6 +275,7 @@ def main():
     ap.add_argument("--depth", type=int, default=8)
     ap.add_argument("--procs", type=int, default=8, help="client processes per protocol, pipelined shape")
     ap.add_argument("--buffer-size", type=int, default=100_000)
+    ap.add_argument("--device", action="append", help="the native server's --device (repeat to compare several)")
     ap.add_argument("--baseline-server", action="store_true", help=argparse.SUPPRESS)
     a = ap.parse_args()
     if a.baseline_server:
@@ -285,8 +288,9 @@ def main():
     except OSError:
         gpu = "unknown"
     print(json.dumps({"gpu": gpu, "cpus": os.cpu_count(), "nofile": hard}), flush=True)
+    kinds = ["native --device " + d for d in a.device] if a.device else ["native", "python"]
     for rep in range(a.reps):
-        for kind in (("native", "python") if rep % 2 == 0 else ("python", "native")):
+        for kind in (kinds if rep % 2 == 0 else kinds[::-1]):
             print(json.dumps(one_run(kind, a, rep)), flush=True)
 
 
