@@ -362,7 +362,9 @@ uint64_t gcra_launch_count(gcra_engine *h);
 uint32_t gcra_owner_of(uint64_t key_hash, uint32_t n_shards);
 /* stable partition of a device-resident batch by owner shard: writes the requests grouped by
  * owner (order inside a group = input order), per-owner counts, and for every output row its
- * input index.  All pointers are device pointers except none; asynchronous on `stream`. */
+ * input index.  All pointers are device pointers except none; asynchronous on `stream`.
+ * The partition's per-tile counts live in one scratch buffer per engine, which gcra_shard_submit uses too, whatever
+ * stream either is given: an engine's partitions must be ordered, for example issued on one stream. */
 int32_t gcra_route_partition(gcra_engine *h, uint64_t n, const gcra_request *d_req,
                              uint32_t n_shards, gcra_request *d_out, uint32_t *d_src_index,
                              uint32_t *d_counts, void *stream);

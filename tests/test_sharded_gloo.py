@@ -2,7 +2,9 @@
 count exchange, variable-size all-to-all, result return and inverse permutation, and the global
 ordering rule.  The three DEVICE steps (partition / decide / unpermute) are CUDA-only in the
 product; here they are replaced by numpy stand-ins defined in THIS test (the decide stand-in is the
-CPU oracle, used as the checker's engine), so only the routing logic around them is under test."""
+CPU oracle, used as the checker's engine), so only the routing logic around them is under test.  The real kernels
+under the same host logic (ShardedLimiter over gloo with CUDA tensors, worlds 2-4 on one GPU) are tested in
+test_gpu_route_nccl.py."""
 import os
 import socket
 import sys
