@@ -631,7 +631,8 @@ gcra_grpc_outcome *gcra_grpc_ring_outcome(gcra_engine *h, uint32_t slot);  /* pi
  * gcra_resp_ring_input, its protocol and, for a gRPC connection, grpc_state = k, the row of gcra_grpc_ring_conns
  * (h, slot) that holds its HTTP/2 state (whose off and len are not read) and of gcra_grpc_ring_outcome(h, slot) that
  * receives its outcome.  Every other call is the rings' own: gcra_resp_ring_input, _submit, _replies, _outcome, _rows,
- * gcra_ring_wait and gcra_ring_poll.
+ * gcra_ring_wait and gcra_ring_poll.  A submit writes the gRPC outcome rows of its gRPC connections only; the rows
+ * past them hold what an earlier submit wrote, or zeros (every ring's replies and outcomes start zeroed).
  *
  * Contract: for connection c, in table order, with base_c the rows of the connections before it, the GPU takes
  * exactly what its protocol's host walk takes at max_frames = row_capacity - base_c:

@@ -18,6 +18,10 @@ mixed.process_connections_sharded over the engines' connections (gcra_server_cre
 Configuration mirrors config.rs: the same flags, THROTTLECRAB_* environment variables and defaults, CLI over env over
 default; one addition, --device / THROTTLECRAB_DEVICE.  --buffer-size bounds the reference's actor channel; here it is
 the ring's row_capacity, the most requests one submit decides.
+
+Persistence (SNAPSHOT_FLAGS, off by default; the reference keeps its state in memory only): with --snapshot-dir the
+server restores the directory's committed snapshot into its engines before it binds a port, saves in the background
+every --snapshot-interval seconds between serves, and saves once more at shutdown (persist.SnapshotDir).
 """
 import argparse
 import ctypes as C
@@ -37,6 +41,7 @@ from . import http as _http
 from . import mixed as _mixed
 from . import resp as _resp
 from .metrics import Metrics, ShardedMetrics, MAX_DENIED_KEYS_LIMIT
+from .persist import SnapshotDir, SnapshotError
 
 MAX_CONNS = 16384             # connections per ring submit: more open connections take several submits per round
 IN_CAPACITY = 16 << 20        # bytes of requests per ring submit (256 full connection buffers)
@@ -79,6 +84,13 @@ FLAGS = [
     ("--log-level", "THROTTLECRAB_LOG_LEVEL", "info", "Log level: error, warn, info, debug, trace"),
     ("--device", "THROTTLECRAB_DEVICE", 0,
      "CUDA device of the engine, or a comma-separated list: one engine per entry (repeats allowed)"),
+]
+# additions of this server, not of config.rs: persistence, off unless --snapshot-dir is given
+SNAPSHOT_FLAGS = [
+    ("--snapshot-dir", "THROTTLECRAB_SNAPSHOT_DIR", None,
+     "Directory to restore the limits from at start and save them to (unset: state is not persisted)"),
+    ("--snapshot-interval", "THROTTLECRAB_SNAPSHOT_INTERVAL", 60,
+     "Seconds between background saves to the snapshot directory (0: save only at shutdown)"),
 ]
 STORE_TYPES = ("periodic", "probabilistic", "adaptive")
 NO_TRANSPORT = ("At least one transport must be specified.\n\n"
@@ -123,6 +135,8 @@ class Config:
     max_denied_keys: int
     log_level: str
     device: object                    # an int, or a tuple of them for several engines (--device 0,1)
+    snapshot_dir: object = None       # a path, or None: no persistence
+    snapshot_interval: int = 60
 
     def devices(self):
         """the engines' devices, one per engine"""
@@ -167,6 +181,8 @@ def _value(flag, default, text, origin):
         if v < 0 or (flag.endswith("-port") and v > 65535):
             raise ConfigError("invalid value '%s' for '%s': out of range (%s)" % (text, flag, origin), 2)
         return v
+    if flag == "--snapshot-dir" and not text:
+        raise ConfigError("invalid value '' for '--snapshot-dir': an empty path (%s)" % origin, 2)
     if flag == "--store" and text.lower() not in STORE_TYPES:
         raise ConfigError("invalid value '%s' for '--store': Invalid store type: %s. Valid options are: periodic, "
                           "probabilistic, adaptive" % (text, text), 2)
@@ -176,7 +192,7 @@ def _value(flag, default, text, origin):
 def env_vars_text():
     """--list-env-vars: every THROTTLECRAB_* variable, what it sets and its default"""
     lines = ["ThrottleCrab environment variables (CLI arguments take precedence over them):", ""]
-    for flag, env, default, help_ in FLAGS:
+    for flag, env, default, help_ in FLAGS + SNAPSHOT_FLAGS:
         value = "true|false" if isinstance(default, bool) else "<%s>" % flag.rsplit("-", 1)[-1]
         lines.append("  %-48s %s [default: %s]" % (env + "=" + value, help_, str(default).lower()))
     return "\n".join(lines) + "\n"
@@ -190,7 +206,7 @@ def parse_config(argv=None, environ=None):
                                  description="Rate limiting server on the GPU.  At least one transport must be "
                                              "specified.  CLI arguments take precedence over THROTTLECRAB_* "
                                              "environment variables.")
-    for flag, env, default, help_ in FLAGS:
+    for flag, env, default, help_ in FLAGS + SNAPSHOT_FLAGS:
         if isinstance(default, bool):
             ap.add_argument(flag, action="store_const", const=True, default=None, help=help_ + " [env: %s]" % env)
         else:
@@ -201,7 +217,7 @@ def parse_config(argv=None, environ=None):
         sys.stdout.write(env_vars_text())
         return None
     kw = {}
-    for flag, env, default, _ in FLAGS:
+    for flag, env, default, _ in FLAGS + SNAPSHOT_FLAGS:
         cli = getattr(a, _dest(flag))
         if cli is not None:
             kw[_dest(flag)] = cli if isinstance(default, bool) else _value(flag, default, cli, "argument")
@@ -374,12 +390,17 @@ class Server:
             return 1
 
 
-def serve_config(cfg, log):
-    """build the stores, the rings, the metrics and the server of `cfg` -> (server, [store per engine])"""
+def serve_config(cfg, log, snapshots=None):
+    """build the stores, the rings, the metrics and the server of `cfg` -> (server, [store per engine]).  With
+    `snapshots` (a persist.SnapshotDir) its committed generation is restored into the stores as soon as they are made,
+    before anything else is built and before any port is bound; a failed restore closes the stores and raises
+    persist.SnapshotError."""
     devices = cfg.devices()
     if len(devices) == 1:
         store = make_store(cfg)
         try:
+            if snapshots is not None:
+                snapshots.restore([store])
             lim = RateLimiter(store)
             ring = MixedRing(lim, 1, MAX_CONNS, IN_CAPACITY, cfg.buffer_size)
             metrics = Metrics(lim, cfg.max_denied_keys)
@@ -389,7 +410,7 @@ def serve_config(cfg, log):
             raise
         stores = [store]
     else:
-        srv, stores = _serve_sharded(cfg, devices)
+        srv, stores = _serve_sharded(cfg, devices, snapshots)
     for t, host, _ in cfg.listens():
         log.info("Starting %s transport on %s:%d", _NAMES[t], host, srv.port(t))
     log.info("ThrottleCrab server started with store type: %s", cfg.store.capitalize())
@@ -400,16 +421,18 @@ def serve_config(cfg, log):
     return srv, stores
 
 
-def _serve_sharded(cfg, devices):
-    """one engine per device, each with a 1/world share of the capacity, connected over peer memory, each with its
-    mixed ring switched to peer-memory ticks; ShardedMetrics; the server -> (server, stores).  A failed step closes
-    what was made, in reverse order."""
+def _serve_sharded(cfg, devices, snapshots=None):
+    """one engine per device, each with a 1/world share of the capacity (each restoring its shard of `snapshots`
+    before the engines connect), connected over peer memory, each with its mixed ring switched to peer-memory ticks;
+    ShardedMetrics; the server -> (server, stores).  A failed step closes what was made, in reverse order."""
     from .sharded import connect_local                 # (sharded imports torch: only several engines need it)
     world = len(devices)
     made = []                                          # what has a close(), in the order made
     try:
         for d in devices:
             made.append(make_store(cfg, d, -(-cfg.store_capacity // world)))
+        if snapshots is not None:
+            snapshots.restore(made)
         limiters = [RateLimiter(st) for st in made]
         connect_local(limiters, cfg.buffer_size)
         rings = [MixedRing(lim, 1, MAX_CONNS, IN_CAPACITY, cfg.buffer_size) for lim in limiters]
@@ -432,6 +455,13 @@ def main(argv=None):
         return e.status
     if cfg is None:
         return 0
+    snapshots = None
+    if cfg.snapshot_dir is not None:
+        try:                                           # (before any CUDA work: a locked directory refuses the start)
+            snapshots = SnapshotDir(cfg.snapshot_dir, cfg.store)
+        except SnapshotError as e:
+            sys.stderr.write("Error: %s\n" % e)
+            return e.status
     if len(cfg.devices()) > 1:
         # read when the process first touches CUDA, which nothing imported so far has done (parse_config refused a
         # value below MIN_DEVICE_CONNECTIONS)
@@ -444,22 +474,50 @@ def main(argv=None):
     stop = []
     for sig in (signal.SIGINT, signal.SIGTERM):
         signal.signal(sig, lambda s, _f: stop.append(s))
-    srv, stores = serve_config(cfg, log)
+    status = 0
     try:
-        # A signal is seen here, between polls, never inside one: a poll ends every tick it started on every engine,
-        # so no engine is left owing its peers a tick at exit.
-        while not stop:
-            try:
-                srv.poll(100, time.time_ns())
-            except GeneralPathError as e:
-                log.warning("%s", e)
-        log.info("Received %s, initiating graceful shutdown...", signal.Signals(stop[0]).name)
+        if snapshots is not None:
+            snapshots.log = log
+        try:
+            srv, stores = serve_config(cfg, log, snapshots)
+        except SnapshotError as e:                     # (the stores are closed and no port was bound)
+            sys.stderr.write("Error: %s\n" % e)
+            return e.status
+        try:
+            interval = cfg.snapshot_interval
+            due = time.monotonic() + interval
+            # A signal is seen here, between polls, never inside one: a poll ends every tick it started on every
+            # engine, so no engine is left owing its peers a tick at exit, and a save begun here is one cut of the
+            # whole table.
+            while not stop:
+                try:
+                    srv.poll(100, time.time_ns())
+                except GeneralPathError as e:
+                    log.warning("%s", e)
+                if snapshots is not None:
+                    snapshots.poll()
+                    if interval and time.monotonic() >= due:
+                        snapshots.begin()
+                        due = time.monotonic() + interval
+            log.info("Received %s, initiating graceful shutdown...", signal.Signals(stop[0]).name)
+            srv.close()
+            if snapshots is not None:
+                t0 = time.monotonic()
+                try:
+                    g = snapshots.save()
+                    log.info("Saved snapshot generation %d to %s in %.3f s", g, snapshots.path, time.monotonic() - t0)
+                except SnapshotError as e:
+                    log.error("%s", e)
+                    status = 1
+        finally:
+            srv.close()                                # (the server before the engines whose rings it drives)
+            for store in reversed(stores):
+                store.close()
     finally:
-        srv.close()                                    # (the server before the engines whose rings it drives)
-        for store in reversed(stores):
-            store.close()
+        if snapshots is not None:
+            snapshots.close()
     log.info("ThrottleCrab server shutdown complete")
-    return 0
+    return status
 
 
 if __name__ == "__main__":
